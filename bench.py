@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py — tokens/s of the llama2.zig decode hot path on B200, with its HBM roofline.
+"""bench.py — tokens/s of the llama2.zig decode hot path on H100, with its HBM roofline.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--workload ...]
+                  [--dump-outputs DIR]
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 \
          --master-port P bench.py --gpus N --steps K --warmup W
 
@@ -23,9 +24,12 @@ A "step" is ONE decode run of the workload's positions from an empty KV cache.
                every position pays its H2D (token,pos) and D2H (vocab*4 bytes of logits).
   roofline   = dominant kernel's algorithmic bytes / its CUDA-event duration inside real steps,
                against the measured HBM copy bandwidth in MEASURED_PEAKS.json.
-  cpu_baseline = the oracle's -O3 build (a C port of the reference, NOT the Zig binary: no Zig
-               toolchain exists here) on one host core, on a bounded sample.
+  cpu_baseline = the oracle's -O3 build (a C port of the reference, NOT the Zig binary: the
+               project builds no Zig toolchain) on one host core, on a bounded sample.
 `--impl reference` times that CPU port alone and prints the same JSON shape.
+`--dump-outputs DIR` writes what the last timed step of the headline workload computed as DIR/<name>.npy
+(float32 / float64): its tokens, the logits and residual stream x of its last position, and a fixed
+seeded sample of the KV cache it filled.  The inputs depend only on the arguments.  Single-GPU arm only.
 """
 import argparse
 import ctypes as C
@@ -51,7 +55,9 @@ WORKLOADS = {
     "llama2-7B": ("llama2-7B", 256, False),
 }
 SYNTH_SEED = {"stories15M": 15, "stories110M": 110, "llama2-7B": 7}
-L2_FLUSH_BYTES = 256 << 20   # > 126 MB L2
+L2_FLUSH_BYTES = 256 << 20   # > 50 MB L2
+HBM_NOMINAL_GBS = 3350.0     # H100 SXM data sheet (700 W card); not a measured figure
+DUMP_KV_SAMPLE = 1 << 20     # KV-cache elements drawn per cache for --dump-outputs
 SYNTH_DESC = "synthetic (counter-based N(0,s) weights, same generator on GPU and CPU; teacher-forced tokens)"
 
 
@@ -85,7 +91,7 @@ def measured_peak():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return HBM_NOMINAL_GBS, "fallback (H100 SXM data sheet, not measured)"
 
 
 class ClockSampler:
@@ -221,28 +227,16 @@ def run_reference_arm(args, rank, world):
 # ----------------------------------------------------------------------------------------------
 # GPU arm
 # ----------------------------------------------------------------------------------------------
-def kernel_source_sha():
-    import hashlib
-    h = hashlib.sha256()
-    for fn in ("l2b_device.cuh", "llama2_b200.cu"):
-        with open(os.path.join(ROOT, "llama2.zig_b200", "csrc", fn), "rb") as f:
-            h.update(f.read())
-    return h.hexdigest()[:16]
-
-
-def ncu_traffic(workload, kernel):
-    """roofline.traffic = dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant
-    kernel.  It can only come from an `ncu --set full` capture (never from a run under this script), so
-    it is taken from profiles/r02_traffic.json — but ONLY if that capture was made from the kernel
-    sources this run was built from (sha recorded by scripts/summarize_ncu.py); otherwise null."""
-    try:
-        rec = json.load(open(os.path.join(ROOT, "profiles", "r02_traffic.json")))
-        if rec.get("kernel_source_sha16") != kernel_source_sha():
-            return None, None
-        e = rec[workload][kernel]
-        return float(e["traffic"]), e.get("source")
-    except Exception:
-        return None, None
+def dump_outputs(t, ck, positions, tokens, out_dir):
+    """What the last timed step computed, as out_dir/<name>.npy (~8.5 MB for llama2-7B)."""
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"tokens": tokens.astype(np.float64), "logits": t.state("logits"), "x": t.state("x")}
+    for name in ("key_cache", "value_cache"):
+        kv = t.state(name).reshape(ck.n_layers, ck.seq_len, -1)[:, :positions].reshape(-1)
+        idx = np.unique(np.random.default_rng(1234).integers(0, kv.size, DUMP_KV_SAMPLE))
+        arrays[name + "_sample"] = kv[idx]
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def load_host_twin():
@@ -288,7 +282,7 @@ def tp_parity(t, ck, workload, rank, device, n_pos=4):
             "ok": bool(worst <= 1e-4 and argmax_equal)}
 
 
-def run_workload(workload, args, rank, world, dist, sync, flush, clock_index):
+def run_workload(workload, args, rank, world, dist, sync, flush, clock_index, dump_dir=None):
     """Returns the result dict for one workload (all ranks participate; rank 0's dict is complete)."""
     import torch
     import llama2_zig_b200 as l2b
@@ -322,10 +316,13 @@ def run_workload(workload, args, rank, world, dist, sync, flush, clock_index):
         data_desc = SYNTH_DESC
         forced = teacher_tokens(positions + 1, ck.vocab_size)[1:]
 
+    last_tokens = []
+
     def device_run():
         t.reset()
         out = t.generate_argmax(1, 0, positions, forced=forced, stop_on_bos=False)
         assert len(out) == positions
+        last_tokens[:] = [out]
         return t.last_timing()
 
     host_lib, GenOptions, GenResult = load_host_twin()
@@ -357,6 +354,8 @@ def run_workload(workload, args, rank, world, dist, sync, flush, clock_index):
             step_s.append(time.perf_counter() - t0)
             dev_ms.append(ms)
             launches += k
+        if dump_dir:
+            dump_outputs(t, ck, positions, last_tokens[0], dump_dir)
         # ---- e2e: same positions through l2b_forward with host buffers
         e2e_s, h2d, d2h = [], 0, 0
         for _ in range(max(1, min(args.steps, 5))):
@@ -408,7 +407,6 @@ def run_workload(workload, args, rank, world, dist, sync, flush, clock_index):
     kernels = {n: {"ms": a[0] / a[2], "bytes": a[1] // a[2], "gbs": (a[1] / a[2]) / (a[0] / a[2] * 1e-3) / 1e9,
                    "launches_sampled": a[2]} for n, a in acc.items()}
     dom = max(kernels, key=lambda n: kernels[n]["bytes"] * kernels[n]["launches_sampled"])
-    traffic, traffic_src = ncu_traffic(workload, dom) if world == 1 else (None, None)
     value = positions * args.steps / tot
     out = {
         "workload": workload, "positions": positions, "value": value,
@@ -419,16 +417,15 @@ def run_workload(workload, args, rank, world, dist, sync, flush, clock_index):
                 "path": "C++ host loop (twin of src/main.zig:995-1042) -> l2b_forward(host logits) -> host argmax",
                 "device_argmax_variant": (positions / float(np.mean(am_s))) if am_s else None},
         "roofline": {"bound": "hbm", "kernel": dom, "achieved": kernels[dom]["gbs"], "peak": peak, "unit": "GB/s",
-                     "frac": kernels[dom]["gbs"] / peak, "traffic": traffic, "traffic_source": traffic_src,
-                     "frac_of_8TBps_nominal": kernels[dom]["gbs"] / 8000.0, "peak_source": peak_src,
+                     "frac": kernels[dom]["gbs"] / peak,
+                     "frac_of_nominal": kernels[dom]["gbs"] / HBM_NOMINAL_GBS, "peak_source": peak_src,
                      "algorithmic_bytes_per_launch": kernels[dom]["bytes"],
                      "avg_launch_ms": kernels[dom]["ms"]},
         "whole_step": {"algorithmic_bytes_per_run_per_gpu": int(step_bytes_total),
                        "achieved_gbs_per_gpu": step_bytes_total * args.steps / (dev_tot * 1e-3) / 1e9,
                        "frac_of_peak": step_bytes_total * args.steps / (dev_tot * 1e-3) / 1e9 / peak,
-                       "frac_of_8TBps_nominal": step_bytes_total * args.steps / (dev_tot * 1e-3) / 1e9 / 8000.0,
-                       "note": "stories15M's 61 MB of weights stay in the 126 MB L2 after the first token"
-                               if workload == "stories15M" else "weights exceed L2: HBM-served"},
+                       "frac_of_nominal": step_bytes_total * args.steps / (dev_tot * 1e-3) / 1e9 / HBM_NOMINAL_GBS,
+                       "note": "weights exceed the 50 MB L2: HBM-served"},
         "kernels": kernels, "clocks": clocks.summary(), "data": data_desc,
         "weights_bytes_per_token_per_gpu": int(wbytes),
     }
@@ -462,17 +459,24 @@ def main():
     ap.add_argument("--in-process", type=int, default=0, metavar="N",
                     help="ONE process drives N GPUs (l2b_create(.., n_gpus=N), what the Zig CLI's --gpus uses) "
                          "instead of one process per GPU; run without torchrun")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs of the headline workload as DIR/<name>.npy "
+                         "(single-GPU arm only)")
     args = ap.parse_args()
 
     rank = int(os.environ.get("RANK", 0))
     world = int(os.environ.get("WORLD_SIZE", 1))
+    if args.dump_outputs and (args.impl != "b200" or world > 1 or args.in_process > 1):
+        # under tensor parallelism the argmax loop leaves the gathered logits unwritten and every
+        # rank holds only its shard of the KV cache, so only the single-GPU arm can dump its step
+        raise SystemExit("--dump-outputs needs the single-GPU arm (--impl b200, one process, one GPU)")
     if args.impl == "reference":
         run_reference_arm(args, rank, world)
         return
 
     import torch
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py needs a B200: there is no CPU fallback for the hot path")
+        raise SystemExit("bench.py needs an H100: there is no CPU fallback for the hot path")
     dist = None
     if world > 1:
         import torch.distributed as dist
@@ -493,7 +497,7 @@ def main():
 
     workload = pick_workload(args)
     clock_index = int(os.environ.get("LOCAL_RANK", 0))
-    main_res = run_workload(workload, args, rank, world, dist, sync, flush, clock_index)
+    main_res = run_workload(workload, args, rank, world, dist, sync, flush, clock_index, args.dump_outputs)
     also = {}
     if world == 1 and args.also != "none" and args.in_process <= 1:
         extra = ["stories15M", "stories110M"] if args.also == "auto" else [w for w in args.also.split(",") if w]

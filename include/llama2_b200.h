@@ -1,5 +1,5 @@
 /*
- * llama2_b200.h — C ABI of the B200 (sm_100a) decode hot path for cgbur/llama2.zig.
+ * llama2_b200.h — C ABI of the H100 (sm_90a) decode hot path for cgbur/llama2.zig.
  *
  * This library replaces ONE internal call of the reference,
  *     transformer(token, pos, &config, &state, &weights)      src/main.zig:285, call site :996
@@ -15,7 +15,7 @@
  *   - host pointers are borrowed for the duration of the call only;
  *   - one context = one decode stream on 1, 2, 4 or 8 GPUs; not thread-safe (the reference is
  *     single-threaded);
- *   - there is NO CPU fallback: if no sm_100 device is usable the call fails with
+ *   - there is NO CPU fallback: if no sm_90 device is usable the call fails with
  *     L2B_ERR_CUDA / L2B_ERR_NO_DEVICE.
  */
 #ifndef LLAMA2_B200_H

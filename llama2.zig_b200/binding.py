@@ -1,6 +1,6 @@
 """ctypes binding of include/llama2_b200.h (the C ABI that replaces transformer()).
 
-Function names follow the reference (/root/reference/src/main.zig): `Transformer.forward`
+Function names follow the reference (src/main.zig): `Transformer.forward`
 is `transformer(token, pos, ...)` (:285), and the module-level `matmul`, `rmsnorm`,
 `softmax`, `vector_weighted_sum_rows` run the same device code on host buffers so the
 reference's unit tests (:1078-1150) can be replayed against the GPU.

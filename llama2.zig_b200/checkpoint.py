@@ -1,7 +1,7 @@
 """Legacy llama2.c checkpoint files: 28-byte header + flat fp32 payload.
 
 Mirrors what the reference's host does before the hot path starts
-(/root/reference/src/main.zig:936-967: read ConfigReader, sign of vocab_size => shared
+(src/main.zig:936-967: read ConfigReader, sign of vocab_size => shared
 classifier, slurp the rest of the file).  Host-side plumbing only; no arithmetic.
 """
 import os

@@ -1,8 +1,8 @@
-// l2b_device.cuh — sm_100a device building blocks for the llama2.zig decode step.
+// l2b_device.cuh — sm_90a device building blocks for the llama2.zig decode step.
 //
 // Everything here is fp32 and HBM/L2-bandwidth bound (batch-1 decode is a vector
 // contraction: 0.5 flop per weight byte), so there is deliberately no tensor-core code.
-// What matters on B200 for this path: 128-bit coalesced streaming loads with many of them
+// What matters on H100 for this path: 128-bit coalesced streaming loads with many of them
 // in flight per SM, the activation vector staged once per CTA into shared memory by a TMA
 // bulk copy (cp.async.bulk + mbarrier), persistent CTAs sized from the SM count, and
 // warp-shuffle reductions.
@@ -763,9 +763,9 @@ __global__ void __launch_bounds__(NT, 2) gemv8_kernel(const GemvParams p) {
 
 // ---- v3: TMA-fed streaming GEMV for bandwidth-bound shapes.
 //
-// Measured on this B200 (profiles/microbench/read_bw.cu): a pure read stream needs ~128 KB in
+// A pure read stream needs ~128 KB in
 // flight per SM; register-fed LDG loops only get there with >= 1024 resident threads per SM,
-// while a shared-memory ring filled by cp.async.bulk reaches 7.2 TB/s with one small CTA.  So:
+// while a shared-memory ring filled by cp.async.bulk keeps as many bytes in flight with one small CTA.  So:
 // one persistent CTA per SM; a producer thread streams 32 KB stages (8 rows x 256 float4, one
 // 4 KB bulk copy per row) of this CTA's contiguous row range into an NSTAGE ring, starting
 // BEFORE griddepcontrol.wait (weights are immutable), so the ring is already full when the
@@ -1258,7 +1258,7 @@ __global__ void __launch_bounds__(NT) attention_kernel(const AttnParams p) {
 // ---------------------------------------------------------------------------------------
 // attention, flash-decoding form (default).  The three-pass kernel above has a long dependent
 // chain (scores -> barrier -> max -> barrier -> exp -> barrier -> sum -> V pass -> barrier ->
-// fold; 9.7 us per layer at pos 40 on llama2-7B, profiles/r01_trace_7b.txt).  Here every group
+// fold).  Here every group
 // of LPR lanes owns whole timeline rows and keeps a running (max, sum, weighted V slice) in
 // registers, with the K and V loads of two rows in flight together, so the only barriers are the
 // two around the final merge of the 8 * (32/LPR) groups in shared memory.
@@ -1463,7 +1463,7 @@ __global__ void __launch_bounds__(NT) attention_flash_kernel(const AttnParams p)
 // ---------------------------------------------------------------------------------------
 // Small models (stories15M / 110M): a decode step there is a chain of ~3 us kernels that move
 // <= 2 MB each, so the step time is the NUMBER of kernels.  One fusion survived measurement
-// (profiles/r02_small_models.md; the fused-FFN kernel and the all-layers cluster kernel that were
+// (the fused-FFN kernel and the all-layers cluster kernel that were
 // also built are parked in scripts/experiments/):
 //
 // attn_wo_kernel: attention of one head (:361-389) + that head's column slice of wo (:392) in one

@@ -1,4 +1,4 @@
-// llama2_b200.cu — C ABI (include/llama2_b200.h) over the sm_100a kernels in l2b_device.cuh.
+// llama2_b200.cu — C ABI (include/llama2_b200.h) over the sm_90a kernels in l2b_device.cuh.
 //
 // Replaces transformer() of the reference (src/main.zig:285-430) and the device-side
 // equivalents of Weights.init (:73-115) / RunState.init (:137-154).  Pure CUDA runtime:
@@ -456,7 +456,7 @@ int launch_gemv(l2b_ctx *ctx, int epi, const GemvParams &p, cudaStream_t st, con
     if (ctx->force_kernel >= 2) big = true;
     // TMA-ring kernel: only x is staged in shared memory, the rest of the SM's 227 KB is the ring
     // (measured: 5-6 stages of 32 KB on ONE CTA per SM beat 2 x 3 stages and beat leaving half
-    // the SM to the successor kernel's pre-fill; profiles/r01_tma_ring_variants.md)
+    // the SM to the successor kernel's pre-fill)
     const size_t stage_bytes = (size_t)TMA_STAGE_FLOATS * 4;
     const size_t xonly = (size_t)p.n * 4;
     int nstage = ctx->tma_stages > 0 ? ctx->tma_stages : (int)(((size_t)kMaxSmemOptin - xonly) / stage_bytes);
@@ -974,7 +974,7 @@ int create_rank(l2b_ctx *ctx, const l2b_config *cfg, const Source &src, const fl
                 const float *rope_sin, int rank, int world, int device) {
     cudaDeviceProp prop{};
     if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) { ctx->err = "cudaGetDeviceProperties failed"; g_create_error = ctx->err; return L2B_ERR_CUDA; }
-    if (prop.major != 10) { ctx->err = "device is not compute capability 10.x (built for sm_100a only)"; g_create_error = ctx->err; return L2B_ERR_NO_DEVICE; }
+    if (prop.major != 9 || prop.minor != 0) { ctx->err = "device is not compute capability 9.0 (built for sm_90a only)"; g_create_error = ctx->err; return L2B_ERR_NO_DEVICE; }
     ctx->cfg = *cfg;
     ctx->rank = rank; ctx->world = world; ctx->device = device;
     ctx->num_sms = prop.multiProcessorCount;
@@ -1042,9 +1042,10 @@ int create_rank(l2b_ctx *ctx, const l2b_config *cfg, const Source &src, const fl
     L2B_TRY(dev_alloc(ctx, &ctx->X, dim));
     L2B_TRY(dev_alloc(ctx, &ctx->Xalt, dim));
     {
-        // small-model fusion (measured on B200, profiles/r02_small_models.md): attention + wo as one
-        // cluster kernel (8 CTAs per head) is +7 % on stories15M (31 -> 25 kernels per token) and -1 % on
-        // stories110M, so it is on for dim <= 512 only (L2B_FUSE=0|1 overrides)
+        // small-model fusion: attention + wo as one cluster kernel (8 CTAs per head; 4 or 2 are slower
+        // on H100) is +1.0 % on stories15M on H100 and +0.5 % on stories110M, too little there to change
+        // its summation order, so it is on for dim <= 512 only (L2B_FUSE=0|1 overrides;
+        // results/h100_policy_ab.txt)
         const char *ef = getenv("L2B_FUSE");
         const int want = ef ? atoi(ef) : (dim <= 512 ? 1 : 0);
         size_t smem_aw = 0;
@@ -1463,7 +1464,7 @@ const char *l2b_status_string(int32_t s) {
     case L2B_ERR_INVALID_ARG: return "invalid argument";
     case L2B_ERR_UNSUPPORTED: return "unsupported shape";
     case L2B_ERR_CUDA: return "CUDA error";
-    case L2B_ERR_NO_DEVICE: return "no usable sm_100 device";
+    case L2B_ERR_NO_DEVICE: return "no usable sm_90 device";
     case L2B_ERR_OOM: return "out of memory";
     case L2B_ERR_COMM: return "communication error";
     case L2B_ERR_STATE: return "call order violated";

@@ -1,5 +1,5 @@
 // llama2_b200 — command-line twin of the reference's `llama2` binary (src/main.zig:823-1051)
-// with transformer() served by the B200 library.  Same flags and usage text (:800-813).
+// with transformer() served by the H100 library.  Same flags and usage text (:800-813).
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>

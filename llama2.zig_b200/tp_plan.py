@@ -55,7 +55,7 @@ def shard_plan(ck, rank, world):
 
 def payload_views(ck):
     """Full tensors as numpy views over the checkpoint payload, in file order
-    (/root/reference/src/main.zig:85-112)."""
+    (src/main.zig:85-112)."""
     import numpy as np
     dim, hid, L, V, S = ck.dim, ck.hidden_dim, ck.n_layers, ck.vocab_size, ck.seq_len
     hs = dim // ck.n_heads

@@ -1,6 +1,6 @@
 /*
  * llama2_oracle.c — CPU parity oracle (TEST INFRASTRUCTURE, see llama2_oracle.h).
- * Restates /root/reference/src/main.zig:285-713 plus the checkpoint layout
+ * Restates src/main.zig:285-713 plus the checkpoint layout
  * (:73-115, :936-967) and the temperature-0 generation loop (:995-1042).
  */
 #define _POSIX_C_SOURCE 200809L

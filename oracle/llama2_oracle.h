@@ -5,7 +5,7 @@
  * bench.py's cpu_baseline / `--impl reference` legs may load this library.  The
  * product (libllama2_b200.so) never links, loads or calls anything in oracle/.
  *
- * What it is: a plain-C restatement of /root/reference/src/main.zig:285-713
+ * What it is: a plain-C restatement of src/main.zig:285-713
  * (transformer() and the numeric helpers it calls) that keeps the reference's
  * exact SIMD lane / accumulator summation order, parameterised by the vector
  * width W = DEFAULT_VECTOR_WIDTH (src/main.zig:7; 4, 8 or 16 depending on the

@@ -1,6 +1,5 @@
 // Parked experiment (round 2): rmsnorm + w1/w3 + SiLU + the matching column slice of w2 per 32 hidden units in
-// one kernel.  Parity-green, slower than the PDL-chained w13_silu + w2 kernels on every model
-// (profiles/r02_small_models.md).  Was part of csrc/l2b_device.cuh; needs GemvParams / gemv_stage_input from there.
+// one kernel.  Parity-green; not part of the build and not measured on H100.  Was part of csrc/l2b_device.cuh; needs GemvParams / gemv_stage_input from there.
 constexpr int FFN_HSZ = 32;       // hidden units per CTA = NT / 8 (one (w1, w3) row pair per 8-lane group)
 constexpr int FFN_MAXU = 16;      // float4 columns per lane: dim <= 8 * 16 * 4 = 512
 struct FfnParams {

@@ -17,8 +17,8 @@
 // the consumers read it through DSMEM after the barrier (a slice buffer is rewritten five barriers
 // later, so no reader can still be on it).  The first weight tile of the NEXT phase is requested
 // before each barrier, so its L2 round trip overlaps the barrier and the gather.
-// Only 16 SMs work on the layers (16 x ~120 GB/s out of L2 ~ 2 TB/s: 24 MB of stories15M layer weights
-// in ~12 us); the classifier (60 % of the bytes) stays a separate full-chip kernel.
+// Only 16 SMs work on the layers, so each phase is bound by those SMs' L2 ports; the classifier
+// (60 % of the bytes) stays a separate full-chip kernel.
 #pragma once
 
 #include <cooperative_groups.h>

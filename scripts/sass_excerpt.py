@@ -1,9 +1,9 @@
 #!/usr/bin/env python
-"""Writes profiles/<tag>_sass_excerpt.md: per hot kernel of libllama2_b200.so, the SASS mnemonics that
-prove the Blackwell-native mechanisms (VERDICT r1 #9): UBLKCP = cp.async.bulk (TMA bulk copy),
+"""Prints a markdown excerpt: per hot kernel of libllama2_b200.so, the SASS mnemonics that
+prove the Hopper-native mechanisms (VERDICT r1 #9): UBLKCP = cp.async.bulk (TMA bulk copy),
 SYNCS = mbarrier ops, ACQBULK/PREEXIT = griddepcontrol.wait / launch_dependents (PDL),
 LDG.E.128 / LDS.128 = 128-bit loads, STG/LDG.E.128.STRONG.SYS = the LL units that cross NVLink.
-Runs here (no GPU): `python scripts/sass_excerpt.py r02`."""
+Needs no GPU: `python scripts/sass_excerpt.py TAG > sass_excerpt.md`."""
 import collections
 import os
 import re
@@ -32,7 +32,7 @@ HOT = ["gemv_tma_kernel<2>", "gemv_tma_kernel<3>", "gemv_tma_kernel<5>", "gemv_t
        "gemv_tma_kernel<1>", "gemv_kernel<32, 2>", "gemv_kernel<8, 1>", "attention_flash_kernel<3>",
        "attention_flash_kernel<8>", "attn_wo_kernel", "ffn_fused_kernel", "advance_kernel", "gather_logits_kernel",
        "sample_prep_kernel"]
-out = [f"# SASS evidence, {tag} (cuobjdump -sass llama2.zig_b200/lib/libllama2_b200.so; single sm_100a cubin)", "",
+out = [f"# SASS evidence, {tag} (cuobjdump -sass llama2.zig_b200/lib/libllama2_b200.so; single sm_90a cubin)", "",
        "ELF list: " + ", ".join(l.split()[-1] for l in elf.splitlines() if "sm_" in l), "",
        "Counts of the mnemonics that matter per hot kernel (EPI template index: 0 store, 1 argmax, 2 qkv+rope, "
        "3 silu, 4 tensor-parallel LL exchange, 5 residual add):", "",
@@ -61,6 +61,4 @@ for short, body in picked:
     if "gemv_tma_kernel<3>" in short:
         out += [l.rstrip()[:150] for l in body if re.search(r"\bLDG\.E\.128\.STRONG\.SYS", l)][:2]
 out += ["```", ""]
-path = os.path.join(ROOT, "profiles", f"{tag}_sass_excerpt.md")
-open(path, "w").write("\n".join(out))
-print(path)
+print("\n".join(out))

@@ -1,11 +1,10 @@
-"""Turn ncu outputs (read here, on the CPU box) into the small tracked summaries under profiles/.
+"""Turn Nsight Compute outputs into small markdown / JSON summaries (on any machine with ncu).
 
-  python scripts/summarize_ncu.py launches gpurun_out/launches_X.csv   > profiles/rNN_launches_X.md
-  python scripts/summarize_ncu.py full     gpurun_out/prof_X.ncu-rep   > profiles/rNN_ncu_X.md
-  python scripts/summarize_ncu.py traffic  gpurun_out/prof_X.ncu-rep WORKLOAD LABEL 'REGEX' SHA16 profiles/rNN_traffic.json
+  python scripts/summarize_ncu.py launches launches_X.csv   > launches_X.md
+  python scripts/summarize_ncu.py full     prof_X.ncu-rep   > ncu_X.md
+  python scripts/summarize_ncu.py traffic  prof_X.ncu-rep WORKLOAD LABEL 'REGEX' SHA16 traffic.json
       (adds dram__bytes_read.sum + dram__bytes_write.sum per launch of the kernels matching REGEX as
-       WORKLOAD/LABEL, tagged with the kernel-source sha the capture was built from: bench.py only
-       reports roofline.traffic when that sha equals the running build's)
+       WORKLOAD/LABEL, tagged with the kernel-source sha the capture was built from)
 """
 import collections
 import csv

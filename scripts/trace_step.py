@@ -1,5 +1,5 @@
 """In-kernel timeline of one llama2-7B decode step (graph + PDL), from %globaltimer stamps.
-Run on the GPU box:  python scripts/trace_step.py [workload] > gpurun_out/trace.txt
+Run on the GPU box:  python scripts/trace_step.py [workload] > trace.txt
 Tensor parallel: launch it under torchrun (one process per GPU); rank 0 prints its own timeline."""
 import ctypes as C
 import os

@@ -10,25 +10,15 @@ for p in (ROOT, os.path.join(ROOT, "tests")):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs a real H100 (run with -m gpu on a GPU machine)")
     config.addinivalue_line("markers", "slow: multi-GB allocations (full llama2-7B shape)")
 
 
-def stories15m_path():
-    """Real stories15M.bin: staged by __graft_entry__.build() into assets/ (the GPU box has no
-    /root/reference), or straight from the reference mount in the build container."""
-    for p in (os.path.join(ROOT, "assets", "stories15M.bin"), "/root/reference/stories15M.bin"):
-        if os.path.exists(p):
-            return p
-    return None
-
-
 @pytest.fixture(scope="session")
-def stories15m():
-    p = stories15m_path()
-    if p is None:
-        pytest.skip("stories15M.bin not staged (run __graft_entry__.build() where /root/reference exists)")
-    return p
+def stories15m(tmp_path_factory, oracle):
+    """Path of a stories15M-shaped checkpoint file with seeded synthetic weights
+    (oracle_lib.write_stories15m_checkpoint; the golden fixtures are computed on it)."""
+    return oracle.write_stories15m_checkpoint(str(tmp_path_factory.mktemp("ckpt") / "stories15M.bin"))
 
 
 @pytest.fixture(scope="session")

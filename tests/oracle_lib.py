@@ -147,3 +147,34 @@ def synth_checkpoint(cfg, shared_weights, seed, kind="strict"):
     data = np.empty(n, dtype=np.float32)
     lib.orc_synth_checkpoint(C.byref(cfg), int(shared_weights), seed, _fp(data))
     return data
+
+
+# stories15M shape, synthetic weights.  Seed 10 keeps every greedy step's top-2 logit margin >= 0.016
+# over all 256 positions (the shipped stories15M.bin has 0.0100), so free-running streams are stable.
+STORIES15M_SHAPE = (288, 768, 6, 6, 6, 32000, 256)
+STORIES15M_SEED = 10
+
+
+def write_stories15m_checkpoint(path):
+    """A stories15M-shaped llama2.c checkpoint file (28-byte header + payload, freq_cis included)."""
+    cfg = make_config(*STORIES15M_SHAPE)
+    data = synth_checkpoint(cfg, True, STORIES15M_SEED)
+    with open(path, "wb") as f:
+        f.write(np.array(STORIES15M_SHAPE, dtype="<i4").tobytes())
+        f.write(data.astype("<f4").tobytes())
+    return path
+
+
+# stories15M shape with an unshared classifier (header vocab -32000), seed 10, classifier row 1 (BOS)
+# scaled by 4: the greedy stream from BOS ends on BOS at position 19 (top-2 margin >= 0.098 at every
+# step), so it exercises the BOS stop of src/main.zig:1017-1019.
+BOS_STOP_SHAPE = (288, 768, 6, 6, 6, -32000, 256)
+BOS_STOP_POS = 19
+
+
+def bos_stop_payload():
+    dim, vocab = BOS_STOP_SHAPE[0], -BOS_STOP_SHAPE[5]
+    data = synth_checkpoint(make_config(*BOS_STOP_SHAPE[:5], vocab, BOS_STOP_SHAPE[6]), False, STORIES15M_SEED)
+    wcls = data.size - vocab * dim
+    data[wcls + dim:wcls + 2 * dim] *= 4.0
+    return data

@@ -21,10 +21,10 @@ def test_library_exports_every_declared_symbol(l2b):
     assert lib.l2b_abi_version() == 2
 
 
-def test_library_is_sm100a_only(l2b):
+def test_library_is_sm90a_only(l2b):
     out = subprocess.run(["cuobjdump", "-lelf", l2b.lib_path()], capture_output=True, text=True).stdout
     archs = {tok for line in out.splitlines() for tok in line.replace(".", " ").split() if tok.startswith("sm_")}
-    assert archs == {"sm_100a"}, archs
+    assert archs == {"sm_90a"}, archs
 
 
 def test_status_strings(l2b):

@@ -1,4 +1,4 @@
-"""GPU: the reference's own hot-path unit tests (/root/reference/src/main.zig:1078-1150)
+"""GPU: the reference's own hot-path unit tests (src/main.zig:1078-1150 of the reference)
 replayed against the device ops through the C ABI, plus oracle comparisons on random
 shapes covering the vector-tail edge cases (n < W, n % W != 0, n % 4 != 0)."""
 import numpy as np

@@ -1,6 +1,6 @@
 """GPU (>= 2 devices): tensor-parallel shards + all-reduce reproduce the single-GPU logits
 (BASELINE.json config 5).  Launches scripts/tp_check.py under torchrun; skipped on 1-GPU boxes
-(the driver's round-end `pytest -m gpu` runs on one GPU; `gpurun --gpus 2` runs this for real)."""
+(runs for real on a machine with 2, 4 or 8 GPUs)."""
 import os
 import subprocess
 import sys

@@ -31,7 +31,7 @@ def make_pair(l2b, oracle, shape, seed):
 
 
 def test_stories15m_logits_and_tokens_match_oracle(l2b, oracle, stories15m):
-    """configs[1]: stories15M.bin fp32 on 1xB200, -t 0, 256-token decode, bit-exact tokens."""
+    """configs[1]: stories15M-shaped checkpoint fp32 on 1xH100, -t 0, 256-token decode, bit-exact tokens."""
     with open(os.path.join(GOLDEN, "stories15M_t0_tokens.json")) as f:
         gold = json.load(f)
     ck = l2b.read_checkpoint(stories15m, mmap=False)
@@ -89,18 +89,44 @@ def test_stories15m_argmax_and_generate_paths(l2b, stories15m):
         assert toks == gold["tokens"]
         t.reset()
         out = t.generate_argmax(1, 0, 256, stop_on_bos=True)
-        assert out[-1] == 1 and out[:-1].tolist() == gold["tokens"]
+        assert out.tolist() == gold["tokens"] + ([gold["terminator"]] if gold["terminator"] is not None else [])
         assert len(out) == gold["forward_calls"]
         # without BOS-stop the loop runs all 256 positions; prefix is unchanged
         t.reset()
         out2 = t.generate_argmax(1, 0, 256, stop_on_bos=False)
-        assert len(out2) == 256 and out2[:222].tolist() == out.tolist()
+        assert len(out2) == 256 and out2[:len(out)].tolist() == out.tolist()
         # prompt forcing (src/main.zig:999-1000): forced tokens are fed, the rest free-runs
         t.reset()
         forced = np.full(256, -1, np.int32)
         forced[:5] = gold["tokens"][:5]
         out3 = t.generate_argmax(1, 0, 40, forced=forced, stop_on_bos=True)
         assert out3.tolist() == gold["tokens"][:40]
+
+
+def test_generate_argmax_stops_on_bos_like_oracle(l2b, oracle):
+    """l2b_generate_argmax(stop_on_bos) ends on the position where the oracle's loop produces BOS
+    (src/main.zig:1017-1019), and without the stop runs on past it over the same prefix."""
+    from llama2_zig_b200.checkpoint import shape_checkpoint
+    shape, k = oracle.BOS_STOP_SHAPE, oracle.BOS_STOP_POS
+    ck = shape_checkpoint(shape)
+    ck.data = oracle.bos_stop_payload()
+    om = oracle.OracleModel(oracle.make_config(*shape[:5], -shape[5], shape[6]), ck.data, False, W=8, kind="strict")
+    calls, want, _ = om.generate(1, 256)
+    assert calls == k + 1 and want[k] == 1
+    with l2b.Transformer(ck) as t:
+        out = t.generate_argmax(1, 0, 256, stop_on_bos=True)
+        assert out.tolist() == want[:k + 1].tolist()
+        t.reset()
+        toks, token = [], 1
+        for pos in range(256):
+            token = t.forward_argmax(token, pos)
+            toks.append(token)
+            if token == 1:
+                break
+        assert toks == out.tolist()
+        t.reset()
+        out2 = t.generate_argmax(1, 0, 256, stop_on_bos=False)
+        assert len(out2) == 256 and out2[:k + 1].tolist() == out.tolist()
 
 
 def test_rope_table_from_host_is_used(l2b, oracle, stories15m):

@@ -1,8 +1,10 @@
 """CPU: the C++ twin of the reference's Zig host (llama2.zig_b200/host) — loader, tokenizer and
 sampler behave like src/main.zig.  The tokenizer checks are the reference's own `bpe` test
-(src/main.zig:1152-1180) replayed on the shipped tokenizer.bin."""
+(src/main.zig:1152-1180) replayed on the shipped tokenizer.bin's entries (tests/golden)."""
 import ctypes as C
+import json
 import os
+import struct
 
 import numpy as np
 import pytest
@@ -32,18 +34,25 @@ def host():
     return lib
 
 
-def tokenizer_path():
-    for p in (os.path.join(ROOT, "assets", "tokenizer.bin"), "/root/reference/tokenizer.bin"):
-        if os.path.exists(p):
-            return p
-    return None
+@pytest.fixture(scope="module")
+def tokenizer_path(tmp_path_factory):
+    """A full-size tokenizer.bin rebuilt from tests/golden/tokenizer_subset.json: the shipped
+    vocabulary's entries the tests can reach, unique placeholders everywhere else."""
+    with open(os.path.join(ROOT, "tests", "golden", "tokenizer_subset.json")) as f:
+        sub = json.load(f)
+    known = {i: (score, bytes.fromhex(s)) for i, score, s in sub["entries"]}
+    path = tmp_path_factory.mktemp("tokenizer") / "tokenizer.bin"
+    with open(path, "wb") as f:
+        f.write(struct.pack("<i", sub["max_token_len"]))
+        for i in range(sub["vocab_size"]):
+            score, s = known.get(i, (-1e9, b"\x01%05d" % i))
+            f.write(struct.pack("<fi", score, len(s)) + s)
+    return str(path)
 
 
-def test_bpe(host):
+def test_bpe(host, tokenizer_path):
     """test "bpe", src/main.zig:1152-1180."""
-    path = tokenizer_path()
-    if path is None:
-        pytest.skip("tokenizer.bin not staged")
+    path = tokenizer_path
     tk = C.c_void_p()
     assert host.l2h_tokenizer_load(path.encode(), 32000, C.byref(tk)) == 0
     assert host.l2h_tokenizer_lookup(tk, "æ".encode(), 2) == 233
@@ -81,12 +90,10 @@ def test_sampler_helpers(host):
         assert host.l2h_sample_top_p(peaked.ctypes.data_as(FP), 4, 0.9, scratch) == 1
 
 
-def test_tokenizer_hash_lookup_equals_first_match_scan(host):
+def test_tokenizer_hash_lookup_equals_first_match_scan(host, tokenizer_path):
     """SURVEY 8f.4: the O(1) lookup must answer exactly like the reference's linear scan (:208-215):
     the FIRST id whose bytes match — the shipped vocabulary has 204 duplicated strings."""
-    path = tokenizer_path()
-    if path is None:
-        pytest.skip("tokenizer.bin not staged")
+    path = tokenizer_path
     tk = C.c_void_p()
     assert host.l2h_tokenizer_load(path.encode(), 32000, C.byref(tk)) == 0
     first, dups = {}, 0

@@ -5,7 +5,7 @@ golden token stream and agrees with the C oracle's logits.
 Why: the reference has no test that pins transformer() and no Zig toolchain exists here (SURVEY 8c),
 so the golden stream is derived.  Two restatements in different languages, arithmetic (fp64 vs the
 reference's fp32 lane order) and authorship agreeing token for token — with a minimum top-2 margin
-of 0.01 along the stream, ~10^4 x the reordering noise — is the strongest pin available offline
+of 0.016 along the stream, ~10^4 x the reordering noise — is the strongest pin available offline
 (ADVICE r1: "a shared misreading of main.zig would pass every test")."""
 import hashlib
 import json
@@ -84,7 +84,7 @@ def test_numpy_restatement_reproduces_golden_stream_and_oracle_logits(l2b, oracl
             break
         toks.append(nxt)
         token = nxt
-    assert toks == gold["tokens"] and len(toks) == 221
+    assert toks == gold["tokens"] and len(toks) == 256
     assert hashlib.sha256(np.array(toks, "<u4").tobytes()).hexdigest() == gold["sha256_le_u32"]
     assert worst <= 1e-5, worst                  # fp64 vs the fp32 lane-ordered oracle
-    assert min_margin >= 0.009                   # SURVEY App. B: 0.0100 at pos 98
+    assert min_margin >= 0.015                   # 0.0166; see oracle_lib.STORIES15M_SEED

@@ -1,5 +1,5 @@
 """CPU: pins the oracle against everything the reference's own tests hold for the hot path
-(/root/reference/src/main.zig:1078-1150) and against the committed golden fixtures."""
+(src/main.zig:1078-1150 of the reference) and against the committed golden fixtures."""
 import hashlib
 import json
 import os
@@ -122,21 +122,35 @@ def test_argmax_first_maximum_wins(oracle):
 
 
 def test_golden_token_stream(oracle, stories15m):
-    """configs[0]: stories15M.bin, -t 0, 256 tokens on CPU.  The stream is what SURVEY.md
-    Appendix B derived independently (sha256 506dd3f7...)."""
+    """configs[0]: the stories15M-shaped checkpoint, -t 0, 256 tokens on CPU."""
     with open(os.path.join(GOLDEN, "stories15M_t0_tokens.json")) as f:
         gold = json.load(f)
-    assert gold["sha256_le_u32"] == "506dd3f7fa602cfdf63f6af15be1c82797012fee4040c950299f1290c0bc2bbb"
+    assert gold["sha256_le_u32"] == "76f4096890fb99d6e0c8abca87b777dc9a20c8e47085da5d3ff50ed6dac7f808"
     cfg, shared, data = oracle.read_checkpoint(stories15m)
     assert (cfg.dim, cfg.hidden_dim, cfg.n_layers, cfg.n_heads, cfg.n_kv_heads, cfg.vocab_size,
             cfg.seq_len, shared) == (288, 768, 6, 6, 6, 32000, 256, True)
+    assert os.path.getsize(stories15m) == gold["checkpoint_bytes"]
     m = oracle.OracleModel(cfg, data, shared, W=8, kind="strict")
     calls, out, _ = m.generate(1, 256)
-    assert calls == gold["forward_calls"] == 222
-    assert out[calls - 1] == 1  # BOS ends the loop (src/main.zig:1017-1019)
-    toks = out[:calls - 1]
+    assert calls == gold["forward_calls"] == 256
+    assert gold["terminator"] is None and 1 not in out[:calls]   # no BOS: the loop runs to seq_len (src/main.zig:1017-1019)
+    toks = out[:calls]
     assert toks.tolist() == gold["tokens"]
     assert hashlib.sha256(toks.astype("<u4").tobytes()).hexdigest() == gold["sha256_le_u32"]
+
+
+def test_generate_stops_on_bos(oracle):
+    """BOS ends the loop (src/main.zig:1017-1019) on the position it is produced; without the stop the
+    loop runs on to n_steps over the same prefix."""
+    shape = oracle.BOS_STOP_SHAPE
+    cfg = oracle.make_config(*shape[:5], -shape[5], shape[6])
+    m = oracle.OracleModel(cfg, oracle.bos_stop_payload(), False, W=8, kind="strict")
+    calls, out, _ = m.generate(1, 256)
+    k = oracle.BOS_STOP_POS
+    assert calls == k + 1 and out[k] == 1 and 1 not in out[:k].tolist()
+    m2 = oracle.OracleModel(cfg, oracle.bos_stop_payload(), False, W=8, kind="strict")
+    calls2, out2, _ = m2.generate(1, 256, stop_on_bos=False)
+    assert calls2 == 256 and np.array_equal(out2[:k + 1], out[:k + 1])
 
 
 def test_golden_logits_fixture(oracle, stories15m):
