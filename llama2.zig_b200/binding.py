@@ -264,19 +264,22 @@ class Transformer:
         """The library's pinned logits buffer as a numpy view (state.logits of the host, zero copy)."""
         return np.ctypeslib.as_array(self.lib.l2b_logits_buffer(self.h), shape=(self.ck.vocab_size,))
 
-    def forward_sample(self, token, pos, temperature, top_p, cand_cap=8192):
+    def forward_sample(self, token, pos, temperature, top_p, cand_cap=8192, with_count=False):
         """transformer() + logits/=T, softmax (:1005-1008) and the top-p prefilter (:761-768) on the
         device.  Returns (probs, candidates or None); candidates is a structured array
-        (prob, index) in index order, or None when top_p is 0/1 or too many passed the filter."""
+        (prob, index) in index order, or None when top_p is 0/1 or too many passed the filter.
+        with_count=True appends n_cand: the number of candidates, 0 when top_p is 0/1, and minus
+        the number that passed when there were more than cand_cap (the caller then filters probs
+        itself)."""
         probs = np.empty(self.ck.vocab_size, dtype=np.float32)
         cand = (L2BProbIndex * cand_cap)()
         n = C.c_int32()
         _check(self.lib.l2b_forward_sample(self.h, int(token), int(pos), float(temperature), float(top_p),
                                            probs.ctypes.data_as(FP), cand, cand_cap, C.byref(n)), self.h)
-        if n.value <= 0:
-            return probs, None
-        arr = np.frombuffer(cand, dtype=[("prob", "<f4"), ("index", "<i4")], count=n.value).copy()
-        return probs, arr
+        arr = None
+        if n.value > 0:
+            arr = np.frombuffer(cand, dtype=[("prob", "<f4"), ("index", "<i4")], count=n.value).copy()
+        return (probs, arr, n.value) if with_count else (probs, arr)
 
     def load_stats(self):
         ms = C.c_double()

@@ -108,11 +108,36 @@ def test_softmax_vs_oracle(l2b, oracle, n):
     assert abs(float(got.astype(np.float64).sum()) - 1.0) < 1e-5
 
 
-@pytest.mark.parametrize("hs,stride,npos", [(48, 288, 1), (48, 288, 7), (48, 288, 256), (64, 768, 300),
-                                            (128, 4096, 65), (128, 512, 1500), (32, 32, 40), (80, 160, 100)])
+ATTN_SHAPES = [(48, 288, 1), (48, 288, 7), (48, 288, 256), (64, 768, 300),
+               (128, 4096, 65), (128, 512, 1500), (32, 32, 40), (80, 160, 100)]
+
+
+@pytest.mark.parametrize("hs,stride,npos", ATTN_SHAPES)
 def test_attention_head_vs_oracle(l2b, oracle, hs, stride, npos):
     """One head of src/main.zig:361-389 (dot / sqrt(hs), softmax, weighted V rows) vs the
     oracle's three helpers composed the same way; npos > 256 exercises the split + merge."""
+    _check_attention_head(l2b, oracle, hs, stride, npos)
+
+
+# every flash NF / lanes-per-row branch, the head sizes only the 3-pass kernel takes (28, 224), and the
+# documented maximum 256, on both sides of the split
+MORE_ATTN_SHAPES = [(hs, 2 * hs, npos) for hs in (4, 8, 12, 20, 24, 28, 192, 224, 256) for npos in (200, 300)]
+
+
+@pytest.mark.parametrize("hs,stride,npos,attn", [s + ("default",) for s in MORE_ATTN_SHAPES] +
+                         [s + ("3pass",) for s in ATTN_SHAPES + MORE_ATTN_SHAPES])
+def test_attention_head_kernels_vs_oracle(l2b, oracle, monkeypatch, hs, stride, npos, attn):
+    """The same comparison for every head size the attention kernels branch on, under the library's
+    own kernel choice and with L2B_ATTN=3pass (read on every call), which forces the 3-pass kernel;
+    test_attention_head_vs_oracle covers the original shapes under the library's choice."""
+    if attn == "3pass":
+        monkeypatch.setenv("L2B_ATTN", "3pass")
+    else:
+        monkeypatch.delenv("L2B_ATTN", raising=False)
+    _check_attention_head(l2b, oracle, hs, stride, npos)
+
+
+def _check_attention_head(l2b, oracle, hs, stride, npos):
     import ctypes as C
     FP = C.POINTER(C.c_float)
     lib = oracle.load("strict")
