@@ -89,7 +89,13 @@ typedef struct l2b_ctx l2b_ctx;
  *                  (see l2b_load_stats).
  * Supported shapes: dim % 4 == 0, hidden_dim % 4 == 0, head_size = dim/n_heads a multiple of
  * 4 and <= 256, n_heads % n_kv_heads == 0; for n_gpus > 1 also n_kv_heads, hidden_dim/4 and
- * vocab_size/2 divisible by n_gpus.  Anything else => L2B_ERR_UNSUPPORTED.                  */
+ * vocab_size/2 divisible by n_gpus.  Anything else => L2B_ERR_UNSUPPORTED.  Two shared-memory
+ * limits are also refused here with L2B_ERR_UNSUPPORTED and a message:
+ *   - a GEMV input that does not fit in shared memory: hidden_dim > 57600 on H100, or
+ *     dim > 28800 where the rmsnorm gain is staged next to it;
+ *   - a seq_len whose timeline split (seq_len / nsplit, at most 32 splits) no longer fits the
+ *     3-pass attention kernel's 200 KB score buffer: seq_len > 1,605,632 with 8 heads or fewer.
+ * DESIGN.md §4.5c tabulates which kernel runs at which limit.                              */
 int32_t l2b_create(l2b_ctx **out, const l2b_config *cfg, const float *host_weights,
                    uint64_t n_floats, const float *rope_cos, const float *rope_sin,
                    int32_t n_gpus);
@@ -148,7 +154,8 @@ float *l2b_logits_buffer(l2b_ctx *ctx);
  *                only the candidates are wanted, or l2b_logits_buffer(ctx) for zero copy.
  *   cand/n_cand: for 0 < top_p < 1: *n_cand candidates (prob, index); if more than cand_cap (or
  *                8192) passed the filter, *n_cand = -(their number) and the host filters
- *                host_probs itself.  Ignored (may be NULL) for top_p == 0 or 1 (:1009).         */
+ *                host_probs itself.  Ignored (may be NULL) for top_p == 0 or 1 (:1009).
+ * vocab_size 1 => L2B_ERR_INVALID_ARG, as for l2b_op_sample_prep (the cutoff divides by n-1).  */
 typedef struct l2b_prob_index { float prob; int32_t index; } l2b_prob_index;
 int32_t l2b_forward_sample(l2b_ctx *ctx, int32_t token, int32_t pos, float temperature, float top_p,
                            float *host_probs, l2b_prob_index *cand, int32_t cand_cap,

@@ -459,7 +459,8 @@ int launch_gemv(l2b_ctx *ctx, int epi, const GemvParams &p, cudaStream_t st, con
     // the SM to the successor kernel's pre-fill)
     const size_t stage_bytes = (size_t)TMA_STAGE_FLOATS * 4;
     const size_t xonly = (size_t)p.n * 4;
-    int nstage = ctx->tma_stages > 0 ? ctx->tma_stages : (int)(((size_t)kMaxSmemOptin - xonly) / stage_bytes);
+    const size_t ring_room = xonly < (size_t)kMaxSmemOptin ? (size_t)kMaxSmemOptin - xonly : 0;   // never wraps
+    int nstage = ctx->tma_stages > 0 ? ctx->tma_stages : (int)(ring_room / stage_bytes);
     if (nstage > TMA_MAX_STAGES) nstage = TMA_MAX_STAGES;
     const bool fused_ok = !p.gamma || p.n <= 5 * (TMA_THREADS - 32) * 4;   // register slices of the rmsnorm gain (MAXV x prologue threads)
     if (p.parts && big) return fail(ctx, L2B_ERR_UNSUPPORTED, "partial-vector prologue is only in the latency kernel");
@@ -469,6 +470,8 @@ int launch_gemv(l2b_ctx *ctx, int epi, const GemvParams &p, cudaStream_t st, con
     if (ctx->force_kernel == 3 && !tma) return fail(ctx, L2B_ERR_UNSUPPORTED, "shape does not fit the TMA-ring kernel");
     const size_t smem = tma ? (size_t)nstage * stage_bytes + xonly : xbytes;
     if (smem > (size_t)kMaxSmemOptin) return fail(ctx, L2B_ERR_UNSUPPORTED, "activation vector too large for shared memory");
+    // hard invariant of the ring kernel, whatever the budget arithmetic above decided
+    if (tma && nstage < 2) return fail(ctx, L2B_ERR_UNSUPPORTED, "TMA ring of fewer than 2 stages");
     int tpr = gemv_tpr(p.n);
     // many-row matrices (the classifier): fewer threads per row = more 128-bit loads in flight per
     // thread and fewer shuffle steps per row, as long as the grid still covers the SMs
@@ -1562,6 +1565,8 @@ int32_t l2b_forward_sample(l2b_ctx *ctx, int32_t token, int32_t pos, float tempe
     if (rc) return rc;
     if (!(temperature > 0.0f)) return fail(ctx, L2B_ERR_INVALID_ARG, "temperature must be > 0 (use l2b_forward_argmax for 0)");
     if (top_p < 0.0f || top_p > 1.0f) return fail(ctx, L2B_ERR_INVALID_ARG, "top_p must be in [0, 1]");
+    // like l2b_op_sample_prep: the top-p cutoff (1-p)/(n-1) has no meaning for a single entry
+    if (ctx->cfg.vocab_size < 2) return fail(ctx, L2B_ERR_INVALID_ARG, "sampling needs vocab_size >= 2");
     const bool filter = (top_p != 0.0f && top_p != 1.0f);            // :1009
     if (filter && (!cand || !n_cand || cand_cap <= 0)) return fail(ctx, L2B_ERR_INVALID_ARG, "candidate buffer missing");
     rc = run_step(ctx, token, pos, G_SAMPLE, temperature, filter ? top_p : -1.0f);
@@ -1592,6 +1597,11 @@ pf_fn pf_pick(int epi) {
     }
 }
 constexpr size_t kPfSmemBudget = 227 * 1024 - 8192;   // the prefill kernels keep ~6.5 KB of static shared memory
+constexpr size_t kPfStageBytes = (size_t)TMA_STAGE_FLOATS * 4;
+
+// does a ring of at least 2 stages fit next to xbytes of activation vectors?  Compared before any
+// subtraction: (budget - xbytes) in unsigned arithmetic wraps once xbytes exceeds the budget.
+static bool pf_ring_fits(uint64_t xbytes) { return xbytes + 2 * kPfStageBytes <= kPfSmemBudget; }
 
 // can this context prefill PF_MAXB positions per weight pass?  Single GPU, flash attention, and all
 // four per-layer GEMVs bandwidth-bound shapes of the TMA-ring kernel; otherwise l2b_prefill runs the
@@ -1607,8 +1617,7 @@ static int pf_prepare(l2b_ctx *ctx) {
                            dim <= 5 * (TMA_THREADS - 32) * 4 && ctx->gemv8_min_bytes >= 0 &&
                            dim * dim * 4 >= (uint64_t)ctx->gemv8_min_bytes && ctx->attn_flash &&
                            pick_attention(ctx->head_size, true, &smem) != attention_kernel &&
-                           (kPfSmemBudget - PF_MAXB * dim * 4) / ((size_t)TMA_STAGE_FLOATS * 4) >= 2 &&
-                           (kPfSmemBudget - 2 * hid * 4) / ((size_t)TMA_STAGE_FLOATS * 4) >= 2;
+                           pf_ring_fits(PF_MAXB * dim * 4) && pf_ring_fits(2 * hid * 4);
     if (!shapes_ok) return L2B_OK;
     L2B_CUDA(ctx, cudaSetDevice(ctx->device));
     int rc;
@@ -1632,7 +1641,7 @@ static int pf_prepare(l2b_ctx *ctx) {
 template <int NB>
 static int pf_launch(l2b_ctx *ctx, int epi, PrefillParams p, cudaStream_t st) {
     const size_t xbytes = (size_t)NB * p.n * 4;
-    int nstage = (int)((kPfSmemBudget - xbytes) / ((size_t)TMA_STAGE_FLOATS * 4));
+    int nstage = xbytes < kPfSmemBudget ? (int)((kPfSmemBudget - xbytes) / kPfStageBytes) : 0;
     if (nstage > TMA_MAX_STAGES) nstage = TMA_MAX_STAGES;
     p.nstage = nstage;
     int grid = ctx->num_sms;
@@ -1641,7 +1650,10 @@ static int pf_launch(l2b_ctx *ctx, int epi, PrefillParams p, cudaStream_t st) {
     cudaLaunchConfig_t lc{};
     lc.gridDim = dim3(grid);
     lc.blockDim = dim3(TMA_THREADS);
-    lc.dynamicSmemBytes = (size_t)nstage * TMA_STAGE_FLOATS * 4 + xbytes;
+    lc.dynamicSmemBytes = (size_t)nstage * kPfStageBytes + xbytes;
+    // hard invariant, whatever pf_prepare decided: a ring kernel never launches with fewer than 2 stages
+    if (nstage < 2 || lc.dynamicSmemBytes > kPfSmemBudget)
+        return fail(ctx, L2B_ERR_UNSUPPORTED, "batched prefill: TMA ring of fewer than 2 stages or past the shared-memory budget");
     lc.stream = st;
     cudaLaunchAttribute at[1] = {pdl_attr()};
     lc.attrs = at;

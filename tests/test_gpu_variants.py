@@ -48,6 +48,21 @@ Ledger: kernel instantiation -> a test that runs it (ids relative to this module
   position-by-position device prefill loop               test_variant[B-prefill-batch0] and every small model
   eager launches / launches without PDL                  test_variant[*-no-graph], [*-no-pdl], [*-no-graph-no-pdl]
   sample_prep_kernel past the candidate capacity          test_sampler_candidate_overflow
+
+At the resource limits (tests/test_gpu_envelope.py, ids relative to test_envelope):
+  gemv_tma_kernel, fused rmsnorm with all 5 gain slices    [dim5760-default], [llama2-13B-default]
+  gemv8_kernel<QKV | SILU | ARGMAX> just past them         [dim5888-default], [llama2-70B-default] (dim 8192)
+  gemv_tma_kernel ring depth 2 / 3 chosen by the budget    [w2-hid41216-default] / [pf-hid28672-default],
+                                                         [llama2-70B-default]
+  gemv8_kernel<RESID> with the whole shared memory as x     [x-hid57600-default]; one float more:
+                                                         test_envelope_refused_at_create[x-hid57604]
+  prefill_gemm_kernel<*, 4> at 4 ring stages, <RESID, 2> at 2   [dim5760-default], [pf-hid19840-default]
+  position-loop prefill past the NB = 2 budget            [pf-hid19844-default], [pf-hid28672-default]
+  attention_flash_kernel / attention_kernel / attn_wo_kernel, splits longer than min_chunk
+                                                         [ctx4096-h32-*], [ctx16384-h1-*]
+  attention_kernel at the longest accepted context        [ctx1605632-attn-3pass]
+  single-CTA grids, odd last row pair, kv_mul 64          [vocab1-*], [vocab2-seq1-*], [vocab3-2layers-*], [mqa64-*]
+  sample_prep_kernel over 128256 entries                  [llama3-8B-default]
 """
 import contextlib
 import os
@@ -155,6 +170,10 @@ def l2b_env(env):
         os.environ.update(saved)
 
 
+PF_SMEM_BUDGET = 227 * 1024 - 8192               # kPfSmemBudget: dynamic shared memory of prefill_gemm_kernel
+TMA_STAGE_BYTES = 8 * 256 * 16                   # one ring stage: 8 rows x 256 float4
+
+
 def batched_prefill(shape, env):
     """Whether l2b_prefill takes the batched kernel under `env` (the shape test of pf_prepare)."""
     dim, hid, _, heads = shape[:4]
@@ -164,7 +183,20 @@ def batched_prefill(shape, env):
     big_min_n = big_min_n if big_min_n >= 4 else 1024
     min_bytes = int(env.get("L2B_GEMV8_MIN_BYTES", str(8 << 20)))
     return (dim >= big_min_n and hid >= big_min_n and dim <= 5760 and 0 <= min_bytes <= dim * dim * 4
-            and _flash_nf(dim // heads) is not None)
+            and _flash_nf(dim // heads) is not None
+            # a ring of >= 2 stages next to 4 dim-wide inputs (qkv, wo, w13) and 2 hidden-wide ones (w2)
+            and 4 * dim * 4 + 2 * TMA_STAGE_BYTES <= PF_SMEM_BUDGET
+            and 2 * hid * 4 + 2 * TMA_STAGE_BYTES <= PF_SMEM_BUDGET)
+
+
+def prefill_launches(shape, env, n_tokens, step_launches):
+    """Kernels one logits-free l2b_prefill of n_tokens launches: per layer and chunk of 4 positions the
+    batched path runs qkv, attention, wo, w13 and one w2 per pair of positions; the position loop
+    runs one decode step (without the classifier, plus the token advance) per position."""
+    if not batched_prefill(shape, env):
+        return n_tokens * step_launches
+    chunks = [min(4, n_tokens - i) for i in range(0, n_tokens, 4)]
+    return shape[2] * sum(4 + (nb + 1) // 2 for nb in chunks)
 
 
 _payloads, _refs, _defaults = {}, {}, {}
@@ -180,19 +212,25 @@ def payload(l2b, name):
     return _payloads[name]
 
 
+def oracle_run(oracle, ck, n, check):
+    """Strict-oracle logits at the check positions of a teacher-forced run of n positions, and the KV
+    caches after the last position."""
+    om = oracle.OracleModel(oracle.make_config(*ck.shape_tuple), ck.data, ck.shared_weights, W=8, kind="strict")
+    logits = {}
+    for pos, tok in enumerate(teacher_tokens(n, ck.vocab_size)):
+        lg = om.forward(tok, pos)
+        if pos in check:
+            logits[pos] = lg
+    ref = (logits, om.state("key_cache"), om.state("value_cache"))
+    om.close()
+    return ref
+
+
 def oracle_ref(l2b, oracle, name):
-    """Strict-oracle logits at the check positions and KV caches after the last position (once per model)."""
+    """oracle_run of a model of MODELS (once per model)."""
     if name not in _refs:
-        ck = payload(l2b, name)
         _, _, n, check, _ = MODELS[name]
-        om = oracle.OracleModel(oracle.make_config(*ck.shape_tuple), ck.data, ck.shared_weights, W=8, kind="strict")
-        logits = {}
-        for pos, tok in enumerate(teacher_tokens(n, ck.vocab_size)):
-            lg = om.forward(tok, pos)
-            if pos in check:
-                logits[pos] = lg
-        _refs[name] = (logits, om.state("key_cache"), om.state("value_cache"))
-        om.close()
+        _refs[name] = oracle_run(oracle, payload(l2b, name), n, check)
     return _refs[name]
 
 
@@ -208,9 +246,15 @@ def host_candidates(probs, top_p):
 
 def run_case(l2b, oracle, name, env):
     """Create a context under `env`, run every checker on it, return (logits by position, kcache, vcache)."""
-    ck = payload(l2b, name)
     _, _, n, check, n_prompt = MODELS[name]
-    want, kref, vref = oracle_ref(l2b, oracle, name)
+    return check_context(l2b, payload(l2b, name), n, check, n_prompt, oracle_ref(l2b, oracle, name), env)
+
+
+def check_context(l2b, ck, n, check, n_prompt, ref, env):
+    """Every checker on a context of checkpoint `ck` created under `env`: n teacher-forced positions
+    against ref = oracle_run(.., n, check), prefill of the first n_prompt tokens (n_prompt - 1 in
+    check).  Returns (logits by position, kcache, vcache)."""
+    want, kref, vref = ref
     toks = teacher_tokens(n, ck.vocab_size)
     kv = ck.seq_len * (ck.dim // ck.n_heads) * ck.n_kv_heads          # floats per layer of one cache
     with l2b_env(env), l2b.Transformer(ck) as t:
@@ -220,6 +264,7 @@ def run_case(l2b, oracle, name, env):
             if pos in check:
                 got[pos] = lg
                 assert rel_err(lg, want[pos]) <= REL_TOL, (pos, rel_err(lg, want[pos]))
+        _, step_launches = t.last_timing()
         kc, vc = t.state("key_cache"), t.state("value_cache")
         np.testing.assert_allclose(kc, kref, rtol=0, atol=1e-4 * np.max(np.abs(kref)))
         np.testing.assert_allclose(vc, vref, rtol=0, atol=1e-4 * np.max(np.abs(vref)))
@@ -228,31 +273,44 @@ def run_case(l2b, oracle, name, env):
         for pos in check:
             assert t.forward_argmax(toks[pos], pos) == int(np.argmax(got[pos])), pos
 
-        # one sampler step on the last checked position
+        # one sampler step on the last checked position; a single-entry vocabulary is refused
         p = check[-1]
-        probs, cand, n_cand = t.forward_sample(toks[p], p, 1.0, 0.9, with_count=True)
-        ref = softmax64(got[p])
-        assert np.max(np.abs(probs - ref)) <= 1e-4 * np.max(ref)
-        keep = host_candidates(probs, 0.9)
-        if keep.size <= 8192:
-            assert n_cand == keep.size and np.array_equal(cand["index"], keep.astype(np.int32))
-            assert np.array_equal(cand["prob"], probs[keep])
+        if ck.vocab_size < 2:
+            with pytest.raises(l2b.L2BError) as e:
+                t.forward_sample(toks[p], p, 1.0, 0.9)
+            assert e.value.status == -1
         else:
-            assert n_cand == -keep.size and cand is None
+            probs, cand, n_cand = t.forward_sample(toks[p], p, 1.0, 0.9, with_count=True)
+            ref = softmax64(got[p])
+            assert np.max(np.abs(probs - ref)) <= 1e-4 * np.max(ref)
+            keep = host_candidates(probs, 0.9)
+            if keep.size <= 8192:
+                assert n_cand == keep.size and np.array_equal(cand["index"], keep.astype(np.int32))
+                assert np.array_equal(cand["prob"], probs[keep])
+            else:
+                assert n_cand == -keep.size and cand is None
 
-        # on-device loop: 4 forced steps, then 8 free-running ones == host loop of forward_argmax
-        steps = 12
+        # on-device loop: 4 forced steps, then free-running ones (12 in all, or up to seq_len) ==
+        # host loop of forward_argmax
+        steps = min(12, ck.seq_len)
+        gen = teacher_tokens(steps + 1, ck.vocab_size)
         forced = np.full(steps, -1, np.int32)
-        forced[:4] = toks[1:5]
+        forced[:4] = gen[1:min(5, steps + 1)]
         t.reset()
-        out = t.generate_argmax(toks[0], 0, steps, forced=forced, stop_on_bos=False)
+        out = t.generate_argmax(gen[0], 0, steps, forced=forced, stop_on_bos=False)
         t.reset()
-        host, tok = [], toks[0]
+        host, tok = [], gen[0]
         for pos in range(steps):
             nxt = t.forward_argmax(tok, pos)
             tok = int(forced[pos]) if forced[pos] >= 0 else nxt
             host.append(tok)
         assert out.tolist() == host
+
+        # which path l2b_prefill takes (batched kernel or position loop): its launch count
+        if n_prompt > 1:
+            t.reset()
+            t.prefill(toks[:n_prompt - 1], 0, want_logits=False)
+            assert t.last_timing()[1] == prefill_launches(ck.shape_tuple, env, n_prompt - 1, step_launches)
 
         # prefill of the first n_prompt teacher tokens == the token-by-token logits and KV rows
         t.reset()
