@@ -277,6 +277,11 @@ struct GemvParams {
     int bump_epoch;            // set on the first kernel of a step: CTA 0 increments ctl[CTL_EPOCH]
     unsigned long long spin_ns;  // bound on every peer wait (SpinGuard)
     unsigned long long *trace;   // nullptr or this launch's [grid][TRACE_SLOTS] timeline
+    // ---- batched prefill (prefill_gemm_kernel): nb <= NB input vectors at positions pos0 .. pos0+nb-1.
+    // x_in holds them contiguously, or (layer 0, emb != nullptr) they are the embedding rows of tokens[b].
+    // Appended last so the decode kernels' parameter offsets stay where they are.
+    const int *tokens;
+    int nb, pos0;
 };
 
 template <int EPI>
@@ -291,6 +296,27 @@ __device__ __forceinline__ const float *gemv_row_ptr(const GemvParams &p, int v)
         return ((v & 1) ? p.w1 : p.w0) + (size_t)(v >> 1) * p.n;
     } else {
         return p.w0 + (size_t)v * p.n;
+    }
+}
+
+// EPI_QKV, rows (v, v+1): an adjacent pair of q, k or v (segment sizes are even).  q and k pairs are
+// rotated by the RoPE row (rc, rs) of position `pos`; q goes to `q`, k and v to row `pos` of the caches.
+// The ring kernels' epilogue warps use it with the RoPE rows they staged in shared memory.
+__device__ __forceinline__ void qkv_store_pair(const GemvParams &p, float *q, int pos, const float *rc,
+                                               const float *rs, int v, float a0, float a1) {
+    if (v < p.rows0 + p.rows1) {
+        const bool is_q = v < p.rows0;
+        const int i = is_q ? v : v - p.rows0;            // index within q / k
+        const int pr = (i % p.head_size) >> 1;           // :338 (i % head_size)
+        const float fcr = rc[pr], fci = rs[pr];
+        // :348-349, evaluated without FMA contraction like the reference
+        const float r0 = __fsub_rn(__fmul_rn(a0, fcr), __fmul_rn(a1, fci));
+        const float r1 = __fadd_rn(__fmul_rn(a0, fci), __fmul_rn(a1, fcr));
+        float *dst = is_q ? q + i : p.kcache + (size_t)pos * p.kv_dim + i;   // :355,:357
+        *reinterpret_cast<float2 *>(dst) = make_float2(r0, r1);
+    } else {
+        const int i = v - p.rows0 - p.rows1;
+        *reinterpret_cast<float2 *>(p.vcache + (size_t)pos * p.kv_dim + i) = make_float2(a0, a1);  // :356,:358
     }
 }
 
@@ -637,6 +663,63 @@ __global__ void __launch_bounds__(NT) gemv_kernel(const GemvParams p) {
 // range of row pairs (+-1 pair), so all CTAs stream the same number of bytes and finish together.
 constexpr int GEMV8_R = 8;
 
+// This CTA's balanced contiguous range of row pairs: virtual rows [r0, r1), ntiles tiles of GEMV8_R rows.
+struct RowSplit {
+    int r0, r1, ntiles;
+};
+__device__ __forceinline__ RowSplit cta_row_split(int total_rows) {
+    const int npairs = (total_rows + 1) >> 1;
+    const int base = npairs / (int)gridDim.x, rem = npairs % (int)gridDim.x;
+    const int b = blockIdx.x;
+    const int pair0 = b * base + min(b, rem);
+    const int pair1 = pair0 + base + (b < rem ? 1 : 0);
+    RowSplit s;
+    s.r0 = pair0 * 2;
+    s.r1 = min(pair1 * 2, total_rows);
+    s.ntiles = (s.r1 - s.r0 + GEMV8_R - 1) / GEMV8_R;
+    return s;
+}
+
+// Transposing butterfly over the 8 per-row partials of a tile: afterwards lane L (L % 4 == 0) holds
+// the warp's sum of row L / 4 in a[0] (9 shuffles for 8 rows instead of 40).
+__device__ __forceinline__ void butterfly8(float (&a)[GEMV8_R], int lane) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        const float send = (lane & 16) ? a[i] : a[i + 4];
+        const float keep = (lane & 16) ? a[i + 4] : a[i];
+        a[i] = keep + __shfl_xor_sync(0xffffffffu, send, 16);
+    }
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+        const float send = (lane & 8) ? a[i] : a[i + 2];
+        const float keep = (lane & 8) ? a[i + 2] : a[i];
+        a[i] = keep + __shfl_xor_sync(0xffffffffu, send, 8);
+    }
+    {
+        const float send = (lane & 4) ? a[0] : a[1];
+        const float keep = (lane & 4) ? a[1] : a[0];
+        a[0] = keep + __shfl_xor_sync(0xffffffffu, send, 4);
+    }
+    a[0] += __shfl_xor_sync(0xffffffffu, a[0], 2);
+    a[0] += __shfl_xor_sync(0xffffffffu, a[0], 1);
+}
+
+// Per-warp row sums of one tile for NB input vectors, double-buffered by tile parity: red[t & 1].
+template <int NB>
+using TileRed = float[2][NWARP][GEMV8_R][NB];
+
+// Rows (2 * pair, 2 * pair + 1) of vector b: the warps' partials summed in fixed warp order.
+template <int NB>
+__device__ __forceinline__ float2 sum_warp_partials(const float (&red)[NWARP][GEMV8_R][NB], int pair, int b) {
+    float s0 = 0.0f, s1 = 0.0f;
+#pragma unroll
+    for (int w8 = 0; w8 < NWARP; ++w8) {
+        s0 += red[w8][2 * pair][b];
+        s1 += red[w8][2 * pair + 1][b];
+    }
+    return make_float2(s0, s1);
+}
+
 template <int EPI>
 __global__ void __launch_bounds__(NT, 2) gemv8_kernel(const GemvParams p) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -644,20 +727,14 @@ __global__ void __launch_bounds__(NT, 2) gemv8_kernel(const GemvParams p) {
     float *aux = xs + p.n;
     __shared__ uint64_t bar;
     __shared__ float scratch[NWARP + 1];
-    __shared__ float red[2][NWARP][GEMV8_R];
+    __shared__ TileRed<1> red;
     __shared__ unsigned long long blk_key;
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int n4 = p.n >> 2;
     const int nsteps = (n4 + NT - 1) / NT;             // column steps per tile
-    // balanced contiguous ranges of row pairs
-    const int npairs = (p.total_rows + 1) >> 1;
-    const int base = npairs / (int)gridDim.x, rem = npairs % (int)gridDim.x;
-    const int b = blockIdx.x;
-    const int pair0 = b * base + min(b, rem);
-    const int pair1 = pair0 + base + (b < rem ? 1 : 0);
-    const int r0 = pair0 * 2, r1 = min(pair1 * 2, p.total_rows);
-    const int ntiles = (r1 - r0 + GEMV8_R - 1) / GEMV8_R;
+    const RowSplit rs = cta_row_split(p.total_rows);
+    const int r0 = rs.r0, r1 = rs.r1, ntiles = rs.ntiles;
     const int total = ntiles * nsteps;                 // flattened (tile, step) space
 
     float4 wa[GEMV8_R], wb[GEMV8_R];
@@ -707,38 +784,14 @@ __global__ void __launch_bounds__(NT, 2) gemv8_kernel(const GemvParams p) {
             for (int r = 0; r < GEMV8_R; ++r) acc[r] = dot4(w[r], xv, acc[r]);
         }
         if (st != nsteps - 1) return;
-        // ---- end of a tile: transposing butterfly, lane L (L % 4 == 0) ends with row L / 4
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-            const float send = (lane & 16) ? acc[i] : acc[i + 4];
-            const float keep = (lane & 16) ? acc[i + 4] : acc[i];
-            acc[i] = keep + __shfl_xor_sync(0xffffffffu, send, 16);
-        }
-#pragma unroll
-        for (int i = 0; i < 2; ++i) {
-            const float send = (lane & 8) ? acc[i] : acc[i + 2];
-            const float keep = (lane & 8) ? acc[i + 2] : acc[i];
-            acc[i] = keep + __shfl_xor_sync(0xffffffffu, send, 8);
-        }
-        {
-            const float send = (lane & 4) ? acc[0] : acc[1];
-            const float keep = (lane & 4) ? acc[1] : acc[0];
-            acc[0] = keep + __shfl_xor_sync(0xffffffffu, send, 4);
-        }
-        acc[0] += __shfl_xor_sync(0xffffffffu, acc[0], 2);
-        acc[0] += __shfl_xor_sync(0xffffffffu, acc[0], 1);
+        butterfly8(acc, lane);                         // end of a tile
         const int par = t & 1;                         // double-buffered: one barrier per tile
-        if ((lane & 3) == 0) red[par][warp][lane >> 2] = acc[0];
+        if ((lane & 3) == 0) red[par][warp][lane >> 2][0] = acc[0];
         __syncthreads();
         if (tid < GEMV8_R / 2) {
-            float s0 = 0.0f, s1 = 0.0f;
-#pragma unroll
-            for (int w8 = 0; w8 < NWARP; ++w8) {       // fixed order
-                s0 += red[par][w8][2 * tid];
-                s1 += red[par][w8][2 * tid + 1];
-            }
+            const float2 s = sum_warp_partials<1>(red[par], tid, 0);
             const int v0 = r0 + t * GEMV8_R + 2 * tid;
-            if (v0 < r1) gemv_epilogue_pair<EPI>(p, v0, s0, s1, pos, best, epoch, xr);
+            if (v0 < r1) gemv_epilogue_pair<EPI>(p, v0, s.x, s.y, pos, best, epoch, xr);
         }
 #pragma unroll
         for (int r = 0; r < GEMV8_R; ++r) acc[r] = 0.0f;
@@ -787,6 +840,182 @@ __device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
 // produces (TMA), warp 9 runs the epilogues (RoPE / KV append / SiLU / argmax) off the consumers'
 // critical path: consumers hand it the 8x8 per-warp partial sums through a double-buffered
 // shared array guarded by two mbarrier pairs, so no block-wide barrier exists in the main loop.
+//
+// Two kernels run this stream: gemv_tma_kernel (decode, one activation vector) and
+// prefill_gemm_kernel (batched prefill, NB vectors).  The producer step, the consumer loop, the
+// rmsnorm prologue, the fixed-order warp-partial sum and the QKV pair store below are the one
+// implementation both use, so per (row, vector) a prefilled position is summed in the decode order.
+
+// One CTA's ring: rows [r0, r1) stream as `total` (tile, column step) stages of GEMV8_R rows x NT
+// float4 through the nstage slots of `ring`.  full[s]: slot s has landed (producer -> consumers);
+// empty[s]: all NWARP consumer warps are done with it.
+struct TmaRing {
+    float *ring;
+    uint64_t *full, *empty;
+    int nstage, n4, nsteps, r0, r1, total;
+};
+
+// The producer warp's place in the stream.  produce_one is executed by all 32 lanes of the warp:
+// lane r issues row r's bulk copy of the next stage, lane 0 owns the barriers.
+struct RingProducer {
+    int it = 0, stage = 0, tile = 0, step = 0;
+    uint32_t phase = 0;
+    const float *row = nullptr;                                        // this lane's row in the current tile
+
+    template <int EPI>
+    __device__ __forceinline__ void produce_one(const GemvParams &p, const TmaRing &R, int lane) {
+        const int c0 = step * NT;                                      // first float4 column
+        const int cols4 = min(NT, R.n4 - c0);
+        const int v0 = R.r0 + tile * GEMV8_R;
+        const int rows = min(GEMV8_R, R.r1 - v0);
+        if (step == 0 && lane < rows) row = gemv_row_ptr<EPI>(p, v0 + lane);
+        if (lane == 0) {
+            mbar_wait(&R.empty[stage], phase ^ 1);
+            mbar_expect_tx(&R.full[stage], (uint32_t)(rows * cols4 * 16));
+        }
+        __syncwarp();
+        if (lane < rows)
+            tma_load_1d(R.ring + (size_t)stage * TMA_STAGE_FLOATS + lane * NT * 4, row + (size_t)c0 * 4,
+                        (uint32_t)(cols4 * 16), &R.full[stage]);
+        ++it;
+        if (++step == R.nsteps) { step = 0; ++tile; }
+        if (++stage == R.nstage) { stage = 0; phase ^= 1; }
+    }
+};
+
+// The prologue runs on the consumer warps and the epilogue warp (TMA_PRO_THREADS; named barrier 1 is
+// theirs).  Thread ptid owns the float4 columns ptid + k * TMA_PRO_THREADS, k < TMA_MAXV, so the fused
+// rmsnorm takes n <= 5 * 288 * 4 = 5760 floats.
+constexpr int TMA_MAXV = 5;
+constexpr int TMA_PRO_THREADS = TMA_THREADS - 32;
+
+// this thread's slices of the rmsnorm gain, held in registers through the prologue
+__device__ __forceinline__ void tma_fetch_gain(const GemvParams &p, float4 (&gv)[TMA_MAXV], int ptid, int n4) {
+    const float4 *g4 = reinterpret_cast<const float4 *>(p.gamma);
+#pragma unroll
+    for (int k = 0; k < TMA_MAXV; ++k) {
+        const int i = ptid + k * TMA_PRO_THREADS;
+        gv[k] = (i < n4) ? __ldg(g4 + i) : make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+}
+
+// With the nb vectors staged in xs ([nb][n]): CTA 0 copies them to x_out, and with a gain each one
+// is normalised in place with the reference's rounding points, (x*s)*w.  Ends at barrier 1.
+template <int NB>
+__device__ __forceinline__ void tma_rmsnorm(const GemvParams &p, float *xs, const float4 (&gv)[TMA_MAXV],
+                                            float (*scratch)[NWARP + 2], int nb, int ptid, int lane, int n4) {
+    if (p.gamma || p.x_out) {
+        float4 *xs4w = reinterpret_cast<float4 *>(xs);
+        float ssq[NB];
+#pragma unroll
+        for (int b = 0; b < NB; ++b) {
+            ssq[b] = 0.0f;
+            if (b < nb) {
+#pragma unroll
+                for (int k = 0; k < TMA_MAXV; ++k) {
+                    const int i = ptid + k * TMA_PRO_THREADS;
+                    if (i < n4) {
+                        const float4 v = xs4w[(size_t)b * n4 + i];
+                        if (p.x_out && blockIdx.x == 0) reinterpret_cast<float4 *>(p.x_out)[(size_t)b * n4 + i] = v;
+                        ssq[b] = fmaf(v.x, v.x, ssq[b]); ssq[b] = fmaf(v.y, v.y, ssq[b]);
+                        ssq[b] = fmaf(v.z, v.z, ssq[b]); ssq[b] = fmaf(v.w, v.w, ssq[b]);
+                    }
+                }
+            }
+        }
+        if (p.gamma) {
+#pragma unroll
+            for (int b = 0; b < NB; ++b) {
+                const float w = warp_sum(ssq[b]);
+                if (lane == 0) scratch[b][ptid >> 5] = w;
+            }
+            named_bar_sync(1, TMA_PRO_THREADS);
+#pragma unroll
+            for (int b = 0; b < NB; ++b) {
+                if (b >= nb) continue;
+                float ss = (lane < TMA_PRO_THREADS / 32) ? scratch[b][lane] : 0.0f;
+                ss = warp_sum(ss);
+                ss /= (float)p.n;            // :452
+                ss += 1e-5f;                 // :453
+                const float sc = 1.0f / sqrtf(ss);  // :454
+#pragma unroll
+                for (int k = 0; k < TMA_MAXV; ++k) {
+                    const int i = ptid + k * TMA_PRO_THREADS;
+                    if (i < n4) {
+                        float4 v = xs4w[(size_t)b * n4 + i];
+                        v.x = __fmul_rn(__fmul_rn(v.x, sc), gv[k].x);   // (x*s)*w, :462
+                        v.y = __fmul_rn(__fmul_rn(v.y, sc), gv[k].y);
+                        v.z = __fmul_rn(__fmul_rn(v.z, sc), gv[k].z);
+                        v.w = __fmul_rn(__fmul_rn(v.w, sc), gv[k].w);
+                        xs4w[(size_t)b * n4 + i] = v;
+                    }
+                }
+            }
+        }
+    }
+    named_bar_sync(1, TMA_PRO_THREADS);
+}
+
+// Consumer warps 0..NWARP-1: acc[b][r] += w_r . x_b over this thread's float4 columns, stage by stage
+// (one LDS.128 of each x_b serves the tile's rows; vectors b >= nb read x_0 and are never stored).
+// At a tile's end the butterfly leaves the warp's row sums in red[t & 1] for the epilogue warp.
+// trace (decode only, else nullptr): the first stage's arrival (slot 4), the last one consumed (5).
+template <int NB>
+__device__ __forceinline__ void tma_consume(const TmaRing &R, const float *xs, int nb, TileRed<NB> &red,
+                                            uint64_t *tile_full, uint64_t *tile_free, unsigned long long *trace) {
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const float4 *xs4 = reinterpret_cast<const float4 *>(xs);
+    float acc[NB][GEMV8_R];
+#pragma unroll
+    for (int b = 0; b < NB; ++b)
+#pragma unroll
+        for (int r = 0; r < GEMV8_R; ++r) acc[b][r] = 0.0f;
+    int c_stage = 0;
+    uint32_t c_phase = 0;
+    int t = 0, st = 0;
+    for (int it = 0; it < R.total; ++it, ++st) {
+        if (st == R.nsteps) { st = 0; ++t; }
+        const int c = st * NT + tid;
+        const int v0 = R.r0 + t * GEMV8_R;
+        const int rows = min(GEMV8_R, R.r1 - v0);
+        mbar_wait(&R.full[c_stage], c_phase);
+        if (it == 0 && tid == 0) L2B_STAMP(trace, 4);
+        if (c < R.n4) {
+            const float4 *w4 = reinterpret_cast<const float4 *>(R.ring + (size_t)c_stage * TMA_STAGE_FLOATS) + tid;
+            float4 xv[NB];
+#pragma unroll
+            for (int b = 0; b < NB; ++b) xv[b] = xs4[(size_t)(b < nb ? b : 0) * R.n4 + c];
+#pragma unroll
+            for (int r = 0; r < GEMV8_R; ++r) {
+                if (r < rows) {
+                    const float4 w = w4[r * NT];
+#pragma unroll
+                    for (int b = 0; b < NB; ++b) acc[b][r] = dot4(w, xv[b], acc[b][r]);
+                }
+            }
+        }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&R.empty[c_stage]);      // this warp is done with the stage
+        if (++c_stage == R.nstage) { c_stage = 0; c_phase ^= 1; }
+        if (it == R.total - 1 && tid == 0) L2B_STAMP(trace, 5);
+        if (st != R.nsteps - 1) continue;
+#pragma unroll
+        for (int b = 0; b < NB; ++b) butterfly8(acc[b], lane);  // end of a tile
+        const int par = t & 1, use = t >> 1;
+        mbar_wait(&tile_free[par], (use & 1) ^ 1);            // epilogue warp has read use-1 of red[par]
+        if ((lane & 3) == 0) {
+#pragma unroll
+            for (int b = 0; b < NB; ++b) red[par][warp][lane >> 2][b] = acc[b][0];
+        }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&tile_full[par]);
+#pragma unroll
+        for (int b = 0; b < NB; ++b)
+#pragma unroll
+            for (int r = 0; r < GEMV8_R; ++r) acc[b][r] = 0.0f;
+    }
+}
+
 template <int EPI>
 __global__ void __launch_bounds__(TMA_THREADS, 2) gemv_tma_kernel(const GemvParams p) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -794,21 +1023,17 @@ __global__ void __launch_bounds__(TMA_THREADS, 2) gemv_tma_kernel(const GemvPara
     float *ring = reinterpret_cast<float *>(smem_raw);                 // NSTAGE x 32 KB
     float *xs = ring + (size_t)NSTAGE * TMA_STAGE_FLOATS;              // n floats
     __shared__ uint64_t full[TMA_MAX_STAGES], empty[TMA_MAX_STAGES], xbar, tile_full[2], tile_free[2];
-    __shared__ float scratch[NWARP + 2];
-    __shared__ float red[2][NWARP][GEMV8_R];
+    __shared__ float scratch[1][NWARP + 2];
+    __shared__ TileRed<1> red;
     __shared__ float rope_s[2][128];                                   // cos/sin row of `pos` (head_size/2 <= 128)
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int n4 = p.n >> 2;
     const int nsteps = (n4 + NT - 1) / NT;
-    const int npairs = (p.total_rows + 1) >> 1;
-    const int base = npairs / (int)gridDim.x, rem = npairs % (int)gridDim.x;
-    const int b = blockIdx.x;
-    const int pair0 = b * base + min(b, rem);
-    const int pair1 = pair0 + base + (b < rem ? 1 : 0);
-    const int r0 = pair0 * 2, r1 = min(pair1 * 2, p.total_rows);
-    const int ntiles = (r1 - r0 + GEMV8_R - 1) / GEMV8_R;
+    const RowSplit split = cta_row_split(p.total_rows);
+    const int r0 = split.r0, r1 = split.r1, ntiles = split.ntiles;
     const int total = ntiles * nsteps;
+    const TmaRing R = {ring, full, empty, NSTAGE, n4, nsteps, r0, r1, total};
 
     if (tid == 0) {
         L2B_STAMP(p.trace, 0);
@@ -819,45 +1044,24 @@ __global__ void __launch_bounds__(TMA_THREADS, 2) gemv_tma_kernel(const GemvPara
     }
     __syncthreads();
 
-    // ---- producer state (warp 8): lane r issues row r's bulk copy, lane 0 owns the barriers.
-    // The ring is filled before waiting on the previous kernel (weights are immutable).
-    int p_it = 0, p_stage = 0, p_tile = 0, p_step = 0;
-    uint32_t p_phase = 0;
-    const float *p_row = nullptr;                                      // this lane's row in the current tile
-    auto produce_one = [&]() {                                         // executed by all 32 lanes of warp 8
-        const int c0 = p_step * NT;                                    // first float4 column
-        const int cols4 = min(NT, n4 - c0);
-        const int v0 = r0 + p_tile * GEMV8_R;
-        const int rows = min(GEMV8_R, r1 - v0);
-        if (p_step == 0 && lane < rows) p_row = gemv_row_ptr<EPI>(p, v0 + lane);
-        if (lane == 0) {
-            mbar_wait(&empty[p_stage], p_phase ^ 1);
-            mbar_expect_tx(&full[p_stage], (uint32_t)(rows * cols4 * 16));
-        }
-        __syncwarp();
-        if (lane < rows)
-            tma_load_1d(ring + (size_t)p_stage * TMA_STAGE_FLOATS + lane * NT * 4, p_row + (size_t)c0 * 4,
-                        (uint32_t)(cols4 * 16), &full[p_stage]);
-        ++p_it;
-        if (++p_step == nsteps) { p_step = 0; ++p_tile; }
-        if (++p_stage == NSTAGE) { p_stage = 0; p_phase ^= 1; }
-    };
+    RingProducer prod;
     if (warp == NWARP) {
         // ---- producer warp.  It runs on its own: issuing one stage costs ~0.5 us (8 bulk copies), so
         // the other warps must not meet it at a barrier (measured r02: with the producer inside the
         // prologue's barriers the activation vector was staged 5.3 us after the dependency wait, and
-        // the memory pipe sat idle behind a full ring).
+        // the memory pipe sat idle behind a full ring).  The ring is filled before waiting on the
+        // previous kernel (weights are immutable).
         // Only nprefill stages go out before the wait: the activation vector's bulk copy is issued by
         // warp 0 right after the wait and is served behind everything this SM already requested
         // (~47 GB/s of HBM per SM: a full 192 KB ring ahead of it costs 4 us).
-        while (p_it < total && p_it < p.nprefill) produce_one();
-        if (p_it >= total) pdl_launch_dependents();
+        while (prod.it < total && prod.it < p.nprefill) prod.produce_one<EPI>(p, R, lane);
+        if (prod.it >= total) pdl_launch_dependents();
         if (lane == 0) L2B_STAMP(p.trace, 1);
         pdl_wait();
         if (!p.ctl[CTL_DONE]) {
-            while (p_it < total) {
-                produce_one();
-                if (p_it == total) pdl_launch_dependents();   // last stage in flight
+            while (prod.it < total) {
+                prod.produce_one<EPI>(p, R, lane);
+                if (prod.it == total) pdl_launch_dependents();   // last stage in flight
             }
             if (lane == 0) L2B_STAMP(p.trace, 6);
             return;
@@ -867,18 +1071,9 @@ __global__ void __launch_bounds__(TMA_THREADS, 2) gemv_tma_kernel(const GemvPara
     // the rmsnorm gain is immutable: fetch this thread's slice before waiting on the previous
     // kernel (on big models it has been evicted from L2 by the weight stream, and after the wait
     // its DRAM round trip would queue behind this CTA's own ring traffic)
-    constexpr int MAXV = 5;                               // n <= 5 * 288 * 4 = 5760 floats when fused
-    constexpr int PRO_THREADS = TMA_THREADS - 32;         // consumers + epilogue warp
     const int ptid = tid < NT ? tid : tid - 32;           // index among the prologue's threads
-    float4 gv[MAXV];
-    if (p.gamma && warp != NWARP) {
-        const float4 *g4 = reinterpret_cast<const float4 *>(p.gamma);
-#pragma unroll
-        for (int k = 0; k < MAXV; ++k) {
-            const int i = ptid + k * PRO_THREADS;
-            gv[k] = (i < n4) ? __ldg(g4 + i) : make_float4(0.f, 0.f, 0.f, 0.f);
-        }
-    }
+    float4 gv[TMA_MAXV];
+    if (p.gamma && warp != NWARP) tma_fetch_gain(p, gv, ptid, n4);
 
     // ---- everything below reads what earlier kernels of this step wrote
     if (warp != NWARP) pdl_wait();
@@ -916,43 +1111,7 @@ __global__ void __launch_bounds__(TMA_THREADS, 2) gemv_tma_kernel(const GemvPara
             }
         }
         mbar_wait(&xbar, 0);
-        if (p.gamma || p.x_out) {
-            float4 *xs4w = reinterpret_cast<float4 *>(xs);
-            float ssq = 0.0f;
-#pragma unroll
-            for (int k = 0; k < MAXV; ++k) {
-                const int i = ptid + k * PRO_THREADS;
-                if (i < n4) {
-                    const float4 v = xs4w[i];
-                    if (p.x_out && blockIdx.x == 0) reinterpret_cast<float4 *>(p.x_out)[i] = v;
-                    ssq = fmaf(v.x, v.x, ssq); ssq = fmaf(v.y, v.y, ssq);
-                    ssq = fmaf(v.z, v.z, ssq); ssq = fmaf(v.w, v.w, ssq);
-                }
-            }
-            if (p.gamma) {
-                ssq = warp_sum(ssq);
-                if (lane == 0) scratch[ptid >> 5] = ssq;
-                named_bar_sync(1, PRO_THREADS);
-                float ss = (lane < PRO_THREADS / 32) ? scratch[lane] : 0.0f;
-                ss = warp_sum(ss);
-                ss /= (float)p.n;            // :452
-                ss += 1e-5f;                 // :453
-                const float sc = 1.0f / sqrtf(ss);  // :454
-#pragma unroll
-                for (int k = 0; k < MAXV; ++k) {
-                    const int i = ptid + k * PRO_THREADS;
-                    if (i < n4) {
-                        float4 v = xs4w[i];
-                        v.x = __fmul_rn(__fmul_rn(v.x, sc), gv[k].x);   // (x*s)*w, :462
-                        v.y = __fmul_rn(__fmul_rn(v.y, sc), gv[k].y);
-                        v.z = __fmul_rn(__fmul_rn(v.z, sc), gv[k].z);
-                        v.w = __fmul_rn(__fmul_rn(v.w, sc), gv[k].w);
-                        xs4w[i] = v;
-                    }
-                }
-            }
-        }
-        named_bar_sync(1, PRO_THREADS);
+        tma_rmsnorm<1>(p, xs, gv, scratch, 1, ptid, lane, n4);
         if (EPI == EPI_QKV && tid >= NT + 32) {
             const int half = p.head_size >> 1;
 #pragma unroll
@@ -979,30 +1138,14 @@ __global__ void __launch_bounds__(TMA_THREADS, 2) gemv_tma_kernel(const GemvPara
                 xr_next = gemv_resid_fetch<EPI>(p, (lane < GEMV8_R / 2 && vn < r1) ? vn : p.total_rows);
             }
             mbar_wait(&tile_full[par], use & 1);
-            float s0 = 0.0f, s1 = 0.0f;
-            if (lane < GEMV8_R / 2) {
-#pragma unroll
-                for (int w8 = 0; w8 < NWARP; ++w8) {       // fixed order
-                    s0 += red[par][w8][2 * lane];
-                    s1 += red[par][w8][2 * lane + 1];
-                }
-            }
+            float2 s = make_float2(0.0f, 0.0f);
+            if (lane < GEMV8_R / 2) s = sum_warp_partials<1>(red[par], lane, 0);
             __syncwarp();
             if (lane == 0) mbar_arrive(&tile_free[par]);  // consumers may overwrite red[par]
             const int vp = r0 + t * GEMV8_R + 2 * lane;
             if (lane < GEMV8_R / 2 && vp < r1) {
-                if (EPI == EPI_QKV && vp < p.rows0 + p.rows1) {
-                    const bool is_q = vp < p.rows0;
-                    const int i = is_q ? vp : vp - p.rows0;
-                    const int pr = (i % p.head_size) >> 1;                                  // :338
-                    const float fcr = rope_s[0][pr], fci = rope_s[1][pr];
-                    const float q0 = __fsub_rn(__fmul_rn(s0, fcr), __fmul_rn(s1, fci));      // :348
-                    const float q1 = __fadd_rn(__fmul_rn(s0, fci), __fmul_rn(s1, fcr));      // :349
-                    float *dst = is_q ? p.out0 + i : p.kcache + (size_t)pos * p.kv_dim + i;  // :355,:357
-                    *reinterpret_cast<float2 *>(dst) = make_float2(q0, q1);
-                } else {
-                    gemv_epilogue_pair<EPI>(p, vp, s0, s1, pos, best, epoch, xr);
-                }
+                if (EPI == EPI_QKV) qkv_store_pair(p, p.out0, pos, rope_s[0], rope_s[1], vp, s.x, s.y);
+                else gemv_epilogue_pair<EPI>(p, vp, s.x, s.y, pos, best, epoch, xr);
             }
         }
         if (EPI == EPI_ARGMAX) {
@@ -1018,61 +1161,113 @@ __global__ void __launch_bounds__(TMA_THREADS, 2) gemv_tma_kernel(const GemvPara
         return;
     }
 
-    // ---- consumers (warps 0..7)
-    const float4 *xs4 = reinterpret_cast<const float4 *>(xs);
-    float acc[GEMV8_R];
-#pragma unroll
-    for (int r = 0; r < GEMV8_R; ++r) acc[r] = 0.0f;
-    int c_stage = 0;
-    uint32_t c_phase = 0;
-    int t = 0, st = 0;
-    for (int it = 0; it < total; ++it, ++st) {
-        if (st == nsteps) { st = 0; ++t; }
-        const int c = st * NT + tid;
-        const int v0 = r0 + t * GEMV8_R;
-        const int rows = min(GEMV8_R, r1 - v0);
-        mbar_wait(&full[c_stage], c_phase);
-        if (it == 0 && tid == 0) L2B_STAMP(p.trace, 4);
-        if (c < n4) {
-            const float4 *w4 = reinterpret_cast<const float4 *>(ring + (size_t)c_stage * TMA_STAGE_FLOATS) + tid;
-            const float4 xv = xs4[c];
-#pragma unroll
-            for (int r = 0; r < GEMV8_R; ++r)
-                if (r < rows) acc[r] = dot4(w4[r * NT], xv, acc[r]);
-        }
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&empty[c_stage]);      // this warp is done with the stage
-        if (++c_stage == NSTAGE) { c_stage = 0; c_phase ^= 1; }
-        if (it == total - 1 && tid == 0) L2B_STAMP(p.trace, 5);
-        if (st != nsteps - 1) continue;
-        // ---- end of a tile: transposing butterfly, lane L (L % 4 == 0) ends with row L / 4
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-            const float send = (lane & 16) ? acc[i] : acc[i + 4];
-            const float keep = (lane & 16) ? acc[i + 4] : acc[i];
-            acc[i] = keep + __shfl_xor_sync(0xffffffffu, send, 16);
-        }
-#pragma unroll
-        for (int i = 0; i < 2; ++i) {
-            const float send = (lane & 8) ? acc[i] : acc[i + 2];
-            const float keep = (lane & 8) ? acc[i + 2] : acc[i];
-            acc[i] = keep + __shfl_xor_sync(0xffffffffu, send, 8);
-        }
-        {
-            const float send = (lane & 4) ? acc[0] : acc[1];
-            const float keep = (lane & 4) ? acc[1] : acc[0];
-            acc[0] = keep + __shfl_xor_sync(0xffffffffu, send, 4);
-        }
-        acc[0] += __shfl_xor_sync(0xffffffffu, acc[0], 2);
-        acc[0] += __shfl_xor_sync(0xffffffffu, acc[0], 1);
-        const int par = t & 1, use = t >> 1;
-        mbar_wait(&tile_free[par], (use & 1) ^ 1);        // epilogue warp has read use-1 of red[par]
-        if ((lane & 3) == 0) red[par][warp][lane >> 2] = acc[0];
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&tile_full[par]);
-#pragma unroll
-        for (int r = 0; r < GEMV8_R; ++r) acc[r] = 0.0f;
+    tma_consume<1>(R, xs, 1, red, tile_full, tile_free, p.trace);   // warps 0..7
+}
+
+// ---- batched prompt prefill (SURVEY 8f.2): NB consecutive prompt positions share one pass over the
+// weights.
+//
+// The reference feeds prompt tokens through transformer() one at a time (src/main.zig:996-1000) and
+// streams every weight once per token.  For bandwidth-bound shapes (llama2-7B) this kernel runs the
+// decode kernel's stream (the shared producer, consumer loop and prologue above) with NB activation
+// vectors instead of one: each 128-bit weight load feeds NB x 4 FMAs, so the weight traffic per prompt
+// token drops NB-fold while fp32 CUDA-core arithmetic stays far below its roof (NB = 4: 2 flop/B).
+// Per (row, position) the summation order is the decode kernel's, so a prefilled position holds what
+// the token-by-token path would have computed.  Epilogue warp: lane b * 4 + pair handles (row pair,
+// position b) of each tile.  Outputs: EPI_QKV: q batch [nb][rows0]; EPI_SILU: hb batch [nb][rows0];
+// EPI_RESID: x batch [nb][total_rows].
+constexpr int PF_MAXB = 4;
+
+template <int EPI, int NB>
+__global__ void __launch_bounds__(TMA_THREADS, 1) prefill_gemm_kernel(const GemvParams p) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    const int NSTAGE = p.nstage;
+    float *ring = reinterpret_cast<float *>(smem_raw);                 // NSTAGE x 32 KB
+    float *xs = ring + (size_t)NSTAGE * TMA_STAGE_FLOATS;              // NB x n floats
+    __shared__ uint64_t full[TMA_MAX_STAGES], empty[TMA_MAX_STAGES], xbar, tile_full[2], tile_free[2];
+    __shared__ float scratch[NB][NWARP + 2];
+    __shared__ TileRed<NB> red;
+    __shared__ float rope_s[NB][2][128];                               // cos/sin rows of pos0 .. pos0+NB-1
+
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int n4 = p.n >> 2;
+    const int nsteps = (n4 + NT - 1) / NT;
+    const RowSplit split = cta_row_split(p.total_rows);
+    const int r0 = split.r0, r1 = split.r1, ntiles = split.ntiles;
+    const int total = ntiles * nsteps;
+    const TmaRing R = {ring, full, empty, NSTAGE, n4, nsteps, r0, r1, total};
+
+    if (tid == 0) {
+        for (int s = 0; s < NSTAGE; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], NWARP); }
+        mbar_init(&xbar, 1);
+        for (int s = 0; s < 2; ++s) { mbar_init(&tile_full[s], NWARP); mbar_init(&tile_free[s], 1); }
+        mbar_fence_init();
     }
+    __syncthreads();
+
+    if (warp == NWARP) {
+        RingProducer prod;
+        while (prod.it < total) prod.produce_one<EPI>(p, R, lane);
+        pdl_launch_dependents();
+        return;
+    }
+
+    const int ptid = tid < NT ? tid : tid - 32;
+    float4 gv[TMA_MAXV];
+    if (p.gamma) tma_fetch_gain(p, gv, ptid, n4);
+    pdl_wait();
+    if (tid == 0) {
+        const uint32_t bytes = (uint32_t)p.n * 4u;
+        mbar_expect_tx(&xbar, bytes * (uint32_t)p.nb);
+        if (p.emb) {
+            for (int b = 0; b < p.nb; ++b)                              // x[b] = token_embedding_table[tokens[b]], :295-296
+                tma_load_1d(xs + (size_t)b * p.n, p.emb + (size_t)p.tokens[b] * p.n, bytes, &xbar);
+        } else {
+            tma_load_1d(xs, p.x_in, bytes * (uint32_t)p.nb, &xbar);
+        }
+    }
+    if (EPI == EPI_QKV && tid >= NT + 32) {                            // epilogue warp: RoPE rows of the chunk's positions
+        const int half = p.head_size >> 1;
+        for (int b = 0; b < p.nb; ++b)
+            for (int i = lane; i < half; i += 32) {
+                rope_s[b][0][i] = __ldg(p.rope_cos + (size_t)(p.pos0 + b) * half + i);
+                rope_s[b][1][i] = __ldg(p.rope_sin + (size_t)(p.pos0 + b) * half + i);
+            }
+    }
+    mbar_wait(&xbar, 0);
+    tma_rmsnorm<NB>(p, xs, gv, scratch, p.nb, ptid, lane, n4);
+
+    if (warp == NWARP + 1) {
+        const int eb = lane >> 2, ep = lane & 3;
+        const bool active = lane < 4 * NB && eb < p.nb;
+        for (int t = 0; t < ntiles; ++t) {
+            const int par = t & 1, use = t >> 1;
+            mbar_wait(&tile_full[par], use & 1);
+            float2 s = make_float2(0.0f, 0.0f);
+            if (lane < 4 * NB) s = sum_warp_partials<NB>(red[par], ep, eb);
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&tile_free[par]);
+            const int vp = r0 + t * GEMV8_R + 2 * ep;
+            if (!active || vp >= r1) continue;
+            if (EPI == EPI_QKV) {
+                qkv_store_pair(p, p.out0 + (size_t)eb * p.rows0, p.pos0 + eb, rope_s[eb][0], rope_s[eb][1], vp, s.x, s.y);
+            } else if (EPI == EPI_SILU) {
+                const float sg = __fmul_rn(s.x, __fdiv_rn(1.0f, __fadd_rn(1.0f, expf(-s.x))));   // :412
+                p.out0[(size_t)eb * p.rows0 + (vp >> 1)] = __fmul_rn(sg, s.y);                     // :416
+            } else {   // EPI_RESID: x[b][row] += acc (:395, :422)
+                float *dst = p.out0 + (size_t)eb * p.total_rows + vp;
+                if (vp + 1 < p.total_rows) {
+                    const float2 o = *reinterpret_cast<const float2 *>(dst);
+                    *reinterpret_cast<float2 *>(dst) = make_float2(o.x + s.x, o.y + s.y);
+                } else {
+                    dst[0] += s.x;
+                }
+            }
+        }
+        return;
+    }
+
+    tma_consume<NB>(R, xs, p.nb, red, tile_full, tile_free, nullptr);   // warps 0..7
 }
 
 // Scalar fallback for shapes the vector kernel cannot take (n % 4 != 0 or unaligned rows):

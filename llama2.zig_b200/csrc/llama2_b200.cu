@@ -21,7 +21,6 @@
 #include <vector>
 
 #include "l2b_device.cuh"
-#include "l2b_prefill.cuh"
 
 using namespace l2b;
 
@@ -441,6 +440,14 @@ unsigned long long *trace_slot(l2b_ctx *ctx) {
     return ctx->trace + (size_t)(ctx->last_launches % ctx->trace_launches) * TRACE_MAX_CTAS * TRACE_SLOTS;
 }
 
+// TMA-ring stages (at most TMA_MAX_STAGES) that fit next to xbytes of activation vectors under a
+// dynamic shared-memory budget.  Compared before subtracting: (budget - xbytes) in unsigned
+// arithmetic wraps once xbytes exceeds the budget.
+int tma_ring_stages(size_t budget, size_t xbytes) {
+    const int n = xbytes < budget ? (int)((budget - xbytes) / ((size_t)TMA_STAGE_FLOATS * 4)) : 0;
+    return n < TMA_MAX_STAGES ? n : TMA_MAX_STAGES;
+}
+
 int launch_gemv(l2b_ctx *ctx, int epi, const GemvParams &p, cudaStream_t st, const char *name = "gemv",
                 int layer = -1) {
     {
@@ -459,10 +466,9 @@ int launch_gemv(l2b_ctx *ctx, int epi, const GemvParams &p, cudaStream_t st, con
     // the SM to the successor kernel's pre-fill)
     const size_t stage_bytes = (size_t)TMA_STAGE_FLOATS * 4;
     const size_t xonly = (size_t)p.n * 4;
-    const size_t ring_room = xonly < (size_t)kMaxSmemOptin ? (size_t)kMaxSmemOptin - xonly : 0;   // never wraps
-    int nstage = ctx->tma_stages > 0 ? ctx->tma_stages : (int)(ring_room / stage_bytes);
-    if (nstage > TMA_MAX_STAGES) nstage = TMA_MAX_STAGES;
-    const bool fused_ok = !p.gamma || p.n <= 5 * (TMA_THREADS - 32) * 4;   // register slices of the rmsnorm gain (MAXV x prologue threads)
+    int nstage = tma_ring_stages(kMaxSmemOptin, xonly);
+    if (ctx->tma_stages > 0) nstage = ctx->tma_stages < TMA_MAX_STAGES ? ctx->tma_stages : TMA_MAX_STAGES;
+    const bool fused_ok = !p.gamma || p.n <= TMA_MAXV * TMA_PRO_THREADS * 4;   // register slices of the rmsnorm gain
     if (p.parts && big) return fail(ctx, L2B_ERR_UNSUPPORTED, "partial-vector prologue is only in the latency kernel");
     bool tma = big && ctx->big_kernel_tma && nstage >= 2 && fused_ok && p.head_size <= 256 &&
                (size_t)nstage * stage_bytes + xonly <= (size_t)kMaxSmemOptin;
@@ -601,7 +607,11 @@ int launch_attn_wo(l2b_ctx *ctx, int layer, cudaStream_t st) {
     return L2B_OK;
 }
 
-int launch_attention(l2b_ctx *ctx, int layer, cudaStream_t st) {
+// Attention of one layer for nb queries (gridDim.z).  Decode: one query at the control block's
+// position (pos_base < 0).  Batched prefill: query z at position pos_base + z, q_stride floats apart
+// in q and xb, with its own partial buffers and counters; it is not traced.
+int launch_attention(l2b_ctx *ctx, int layer, cudaStream_t st, const float *q, float *xb, float *part_o,
+                     float *part_ml, unsigned int *counters, int pos_base = -1, int q_stride = 0, int nb = 1) {
     if (ctx->profiling) {
         const int hpos = ctx->n_appended > 0 ? ctx->n_appended - 1 : 0;
         int prc = prof_mark(ctx, "attention", layer, 2ull * (uint64_t)(hpos + 1) * ctx->kv_loc * 4ull, st);
@@ -609,26 +619,27 @@ int launch_attention(l2b_ctx *ctx, int layer, cudaStream_t st) {
     }
     AttnParams a{};
     a.ctl = ctx->ctl;
-    a.q = ctx->q;
+    a.q = q;
     const size_t loff = (size_t)layer * ctx->cfg.seq_len * ctx->kv_loc;   // :354
     a.kcache = ctx->kcache + loff;
     a.vcache = ctx->vcache + loff;
-    a.xb = ctx->xb;
-    a.part_o = ctx->part_o;
-    a.part_ml = ctx->part_ml;
-    a.counters = ctx->counters;
+    a.xb = xb;
+    a.part_o = part_o;
+    a.part_ml = part_ml;
+    a.counters = counters;
     a.head_size = ctx->head_size;
     a.kv_dim = ctx->kv_loc;
     a.kv_mul = ctx->kv_mul;
     a.nsplit = ctx->nsplit;
     a.min_chunk = ctx->min_chunk;
-    a.pos_base = -1;
+    a.pos_base = pos_base;
+    a.q_stride = q_stride;
     a.seq_len = ctx->cfg.seq_len;
-    a.trace = trace_slot(ctx);
+    a.trace = pos_base < 0 ? trace_slot(ctx) : nullptr;
     size_t smem = ctx->attn_smem;
     attn_fn fn = pick_attention(ctx->head_size, ctx->attn_flash, &smem);
     cudaLaunchConfig_t lc{};
-    lc.gridDim = dim3(ctx->heads_loc, ctx->nsplit);
+    lc.gridDim = dim3(ctx->heads_loc, ctx->nsplit, nb);
     lc.blockDim = dim3(NT);
     lc.dynamicSmemBytes = smem;
     lc.stream = st;
@@ -683,6 +694,51 @@ int launch_advance(l2b_ctx *ctx, cudaStream_t st, bool forced, bool exchange) {
     return launch_small(ctx, (const void *)advance_kernel, dim3(1), dim3(32), args, st, true);
 }
 
+// The four GEMVs of layer l, as the decode step and batched prefill share them: columns, rmsnorm gains,
+// weights and row counts, and for qkv the caches, RoPE table and head size.  Inputs, outputs and
+// whatever else is per launch are the caller's.
+struct LayerGemvs {
+    GemvParams qkv, wo, w13, w2;
+};
+LayerGemvs layer_gemvs(const l2b_ctx *ctx, int l) {
+    const int dim = ctx->dim;
+    LayerGemvs g{};
+    // rmsnorm + q,k,v + RoPE + KV append (:305-358)
+    GemvParams &p = g.qkv;
+    p.ctl = ctx->ctl;
+    p.n = dim;
+    p.gamma = ctx->rms_att + (size_t)l * dim;
+    p.w0 = ctx->wq + (size_t)l * ctx->q_loc * dim;
+    p.w1 = ctx->wk + (size_t)l * ctx->kv_loc * dim;
+    p.w2 = ctx->wv + (size_t)l * ctx->kv_loc * dim;
+    p.rows0 = ctx->q_loc; p.rows1 = ctx->kv_loc; p.rows2 = ctx->kv_loc;
+    p.total_rows = ctx->q_loc + 2 * ctx->kv_loc;
+    const size_t loff = (size_t)l * ctx->cfg.seq_len * ctx->kv_loc;
+    p.kcache = ctx->kcache + loff;
+    p.vcache = ctx->vcache + loff;
+    p.rope_cos = ctx->rope_cos; p.rope_sin = ctx->rope_sin;
+    p.head_size = ctx->head_size; p.kv_dim = ctx->kv_loc;
+    // wo, whose result is added to the residual stream (:392-395)
+    g.wo.ctl = ctx->ctl;
+    g.wo.n = ctx->q_loc;
+    g.wo.w0 = ctx->wo + (size_t)l * dim * ctx->q_loc;
+    g.wo.total_rows = dim; g.wo.rows0 = dim;
+    // rmsnorm + w1,w3 + SiLU*mul (:398-416)
+    g.w13.ctl = ctx->ctl;
+    g.w13.n = dim;
+    g.w13.gamma = ctx->rms_ffn + (size_t)l * dim;
+    g.w13.w0 = ctx->w1 + (size_t)l * ctx->hid_loc * dim;
+    g.w13.w1 = ctx->w3 + (size_t)l * ctx->hid_loc * dim;
+    g.w13.rows0 = ctx->hid_loc;
+    g.w13.total_rows = 2 * ctx->hid_loc;
+    // w2, added to the residual stream (:419-422)
+    g.w2.ctl = ctx->ctl;
+    g.w2.n = ctx->hid_loc;
+    g.w2.w0 = ctx->w2 + (size_t)l * dim * ctx->hid_loc;
+    g.w2.total_rows = dim; g.w2.rows0 = dim;
+    return g;
+}
+
 // One decode step on `st` (transformer(), src/main.zig:285-430).  All (token, pos) dependence is
 // through ctx->ctl, so the sequence is capturable once and replayed.
 int enqueue_step(l2b_ctx *ctx, cudaStream_t st, StepMode mode) {
@@ -700,7 +756,6 @@ int enqueue_step(l2b_ctx *ctx, cudaStream_t st, StepMode mode) {
     };
     // wo / w2: row-parallel GEMV whose result is added to the residual stream (:392-395, :419-422)
     auto residual_gemv = [&](GemvParams &g, float *x, int slot, const char *name, int l) -> int {
-        g.total_rows = dim; g.rows0 = dim;
         int rc;
         if (!tp) {
             g.out0 = x;
@@ -735,29 +790,16 @@ int enqueue_step(l2b_ctx *ctx, cudaStream_t st, StepMode mode) {
         }
     };
     for (int l = 0; l < c.n_layers; ++l) {
+        LayerGemvs g = layer_gemvs(ctx, l);
         // ---- rmsnorm + q,k,v + RoPE + KV append (:305-358)
-        GemvParams p{};
-        p.ctl = ctx->ctl;
-        p.n = dim;
-        fold_pending(p);
+        fold_pending(g.qkv);
         if (l == 0) {
-            p.emb = ctx->emb;                 // :295-296
-            p.x_out = Xc;
-            p.bump_epoch = 1;
+            g.qkv.emb = ctx->emb;             // :295-296
+            g.qkv.x_out = Xc;
+            g.qkv.bump_epoch = 1;
         }
-        p.gamma = ctx->rms_att + (size_t)l * dim;
-        p.w0 = ctx->wq + (size_t)l * ctx->q_loc * dim;
-        p.w1 = ctx->wk + (size_t)l * ctx->kv_loc * dim;
-        p.w2 = ctx->wv + (size_t)l * ctx->kv_loc * dim;
-        p.rows0 = ctx->q_loc; p.rows1 = ctx->kv_loc; p.rows2 = ctx->kv_loc;
-        p.total_rows = ctx->q_loc + 2 * ctx->kv_loc;
-        p.out0 = ctx->q;
-        const size_t loff = (size_t)l * c.seq_len * ctx->kv_loc;
-        p.kcache = ctx->kcache + loff;
-        p.vcache = ctx->vcache + loff;
-        p.rope_cos = ctx->rope_cos; p.rope_sin = ctx->rope_sin;
-        p.head_size = ctx->head_size; p.kv_dim = ctx->kv_loc;
-        int rc = launch_gemv(ctx, EPI_QKV, p, st, "qkv_rope", l);
+        g.qkv.out0 = ctx->q;
+        int rc = launch_gemv(ctx, EPI_QKV, g.qkv, st, "qkv_rope", l);
         if (rc) return rc;
 
         if (ctx->fuse_attn) {
@@ -767,39 +809,23 @@ int enqueue_step(l2b_ctx *ctx, cudaStream_t st, StepMode mode) {
             pend = ctx->attn_parts; npend = ctx->heads_loc;
         } else {
             // ---- attention (:361-389)
-            rc = launch_attention(ctx, l, st);
+            rc = launch_attention(ctx, l, st, ctx->q, ctx->xb, ctx->part_o, ctx->part_ml, ctx->counters);
             if (rc) return rc;
             // ---- wo + residual (:392-395)
-            GemvParams o{};
-            o.ctl = ctx->ctl;
-            o.n = ctx->q_loc;
-            o.x_in = ctx->xb;
-            o.w0 = ctx->wo + (size_t)l * dim * ctx->q_loc;
-            rc = residual_gemv(o, Xc, 2 * l, "wo", l);
+            g.wo.x_in = ctx->xb;
+            rc = residual_gemv(g.wo, Xc, 2 * l, "wo", l);
             if (rc) return rc;
         }
 
         // ---- rmsnorm + w1,w3 + SiLU*mul (:398-416)
-        GemvParams f{};
-        f.ctl = ctx->ctl;
-        f.n = dim;
-        fold_pending(f);
-        f.gamma = ctx->rms_ffn + (size_t)l * dim;
-        f.w0 = ctx->w1 + (size_t)l * ctx->hid_loc * dim;
-        f.w1 = ctx->w3 + (size_t)l * ctx->hid_loc * dim;
-        f.rows0 = ctx->hid_loc;
-        f.total_rows = 2 * ctx->hid_loc;
-        f.out0 = ctx->hb;
-        rc = launch_gemv(ctx, EPI_SILU, f, st, "w13_silu", l);
+        fold_pending(g.w13);
+        g.w13.out0 = ctx->hb;
+        rc = launch_gemv(ctx, EPI_SILU, g.w13, st, "w13_silu", l);
         if (rc) return rc;
 
         // ---- w2 + residual (:419-422)
-        GemvParams d{};
-        d.ctl = ctx->ctl;
-        d.n = ctx->hid_loc;
-        d.x_in = ctx->hb;
-        d.w0 = ctx->w2 + (size_t)l * dim * ctx->hid_loc;
-        rc = residual_gemv(d, Xc, 2 * l + 1, "w2", l);
+        g.w2.x_in = ctx->hb;
+        rc = residual_gemv(g.w2, Xc, 2 * l + 1, "w2", l);
         if (rc) return rc;
     }
     if (mode == MODE_NOCLS) {   // prompt prefill: the logits of this position are never looked at (:996-1000)
@@ -1586,10 +1612,9 @@ int32_t l2b_forward_sample(l2b_ctx *ctx, int32_t token, int32_t pos, float tempe
 
 }  // extern "C" (templates below)
 
-// ---- batched prompt prefill (csrc/l2b_prefill.cuh) --------------------------------------------
-typedef void (*pf_fn)(const PrefillParams);
+// ---- batched prompt prefill (prefill_gemm_kernel in l2b_device.cuh) -----------------------------
 template <int NB>
-pf_fn pf_pick(int epi) {
+gemv_fn pf_pick(int epi) {
     switch (epi) {
     case EPI_QKV: return prefill_gemm_kernel<EPI_QKV, NB>;
     case EPI_SILU: return prefill_gemm_kernel<EPI_SILU, NB>;
@@ -1597,11 +1622,6 @@ pf_fn pf_pick(int epi) {
     }
 }
 constexpr size_t kPfSmemBudget = 227 * 1024 - 8192;   // the prefill kernels keep ~6.5 KB of static shared memory
-constexpr size_t kPfStageBytes = (size_t)TMA_STAGE_FLOATS * 4;
-
-// does a ring of at least 2 stages fit next to xbytes of activation vectors?  Compared before any
-// subtraction: (budget - xbytes) in unsigned arithmetic wraps once xbytes exceeds the budget.
-static bool pf_ring_fits(uint64_t xbytes) { return xbytes + 2 * kPfStageBytes <= kPfSmemBudget; }
 
 // can this context prefill PF_MAXB positions per weight pass?  Single GPU, flash attention, and all
 // four per-layer GEMVs bandwidth-bound shapes of the TMA-ring kernel; otherwise l2b_prefill runs the
@@ -1614,10 +1634,11 @@ static int pf_prepare(l2b_ctx *ctx) {
     const uint64_t dim = ctx->dim, hid = ctx->hid_loc, q = ctx->q_loc;
     size_t smem = 0;
     const bool shapes_ok = ctx->world == 1 && !ctx->leader && dim >= (uint64_t)ctx->big_min_n && hid >= (uint64_t)ctx->big_min_n &&
-                           dim <= 5 * (TMA_THREADS - 32) * 4 && ctx->gemv8_min_bytes >= 0 &&
+                           dim <= TMA_MAXV * TMA_PRO_THREADS * 4 && ctx->gemv8_min_bytes >= 0 &&
                            dim * dim * 4 >= (uint64_t)ctx->gemv8_min_bytes && ctx->attn_flash &&
                            pick_attention(ctx->head_size, true, &smem) != attention_kernel &&
-                           pf_ring_fits(PF_MAXB * dim * 4) && pf_ring_fits(2 * hid * 4);
+                           tma_ring_stages(kPfSmemBudget, PF_MAXB * dim * 4) >= 2 &&
+                           tma_ring_stages(kPfSmemBudget, 2 * hid * 4) >= 2;
     if (!shapes_ok) return L2B_OK;
     L2B_CUDA(ctx, cudaSetDevice(ctx->device));
     int rc;
@@ -1639,10 +1660,9 @@ static int pf_prepare(l2b_ctx *ctx) {
 }
 
 template <int NB>
-static int pf_launch(l2b_ctx *ctx, int epi, PrefillParams p, cudaStream_t st) {
+static int pf_launch(l2b_ctx *ctx, int epi, GemvParams p, cudaStream_t st) {
     const size_t xbytes = (size_t)NB * p.n * 4;
-    int nstage = xbytes < kPfSmemBudget ? (int)((kPfSmemBudget - xbytes) / kPfStageBytes) : 0;
-    if (nstage > TMA_MAX_STAGES) nstage = TMA_MAX_STAGES;
+    const int nstage = tma_ring_stages(kPfSmemBudget, xbytes);
     p.nstage = nstage;
     int grid = ctx->num_sms;
     const int npairs = (p.total_rows + 1) / 2;
@@ -1650,7 +1670,7 @@ static int pf_launch(l2b_ctx *ctx, int epi, PrefillParams p, cudaStream_t st) {
     cudaLaunchConfig_t lc{};
     lc.gridDim = dim3(grid);
     lc.blockDim = dim3(TMA_THREADS);
-    lc.dynamicSmemBytes = (size_t)nstage * kPfStageBytes + xbytes;
+    lc.dynamicSmemBytes = (size_t)nstage * TMA_STAGE_FLOATS * 4 + xbytes;
     // hard invariant, whatever pf_prepare decided: a ring kernel never launches with fewer than 2 stages
     if (nstage < 2 || lc.dynamicSmemBytes > kPfSmemBudget)
         return fail(ctx, L2B_ERR_UNSUPPORTED, "batched prefill: TMA ring of fewer than 2 stages or past the shared-memory budget");
@@ -1675,76 +1695,39 @@ static int prefill_batched(l2b_ctx *ctx, const int32_t *tokens, int n_tokens, in
     L2B_CUDA(ctx, cudaMemcpyAsync(ctx->ctl, ctx->h_ctl, CTL_HOST_WORDS * sizeof(int), cudaMemcpyHostToDevice, st));
     L2B_CUDA(ctx, cudaEventRecord(ctx->ev0, st));
     ctx->last_launches = 0;
-    size_t attn_smem = 0;
-    attn_fn afn = pick_attention(ctx->head_size, true, &attn_smem);
     for (int done = 0; done < n_tokens; done += PF_MAXB) {
         const int nb = n_tokens - done < PF_MAXB ? n_tokens - done : PF_MAXB;
         const int pos = pos0 + done;
         for (int l = 0; l < c.n_layers; ++l) {
+            LayerGemvs g = layer_gemvs(ctx, l);
             // ---- rmsnorm + q,k,v + RoPE + KV append for nb positions (:305-358)
-            PrefillParams p{};
-            p.n = dim; p.nb = nb; p.pos0 = pos;
-            p.x_in = ctx->pf_x;
-            if (l == 0) { p.emb = ctx->emb; p.tokens = ctx->pf_tokens + done; p.x_out = ctx->pf_x; }
-            p.gamma = ctx->rms_att + (size_t)l * dim;
-            p.w0 = ctx->wq + (size_t)l * ctx->q_loc * dim;
-            p.w1 = ctx->wk + (size_t)l * ctx->kv_loc * dim;
-            p.w2 = ctx->wv + (size_t)l * ctx->kv_loc * dim;
-            p.rows0 = ctx->q_loc; p.rows1 = ctx->kv_loc; p.rows2 = ctx->kv_loc;
-            p.total_rows = ctx->q_loc + 2 * ctx->kv_loc;
-            p.out0 = ctx->pf_q;
-            const size_t loff = (size_t)l * c.seq_len * ctx->kv_loc;
-            p.kcache = ctx->kcache + loff;
-            p.vcache = ctx->vcache + loff;
-            p.rope_cos = ctx->rope_cos; p.rope_sin = ctx->rope_sin;
-            p.head_size = ctx->head_size; p.kv_dim = ctx->kv_loc;
-            int rc = pf_launch<PF_MAXB>(ctx, EPI_QKV, p, st);
+            g.qkv.nb = nb; g.qkv.pos0 = pos;
+            g.qkv.x_in = ctx->pf_x;
+            if (l == 0) { g.qkv.emb = ctx->emb; g.qkv.tokens = ctx->pf_tokens + done; g.qkv.x_out = ctx->pf_x; }
+            g.qkv.out0 = ctx->pf_q;
+            int rc = pf_launch<PF_MAXB>(ctx, EPI_QKV, g.qkv, st);
             if (rc) return rc;
             // ---- attention of the nb queries (:361-389); query z sees positions 0 .. pos+z
-            AttnParams a{};
-            a.ctl = ctx->ctl; a.q = ctx->pf_q; a.kcache = ctx->kcache + loff; a.vcache = ctx->vcache + loff;
-            a.xb = ctx->pf_xb; a.part_o = ctx->pf_part_o; a.part_ml = ctx->pf_part_ml; a.counters = ctx->pf_counters;
-            a.head_size = ctx->head_size; a.kv_dim = ctx->kv_loc; a.kv_mul = ctx->kv_mul;
-            a.nsplit = ctx->nsplit; a.min_chunk = ctx->min_chunk;
-            a.pos_base = pos; a.q_stride = ctx->q_loc; a.seq_len = c.seq_len;
-            cudaLaunchConfig_t lc{};
-            lc.gridDim = dim3(ctx->heads_loc, ctx->nsplit, nb);
-            lc.blockDim = dim3(NT);
-            lc.dynamicSmemBytes = attn_smem;
-            lc.stream = st;
-            cudaLaunchAttribute at[1] = {pdl_attr()};
-            lc.attrs = at;
-            lc.numAttrs = ctx->use_pdl ? 1 : 0;
-            L2B_CUDA(ctx, cudaLaunchKernelEx(&lc, afn, a));
-            ++ctx->last_launches;
+            rc = launch_attention(ctx, l, st, ctx->pf_q, ctx->pf_xb, ctx->pf_part_o, ctx->pf_part_ml, ctx->pf_counters,
+                                  pos, ctx->q_loc, nb);
+            if (rc) return rc;
             // ---- wo + residual (:392-395)
-            PrefillParams o{};
-            o.n = ctx->q_loc; o.nb = nb; o.pos0 = pos;
-            o.x_in = ctx->pf_xb;
-            o.w0 = ctx->wo + (size_t)l * dim * ctx->q_loc;
-            o.total_rows = dim; o.rows0 = dim;
-            o.out0 = ctx->pf_x;
-            rc = pf_launch<PF_MAXB>(ctx, EPI_RESID, o, st);
+            g.wo.nb = nb; g.wo.pos0 = pos;
+            g.wo.x_in = ctx->pf_xb;
+            g.wo.out0 = ctx->pf_x;
+            rc = pf_launch<PF_MAXB>(ctx, EPI_RESID, g.wo, st);
             if (rc) return rc;
             // ---- rmsnorm + w1,w3 + SiLU*mul (:398-416)
-            PrefillParams f{};
-            f.n = dim; f.nb = nb; f.pos0 = pos;
-            f.x_in = ctx->pf_x;
-            f.gamma = ctx->rms_ffn + (size_t)l * dim;
-            f.w0 = ctx->w1 + (size_t)l * ctx->hid_loc * dim;
-            f.w1 = ctx->w3 + (size_t)l * ctx->hid_loc * dim;
-            f.rows0 = ctx->hid_loc;
-            f.total_rows = 2 * ctx->hid_loc;
-            f.out0 = ctx->pf_hb;
-            rc = pf_launch<PF_MAXB>(ctx, EPI_SILU, f, st);
+            g.w13.nb = nb; g.w13.pos0 = pos;
+            g.w13.x_in = ctx->pf_x;
+            g.w13.out0 = ctx->pf_hb;
+            rc = pf_launch<PF_MAXB>(ctx, EPI_SILU, g.w13, st);
             if (rc) return rc;
             // ---- w2 + residual (:419-422); hidden-sized inputs: two positions per pass (shared memory)
             for (int b = 0; b < nb; b += 2) {
-                PrefillParams d{};
-                d.n = ctx->hid_loc; d.nb = nb - b < 2 ? nb - b : 2; d.pos0 = pos + b;
+                GemvParams d = g.w2;
+                d.nb = nb - b < 2 ? nb - b : 2; d.pos0 = pos + b;
                 d.x_in = ctx->pf_hb + (size_t)b * ctx->hid_loc;
-                d.w0 = ctx->w2 + (size_t)l * dim * ctx->hid_loc;
-                d.total_rows = dim; d.rows0 = dim;
                 d.out0 = ctx->pf_x + (size_t)b * dim;
                 rc = pf_launch<2>(ctx, EPI_RESID, d, st);
                 if (rc) return rc;
@@ -1837,7 +1820,7 @@ int32_t l2b_generate_argmax(l2b_ctx *ctx, int32_t token, int32_t pos, int32_t n_
 // the next token forced, the classifier (60 % of stories15M's bytes) is skipped for every position
 // whose logits nobody reads, and no position pays a host round trip.  On bandwidth-bound shapes
 // (llama2-7B on one GPU) PF_MAXB = 4 positions additionally share each pass over the weights
-// (csrc/l2b_prefill.cuh).  Per (row, position) the arithmetic is the decode step's own.
+// (prefill_gemm_kernel).  Per (row, position) the arithmetic is the decode step's own.
 int32_t l2b_prefill(l2b_ctx *ctx, const int32_t *tokens, int32_t n_tokens, int32_t pos0, float *host_logits) {
     if (!ctx || !tokens || n_tokens <= 0) return fail(ctx, L2B_ERR_INVALID_ARG, "bad prefill arguments");
     int rc = check_step_args(ctx, tokens[0], pos0);

@@ -371,7 +371,7 @@ def test_prefill_equals_token_by_token(l2b, oracle, stories15m):
 
 def test_batched_prefill_on_bandwidth_bound_shapes(l2b, oracle):
     """SURVEY 8f.2 on llama2-7B shapes (2 layers): l2b_prefill runs 4 prompt positions per pass over
-    the weights (csrc/l2b_prefill.cuh).  KV cache and the next logits must equal the token-by-token
+    the weights (prefill_gemm_kernel).  KV cache and the next logits must equal the token-by-token
     path (same per-row summation order => expected bit-identical; bar 1e-6) and the oracle (1e-4)."""
     ck, om = make_pair(l2b, oracle, (4096, 11008, 2, 32, 32, -32000, 2048), 7)
     toks = teacher_tokens(12, ck.vocab_size)           # 11 silent positions = 2 full chunks + 3, then 1 with logits

@@ -13,7 +13,8 @@ a context under one environment and runs the same checker on it:
   * one `forward_sample` step: probabilities within 1e-4 of the exact float64 softmax of the step's
     logits, candidates == the host filter (or, past the candidate capacity, their negated count);
   * `prefill` == token-by-token `forward`: bit for bit (include/llama2_b200.h), 1e-6 on the batched
-    kernel of bandwidth-bound shapes (csrc/l2b_prefill.cuh), like test_batched_prefill_on_bandwidth_bound_shapes.
+    kernel of bandwidth-bound shapes (prefill_gemm_kernel, csrc/l2b_device.cuh), like
+    test_batched_prefill_on_bandwidth_bound_shapes.
 
 Switches that change neither the kernels' arithmetic nor their summation order must also reproduce
 the default context's logits and caches bit for bit (`BITWISE`).  The oracle runs once per model.
@@ -43,7 +44,8 @@ Ledger: kernel instantiation -> a test that runs it (ids relative to this module
                                                          [hs192-default] / [hs256-default]
   attn_wo_kernel<2>, <4>                                  test_variant[110M-fuse1] / [hs128-default]
   attn_wo_kernel cluster sizes 1, 2, 4 (default 8)        test_variant[S-attn-r1], [S-attn-r2], [S-attn-r4]
-  prefill_gemm_kernel<QKV | SILU | RESID, NB 4 and 2> with GQA   test_variant[B-default] (prefill check),
+  prefill_gemm_kernel<QKV | SILU | RESID, NB 4 and 2> with GQA (the TMA stream code of gemv_tma_kernel
+  with NB vectors)                                        test_variant[B-default] (prefill check),
                                                          test_variant[S-all-streaming] (head_size 48)
   position-by-position device prefill loop               test_variant[B-prefill-batch0] and every small model
   eager launches / launches without PDL                  test_variant[*-no-graph], [*-no-pdl], [*-no-graph-no-pdl]
