@@ -117,6 +117,15 @@ int32_t l2b_create_synthetic(l2b_ctx **out, const l2b_config *cfg, uint64_t seed
 int32_t l2b_create_synthetic_group(l2b_ctx **out, const l2b_config *cfg, uint64_t seed,
                                    int32_t n_gpus);
 
+/* A new decode stream on the weights of `model` (any context of it, or any session of it), with no
+ * upload: its own KV cache, run state, control block, stream and graphs.  Every entry point that
+ * takes a context accepts a session, and a session steps exactly as a context of the same weights
+ * would.  The weights are freed when the last context or session of the model is destroyed, in
+ * any order.  Single-GPU models only: a tensor-parallel model => L2B_ERR_UNSUPPORTED.
+ * l2b_load_stats of a session reports 0 bytes.  A model and its sessions are not thread-safe:
+ * drive them from one thread, as one context.                                              */
+int32_t l2b_create_session(l2b_ctx **out, l2b_ctx *model);
+
 void l2b_destroy(l2b_ctx *ctx);
 
 /* Forget the KV cache (start a new generation at pos 0).  The reference runs one
@@ -180,6 +189,26 @@ int32_t l2b_generate_argmax(l2b_ctx *ctx, int32_t token, int32_t pos, int32_t n_
  * l2b_forward bit for bit.                                                                 */
 int32_t l2b_prefill(l2b_ctx *ctx, const int32_t *tokens, int32_t n_tokens, int32_t pos0,
                     float *host_logits);
+
+/* One transformer() step for each of n distinct sessions of one model (l2b_create_session; the
+ * model's own context counts as one): sessions[i] runs tokens[i] at pos[i], under l2b_forward's rule
+ * pos[i] <= (positions appended to that session).  host_logits[i] receives session i's logits.
+ * On the shapes where l2b_prefill shares weight passes (bandwidth-bound, single GPU; not with
+ * L2B_PREFILL_BATCH=0), up to 4 sessions share each pass over the weights, and the logits and KV
+ * rows then match n l2b_forward calls to within float rounding (1e-6 relative), not bit for bit.
+ * Elsewhere the sessions are stepped one after another with l2b_forward's own kernels (bit for bit).
+ * Everything is checked before anything runs: n < 1, a NULL entry, the same session twice,
+ * sessions of different models, a token or position out of range => L2B_ERR_INVALID_ARG; a position
+ * past a session's appended count => L2B_ERR_STATE.  A refused call changes no session.  Errors
+ * are reported through l2b_last_error(sessions[0]) (l2b_last_error(NULL) when there is no
+ * sessions[0]), and l2b_last_timing(sessions[0]) gives the call's device time and kernel launches.
+ * Afterwards l2b_read_state of each session returns its own x, key/value cache and logits, as after
+ * l2b_forward; xb, hb and q are not defined after a batched step.  Synchronous.             */
+int32_t l2b_forward_batch(l2b_ctx *const *sessions, int32_t n, const int32_t *tokens,
+                          const int32_t *pos, float *const *host_logits);
+/* Same step with the device argmax (first maximum wins, :715-726): next[i] for session i.      */
+int32_t l2b_forward_argmax_batch(l2b_ctx *const *sessions, int32_t n, const int32_t *tokens,
+                                 const int32_t *pos, int32_t *next);
 
 /* ---- introspection ------------------------------------------------------------------- */
 

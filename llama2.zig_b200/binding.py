@@ -80,6 +80,9 @@ def load_library():
     lib.l2b_create_synthetic.argtypes = [C.POINTER(vp), C.POINTER(L2BConfig), C.c_uint64,
                                          C.POINTER(L2BShard)]
     lib.l2b_create_synthetic_group.argtypes = [C.POINTER(vp), C.POINTER(L2BConfig), C.c_uint64, C.c_int32]
+    lib.l2b_create_session.argtypes = [C.POINTER(vp), vp]
+    lib.l2b_forward_batch.argtypes = [C.POINTER(vp), C.c_int32, IP, IP, C.POINTER(FP)]
+    lib.l2b_forward_argmax_batch.argtypes = [C.POINTER(vp), C.c_int32, IP, IP, IP]
     lib.l2b_destroy.argtypes = [vp]
     lib.l2b_destroy.restype = None
     lib.l2b_reset.argtypes = [vp]
@@ -212,6 +215,18 @@ class Transformer:
         self._logits = np.empty(ck.vocab_size, dtype=np.float32)
 
     # -- lifecycle
+    def session(self):
+        """A new decode stream on this model's weights (l2b_create_session): its own KV cache and run
+        state, no upload.  The weights live until the model and all its sessions are closed."""
+        s = Transformer.__new__(Transformer)
+        s.lib, s.ck, s.cfg, s.h = self.lib, self.ck, self.cfg, C.c_void_p()
+        rc = self.lib.l2b_create_session(C.byref(s.h), self.h)
+        if rc != 0:
+            s.h = C.c_void_p()
+            _check(rc, None)
+        s._logits = np.empty(self.ck.vocab_size, dtype=np.float32)
+        return s
+
     def close(self):
         if getattr(self, "h", None) and self.h.value:
             self.lib.l2b_destroy(self.h)
@@ -328,6 +343,37 @@ class Transformer:
         kv = C.c_uint64()
         _check(self.lib.l2b_step_bytes(self.h, int(pos), C.byref(w), C.byref(kv)), self.h)
         return w.value, kv.value
+
+
+# ---- one step of several sessions of one model ------------------------------------------------
+
+def _batch_args(sessions, tokens, positions):
+    n = len(sessions)
+    hs = (C.c_void_p * max(n, 1))(*[s.h.value for s in sessions])
+    toks = np.ascontiguousarray(tokens, dtype=np.int32)
+    pos = np.ascontiguousarray(positions, dtype=np.int32)
+    assert toks.size == n and pos.size == n
+    return n, hs, toks, pos
+
+
+def forward_batch(sessions, tokens, positions):
+    """transformer(tokens[i], positions[i]) on sessions[i] for every i (l2b_forward_batch); returns the
+    (n, vocab) logits."""
+    n, hs, toks, pos = _batch_args(sessions, tokens, positions)
+    out = np.empty((n, sessions[0].ck.vocab_size if n else 0), dtype=np.float32)
+    rows = (FP * max(n, 1))(*[out[i].ctypes.data_as(FP) for i in range(n)])
+    _check(load_library().l2b_forward_batch(hs, n, toks.ctypes.data_as(IP), pos.ctypes.data_as(IP), rows),
+           hs[0] if n else None)
+    return out
+
+
+def forward_argmax_batch(sessions, tokens, positions):
+    """Same step with the device argmax (l2b_forward_argmax_batch); returns the n next tokens."""
+    n, hs, toks, pos = _batch_args(sessions, tokens, positions)
+    nxt = np.empty(max(n, 1), dtype=np.int32)
+    _check(load_library().l2b_forward_argmax_batch(hs, n, toks.ctypes.data_as(IP), pos.ctypes.data_as(IP),
+                                                   nxt.ctypes.data_as(IP)), hs[0] if n else None)
+    return nxt[:n].copy()
 
 
 # ---- reference-named single ops on host buffers (device = cuda:0) ---------------------------

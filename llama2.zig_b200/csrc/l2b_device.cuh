@@ -239,6 +239,8 @@ enum GemvEpi {
     EPI_COUNT = 6
 };
 
+constexpr int PF_MAXB = 4;   // input vectors per weight pass of the batched kernels (prefill_gemm_kernel)
+
 struct GemvParams {
     // ---- input vector / prologue
     const float *x_in;      // n floats; when emb != nullptr: row `token` of emb is used instead
@@ -277,11 +279,15 @@ struct GemvParams {
     int bump_epoch;            // set on the first kernel of a step: CTA 0 increments ctl[CTL_EPOCH]
     unsigned long long spin_ns;  // bound on every peer wait (SpinGuard)
     unsigned long long *trace;   // nullptr or this launch's [grid][TRACE_SLOTS] timeline
-    // ---- batched prefill (prefill_gemm_kernel): nb <= NB input vectors at positions pos0 .. pos0+nb-1.
-    // x_in holds them contiguously, or (layer 0, emb != nullptr) they are the embedding rows of tokens[b].
+    // ---- batched kernels (prefill_gemm_kernel): nb <= NB input vectors.  x_in holds them contiguously,
+    // or (layer 0, emb != nullptr) they are the embedding rows of tokens[b].  EPI_QKV: vector b is at
+    // position pos_b[b] and appends to this layer's caches kcache_b[b] / vcache_b[b] (a prompt: pos0 + b
+    // on one cache; the batched step: one decode session per vector).
     // Appended last so the decode kernels' parameter offsets stay where they are.
     const int *tokens;
-    int nb, pos0;
+    int nb;
+    int pos_b[PF_MAXB];
+    float *kcache_b[PF_MAXB], *vcache_b[PF_MAXB];
 };
 
 template <int EPI>
@@ -300,10 +306,10 @@ __device__ __forceinline__ const float *gemv_row_ptr(const GemvParams &p, int v)
 }
 
 // EPI_QKV, rows (v, v+1): an adjacent pair of q, k or v (segment sizes are even).  q and k pairs are
-// rotated by the RoPE row (rc, rs) of position `pos`; q goes to `q`, k and v to row `pos` of the caches.
-// The ring kernels' epilogue warps use it with the RoPE rows they staged in shared memory.
-__device__ __forceinline__ void qkv_store_pair(const GemvParams &p, float *q, int pos, const float *rc,
-                                               const float *rs, int v, float a0, float a1) {
+// rotated by the RoPE row (rc, rs) of position `pos`; q goes to `q`, k and v to row `pos` of the caches
+// kc / vc.  The ring kernels' epilogue warps use it with the RoPE rows they staged in shared memory.
+__device__ __forceinline__ void qkv_store_pair(const GemvParams &p, float *q, float *kc, float *vc, int pos,
+                                               const float *rc, const float *rs, int v, float a0, float a1) {
     if (v < p.rows0 + p.rows1) {
         const bool is_q = v < p.rows0;
         const int i = is_q ? v : v - p.rows0;            // index within q / k
@@ -312,12 +318,17 @@ __device__ __forceinline__ void qkv_store_pair(const GemvParams &p, float *q, in
         // :348-349, evaluated without FMA contraction like the reference
         const float r0 = __fsub_rn(__fmul_rn(a0, fcr), __fmul_rn(a1, fci));
         const float r1 = __fadd_rn(__fmul_rn(a0, fci), __fmul_rn(a1, fcr));
-        float *dst = is_q ? q + i : p.kcache + (size_t)pos * p.kv_dim + i;   // :355,:357
+        float *dst = is_q ? q + i : kc + (size_t)pos * p.kv_dim + i;   // :355,:357
         *reinterpret_cast<float2 *>(dst) = make_float2(r0, r1);
     } else {
         const int i = v - p.rows0 - p.rows1;
-        *reinterpret_cast<float2 *>(p.vcache + (size_t)pos * p.kv_dim + i) = make_float2(a0, a1);  // :356,:358
+        *reinterpret_cast<float2 *>(vc + (size_t)pos * p.kv_dim + i) = make_float2(a0, a1);  // :356,:358
     }
+}
+// the decode step's form: the layer's caches of the launch
+__device__ __forceinline__ void qkv_store_pair(const GemvParams &p, float *q, int pos, const float *rc,
+                                               const float *rs, int v, float a0, float a1) {
+    qkv_store_pair(p, q, p.kcache, p.vcache, pos, rc, rs, v, a0, a1);
 }
 
 // ---- tensor-parallel all-reduce, second half, run by ONE warp of a wo / w2 CTA after that CTA has
@@ -1174,10 +1185,11 @@ __global__ void __launch_bounds__(TMA_THREADS, 2) gemv_tma_kernel(const GemvPara
 // token drops NB-fold while fp32 CUDA-core arithmetic stays far below its roof (NB = 4: 2 flop/B).
 // Per (row, position) the summation order is the decode kernel's, so a prefilled position holds what
 // the token-by-token path would have computed.  Epilogue warp: lane b * 4 + pair handles (row pair,
-// position b) of each tile.  Outputs: EPI_QKV: q batch [nb][rows0]; EPI_SILU: hb batch [nb][rows0];
-// EPI_RESID: x batch [nb][total_rows].
-constexpr int PF_MAXB = 4;
-
+// vector b) of each tile.  Outputs: EPI_QKV: q batch [nb][rows0]; EPI_SILU: hb batch [nb][rows0];
+// EPI_RESID: x batch [nb][total_rows]; EPI_STORE / EPI_ARGMAX (the classifier of the batched step):
+// logits batch [nb][total_rows], and for EPI_ARGMAX one packed argmax_key per vector in amax[b] (zeroed
+// before the launch).  The vectors need not be consecutive positions of one sequence: each carries
+// its own position and caches (pos_b, kcache_b, vcache_b).
 template <int EPI, int NB>
 __global__ void __launch_bounds__(TMA_THREADS, 1) prefill_gemm_kernel(const GemvParams p) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -1187,7 +1199,7 @@ __global__ void __launch_bounds__(TMA_THREADS, 1) prefill_gemm_kernel(const Gemv
     __shared__ uint64_t full[TMA_MAX_STAGES], empty[TMA_MAX_STAGES], xbar, tile_full[2], tile_free[2];
     __shared__ float scratch[NB][NWARP + 2];
     __shared__ TileRed<NB> red;
-    __shared__ float rope_s[NB][2][128];                               // cos/sin rows of pos0 .. pos0+NB-1
+    __shared__ float rope_s[NB][2][128];                               // cos/sin rows of pos_b[0 .. NB-1]
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int n4 = p.n >> 2;
@@ -1226,12 +1238,12 @@ __global__ void __launch_bounds__(TMA_THREADS, 1) prefill_gemm_kernel(const Gemv
             tma_load_1d(xs, p.x_in, bytes * (uint32_t)p.nb, &xbar);
         }
     }
-    if (EPI == EPI_QKV && tid >= NT + 32) {                            // epilogue warp: RoPE rows of the chunk's positions
+    if (EPI == EPI_QKV && tid >= NT + 32) {                            // epilogue warp: RoPE rows of the vectors' positions
         const int half = p.head_size >> 1;
         for (int b = 0; b < p.nb; ++b)
             for (int i = lane; i < half; i += 32) {
-                rope_s[b][0][i] = __ldg(p.rope_cos + (size_t)(p.pos0 + b) * half + i);
-                rope_s[b][1][i] = __ldg(p.rope_sin + (size_t)(p.pos0 + b) * half + i);
+                rope_s[b][0][i] = __ldg(p.rope_cos + (size_t)p.pos_b[b] * half + i);
+                rope_s[b][1][i] = __ldg(p.rope_sin + (size_t)p.pos_b[b] * half + i);
             }
     }
     mbar_wait(&xbar, 0);
@@ -1240,6 +1252,7 @@ __global__ void __launch_bounds__(TMA_THREADS, 1) prefill_gemm_kernel(const Gemv
     if (warp == NWARP + 1) {
         const int eb = lane >> 2, ep = lane & 3;
         const bool active = lane < 4 * NB && eb < p.nb;
+        unsigned long long best = 0ull;                                // EPI_ARGMAX: this lane's rows of vector eb
         for (int t = 0; t < ntiles; ++t) {
             const int par = t & 1, use = t >> 1;
             mbar_wait(&tile_full[par], use & 1);
@@ -1250,7 +1263,20 @@ __global__ void __launch_bounds__(TMA_THREADS, 1) prefill_gemm_kernel(const Gemv
             const int vp = r0 + t * GEMV8_R + 2 * ep;
             if (!active || vp >= r1) continue;
             if (EPI == EPI_QKV) {
-                qkv_store_pair(p, p.out0 + (size_t)eb * p.rows0, p.pos0 + eb, rope_s[eb][0], rope_s[eb][1], vp, s.x, s.y);
+                qkv_store_pair(p, p.out0 + (size_t)eb * p.rows0, p.kcache_b[eb], p.vcache_b[eb], p.pos_b[eb],
+                               rope_s[eb][0], rope_s[eb][1], vp, s.x, s.y);
+            } else if (EPI == EPI_STORE || EPI == EPI_ARGMAX) {   // logits[b][row] (:429), as gemv_epilogue_pair
+                float *dst = p.out0 + (size_t)eb * p.total_rows;
+                dst[vp] = s.x;
+                if (vp + 1 < p.total_rows) dst[vp + 1] = s.y;      // the last pair of an odd vocabulary has one row
+                if (EPI == EPI_ARGMAX) {
+                    const unsigned long long k0 = argmax_key(s.x, vp);
+                    best = k0 > best ? k0 : best;
+                    if (vp + 1 < p.total_rows) {
+                        const unsigned long long k1 = argmax_key(s.y, vp + 1);
+                        best = k1 > best ? k1 : best;
+                    }
+                }
             } else if (EPI == EPI_SILU) {
                 const float sg = __fmul_rn(s.x, __fdiv_rn(1.0f, __fadd_rn(1.0f, expf(-s.x))));   // :412
                 p.out0[(size_t)eb * p.rows0 + (vp >> 1)] = __fmul_rn(sg, s.y);                     // :416
@@ -1263,6 +1289,15 @@ __global__ void __launch_bounds__(TMA_THREADS, 1) prefill_gemm_kernel(const Gemv
                     dst[0] += s.x;
                 }
             }
+        }
+        if (EPI == EPI_ARGMAX) {
+            // the four lanes of vector eb (lanes 4*eb .. 4*eb+3), then one 64-bit atomicMax per CTA and vector
+#pragma unroll
+            for (int o = 2; o > 0; o >>= 1) {
+                const unsigned long long other = __shfl_xor_sync(0xffffffffu, best, o);
+                best = other > best ? other : best;
+            }
+            if (active && ep == 0 && best) atomicMax(p.amax + eb, best);
         }
         return;
     }
@@ -1307,11 +1342,27 @@ struct AttnParams {
     unsigned int *counters;  // (n_heads), zero between launches
     int head_size, kv_dim, kv_mul, nsplit, min_chunk;
     unsigned long long *trace;
-    // batched prompt prefill: gridDim.z positions at once; query z sits at position pos_base + z and
-    // uses q / xb / partial buffers offset by z (pos_base < 0: single position from the control block)
-    int pos_base, q_stride;
+    // batched != 0: gridDim.z queries at once (batched prefill, batched step); query z uses q / xb /
+    // partial buffers / counters offset by z, and its position and caches come from the AttnBatch
+    // argument.  batched == 0: one query at the control block's position on kcache / vcache.
+    int batched, q_stride;
     int seq_len;           // rows of the cache (bounds the speculative first pass; 0 = no speculation)
 };
+
+// Query z of a batched launch: position pos[z] over this layer's caches kcache[z] / vcache[z].  The
+// queries of one launch may be positions of one prompt (one cache) or of different sessions.
+struct AttnBatch {
+    const float *kcache[PF_MAXB], *vcache[PF_MAXB];
+    int pos[PF_MAXB];
+};
+// a[z] through compares with constant indices: indexing the parameter by z would copy it to local memory
+template <typename T>
+__device__ __forceinline__ T batch_entry(const T (&a)[PF_MAXB], int z) {
+    T v = a[0];
+#pragma unroll
+    for (int i = 1; i < PF_MAXB; ++i) v = (z == i) ? a[i] : v;
+    return v;
+}
 
 __device__ __forceinline__ int attn_lanes_per_row(int hs4) {
     return (hs4 % 8 == 0) ? 8 : (hs4 % 4 == 0) ? 4 : (hs4 % 2 == 0) ? 2 : 1;
@@ -1362,7 +1413,9 @@ __device__ __forceinline__ void attn_weighted_rows(float *red, const float *w, c
     }
 }
 
-__global__ void __launch_bounds__(NT) attention_kernel(const AttnParams p) {
+// The AttnBatch argument only gives it attention_flash_kernel's signature: batched launches take the
+// flash kernel (pf_prepare), so this kernel never sees one.
+__global__ void __launch_bounds__(NT) attention_kernel(const AttnParams p, const AttnBatch) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     __shared__ int is_last;
     unsigned long long *atr = p.trace ? p.trace + ((size_t)blockIdx.y * gridDim.x) * TRACE_SLOTS : nullptr;
@@ -1491,7 +1544,7 @@ __device__ __forceinline__ void attn_warp_merge(float &m, float &l, float4 (&acc
 }
 
 template <int NF>   // float4 per lane per row: head_size = 4 * NF * LPR
-__global__ void __launch_bounds__(NT) attention_flash_kernel(const AttnParams p) {
+__global__ void __launch_bounds__(NT) attention_flash_kernel(const AttnParams p, const AttnBatch zb) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     __shared__ int is_last;
     unsigned long long *atr = p.trace ? p.trace + ((size_t)blockIdx.y * gridDim.x) * TRACE_SLOTS : nullptr;
@@ -1510,7 +1563,8 @@ __global__ void __launch_bounds__(NT) attention_flash_kernel(const AttnParams p)
     const float *qz = p.q + (size_t)z * p.q_stride;
     const size_t hoff = (size_t)(h / p.kv_mul) * hs;          // :369, :382
     const float4 *q4 = reinterpret_cast<const float4 *>(qz + (size_t)h * hs);
-    const float *kb = p.kcache + hoff, *vb = p.vcache + hoff;
+    const float *kb = (p.batched ? batch_entry(zb.kcache, z) : p.kcache) + hoff;
+    const float *vb = (p.batched ? batch_entry(zb.vcache, z) : p.vcache) + hoff;
 
     // Everything whose ADDRESS does not depend on the position is requested before the position is
     // read from the control block: q, and (timeline split 0) the cache rows of this lane's first pass —
@@ -1539,7 +1593,9 @@ __global__ void __launch_bounds__(NT) attention_flash_kernel(const AttnParams p)
     }
 
     if (p.ctl[CTL_DONE]) return;
-    const int T = (p.pos_base >= 0 ? p.pos_base + z : p.ctl[CTL_POS]) + 1;
+    // each query has its own length: the split count (`active`), the partial buffers and the
+    // last-arriver counter below are all per z
+    const int T = (p.batched ? batch_entry(zb.pos, z) : p.ctl[CTL_POS]) + 1;
     int chunk = (T + p.nsplit - 1) / p.nsplit;
     if (chunk < p.min_chunk) chunk = p.min_chunk;
     const int active = (T + chunk - 1) / chunk;

@@ -86,6 +86,13 @@ enum StepMode { MODE_LOGITS = 0, MODE_ARGMAX = 1, MODE_SAMPLE = 2, MODE_NOCLS = 
 enum GraphId { G_LOGITS = 0, G_ARGMAX_ONE = 1, G_ARGMAX_LOOP = 2, G_SAMPLE = 3, G_PREFILL_LOOP = 4, G_COUNT = 5 };
 constexpr int kCandCap = 8192;               // top-p candidates returned per step (more => host filters itself)
 
+// The device weights and RoPE tables of one loaded model (one rank's shard), shared by the context that
+// loaded them and every session created on it (l2b_create_session); freed with the last of them.
+struct SharedWeights {
+    int refs = 1;
+    std::vector<void *> owned;
+};
+
 struct l2b_ctx {
     l2b_config cfg{};
     int rank = 0, world = 1, device = 0, num_sms = 0;
@@ -96,7 +103,8 @@ struct l2b_ctx {
     int dim = 0, hidden = 0, head_size = 0, kv_mul = 0;
     int q_dim = 0, kv_dim = 0;              // global
     int q_loc = 0, kv_loc = 0, hid_loc = 0, heads_loc = 0, vocab_loc = 0;
-    // device weights (Weights, src/main.zig:53-71), this rank's slices
+    // device weights (Weights, src/main.zig:53-71), this rank's slices, owned by `weights`
+    SharedWeights *weights = nullptr;
     float *emb = nullptr, *rms_att = nullptr, *rms_ffn = nullptr, *rms_final = nullptr;
     float *wq = nullptr, *wk = nullptr, *wv = nullptr, *wo = nullptr;
     float *w1 = nullptr, *w2 = nullptr, *w3 = nullptr, *wcls = nullptr;
@@ -106,8 +114,11 @@ struct l2b_ctx {
     float *final_X = nullptr;                // which of the two holds x after a step
     float *attn_parts = nullptr;             // small-model fusion: (n_heads, dim) partial vectors of attention + wo
     bool fuse_attn = false;
-    // batched prompt prefill (l2b_prefill, bandwidth-bound shapes): PF_MAXB positions per weight pass
+    // batched prompt prefill (l2b_prefill) and batched step (l2b_forward_batch) on bandwidth-bound shapes:
+    // PF_MAXB vectors per weight pass
     float *pf_x = nullptr, *pf_q = nullptr, *pf_xb = nullptr, *pf_hb = nullptr;   // [PF_MAXB][dim | q | q | hidden]
+    float *pf_logits = nullptr;                                                  // [PF_MAXB][vocab]
+    unsigned long long *pf_amax = nullptr;                                       // [PF_MAXB] packed argmax keys
     float *pf_part_o = nullptr, *pf_part_ml = nullptr;
     unsigned int *pf_counters = nullptr;
     int *pf_tokens = nullptr;
@@ -226,11 +237,12 @@ std::vector<l2b_ctx *> locals(l2b_ctx *ctx) {
     return std::vector<l2b_ctx *>{ctx};
 }
 
+// a device allocation freed with the context, or with the model's weights when owner is given
 template <typename T>
-int dev_alloc(l2b_ctx *ctx, T **p, size_t count) {
+int dev_alloc(l2b_ctx *ctx, T **p, size_t count, std::vector<void *> *owner = nullptr) {
     void *q = nullptr;
     L2B_CUDA(ctx, cudaMalloc(&q, (count ? count : 1) * sizeof(T)));
-    ctx->owned.push_back(q);
+    (owner ? owner : &ctx->owned)->push_back(q);
     *p = static_cast<T *>(q);
     return L2B_OK;
 }
@@ -330,7 +342,7 @@ int materialize(l2b_ctx *ctx, float **dptr, const Source &src, uint64_t payload_
     const uint64_t cols_loc = (mode == SH_COLS) ? cols / g : cols;
     const uint64_t row0 = (mode == SH_ROWS) ? r * rows_loc : 0;
     const uint64_t col0 = (mode == SH_COLS) ? r * cols_loc : 0;
-    int rc = dev_alloc(ctx, dptr, L * rows_loc * cols_loc);
+    int rc = dev_alloc(ctx, dptr, L * rows_loc * cols_loc, &ctx->weights->owned);
     if (rc) return rc;
     const uint64_t tensor_seed = mix64(src.seed * 1000003ull + (uint64_t)tensor_id);
     const bool whole = (rows_loc == rows && cols_loc == cols);
@@ -524,7 +536,7 @@ int launch_gemv(l2b_ctx *ctx, int epi, const GemvParams &p, cudaStream_t st, con
 }
 
 // flash-decoding form when head_size/4 splits into 1..8 float4 per lane, else the 3-pass kernel
-typedef void (*attn_fn)(const AttnParams);
+typedef void (*attn_fn)(const AttnParams, const AttnBatch);
 attn_fn pick_attention(int head_size, bool flash, size_t *smem) {
     const int hs4 = head_size / 4;
     const int lpr = (hs4 % 8 == 0) ? 8 : (hs4 % 4 == 0) ? 4 : (hs4 % 2 == 0) ? 2 : 1;
@@ -607,11 +619,13 @@ int launch_attn_wo(l2b_ctx *ctx, int layer, cudaStream_t st) {
     return L2B_OK;
 }
 
-// Attention of one layer for nb queries (gridDim.z).  Decode: one query at the control block's
-// position (pos_base < 0).  Batched prefill: query z at position pos_base + z, q_stride floats apart
-// in q and xb, with its own partial buffers and counters; it is not traced.
+// Attention of one layer for nb queries (gridDim.z).  Decode (zb == nullptr): one query at the control
+// block's position on this context's caches.  Batched: query z at position zb->pos[z] on the caches
+// zb->kcache[z] / vcache[z], q_stride floats apart in q and xb, with its own partial buffers and
+// counters; it is not traced.
 int launch_attention(l2b_ctx *ctx, int layer, cudaStream_t st, const float *q, float *xb, float *part_o,
-                     float *part_ml, unsigned int *counters, int pos_base = -1, int q_stride = 0, int nb = 1) {
+                     float *part_ml, unsigned int *counters, const AttnBatch *zb = nullptr, int q_stride = 0,
+                     int nb = 1) {
     if (ctx->profiling) {
         const int hpos = ctx->n_appended > 0 ? ctx->n_appended - 1 : 0;
         int prc = prof_mark(ctx, "attention", layer, 2ull * (uint64_t)(hpos + 1) * ctx->kv_loc * 4ull, st);
@@ -632,10 +646,11 @@ int launch_attention(l2b_ctx *ctx, int layer, cudaStream_t st, const float *q, f
     a.kv_mul = ctx->kv_mul;
     a.nsplit = ctx->nsplit;
     a.min_chunk = ctx->min_chunk;
-    a.pos_base = pos_base;
+    a.batched = zb ? 1 : 0;
     a.q_stride = q_stride;
     a.seq_len = ctx->cfg.seq_len;
-    a.trace = pos_base < 0 ? trace_slot(ctx) : nullptr;
+    a.trace = zb ? nullptr : trace_slot(ctx);
+    const AttnBatch none{};
     size_t smem = ctx->attn_smem;
     attn_fn fn = pick_attention(ctx->head_size, ctx->attn_flash, &smem);
     cudaLaunchConfig_t lc{};
@@ -646,7 +661,7 @@ int launch_attention(l2b_ctx *ctx, int layer, cudaStream_t st, const float *q, f
     cudaLaunchAttribute at[1] = {pdl_attr()};
     lc.attrs = at;
     lc.numAttrs = ctx->use_pdl ? 1 : 0;
-    L2B_CUDA(ctx, cudaLaunchKernelEx(&lc, fn, a));
+    L2B_CUDA(ctx, cudaLaunchKernelEx(&lc, fn, a, zb ? *zb : none));
     ++ctx->last_launches;
     return L2B_OK;
 }
@@ -999,8 +1014,8 @@ int preload_kernels(l2b_ctx *ctx) {
 }
 
 // ---- creation, stage 1: weights + run state of one rank (no peer is touched) ------------------
-int create_rank(l2b_ctx *ctx, const l2b_config *cfg, const Source &src, const float *rope_cos,
-                const float *rope_sin, int rank, int world, int device) {
+// device, derived sizes, stream and events of one rank
+int init_rank(l2b_ctx *ctx, const l2b_config *cfg, int rank, int world, int device) {
     cudaDeviceProp prop{};
     if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) { ctx->err = "cudaGetDeviceProperties failed"; g_create_error = ctx->err; return L2B_ERR_CUDA; }
     if (prop.major != 9 || prop.minor != 0) { ctx->err = "device is not compute capability 9.0 (built for sm_90a only)"; g_create_error = ctx->err; return L2B_ERR_NO_DEVICE; }
@@ -1022,7 +1037,15 @@ int create_rank(l2b_ctx *ctx, const l2b_config *cfg, const Source &src, const fl
     L2B_TRY(cuda_try(ctx, cudaEventCreate(&ctx->ev0), "cudaEventCreate"));
     L2B_TRY(cuda_try(ctx, cudaEventCreate(&ctx->ev1), "cudaEventCreate"));
     L2B_TRY(preload_kernels(ctx));
+    return L2B_OK;
+}
 
+int create_run_state(l2b_ctx *ctx);
+
+int create_rank(l2b_ctx *ctx, const l2b_config *cfg, const Source &src, const float *rope_cos,
+                const float *rope_sin, int rank, int world, int device) {
+    L2B_TRY(init_rank(ctx, cfg, rank, world, device));
+    ctx->weights = new SharedWeights();
     const uint64_t dim = cfg->dim, hid = cfg->hidden_dim, L = cfg->n_layers, V = cfg->vocab_size, S = cfg->seq_len;
     const uint64_t hs = ctx->head_size, kvd = ctx->kv_dim;
     const double sd = sqrt(288.0 / (double)dim), sh = sqrt(768.0 / (double)hid);
@@ -1067,7 +1090,37 @@ int create_rank(l2b_ctx *ctx, const l2b_config *cfg, const Source &src, const fl
         if (ctx->stage_ev[i]) { cudaEventDestroy(ctx->stage_ev[i]); ctx->stage_ev[i] = nullptr; }
     }
 
-    // ---- run state
+    // ---- RoPE table (:338-342); the host's own libm values when the caller passes them
+    L2B_TRY(dev_alloc(ctx, &ctx->rope_cos, S * hs / 2, &ctx->weights->owned));
+    L2B_TRY(dev_alloc(ctx, &ctx->rope_sin, S * hs / 2, &ctx->weights->owned));
+    {
+        std::vector<float> hc(S * hs / 2), hsn(S * hs / 2);
+        if (rope_cos && rope_sin) {
+            memcpy(hc.data(), rope_cos, hc.size() * sizeof(float));
+            memcpy(hsn.data(), rope_sin, hsn.size() * sizeof(float));
+        } else {
+            for (uint64_t p = 0; p < S; ++p)
+                for (uint64_t j = 0; j < hs / 2; ++j) {
+                    const float head_dim = (float)(2 * j);                                   // i % head_size
+                    const float freq = 1.0f / powf(10000.0f, head_dim / (float)hs);          // :339
+                    const float val = (float)p * freq;                                       // :340
+                    hc[p * (hs / 2) + j] = cosf(val);                                        // :341
+                    hsn[p * (hs / 2) + j] = sinf(val);                                       // :342
+                }
+        }
+        L2B_TRY(cuda_try(ctx, cudaMemcpy(ctx->rope_cos, hc.data(), hc.size() * sizeof(float), cudaMemcpyHostToDevice), "rope upload"));
+        L2B_TRY(cuda_try(ctx, cudaMemcpy(ctx->rope_sin, hsn.data(), hsn.size() * sizeof(float), cudaMemcpyHostToDevice), "rope upload"));
+    }
+    return create_run_state(ctx);
+}
+
+// run state, attention launch shape, pinned host buffers, tensor-parallel landing area and switches
+// of one rank whose weights are in place
+int create_run_state(l2b_ctx *ctx) {
+    const l2b_config *cfg = &ctx->cfg;
+    const int rank = ctx->rank, world = ctx->world;
+    const uint64_t dim = cfg->dim, L = cfg->n_layers, V = cfg->vocab_size, S = cfg->seq_len;
+    const uint64_t hs = ctx->head_size;
     L2B_TRY(dev_alloc(ctx, &ctx->X, dim));
     L2B_TRY(dev_alloc(ctx, &ctx->Xalt, dim));
     {
@@ -1091,8 +1144,6 @@ int create_rank(l2b_ctx *ctx, const l2b_config *cfg, const Source &src, const fl
     if (world > 1) L2B_TRY(dev_alloc(ctx, &ctx->logits_loc, (size_t)ctx->vocab_loc));
     L2B_TRY(dev_alloc(ctx, &ctx->kcache, L * S * ctx->kv_loc));
     L2B_TRY(dev_alloc(ctx, &ctx->vcache, L * S * ctx->kv_loc));
-    L2B_TRY(dev_alloc(ctx, &ctx->rope_cos, S * hs / 2));
-    L2B_TRY(dev_alloc(ctx, &ctx->rope_sin, S * hs / 2));
     L2B_TRY(dev_alloc(ctx, &ctx->ctl, (size_t)CTL_WORDS));
     L2B_TRY(dev_alloc(ctx, &ctx->amax, (size_t)1));
     L2B_TRY(dev_alloc(ctx, &ctx->gen_forced, S));
@@ -1131,26 +1182,6 @@ int create_rank(l2b_ctx *ctx, const l2b_config *cfg, const Source &src, const fl
         L2B_TRY(dev_alloc(ctx, &ctx->part_ml, (size_t)ctx->heads_loc * ns * 2));
         L2B_TRY(dev_alloc(ctx, &ctx->counters, (size_t)ctx->heads_loc));
         L2B_TRY(cuda_try(ctx, cudaMemsetAsync(ctx->counters, 0, ctx->heads_loc * sizeof(unsigned int), ctx->stream), "memset"));
-    }
-
-    // ---- RoPE table (:338-342); the host's own libm values when the caller passes them
-    {
-        std::vector<float> hc(S * hs / 2), hsn(S * hs / 2);
-        if (rope_cos && rope_sin) {
-            memcpy(hc.data(), rope_cos, hc.size() * sizeof(float));
-            memcpy(hsn.data(), rope_sin, hsn.size() * sizeof(float));
-        } else {
-            for (uint64_t p = 0; p < S; ++p)
-                for (uint64_t j = 0; j < hs / 2; ++j) {
-                    const float head_dim = (float)(2 * j);                                   // i % head_size
-                    const float freq = 1.0f / powf(10000.0f, head_dim / (float)hs);          // :339
-                    const float val = (float)p * freq;                                       // :340
-                    hc[p * (hs / 2) + j] = cosf(val);                                        // :341
-                    hsn[p * (hs / 2) + j] = sinf(val);                                       // :342
-                }
-        }
-        L2B_TRY(cuda_try(ctx, cudaMemcpy(ctx->rope_cos, hc.data(), hc.size() * sizeof(float), cudaMemcpyHostToDevice), "rope upload"));
-        L2B_TRY(cuda_try(ctx, cudaMemcpy(ctx->rope_sin, hsn.data(), hsn.size() * sizeof(float), cudaMemcpyHostToDevice), "rope upload"));
     }
 
     // ---- pinned host buffers
@@ -1317,6 +1348,10 @@ void destroy_rank(l2b_ctx *ctx) {
     if (ctx->comm && g_nccl.ok) g_nccl.CommDestroy(ctx->comm);
     for (void *p : ctx->ipc_opened) cudaIpcCloseMemHandle(p);
     for (void *p : ctx->owned) cudaFree(p);
+    if (ctx->weights && --ctx->weights->refs == 0) {   // the last context or session of the model
+        for (void *p : ctx->weights->owned) cudaFree(p);
+        delete ctx->weights;
+    }
     for (int i = 0; i < 2; ++i) {
         if (ctx->stage[i]) cudaFreeHost(ctx->stage[i]);
         if (ctx->stage_ev[i]) cudaEventDestroy(ctx->stage_ev[i]);
@@ -1404,6 +1439,19 @@ int common_create(l2b_ctx **out, const l2b_config *cfg, const Source &src, uint6
     if (in_process) ranks[0]->members = ranks;
     *out = ranks[0];
     return L2B_OK;
+}
+
+// a context on the weights of `model` (single GPU): its own run state, caches, stream and graphs
+int create_session(l2b_ctx *ctx, const l2b_ctx *model) {
+    L2B_TRY(init_rank(ctx, &model->cfg, 0, 1, model->device));
+    ctx->weights = model->weights;
+    ++ctx->weights->refs;
+    ctx->emb = model->emb; ctx->rms_att = model->rms_att; ctx->rms_ffn = model->rms_ffn; ctx->rms_final = model->rms_final;
+    ctx->wq = model->wq; ctx->wk = model->wk; ctx->wv = model->wv; ctx->wo = model->wo;
+    ctx->w1 = model->w1; ctx->w2 = model->w2; ctx->w3 = model->w3; ctx->wcls = model->wcls;
+    ctx->rope_cos = model->rope_cos; ctx->rope_sin = model->rope_sin;
+    L2B_TRY(create_run_state(ctx));
+    return warm_up(std::vector<l2b_ctx *>{ctx});
 }
 #undef L2B_TRY
 
@@ -1541,6 +1589,17 @@ int32_t l2b_create_synthetic_group(l2b_ctx **out, const l2b_config *cfg, uint64_
     return common_create(out, cfg, s, 0, nullptr, nullptr, nullptr, n_gpus);
 }
 
+int32_t l2b_create_session(l2b_ctx **out, l2b_ctx *model) {
+    if (!out || !model) { g_create_error = "NULL argument"; return L2B_ERR_INVALID_ARG; }
+    *out = nullptr;
+    if (model->world > 1) { g_create_error = "sessions need a single-GPU model (tensor parallel is not supported)"; return L2B_ERR_UNSUPPORTED; }
+    l2b_ctx *ctx = new l2b_ctx();
+    const int rc = create_session(ctx, model);
+    if (rc) { destroy_rank(ctx); return rc; }
+    *out = ctx;
+    return L2B_OK;
+}
+
 void l2b_destroy(l2b_ctx *ctx) { destroy_all(ctx); }
 
 int32_t l2b_reset(l2b_ctx *ctx) {
@@ -1618,6 +1677,8 @@ gemv_fn pf_pick(int epi) {
     switch (epi) {
     case EPI_QKV: return prefill_gemm_kernel<EPI_QKV, NB>;
     case EPI_SILU: return prefill_gemm_kernel<EPI_SILU, NB>;
+    case EPI_STORE: return prefill_gemm_kernel<EPI_STORE, NB>;
+    case EPI_ARGMAX: return prefill_gemm_kernel<EPI_ARGMAX, NB>;
     default: return prefill_gemm_kernel<EPI_RESID, NB>;
     }
 }
@@ -1625,7 +1686,9 @@ constexpr size_t kPfSmemBudget = 227 * 1024 - 8192;   // the prefill kernels kee
 
 // can this context prefill PF_MAXB positions per weight pass?  Single GPU, flash attention, and all
 // four per-layer GEMVs bandwidth-bound shapes of the TMA-ring kernel; otherwise l2b_prefill runs the
-// positions one by one on the device (same results, weights streamed once per position).
+// positions one by one on the device (same results, weights streamed once per position).  The batched
+// step (l2b_forward_batch) makes the same choice on its first session; its classifier's dim-wide
+// inputs fit wherever qkv's do.
 static int pf_prepare(l2b_ctx *ctx) {
     if (ctx->pf_ready) return L2B_OK;
     ctx->pf_ready = true;
@@ -1646,12 +1709,14 @@ static int pf_prepare(l2b_ctx *ctx) {
     if ((rc = dev_alloc(ctx, &ctx->pf_q, PF_MAXB * q))) return rc;
     if ((rc = dev_alloc(ctx, &ctx->pf_xb, PF_MAXB * q))) return rc;
     if ((rc = dev_alloc(ctx, &ctx->pf_hb, PF_MAXB * hid))) return rc;
+    if ((rc = dev_alloc(ctx, &ctx->pf_logits, (size_t)PF_MAXB * ctx->vocab_loc))) return rc;
+    if ((rc = dev_alloc(ctx, &ctx->pf_amax, (size_t)PF_MAXB))) return rc;
     if ((rc = dev_alloc(ctx, &ctx->pf_part_o, (size_t)PF_MAXB * ctx->heads_loc * ctx->nsplit * ctx->head_size))) return rc;
     if ((rc = dev_alloc(ctx, &ctx->pf_part_ml, (size_t)PF_MAXB * ctx->heads_loc * ctx->nsplit * 2))) return rc;
     if ((rc = dev_alloc(ctx, &ctx->pf_counters, (size_t)PF_MAXB * ctx->heads_loc))) return rc;
     if ((rc = dev_alloc(ctx, &ctx->pf_tokens, (size_t)ctx->cfg.seq_len))) return rc;
     L2B_CUDA(ctx, cudaMemsetAsync(ctx->pf_counters, 0, (size_t)PF_MAXB * ctx->heads_loc * sizeof(unsigned int), ctx->stream));
-    for (int epi : {(int)EPI_QKV, (int)EPI_SILU, (int)EPI_RESID}) {
+    for (int epi : {(int)EPI_QKV, (int)EPI_SILU, (int)EPI_RESID, (int)EPI_STORE, (int)EPI_ARGMAX}) {
         L2B_CUDA(ctx, cudaFuncSetAttribute(pf_pick<PF_MAXB>(epi), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPfSmemBudget));
         L2B_CUDA(ctx, cudaFuncSetAttribute(pf_pick<2>(epi), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPfSmemBudget));
     }
@@ -1683,10 +1748,62 @@ static int pf_launch(l2b_ctx *ctx, int epi, GemvParams p, cudaStream_t st) {
     return L2B_OK;
 }
 
+// nb <= PF_MAXB vectors through every layer in one pass over the weights, on ctx's stream and batch
+// buffers: vector b enters as the embedding row of d_tokens[b] and runs at position pos[b] on the KV
+// cache of kv[b] (a prompt: one context at consecutive positions; the batched step: one session per
+// vector).  Its x is left in ctx->pf_x[b].
+static int batched_layers(l2b_ctx *ctx, l2b_ctx *const *kv, const int *pos, int nb, const int *d_tokens) {
+    const int dim = ctx->dim;
+    cudaStream_t st = ctx->stream;
+    for (int l = 0; l < ctx->cfg.n_layers; ++l) {
+        LayerGemvs g = layer_gemvs(ctx, l);
+        const size_t loff = (size_t)l * ctx->cfg.seq_len * ctx->kv_loc;
+        AttnBatch zb{};
+        for (int b = 0; b < nb; ++b) {
+            g.qkv.pos_b[b] = zb.pos[b] = pos[b];
+            g.qkv.kcache_b[b] = kv[b]->kcache + loff;
+            g.qkv.vcache_b[b] = kv[b]->vcache + loff;
+            zb.kcache[b] = g.qkv.kcache_b[b];
+            zb.vcache[b] = g.qkv.vcache_b[b];
+        }
+        // ---- rmsnorm + q,k,v + RoPE + KV append for nb vectors (:305-358)
+        g.qkv.nb = nb;
+        g.qkv.x_in = ctx->pf_x;
+        if (l == 0) { g.qkv.emb = ctx->emb; g.qkv.tokens = d_tokens; g.qkv.x_out = ctx->pf_x; }
+        g.qkv.out0 = ctx->pf_q;
+        int rc = pf_launch<PF_MAXB>(ctx, EPI_QKV, g.qkv, st);
+        if (rc) return rc;
+        // ---- attention of the nb queries (:361-389); query z sees positions 0 .. pos[z] of its cache
+        rc = launch_attention(ctx, l, st, ctx->pf_q, ctx->pf_xb, ctx->pf_part_o, ctx->pf_part_ml, ctx->pf_counters,
+                              &zb, ctx->q_loc, nb);
+        if (rc) return rc;
+        // ---- wo + residual (:392-395)
+        g.wo.nb = nb;
+        g.wo.x_in = ctx->pf_xb;
+        g.wo.out0 = ctx->pf_x;
+        rc = pf_launch<PF_MAXB>(ctx, EPI_RESID, g.wo, st);
+        if (rc) return rc;
+        // ---- rmsnorm + w1,w3 + SiLU*mul (:398-416)
+        g.w13.nb = nb;
+        g.w13.x_in = ctx->pf_x;
+        g.w13.out0 = ctx->pf_hb;
+        rc = pf_launch<PF_MAXB>(ctx, EPI_SILU, g.w13, st);
+        if (rc) return rc;
+        // ---- w2 + residual (:419-422); hidden-sized inputs: two vectors per pass (shared memory)
+        for (int b = 0; b < nb; b += 2) {
+            GemvParams d = g.w2;
+            d.nb = nb - b < 2 ? nb - b : 2;
+            d.x_in = ctx->pf_hb + (size_t)b * ctx->hid_loc;
+            d.out0 = ctx->pf_x + (size_t)b * dim;
+            rc = pf_launch<2>(ctx, EPI_RESID, d, st);
+            if (rc) return rc;
+        }
+    }
+    return L2B_OK;
+}
+
 // n_tokens positions starting at pos0, PF_MAXB per pass over the weights; KV cache filled, no logits
 static int prefill_batched(l2b_ctx *ctx, const int32_t *tokens, int n_tokens, int pos0) {
-    const l2b_config &c = ctx->cfg;
-    const int dim = ctx->dim;
     cudaStream_t st = ctx->stream;
     L2B_CUDA(ctx, cudaSetDevice(ctx->device));
     for (int i = 0; i < n_tokens; ++i) ctx->h_gen[i] = tokens[i];
@@ -1697,48 +1814,109 @@ static int prefill_batched(l2b_ctx *ctx, const int32_t *tokens, int n_tokens, in
     ctx->last_launches = 0;
     for (int done = 0; done < n_tokens; done += PF_MAXB) {
         const int nb = n_tokens - done < PF_MAXB ? n_tokens - done : PF_MAXB;
-        const int pos = pos0 + done;
-        for (int l = 0; l < c.n_layers; ++l) {
-            LayerGemvs g = layer_gemvs(ctx, l);
-            // ---- rmsnorm + q,k,v + RoPE + KV append for nb positions (:305-358)
-            g.qkv.nb = nb; g.qkv.pos0 = pos;
-            g.qkv.x_in = ctx->pf_x;
-            if (l == 0) { g.qkv.emb = ctx->emb; g.qkv.tokens = ctx->pf_tokens + done; g.qkv.x_out = ctx->pf_x; }
-            g.qkv.out0 = ctx->pf_q;
-            int rc = pf_launch<PF_MAXB>(ctx, EPI_QKV, g.qkv, st);
-            if (rc) return rc;
-            // ---- attention of the nb queries (:361-389); query z sees positions 0 .. pos+z
-            rc = launch_attention(ctx, l, st, ctx->pf_q, ctx->pf_xb, ctx->pf_part_o, ctx->pf_part_ml, ctx->pf_counters,
-                                  pos, ctx->q_loc, nb);
-            if (rc) return rc;
-            // ---- wo + residual (:392-395)
-            g.wo.nb = nb; g.wo.pos0 = pos;
-            g.wo.x_in = ctx->pf_xb;
-            g.wo.out0 = ctx->pf_x;
-            rc = pf_launch<PF_MAXB>(ctx, EPI_RESID, g.wo, st);
-            if (rc) return rc;
-            // ---- rmsnorm + w1,w3 + SiLU*mul (:398-416)
-            g.w13.nb = nb; g.w13.pos0 = pos;
-            g.w13.x_in = ctx->pf_x;
-            g.w13.out0 = ctx->pf_hb;
-            rc = pf_launch<PF_MAXB>(ctx, EPI_SILU, g.w13, st);
-            if (rc) return rc;
-            // ---- w2 + residual (:419-422); hidden-sized inputs: two positions per pass (shared memory)
-            for (int b = 0; b < nb; b += 2) {
-                GemvParams d = g.w2;
-                d.nb = nb - b < 2 ? nb - b : 2; d.pos0 = pos + b;
-                d.x_in = ctx->pf_hb + (size_t)b * ctx->hid_loc;
-                d.out0 = ctx->pf_x + (size_t)b * dim;
-                rc = pf_launch<2>(ctx, EPI_RESID, d, st);
-                if (rc) return rc;
-            }
-        }
+        l2b_ctx *kv[PF_MAXB];
+        int pos[PF_MAXB];
+        for (int b = 0; b < nb; ++b) { kv[b] = ctx; pos[b] = pos0 + done + b; }
+        int rc = batched_layers(ctx, kv, pos, nb, ctx->pf_tokens + done);
+        if (rc) return rc;
     }
     L2B_CUDA(ctx, cudaEventRecord(ctx->ev1, st));
     L2B_CUDA(ctx, cudaStreamSynchronize(st));
     L2B_CUDA(ctx, cudaGetLastError());
     L2B_CUDA(ctx, cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
     if (pos0 + n_tokens > ctx->n_appended) ctx->n_appended = pos0 + n_tokens;
+    return L2B_OK;
+}
+
+// Everything a batched step checks, before anything is launched: a refused call changes no session.
+static int check_batch_args(l2b_ctx *const *s, int32_t n, const int32_t *tokens, const int32_t *pos) {
+    if (!s || n < 1 || !s[0]) { g_create_error = "sessions is NULL, n < 1 or sessions[0] is NULL"; return L2B_ERR_INVALID_ARG; }
+    l2b_ctx *s0 = s[0];
+    if (!tokens || !pos) return fail(s0, L2B_ERR_INVALID_ARG, "tokens or pos is NULL");
+    std::set<const l2b_ctx *> seen;
+    for (int i = 0; i < n; ++i) {
+        const l2b_ctx *c = s[i];
+        if (!c) return fail(s0, L2B_ERR_INVALID_ARG, "NULL session");
+        if (!seen.insert(c).second) return fail(s0, L2B_ERR_INVALID_ARG, "the same session twice in one batch");
+        if (c->weights != s0->weights) return fail(s0, L2B_ERR_INVALID_ARG, "sessions of different models");
+        if (tokens[i] < 0 || tokens[i] >= c->cfg.vocab_size) return fail(s0, L2B_ERR_INVALID_ARG, "token out of range");
+        if (pos[i] < 0 || pos[i] >= c->cfg.seq_len) return fail(s0, L2B_ERR_INVALID_ARG, "pos out of range");
+    }
+    for (int i = 0; i < n; ++i)
+        if (pos[i] > s[i]->n_appended) return fail(s0, L2B_ERR_STATE, "pos skips ahead of a session's KV cache");
+    return L2B_OK;
+}
+
+// One step of each of n validated sessions.  Where l2b_prefill would batch (pf_prepare on the first
+// session), PF_MAXB sessions share each pass over the weights on the first session's stream and batch
+// buffers; each session's x and logits are then copied to its own buffers (xb, hb and q are not
+// written).  Otherwise each session runs its own step in turn.  Leaves each session's logits in its
+// h_logits, or (argmax) the next token in its h_ints[0]; the call's time and launches on s[0].
+static int step_sessions(l2b_ctx *const *s, int n, const int32_t *tokens, const int32_t *pos, bool argmax) {
+    l2b_ctx *ctx = s[0];
+    int rc = pf_prepare(ctx);
+    if (rc) return rc;
+    cudaStream_t st = ctx->stream;
+    L2B_CUDA(ctx, cudaSetDevice(ctx->device));
+    L2B_CUDA(ctx, cudaEventRecord(ctx->ev0, st));
+    if (!ctx->pf_ok) {
+        int launches = 0;
+        for (int i = 0; i < n; ++i) {
+            rc = run_step(s[i], tokens[i], pos[i], argmax ? G_ARGMAX_ONE : G_LOGITS, 1.0f, 0.0f);
+            if (rc) { ctx->err = s[i]->err; return rc; }
+            launches += s[i]->last_launches;
+        }
+        // every step above ended in a synchronise: ev0 .. ev1 spans them all
+        L2B_CUDA(ctx, cudaEventRecord(ctx->ev1, s[n - 1]->stream));
+        L2B_CUDA(ctx, cudaEventSynchronize(ctx->ev1));
+        L2B_CUDA(ctx, cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
+        ctx->last_launches = launches;
+        return L2B_OK;
+    }
+    const int dim = ctx->dim, V = ctx->cfg.vocab_size;
+    fill_ctl(ctx, tokens[0], pos[0], 0, 1.0f, -1.0f);        // DONE = 0 for the attention kernel
+    L2B_CUDA(ctx, cudaMemcpyAsync(ctx->ctl, ctx->h_ctl, CTL_HOST_WORDS * sizeof(int), cudaMemcpyHostToDevice, st));
+    ctx->last_launches = 0;
+    for (int g = 0; g < n; g += PF_MAXB) {
+        const int nb = n - g < PF_MAXB ? n - g : PF_MAXB;
+        // from the caller's (pageable) array: staged before the call returns, ordered after the previous group
+        L2B_CUDA(ctx, cudaMemcpyAsync(ctx->pf_tokens, tokens + g, (size_t)nb * sizeof(int), cudaMemcpyHostToDevice, st));
+        rc = batched_layers(ctx, s + g, pos + g, nb, ctx->pf_tokens);
+        if (rc) return rc;
+        // ---- final rmsnorm + classifier (:426-429) of the nb vectors
+        GemvParams k{};
+        k.ctl = ctx->ctl;
+        k.n = dim;
+        k.nb = nb;
+        k.x_in = ctx->pf_x;
+        k.gamma = ctx->rms_final;
+        k.w0 = ctx->wcls;
+        k.total_rows = V; k.rows0 = V;
+        k.out0 = ctx->pf_logits;
+        k.amax = ctx->pf_amax;
+        if (argmax) L2B_CUDA(ctx, cudaMemsetAsync(ctx->pf_amax, 0, PF_MAXB * sizeof(unsigned long long), st));
+        rc = pf_launch<PF_MAXB>(ctx, argmax ? EPI_ARGMAX : EPI_STORE, k, st);
+        if (rc) return rc;
+        for (int b = 0; b < nb; ++b) {
+            l2b_ctx *c = s[g + b];
+            L2B_CUDA(ctx, cudaMemcpyAsync(c->X, ctx->pf_x + (size_t)b * dim, dim * sizeof(float), cudaMemcpyDeviceToDevice, st));
+            L2B_CUDA(ctx, cudaMemcpyAsync(c->logits, ctx->pf_logits + (size_t)b * V, V * sizeof(float), cudaMemcpyDeviceToDevice, st));
+            if (argmax)   // the key's low word (little-endian: its first 4 bytes) is 0xFFFFFFFF - index
+                L2B_CUDA(ctx, cudaMemcpyAsync(c->h_ints, ctx->pf_amax + b, sizeof(int), cudaMemcpyDeviceToHost, st));
+            else
+                L2B_CUDA(ctx, cudaMemcpyAsync(c->h_logits, ctx->pf_logits + (size_t)b * V, V * sizeof(float), cudaMemcpyDeviceToHost, st));
+        }
+    }
+    L2B_CUDA(ctx, cudaEventRecord(ctx->ev1, st));
+    L2B_CUDA(ctx, cudaStreamSynchronize(st));
+    L2B_CUDA(ctx, cudaGetLastError());
+    L2B_CUDA(ctx, cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
+    for (int i = 0; i < n; ++i) {
+        l2b_ctx *c = s[i];
+        c->final_X = c->X;
+        if (argmax) c->h_ints[0] = (int)(0xFFFFFFFFu - (uint32_t)c->h_ints[0]);
+        if (pos[i] + 1 > c->n_appended) c->n_appended = pos[i] + 1;
+    }
     return L2B_OK;
 }
 
@@ -1844,6 +2022,32 @@ int32_t l2b_prefill(l2b_ctx *ctx, const int32_t *tokens, int32_t n_tokens, int32
         if (done != n_silent) return fail(ctx, L2B_ERR_STATE, "prefill stopped early");
     }
     if (host_logits) return l2b_forward(ctx, tokens[n_tokens - 1], pos0 + n_tokens - 1, host_logits);
+    return L2B_OK;
+}
+
+int32_t l2b_forward_batch(l2b_ctx *const *sessions, int32_t n, const int32_t *tokens, const int32_t *pos,
+                          float *const *host_logits) {
+    int rc = check_batch_args(sessions, n, tokens, pos);
+    if (rc) return rc;
+    if (!host_logits) return fail(sessions[0], L2B_ERR_INVALID_ARG, "host_logits is NULL");
+    for (int i = 0; i < n; ++i)
+        if (!host_logits[i]) return fail(sessions[0], L2B_ERR_INVALID_ARG, "a host_logits entry is NULL");
+    rc = step_sessions(sessions, n, tokens, pos, false);
+    if (rc) return rc;
+    for (int i = 0; i < n; ++i)
+        if (host_logits[i] != sessions[i]->h_logits)
+            memcpy(host_logits[i], sessions[i]->h_logits, (size_t)sessions[i]->cfg.vocab_size * sizeof(float));
+    return L2B_OK;
+}
+
+int32_t l2b_forward_argmax_batch(l2b_ctx *const *sessions, int32_t n, const int32_t *tokens, const int32_t *pos,
+                                 int32_t *next) {
+    int rc = check_batch_args(sessions, n, tokens, pos);
+    if (rc) return rc;
+    if (!next) return fail(sessions[0], L2B_ERR_INVALID_ARG, "next is NULL");
+    rc = step_sessions(sessions, n, tokens, pos, true);
+    if (rc) return rc;
+    for (int i = 0; i < n; ++i) next[i] = sessions[i]->h_ints[0];
     return L2B_OK;
 }
 
@@ -2128,7 +2332,6 @@ int32_t l2b_op_attention_head(int32_t device, float *out, const float *q, const 
     a.ctl = ctl; a.q = dq; a.kcache = dk; a.vcache = dv; a.xb = dout; a.part_o = po; a.part_ml = pml;
     a.counters = cnt; a.head_size = head_size; a.kv_dim = kv_stride; a.kv_mul = 1; a.nsplit = nsplit;
     a.min_chunk = 64;
-    a.pos_base = -1;
     a.seq_len = n_pos;
     int cap = (n_pos + nsplit - 1) / nsplit;
     if (cap < 64) cap = 64;
@@ -2140,7 +2343,7 @@ int32_t l2b_op_attention_head(int32_t device, float *out, const float *q, const 
         const char *enva = getenv("L2B_ATTN");
         size_t smem2 = smem;
         attn_fn fn = pick_attention(head_size, !(enva && strcmp(enva, "3pass") == 0), &smem2);
-        fn<<<dim3(1, nsplit), NT, smem2>>>(a);
+        fn<<<dim3(1, nsplit), NT, smem2>>>(a, AttnBatch{});
     }
     s.down(out, dout, head_size);
     return s.rc;
