@@ -174,7 +174,9 @@ int32_t l2b_forward_sample(l2b_ctx *ctx, int32_t token, int32_t pos, float tempe
  * `token` at position `pos`, runs up to n_steps steps, feeds forced[i] (if forced != NULL
  * and forced[i] >= 0, like prompt forcing :999-1000) or the on-device argmax back in, and
  * stops after emitting BOS (token 1, :1017-1019) when stop_on_bos != 0.  out_next[i] is the
- * token chosen at step i; *n_done the number of transformer steps executed.                */
+ * token chosen at step i; *n_done the number of transformer steps executed.  At most
+ * seq_len - pos steps run (:992-993).  A forced entry that is read and lies outside
+ * [-1, vocab_size) => L2B_ERR_INVALID_ARG before anything runs.                            */
 int32_t l2b_generate_argmax(l2b_ctx *ctx, int32_t token, int32_t pos, int32_t n_steps,
                             const int32_t *forced, int32_t stop_on_bos, int32_t *out_next,
                             int32_t *n_done);
@@ -209,6 +211,23 @@ int32_t l2b_forward_batch(l2b_ctx *const *sessions, int32_t n, const int32_t *to
 /* Same step with the device argmax (first maximum wins, :715-726): next[i] for session i.      */
 int32_t l2b_forward_argmax_batch(l2b_ctx *const *sessions, int32_t n, const int32_t *tokens,
                                  const int32_t *pos, int32_t *next);
+/* The greedy loop of l2b_generate_argmax on n sessions in one call, with no host round trip per
+ * step.  For each i it does what l2b_generate_argmax(sessions[i], tokens[i], pos[i], n_steps,
+ * forced + i*n_steps, stop_on_bos, out_next + i*n_steps, &n_done[i]) does: forced (may be NULL)
+ * and out_next are row-major n x n_steps, forced[i*n_steps + s] >= 0 replaces session i's argmax at
+ * step s and -1 lets it run free; session i runs at most min(n_steps, seq_len - pos[i]) steps and,
+ * with stop_on_bos, stops after emitting BOS while the others go on.  Afterwards session i has
+ * pos[i] + n_done[i] positions appended; its KV rows from there on are untouched.  The sessions
+ * share weight passes exactly where l2b_forward_batch does, with the same kernels (up to 4 per
+ * pass, all steps enqueued at once); elsewhere each session replays its own device loop on its own
+ * stream, bit for bit l2b_generate_argmax.  Checked before anything runs, as l2b_forward_batch,
+ * plus n_steps < 0, a NULL out_next or n_done, and a forced entry that is read and lies outside
+ * [-1, vocab_size) => L2B_ERR_INVALID_ARG.  n_steps == 0 sets every n_done[i] = 0 and runs
+ * nothing.  l2b_last_timing(sessions[0]) gives the whole call's device time and kernel launches.
+ * x, xb, hb, q and logits of the sessions are not defined afterwards.  Synchronous.           */
+int32_t l2b_generate_argmax_batch(l2b_ctx *const *sessions, int32_t n, const int32_t *tokens,
+                                  const int32_t *pos, int32_t n_steps, const int32_t *forced,
+                                  int32_t stop_on_bos, int32_t *out_next, int32_t *n_done);
 
 /* ---- introspection ------------------------------------------------------------------- */
 

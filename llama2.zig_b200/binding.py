@@ -83,6 +83,7 @@ def load_library():
     lib.l2b_create_session.argtypes = [C.POINTER(vp), vp]
     lib.l2b_forward_batch.argtypes = [C.POINTER(vp), C.c_int32, IP, IP, C.POINTER(FP)]
     lib.l2b_forward_argmax_batch.argtypes = [C.POINTER(vp), C.c_int32, IP, IP, IP]
+    lib.l2b_generate_argmax_batch.argtypes = [C.POINTER(vp), C.c_int32, IP, IP, C.c_int32, IP, C.c_int32, IP, IP]
     lib.l2b_destroy.argtypes = [vp]
     lib.l2b_destroy.restype = None
     lib.l2b_reset.argtypes = [vp]
@@ -374,6 +375,26 @@ def forward_argmax_batch(sessions, tokens, positions):
     _check(load_library().l2b_forward_argmax_batch(hs, n, toks.ctypes.data_as(IP), pos.ctypes.data_as(IP),
                                                    nxt.ctypes.data_as(IP)), hs[0] if n else None)
     return nxt[:n].copy()
+
+
+def generate_argmax_batch(sessions, tokens, positions, n_steps, forced=None, stop_on_bos=True):
+    """Session i's generate_argmax from (tokens[i], positions[i]) for every i, in one call
+    (l2b_generate_argmax_batch).  forced: (n, n_steps) tokens, -1 = free-running.  Returns one array
+    per session: the tokens of the steps it ran."""
+    n, hs, toks, pos = _batch_args(sessions, tokens, positions)
+    width = max(int(n_steps), 1)
+    out = np.full((max(n, 1), width), -1, dtype=np.int32)
+    done = np.zeros(max(n, 1), dtype=np.int32)
+    fp = None
+    if forced is not None:
+        forced = np.ascontiguousarray(forced, dtype=np.int32)
+        assert forced.shape == (n, n_steps), forced.shape
+        fp = forced.ctypes.data_as(IP)
+    _check(load_library().l2b_generate_argmax_batch(hs, n, toks.ctypes.data_as(IP), pos.ctypes.data_as(IP),
+                                                    int(n_steps), fp, 1 if stop_on_bos else 0,
+                                                    out.ctypes.data_as(IP), done.ctypes.data_as(IP)),
+           hs[0] if n else None)
+    return [out[i, :done[i]].copy() for i in range(n)]
 
 
 # ---- reference-named single ops on host buffers (device = cuda:0) ---------------------------

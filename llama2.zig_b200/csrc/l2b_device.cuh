@@ -288,6 +288,9 @@ struct GemvParams {
     int nb;
     int pos_b[PF_MAXB];
     float *kcache_b[PF_MAXB], *vcache_b[PF_MAXB];
+    // EPI_QKV of the batched kernels: vector b appends no KV row when skip_b[b] != 0 (a session that has
+    // stopped in the batched generation loop), or nullptr: every vector appends
+    const int *skip_b;
 };
 
 template <int EPI>
@@ -1189,7 +1192,10 @@ __global__ void __launch_bounds__(TMA_THREADS, 2) gemv_tma_kernel(const GemvPara
 // EPI_RESID: x batch [nb][total_rows]; EPI_STORE / EPI_ARGMAX (the classifier of the batched step):
 // logits batch [nb][total_rows], and for EPI_ARGMAX one packed argmax_key per vector in amax[b] (zeroed
 // before the launch).  The vectors need not be consecutive positions of one sequence: each carries
-// its own position and caches (pos_b, kcache_b, vcache_b).
+// its own position and caches (pos_b, kcache_b, vcache_b).  In the batched generation loop
+// (l2b_generate_argmax_batch) skip_b keeps a stopped session's vector from appending KV rows, and once
+// every session has stopped (CTL_DONE) the launches still queued return at once.  Prefill and the
+// batched step clear CTL_DONE before they launch.
 template <int EPI, int NB>
 __global__ void __launch_bounds__(TMA_THREADS, 1) prefill_gemm_kernel(const GemvParams p) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -1218,7 +1224,16 @@ __global__ void __launch_bounds__(TMA_THREADS, 1) prefill_gemm_kernel(const Gemv
     __syncthreads();
 
     if (warp == NWARP) {
+        // the ring is filled before the dependency wait (weights are immutable); the rest of the stream
+        // only while the batched generation loop is running (CTL_DONE, as in gemv_tma_kernel)
         RingProducer prod;
+        while (prod.it < total && prod.it < NSTAGE) prod.produce_one<EPI>(p, R, lane);
+        pdl_wait();
+        if (p.ctl[CTL_DONE]) {   // the loop has ended: drain the bulk copies already aimed at shared memory
+            if (lane == 0)
+                for (int s = 0; s < prod.it; ++s) mbar_wait(&full[s], 0);
+            return;
+        }
         while (prod.it < total) prod.produce_one<EPI>(p, R, lane);
         pdl_launch_dependents();
         return;
@@ -1228,6 +1243,7 @@ __global__ void __launch_bounds__(TMA_THREADS, 1) prefill_gemm_kernel(const Gemv
     float4 gv[TMA_MAXV];
     if (p.gamma) tma_fetch_gain(p, gv, ptid, n4);
     pdl_wait();
+    const bool done = p.ctl[CTL_DONE] != 0;                            // read while x is staged below
     if (tid == 0) {
         const uint32_t bytes = (uint32_t)p.n * 4u;
         mbar_expect_tx(&xbar, bytes * (uint32_t)p.nb);
@@ -1247,11 +1263,13 @@ __global__ void __launch_bounds__(TMA_THREADS, 1) prefill_gemm_kernel(const Gemv
             }
     }
     mbar_wait(&xbar, 0);
+    if (done) return;                                                  // the producer drains the ring
     tma_rmsnorm<NB>(p, xs, gv, scratch, p.nb, ptid, lane, n4);
 
     if (warp == NWARP + 1) {
         const int eb = lane >> 2, ep = lane & 3;
         const bool active = lane < 4 * NB && eb < p.nb;
+        const bool append = !(EPI == EPI_QKV && active && p.skip_b && p.skip_b[eb]);
         unsigned long long best = 0ull;                                // EPI_ARGMAX: this lane's rows of vector eb
         for (int t = 0; t < ntiles; ++t) {
             const int par = t & 1, use = t >> 1;
@@ -1263,8 +1281,9 @@ __global__ void __launch_bounds__(TMA_THREADS, 1) prefill_gemm_kernel(const Gemv
             const int vp = r0 + t * GEMV8_R + 2 * ep;
             if (!active || vp >= r1) continue;
             if (EPI == EPI_QKV) {
-                qkv_store_pair(p, p.out0 + (size_t)eb * p.rows0, p.kcache_b[eb], p.vcache_b[eb], p.pos_b[eb],
-                               rope_s[eb][0], rope_s[eb][1], vp, s.x, s.y);
+                if (append || vp < p.rows0)                            // q rows always; k / v rows are the KV append
+                    qkv_store_pair(p, p.out0 + (size_t)eb * p.rows0, p.kcache_b[eb], p.vcache_b[eb], p.pos_b[eb],
+                                   rope_s[eb][0], rope_s[eb][1], vp, s.x, s.y);
             } else if (EPI == EPI_STORE || EPI == EPI_ARGMAX) {   // logits[b][row] (:429), as gemv_epilogue_pair
                 float *dst = p.out0 + (size_t)eb * p.total_rows;
                 dst[vp] = s.x;
@@ -1934,6 +1953,42 @@ __global__ void advance_kernel(const AdvanceParams p) {
     ctl[CTL_TOKEN] = next;
     ctl[CTL_POS] = ctl[CTL_POS] + 1;
     ctl[CTL_STEP] = step + 1;
+}
+
+// End of step `step` of the batched on-device loop (l2b_generate_argmax_batch) for one group of nb
+// sessions: thread b is the group's vector b, session i = g0 + b.  The batched counterpart of
+// advance_kernel: next = forced or the vector's argmax key, recorded; the session stops on BOS or at
+// its step limit, else its next token goes to tokens[i], which the next step's qkv kernel embeds.  The
+// session arrays are indexed by i, the [n][stride] token arrays by (i, step).
+struct BatchAdvanceParams {
+    int *ctl;                   // sessions[0]'s control block: CTL_DONE is raised when no session runs
+    unsigned long long *amax;   // [PF_MAXB] packed argmax keys of the group's classifier
+    const int *forced;          // [n][stride], -1 = free-running, or nullptr
+    const int *limit;           // [n] steps session i may run
+    int *tokens, *done, *n_done, *out_next;   // [n] [n] [n] [n][stride]
+    int *live;                  // sessions still running
+    int g0, nb, step, stride, stop_on_bos;
+};
+__global__ void batch_advance_kernel(const BatchAdvanceParams p) {
+    pdl_wait();
+    const int b = threadIdx.x;
+    if (p.ctl[CTL_DONE] || b >= p.nb) return;
+    // the key slot is the next group's too: consume it whether or not this session still runs
+    const unsigned long long key = p.amax[b];
+    p.amax[b] = 0ull;
+    const int i = p.g0 + b;
+    if (p.done[i]) return;
+    const size_t at = (size_t)i * p.stride + p.step;
+    int next = (int)(0xFFFFFFFFu - (unsigned int)(key & 0xFFFFFFFFull));
+    if (p.forced && p.forced[at] >= 0) next = p.forced[at];
+    p.out_next[at] = next;
+    p.n_done[i] = p.step + 1;
+    if ((p.stop_on_bos && next == 1) || p.step + 1 == p.limit[i]) {   // :1017-1019, :992-993
+        p.done[i] = 1;
+        if (atomicSub(p.live, 1) == 1) p.ctl[CTL_DONE] = 1;
+        return;
+    }
+    p.tokens[i] = next;
 }
 
 // Tensor parallel logits: every rank's classifier sent its vocab slice as LL units (EPI_XCHG with

@@ -15,6 +15,7 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <algorithm>
 #include <chrono>
 #include <set>
 #include <string>
@@ -123,6 +124,8 @@ struct l2b_ctx {
     unsigned int *pf_counters = nullptr;
     int *pf_tokens = nullptr;
     bool pf_ready = false, pf_ok = false;
+    int *gb_ints = nullptr;                  // l2b_generate_argmax_batch on the batched path: its per-call
+    size_t gb_cap = 0;                       // session and token arrays (ints), grown on demand
     int attn_R = 1;                          // CTAs per head cluster of attn_wo_kernel
     float *delta = nullptr;                  // L2B_TP=nccl baseline only: partial rows before the NCCL all-reduce
     float *q = nullptr, *xb = nullptr, *hb = nullptr, *logits = nullptr, *logits_loc = nullptr;
@@ -1007,7 +1010,8 @@ int preload_kernels(l2b_ctx *ctx) {
     size_t smem = 0;
     L2B_CUDA(ctx, cudaFuncGetAttributes(&fa, (const void *)pick_attention(ctx->head_size, true, &smem)));
     if (pick_attn_wo(ctx->head_size, &smem)) L2B_CUDA(ctx, cudaFuncGetAttributes(&fa, (const void *)pick_attn_wo(ctx->head_size, &smem)));
-    const void *others[] = {(const void *)attention_kernel, (const void *)advance_kernel, (const void *)gather_logits_kernel,
+    const void *others[] = {(const void *)attention_kernel, (const void *)advance_kernel,
+                            (const void *)batch_advance_kernel, (const void *)gather_logits_kernel,
                             (const void *)resid_add_kernel, (const void *)sample_prep_kernel, (const void *)synth_fill_kernel};
     for (const void *f : others) L2B_CUDA(ctx, cudaFuncGetAttributes(&fa, f));
     return L2B_OK;
@@ -1751,8 +1755,10 @@ static int pf_launch(l2b_ctx *ctx, int epi, GemvParams p, cudaStream_t st) {
 // nb <= PF_MAXB vectors through every layer in one pass over the weights, on ctx's stream and batch
 // buffers: vector b enters as the embedding row of d_tokens[b] and runs at position pos[b] on the KV
 // cache of kv[b] (a prompt: one context at consecutive positions; the batched step: one session per
-// vector).  Its x is left in ctx->pf_x[b].
-static int batched_layers(l2b_ctx *ctx, l2b_ctx *const *kv, const int *pos, int nb, const int *d_tokens) {
+// vector).  Its x is left in ctx->pf_x[b].  d_skip (device, or nullptr): vector b appends no KV row
+// when d_skip[b] is set (a stopped session of the batched generation loop).
+static int batched_layers(l2b_ctx *ctx, l2b_ctx *const *kv, const int *pos, int nb, const int *d_tokens,
+                          const int *d_skip) {
     const int dim = ctx->dim;
     cudaStream_t st = ctx->stream;
     for (int l = 0; l < ctx->cfg.n_layers; ++l) {
@@ -1768,6 +1774,7 @@ static int batched_layers(l2b_ctx *ctx, l2b_ctx *const *kv, const int *pos, int 
         }
         // ---- rmsnorm + q,k,v + RoPE + KV append for nb vectors (:305-358)
         g.qkv.nb = nb;
+        g.qkv.skip_b = d_skip;
         g.qkv.x_in = ctx->pf_x;
         if (l == 0) { g.qkv.emb = ctx->emb; g.qkv.tokens = d_tokens; g.qkv.x_out = ctx->pf_x; }
         g.qkv.out0 = ctx->pf_q;
@@ -1817,7 +1824,7 @@ static int prefill_batched(l2b_ctx *ctx, const int32_t *tokens, int n_tokens, in
         l2b_ctx *kv[PF_MAXB];
         int pos[PF_MAXB];
         for (int b = 0; b < nb; ++b) { kv[b] = ctx; pos[b] = pos0 + done + b; }
-        int rc = batched_layers(ctx, kv, pos, nb, ctx->pf_tokens + done);
+        int rc = batched_layers(ctx, kv, pos, nb, ctx->pf_tokens + done, nullptr);
         if (rc) return rc;
     }
     L2B_CUDA(ctx, cudaEventRecord(ctx->ev1, st));
@@ -1826,6 +1833,22 @@ static int prefill_batched(l2b_ctx *ctx, const int32_t *tokens, int n_tokens, in
     L2B_CUDA(ctx, cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
     if (pos0 + n_tokens > ctx->n_appended) ctx->n_appended = pos0 + n_tokens;
     return L2B_OK;
+}
+
+// final rmsnorm + classifier (:426-429) of the nb vectors in ctx->pf_x: logits to pf_logits, and with
+// argmax one packed key per vector added into pf_amax (zero before the launch)
+static int batched_classifier(l2b_ctx *ctx, int nb, bool argmax) {
+    GemvParams k{};
+    k.ctl = ctx->ctl;
+    k.n = ctx->dim;
+    k.nb = nb;
+    k.x_in = ctx->pf_x;
+    k.gamma = ctx->rms_final;
+    k.w0 = ctx->wcls;
+    k.total_rows = ctx->cfg.vocab_size; k.rows0 = ctx->cfg.vocab_size;
+    k.out0 = ctx->pf_logits;
+    k.amax = ctx->pf_amax;
+    return pf_launch<PF_MAXB>(ctx, argmax ? EPI_ARGMAX : EPI_STORE, k, ctx->stream);
 }
 
 // Everything a batched step checks, before anything is launched: a refused call changes no session.
@@ -1881,21 +1904,10 @@ static int step_sessions(l2b_ctx *const *s, int n, const int32_t *tokens, const 
         const int nb = n - g < PF_MAXB ? n - g : PF_MAXB;
         // from the caller's (pageable) array: staged before the call returns, ordered after the previous group
         L2B_CUDA(ctx, cudaMemcpyAsync(ctx->pf_tokens, tokens + g, (size_t)nb * sizeof(int), cudaMemcpyHostToDevice, st));
-        rc = batched_layers(ctx, s + g, pos + g, nb, ctx->pf_tokens);
+        rc = batched_layers(ctx, s + g, pos + g, nb, ctx->pf_tokens, nullptr);
         if (rc) return rc;
-        // ---- final rmsnorm + classifier (:426-429) of the nb vectors
-        GemvParams k{};
-        k.ctl = ctx->ctl;
-        k.n = dim;
-        k.nb = nb;
-        k.x_in = ctx->pf_x;
-        k.gamma = ctx->rms_final;
-        k.w0 = ctx->wcls;
-        k.total_rows = V; k.rows0 = V;
-        k.out0 = ctx->pf_logits;
-        k.amax = ctx->pf_amax;
         if (argmax) L2B_CUDA(ctx, cudaMemsetAsync(ctx->pf_amax, 0, PF_MAXB * sizeof(unsigned long long), st));
-        rc = pf_launch<PF_MAXB>(ctx, argmax ? EPI_ARGMAX : EPI_STORE, k, st);
+        rc = batched_classifier(ctx, nb, argmax);
         if (rc) return rc;
         for (int b = 0; b < nb; ++b) {
             l2b_ctx *c = s[g + b];
@@ -1922,57 +1934,118 @@ static int step_sessions(l2b_ctx *const *s, int n, const int32_t *tokens, const 
 
 extern "C" {
 
-// n_steps replays of a device-loop graph (G_ARGMAX_LOOP or G_PREFILL_LOOP) starting at (token, pos)
-static int run_device_loop(l2b_ctx *ctx, int which, int token, int pos, int n_steps, const int32_t *forced,
-                           int stop_on_bos, int *done_out) {
-    std::vector<l2b_ctx *> ranks = locals(ctx);
-    int launches = 0, rc;
-    for (l2b_ctx *c : ranks) {
+// One on-device loop of one context: n_steps replays of a device-loop graph (G_ARGMAX_LOOP or
+// G_PREFILL_LOOP) starting at (token, pos).  The loops of one call are the ranks of an in-process group
+// (all but the lead are not sinks: their tokens are the lead's) or several sessions (all sinks).
+struct DeviceLoop {
+    l2b_ctx *c;
+    int token, pos, n_steps;
+    const int32_t *forced;   // n_steps entries, -1 = free-running, or nullptr
+    bool sink;               // its tokens, n_done and appended count are read back
+    int launches = 0, done = 0;
+};
+
+// The enqueue half: every loop's inputs, then its replays, then the copies of its results; nothing is
+// synchronised.  Timing events go on the lead's stream (loops[0]); loops on other streams of the lead's
+// device are bracketed by them too.
+static int enqueue_device_loops(std::vector<DeviceLoop> &loops, int which, int stop_on_bos) {
+    l2b_ctx *ctx = loops[0].c;
+    int rc;
+    for (DeviceLoop &d : loops) {
+        l2b_ctx *c = d.c;
         L2B_CUDA(ctx, cudaSetDevice(c->device));
         // forced tokens (prompt forcing, :999-1000); -1 = free-running
-        for (int i = 0; i < n_steps; ++i) c->h_gen[i] = forced ? forced[i] : -1;
-        L2B_CUDA(ctx, cudaMemcpyAsync(c->gen_forced, c->h_gen, (size_t)n_steps * sizeof(int),
+        for (int i = 0; i < d.n_steps; ++i) c->h_gen[i] = d.forced ? d.forced[i] : -1;
+        L2B_CUDA(ctx, cudaMemcpyAsync(c->gen_forced, c->h_gen, (size_t)d.n_steps * sizeof(int),
                                       cudaMemcpyHostToDevice, c->stream));
         L2B_CUDA(ctx, cudaMemsetAsync(c->gen_ndone, 0, sizeof(int), c->stream));
         L2B_CUDA(ctx, cudaMemsetAsync(c->amax, 0, sizeof(unsigned long long), c->stream));
-        fill_ctl(c, token, pos, stop_on_bos ? 1 : 0, 1.0f, -1.0f);
+        fill_ctl(c, d.token, d.pos, stop_on_bos ? 1 : 0, 1.0f, -1.0f);
         if (c == ctx) L2B_CUDA(ctx, cudaEventRecord(c->ev0, c->stream));
         L2B_CUDA(ctx, cudaMemcpyAsync(c->ctl, c->h_ctl, CTL_HOST_WORDS * sizeof(int), cudaMemcpyHostToDevice, c->stream));
     }
+    for (DeviceLoop &d : loops)
+        if (d.c->device == ctx->device && d.c->stream != ctx->stream)
+            L2B_CUDA(ctx, cudaStreamWaitEvent(d.c->stream, ctx->ev0, 0));
     // the whole step depends on (token,pos) only through ctl, which advance_kernel updates, so the
-    // same graph is replayed back to back with no host round trip; with several local ranks the
-    // launches are interleaved so that no rank's queue runs dry while another's is being filled
-    for (int i = 0; i < n_steps; ++i) {
-        for (l2b_ctx *c : ranks) {
-            if (ranks.size() > 1) L2B_CUDA(ctx, cudaSetDevice(c->device));
+    // same graph is replayed back to back with no host round trip; with several loops the launches
+    // are interleaved so that no stream's queue runs dry while another's is being filled
+    int n_max = 0;
+    for (const DeviceLoop &d : loops) n_max = d.n_steps > n_max ? d.n_steps : n_max;
+    for (int i = 0; i < n_max; ++i) {
+        for (DeviceLoop &d : loops) {
+            l2b_ctx *c = d.c;
+            if (i >= d.n_steps) continue;
+            if (loops.size() > 1) L2B_CUDA(ctx, cudaSetDevice(c->device));
             if (c->use_graphs) {
                 L2B_CUDA(ctx, cudaGraphLaunch(c->graphs[which], c->stream));
-                if (c == ctx) launches += c->launches_per_step + (which == G_PREFILL_LOOP ? 0 : 1);
+                d.launches += c->launches_per_step + (which == G_PREFILL_LOOP ? 0 : 1);
             } else {
                 c->last_launches = 0;
                 rc = enqueue_call(c, c->stream, which);
                 if (rc) { ctx->err = c->err; return rc; }
-                if (c == ctx) launches += c->last_launches;
+                d.launches += c->last_launches;
             }
         }
     }
-    for (l2b_ctx *c : ranks) {
+    // the lead last: its end event follows every other stream of its device
+    for (size_t k = loops.size(); k-- > 0;) {
+        l2b_ctx *c = loops[k].c;
         L2B_CUDA(ctx, cudaSetDevice(c->device));
-        if (c == ctx) {
-            L2B_CUDA(ctx, cudaMemcpyAsync(c->h_gen, c->gen_out, (size_t)n_steps * sizeof(int),
+        if (loops[k].sink) {
+            L2B_CUDA(ctx, cudaMemcpyAsync(c->h_gen, c->gen_out, (size_t)loops[k].n_steps * sizeof(int),
                                           cudaMemcpyDeviceToHost, c->stream));
             L2B_CUDA(ctx, cudaMemcpyAsync(c->h_ints + 1, c->gen_ndone, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
         }
         L2B_CUDA(ctx, cudaMemcpyAsync(c->h_ctl + CTL_WORDS, c->ctl, CTL_WORDS * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-        if (c == ctx) L2B_CUDA(ctx, cudaEventRecord(c->ev1, c->stream));
+        if (c == ctx) {
+            L2B_CUDA(ctx, cudaEventRecord(c->ev1, c->stream));
+        } else if (c->device == ctx->device && c->stream != ctx->stream) {
+            L2B_CUDA(ctx, cudaEventRecord(c->ev1, c->stream));
+            L2B_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, c->ev1, 0));
+        }
     }
-    rc = finish_call(ctx, ranks);
+    return L2B_OK;
+}
+
+// The finish half: one synchronise of every loop's stream, then each sink's steps done (its tokens in
+// h_gen) and appended count; the call's device time on the lead.
+static int finish_device_loops(std::vector<DeviceLoop> &loops) {
+    l2b_ctx *ctx = loops[0].c;
+    std::vector<l2b_ctx *> cs;
+    for (const DeviceLoop &d : loops) cs.push_back(d.c);
+    int rc = finish_call(ctx, cs);
     if (rc) return rc;
     L2B_CUDA(ctx, cudaSetDevice(ctx->device));
     L2B_CUDA(ctx, cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
-    *done_out = ctx->h_ints[1];
-    ctx->last_launches = launches;
-    if (pos + *done_out > ctx->n_appended) ctx->n_appended = pos + *done_out;
+    for (DeviceLoop &d : loops) {
+        if (!d.sink) continue;
+        d.done = d.c->h_ints[1];
+        if (d.pos + d.done > d.c->n_appended) d.c->n_appended = d.pos + d.done;
+    }
+    return L2B_OK;
+}
+
+// n_steps replays of a device-loop graph (G_ARGMAX_LOOP or G_PREFILL_LOOP) on every rank of ctx
+static int run_device_loop(l2b_ctx *ctx, int which, int token, int pos, int n_steps, const int32_t *forced,
+                           int stop_on_bos, int *done_out) {
+    std::vector<DeviceLoop> loops;
+    for (l2b_ctx *c : locals(ctx)) loops.push_back(DeviceLoop{c, token, pos, n_steps, forced, c == ctx});
+    int rc = enqueue_device_loops(loops, which, stop_on_bos);
+    if (rc) return rc;
+    rc = finish_device_loops(loops);
+    if (rc) return rc;
+    *done_out = loops[0].done;
+    ctx->last_launches = loops[0].launches;
+    return L2B_OK;
+}
+
+// forced tokens a generate call reads: -1 (free-running) or a token of the vocabulary, which the next
+// step embeds; anything else is refused before anything runs
+static int check_forced(l2b_ctx *ctx, const int32_t *forced, int count) {
+    if (!forced) return L2B_OK;
+    for (int i = 0; i < count; ++i)
+        if (forced[i] < -1 || forced[i] >= ctx->cfg.vocab_size) return fail(ctx, L2B_ERR_INVALID_ARG, "forced token out of range");
     return L2B_OK;
 }
 
@@ -1983,6 +2056,8 @@ int32_t l2b_generate_argmax(l2b_ctx *ctx, int32_t token, int32_t pos, int32_t n_
     if (rc) return rc;
     if (!out_next || !n_done || n_steps < 0) return fail(ctx, L2B_ERR_INVALID_ARG, "bad generate arguments");
     if (n_steps > ctx->cfg.seq_len - pos) n_steps = ctx->cfg.seq_len - pos;   // :992-993
+    rc = check_forced(ctx, forced, n_steps);
+    if (rc) return rc;
     *n_done = 0;
     if (n_steps == 0) return L2B_OK;
     int done = 0;
@@ -2049,6 +2124,137 @@ int32_t l2b_forward_argmax_batch(l2b_ctx *const *sessions, int32_t n, const int3
     if (rc) return rc;
     for (int i = 0; i < n; ++i) next[i] = sessions[i]->h_ints[0];
     return L2B_OK;
+}
+
+// l2b_generate_argmax_batch where the batched step runs (pf_ok on s[0]): every step of every group of
+// PF_MAXB sessions is enqueued up front on s[0]'s stream, with no host synchronise until the end.  The
+// positions are launch arguments (pos[i] + step, held at seq_len - 1 once session i is past its limit);
+// the tokens stay on the device: batch_advance_kernel writes each session's next token into the call's
+// token array, which the next step's qkv kernel embeds.  A stopped session's vector still flows through
+// its group, appends no KV row (the done flags are qkv's skip mask) and its outputs are ignored; once
+// every session has stopped (CTL_DONE on s[0]) the launches still queued return at once.
+static int generate_batched(l2b_ctx *const *s, int n, const int32_t *tokens, const int32_t *pos, int n_steps,
+                            const int32_t *forced, const int *limit, int stop_on_bos, int32_t *out_next,
+                            int32_t *n_done) {
+    l2b_ctx *ctx = s[0];
+    const int S = ctx->cfg.seq_len;
+    int stride = 0;                          // steps of the longest-running session
+    for (int i = 0; i < n; ++i) stride = limit[i] > stride ? limit[i] : stride;
+    // the call's device ints: tokens, done flags, n_done, limits [n] each, the live count, then forced
+    // and out_next [n][stride]
+    const size_t o_tok = 0, o_done = (size_t)n, o_ndone = 2 * (size_t)n, o_lim = 3 * (size_t)n, o_live = 4 * (size_t)n;
+    const size_t o_forced = o_live + 1, o_out = o_forced + (size_t)n * stride, total = o_out + (size_t)n * stride;
+    L2B_CUDA(ctx, cudaSetDevice(ctx->device));
+    if (ctx->gb_cap < total) {
+        if (ctx->gb_ints) {
+            L2B_CUDA(ctx, cudaFree(ctx->gb_ints));
+            ctx->owned.erase(std::find(ctx->owned.begin(), ctx->owned.end(), (void *)ctx->gb_ints));
+            ctx->gb_ints = nullptr;
+            ctx->gb_cap = 0;
+        }
+        const int rc = dev_alloc(ctx, &ctx->gb_ints, total);
+        if (rc) { cudaGetLastError(); return rc; }
+        ctx->gb_cap = total;
+    }
+    std::vector<int> h(o_out, -1);
+    for (int i = 0; i < n; ++i) {
+        h[o_tok + i] = tokens[i];
+        h[o_done + i] = 0;
+        h[o_ndone + i] = 0;
+        h[o_lim + i] = limit[i];
+        if (forced)
+            for (int k = 0; k < limit[i]; ++k) h[o_forced + (size_t)i * stride + k] = forced[(size_t)i * n_steps + k];
+    }
+    h[o_live] = n;
+    int *d = ctx->gb_ints;
+    cudaStream_t st = ctx->stream;
+    L2B_CUDA(ctx, cudaMemcpyAsync(d, h.data(), o_out * sizeof(int), cudaMemcpyHostToDevice, st));
+    L2B_CUDA(ctx, cudaMemsetAsync(ctx->pf_amax, 0, PF_MAXB * sizeof(unsigned long long), st));
+    fill_ctl(ctx, tokens[0], pos[0], 0, 1.0f, -1.0f);        // DONE = 0 until the last session stops
+    L2B_CUDA(ctx, cudaMemcpyAsync(ctx->ctl, ctx->h_ctl, CTL_HOST_WORDS * sizeof(int), cudaMemcpyHostToDevice, st));
+    L2B_CUDA(ctx, cudaEventRecord(ctx->ev0, st));
+    ctx->last_launches = 0;
+    BatchAdvanceParams a{};
+    a.ctl = ctx->ctl;
+    a.amax = ctx->pf_amax;
+    a.forced = forced ? d + o_forced : nullptr;
+    a.limit = d + o_lim;
+    a.tokens = d + o_tok; a.done = d + o_done; a.n_done = d + o_ndone; a.out_next = d + o_out;
+    a.live = d + o_live;
+    a.stride = stride;
+    a.stop_on_bos = stop_on_bos ? 1 : 0;
+    for (int step = 0; step < stride; ++step) {
+        for (int g = 0; g < n; g += PF_MAXB) {
+            const int nb = n - g < PF_MAXB ? n - g : PF_MAXB;
+            int p[PF_MAXB];
+            for (int b = 0; b < nb; ++b) p[b] = pos[g + b] + step < S ? pos[g + b] + step : S - 1;
+            int rc = batched_layers(ctx, s + g, p, nb, d + o_tok + g, d + o_done + g);
+            if (rc) return rc;
+            rc = batched_classifier(ctx, nb, true);
+            if (rc) return rc;
+            a.g0 = g; a.nb = nb; a.step = step;
+            void *args[] = {&a};
+            rc = launch_small(ctx, (const void *)batch_advance_kernel, dim3(1), dim3(PF_MAXB), args, st, true);
+            if (rc) return rc;
+        }
+    }
+    std::vector<int> back((size_t)n * stride + n);
+    L2B_CUDA(ctx, cudaMemcpyAsync(back.data(), d + o_ndone, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost, st));
+    L2B_CUDA(ctx, cudaMemcpyAsync(back.data() + n, d + o_out, (size_t)n * stride * sizeof(int), cudaMemcpyDeviceToHost, st));
+    L2B_CUDA(ctx, cudaEventRecord(ctx->ev1, st));
+    L2B_CUDA(ctx, cudaStreamSynchronize(st));
+    L2B_CUDA(ctx, cudaGetLastError());
+    L2B_CUDA(ctx, cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
+    for (int i = 0; i < n; ++i) {
+        n_done[i] = back[i];
+        for (int k = 0; k < n_done[i]; ++k) out_next[(size_t)i * n_steps + k] = back[n + (size_t)i * stride + k];
+        if (pos[i] + n_done[i] > s[i]->n_appended) s[i]->n_appended = pos[i] + n_done[i];
+    }
+    return L2B_OK;
+}
+
+// l2b_generate_argmax_batch elsewhere: each session's own device loop (l2b_generate_argmax's graph
+// replays) on its own stream, the sessions' replays interleaved step by step, one synchronise for all
+static int generate_each(l2b_ctx *const *s, int n, const int32_t *tokens, const int32_t *pos, int n_steps,
+                         const int32_t *forced, const int *limit, int stop_on_bos, int32_t *out_next,
+                         int32_t *n_done) {
+    std::vector<DeviceLoop> loops;
+    for (int i = 0; i < n; ++i)
+        loops.push_back(DeviceLoop{s[i], tokens[i], pos[i], limit[i], forced ? forced + (size_t)i * n_steps : nullptr, true});
+    int rc = enqueue_device_loops(loops, G_ARGMAX_LOOP, stop_on_bos);
+    if (rc) return rc;
+    rc = finish_device_loops(loops);
+    if (rc) return rc;
+    int launches = 0;
+    for (int i = 0; i < n; ++i) {
+        launches += loops[i].launches;
+        n_done[i] = loops[i].done;
+        for (int k = 0; k < n_done[i]; ++k) out_next[(size_t)i * n_steps + k] = s[i]->h_gen[k];
+    }
+    s[0]->last_launches = launches;
+    return L2B_OK;
+}
+
+int32_t l2b_generate_argmax_batch(l2b_ctx *const *sessions, int32_t n, const int32_t *tokens, const int32_t *pos,
+                                  int32_t n_steps, const int32_t *forced, int32_t stop_on_bos, int32_t *out_next,
+                                  int32_t *n_done) {
+    int rc = check_batch_args(sessions, n, tokens, pos);
+    if (rc) return rc;
+    l2b_ctx *s0 = sessions[0];
+    if (!out_next || !n_done || n_steps < 0) return fail(s0, L2B_ERR_INVALID_ARG, "bad generate arguments");
+    std::vector<int> limit(n);
+    for (int i = 0; i < n; ++i) {
+        const int left = s0->cfg.seq_len - pos[i];
+        limit[i] = n_steps < left ? n_steps : left;                   // :992-993, per session
+        rc = check_forced(s0, forced ? forced + (size_t)i * n_steps : nullptr, limit[i]);
+        if (rc) return rc;
+    }
+    for (int i = 0; i < n; ++i) n_done[i] = 0;
+    if (n_steps == 0) return L2B_OK;
+    rc = pf_prepare(s0);
+    if (rc) return rc;
+    if (s0->pf_ok) return generate_batched(sessions, n, tokens, pos, n_steps, forced, limit.data(), stop_on_bos, out_next, n_done);
+    return generate_each(sessions, n, tokens, pos, n_steps, forced, limit.data(), stop_on_bos, out_next, n_done);
 }
 
 int32_t l2b_read_state(l2b_ctx *ctx, int32_t which, float *dst, uint64_t n, uint64_t *n_out) {

@@ -1,15 +1,18 @@
 #!/usr/bin/env python
-"""Aggregate decode rate of n sessions on one llama2-7B model (l2b_create_session + l2b_forward_argmax_batch).
+"""Aggregate decode rate of n sessions on one llama2-7B model (l2b_create_session + l2b_forward_argmax_batch /
+l2b_generate_argmax_batch).
 
   python scripts/bench_sessions.py [--sessions 1,2,4,8] [--positions 256] [--warmup 4] [--repeats 2]
 
 One model with synthetic fp32 weights (seed 7, as bench.py) and n-1 sessions on it.  Session b is
 prefilled to 61*b positions (staggered, so the sessions' attention lengths differ), warmed up for
 --warmup batched steps, and then teacher-forced over --positions positions through
-l2b_forward_argmax_batch, one call per position.  The L2 cache is flushed (256 MiB memset) before
+l2b_forward_argmax_batch, one call per position ("batched step"), and in the same repeat through one
+l2b_generate_argmax_batch call over the same positions with the teacher tokens forced ("device loop":
+no host round trip per position).  The two alternate within each repeat.  The L2 cache is flushed (256 MiB memset) before
 each timed run.  Per call the library brackets its work with CUDA events (l2b_last_timing); the device
 time of a run is their sum, and a host clock around the run (every call ends in a synchronise) gives
-the wall time.  The single-stream reference is the on-device loop of one context
+the wall time (the device loop is one call).  The single-stream reference is the on-device loop of one context
 (l2b_generate_argmax, bench.py's headline), timed the same way.  One JSON line per measurement; the
 card's name and power limit (read-only nvidia-smi query) are printed in the same run.
 """
@@ -66,7 +69,7 @@ def main():
     P, W = args.positions, args.warmup
     starts = [61 * b for b in range(max(counts))]
     assert starts[-1] + W + P <= ck.seq_len
-    toks = [teacher(b, starts[b] + W + P, V) for b in range(len(sess))]
+    toks = [teacher(b, starts[b] + W + P + 1, V) for b in range(len(sess))]
 
     # single stream: the on-device loop of one context over the same number of positions
     for r in range(args.repeats + 1):
@@ -82,7 +85,8 @@ def main():
 
     for n in counts:
         group = sess[:n]
-        for r in range(args.repeats + 1):                       # the first run warms every shape up
+        def prepare(group):
+            """Every session prefilled to its start and stepped --warmup positions."""
             for b, s in enumerate(group):
                 s.reset()
                 if starts[b]:
@@ -90,6 +94,9 @@ def main():
             for i in range(W):
                 pos = [starts[b] + i for b in range(n)]
                 l2b.forward_argmax_batch(group, [toks[b][p] for b, p in enumerate(pos)], pos)
+
+        for r in range(args.repeats + 1):                       # the first run warms every shape up
+            prepare(group)
             flush()
             dev_ms, launches = 0.0, 0
             t0 = time.perf_counter()
@@ -104,6 +111,22 @@ def main():
                                   "launches_per_step": launches,
                                   "ms_per_step": round(dev_ms / P, 3),
                                   "tok_s": round(n * P / (dev_ms / 1e3), 2),
+                                  "wall_tok_s": round(n * P / wall, 2)}), flush=True)
+            # the same positions through the device loop, from the same state
+            prepare(group)
+            first = [toks[b][starts[b] + W] for b in range(n)]
+            forced = [toks[b][starts[b] + W + 1:starts[b] + W + P + 1] for b in range(n)]
+            flush()
+            t0 = time.perf_counter()
+            l2b.generate_argmax_batch(group, first, [starts[b] + W for b in range(n)], P, forced=forced,
+                                      stop_on_bos=False)
+            wall = time.perf_counter() - t0
+            ms, launches = group[0].last_timing()
+            if r:
+                print(json.dumps({"what": "device loop", "sessions": n, "positions": P,
+                                  "launches_per_step": launches // P,
+                                  "ms_per_step": round(ms / P, 3),
+                                  "tok_s": round(n * P / (ms / 1e3), 2),
                                   "wall_tok_s": round(n * P / wall, 2)}), flush=True)
     for s in sess[1:]:
         s.close()
