@@ -211,6 +211,23 @@ int32_t l2b_forward_batch(l2b_ctx *const *sessions, int32_t n, const int32_t *to
 /* Same step with the device argmax (first maximum wins, :715-726): next[i] for session i.      */
 int32_t l2b_forward_argmax_batch(l2b_ctx *const *sessions, int32_t n, const int32_t *tokens,
                                  const int32_t *pos, int32_t *next);
+/* Same step with l2b_forward_sample's device sampler preparation.  For each i it does what
+ * l2b_forward_sample(sessions[i], tokens[i], pos[i], temperature[i], top_p[i], host_probs[i],
+ * cand + i*cand_cap, cand_cap, &n_cand[i]) does: temperature and top-p are per session, cand is
+ * row-major n x cand_cap, and n_cand[i] follows the single call's rule (the count, 0 when session i
+ * does not filter, minus the number that passed when more than min(cand_cap, 8192) did).
+ * host_probs, or any entry of it, may be NULL (those probabilities are not copied out); cand and
+ * n_cand may be NULL only when no session filters (top_p 0 or 1).  Where the sessions share weight
+ * passes, the sampler runs on the batched logits, so the probabilities match l2b_forward_sample to
+ * float rounding; elsewhere each session runs l2b_forward_sample's own step (bit for bit).  Checked
+ * before anything runs, as l2b_forward_batch, plus NULL temperature or top_p, a temperature not > 0,
+ * a top_p outside [0, 1], a vocabulary of fewer than 2 entries, and a filtering session without a
+ * candidate buffer or with cand_cap <= 0 => L2B_ERR_INVALID_ARG.  Afterwards l2b_read_state(..,
+ * logits) of each session returns its probabilities; xb, hb and q are not defined.  Synchronous. */
+int32_t l2b_forward_sample_batch(l2b_ctx *const *sessions, int32_t n, const int32_t *tokens,
+                                 const int32_t *pos, const float *temperature, const float *top_p,
+                                 float *const *host_probs, l2b_prob_index *cand, int32_t cand_cap,
+                                 int32_t *n_cand);
 /* The greedy loop of l2b_generate_argmax on n sessions in one call, with no host round trip per
  * step.  For each i it does what l2b_generate_argmax(sessions[i], tokens[i], pos[i], n_steps,
  * forced + i*n_steps, stop_on_bos, out_next + i*n_steps, &n_done[i]) does: forced (may be NULL)

@@ -83,6 +83,8 @@ def load_library():
     lib.l2b_create_session.argtypes = [C.POINTER(vp), vp]
     lib.l2b_forward_batch.argtypes = [C.POINTER(vp), C.c_int32, IP, IP, C.POINTER(FP)]
     lib.l2b_forward_argmax_batch.argtypes = [C.POINTER(vp), C.c_int32, IP, IP, IP]
+    lib.l2b_forward_sample_batch.argtypes = [C.POINTER(vp), C.c_int32, IP, IP, FP, FP, C.POINTER(FP),
+                                             C.POINTER(L2BProbIndex), C.c_int32, IP]
     lib.l2b_generate_argmax_batch.argtypes = [C.POINTER(vp), C.c_int32, IP, IP, C.c_int32, IP, C.c_int32, IP, IP]
     lib.l2b_destroy.argtypes = [vp]
     lib.l2b_destroy.restype = None
@@ -375,6 +377,27 @@ def forward_argmax_batch(sessions, tokens, positions):
     _check(load_library().l2b_forward_argmax_batch(hs, n, toks.ctypes.data_as(IP), pos.ctypes.data_as(IP),
                                                    nxt.ctypes.data_as(IP)), hs[0] if n else None)
     return nxt[:n].copy()
+
+
+def forward_sample_batch(sessions, tokens, positions, temperature, top_p, cand_cap=8192):
+    """Session i's forward_sample(tokens[i], positions[i], temperature[i], top_p[i]) for every i, in one
+    call (l2b_forward_sample_batch).  Returns (probs (n, vocab), candidates, n_cand): candidates[i] is
+    session i's (prob, index) structured array in index order, or None when n_cand[i] <= 0 (0: top_p
+    is 0 or 1; minus the number that passed when more than cand_cap did)."""
+    n, hs, toks, pos = _batch_args(sessions, tokens, positions)
+    temp = np.ascontiguousarray(temperature, dtype=np.float32)
+    tp = np.ascontiguousarray(top_p, dtype=np.float32)
+    assert temp.size == n and tp.size == n
+    probs = np.empty((n, sessions[0].ck.vocab_size if n else 0), dtype=np.float32)
+    rows = (FP * max(n, 1))(*[probs[i].ctypes.data_as(FP) for i in range(n)])
+    cand = (L2BProbIndex * (max(n, 1) * max(cand_cap, 1)))()
+    n_cand = np.zeros(max(n, 1), dtype=np.int32)
+    _check(load_library().l2b_forward_sample_batch(hs, n, toks.ctypes.data_as(IP), pos.ctypes.data_as(IP),
+                                                   temp.ctypes.data_as(FP), tp.ctypes.data_as(FP), rows, cand,
+                                                   cand_cap, n_cand.ctypes.data_as(IP)), hs[0] if n else None)
+    flat = np.frombuffer(cand, dtype=[("prob", "<f4"), ("index", "<i4")])
+    cands = [flat[i * cand_cap:i * cand_cap + n_cand[i]].copy() if n_cand[i] > 0 else None for i in range(n)]
+    return probs, cands, n_cand[:n].copy()
 
 
 def generate_argmax_batch(sessions, tokens, positions, n_steps, forced=None, stop_on_bos=True):

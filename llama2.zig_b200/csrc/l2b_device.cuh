@@ -2023,19 +2023,19 @@ __global__ void __launch_bounds__(NT) resid_add_kernel(float *x, const float *de
 //   logits /= temperature (:1006); softmax in place (:1008, :687-706: max, exp, sum, divide);
 //   top-p prefilter (:761-768): candidates with prob >= (1-p)/(n-1), compacted IN INDEX ORDER.
 // The random draw, the sort of the (few) candidates and the CDF walk stay on the host because they
-// use the host's PRNG (:730, :788).  temperature / top-p come from ctl[CTL_TEMP] / ctl[CTL_TOPP].
+// use the host's PRNG (:730, :788).  top_p < 0: no candidate filter (*n_cand = -1).  One body,
+// sample_prep_row, serves both kernels: sample_prep_kernel (the single step's graph: temperature /
+// top-p from ctl[CTL_TEMP] / ctl[CTL_TOPP], written before each replay) and sample_prep_batch_kernel
+// (one CTA per vector of a batched step), so a batched row holds exactly what the single kernel
+// computes on the same logits.
 // ---------------------------------------------------------------------------------------
 constexpr int SAMP_THREADS = 1024;
 struct ProbIndex { float prob; int index; };
-__global__ void __launch_bounds__(SAMP_THREADS) sample_prep_kernel(float *logits, int n, const int *ctl,
-                                                                   ProbIndex *cand, int cand_cap, int *n_cand) {
-    pdl_wait();
-    if (ctl[CTL_DONE]) return;
+__device__ __forceinline__ void sample_prep_row(float *logits, int n, float temp, float top_p, ProbIndex *cand,
+                                                int cand_cap, int *n_cand) {
     __shared__ float red[SAMP_THREADS / 32 + 1];
     __shared__ int wsum[SAMP_THREADS / 32 + 1];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const float temp = __int_as_float(ctl[CTL_TEMP]);
-    const float top_p = __int_as_float(ctl[CTL_TOPP]);
     // pass 1: scaled logits and their maximum
     float m = -INFINITY;
     for (int i = tid; i < n; i += SAMP_THREADS) {
@@ -2102,6 +2102,32 @@ __global__ void __launch_bounds__(SAMP_THREADS) sample_prep_kernel(float *logits
             ++off;
         }
     }
+}
+__global__ void __launch_bounds__(SAMP_THREADS) sample_prep_kernel(float *logits, int n, const int *ctl,
+                                                                   ProbIndex *cand, int cand_cap, int *n_cand) {
+    pdl_wait();
+    if (ctl[CTL_DONE]) return;
+    sample_prep_row(logits, n, __int_as_float(ctl[CTL_TEMP]), __int_as_float(ctl[CTL_TOPP]), cand, cand_cap, n_cand);
+}
+
+// Sampler preparation of a batched step (l2b_forward_sample_batch): CTA b runs sample_prep_row in place
+// on vector b's logits row of the group, with its session's temperature and top-p, into that session's
+// own candidate buffer and count.
+struct SamplePrepBatchParams {
+    const int *ctl;                 // sessions[0]'s control block (CTL_DONE)
+    float *logits;                  // [nb][stride]: logits in, probabilities out
+    int n, stride, cand_cap;
+    float temperature[PF_MAXB];
+    float top_p[PF_MAXB];           // < 0: no candidate filter
+    ProbIndex *cand[PF_MAXB];       // [cand_cap] each
+    int *n_cand[PF_MAXB];
+};
+__global__ void __launch_bounds__(SAMP_THREADS) sample_prep_batch_kernel(const SamplePrepBatchParams p) {
+    pdl_wait();
+    if (p.ctl[CTL_DONE]) return;
+    const int b = blockIdx.x;
+    sample_prep_row(p.logits + (size_t)b * p.stride, p.n, batch_entry(p.temperature, b), batch_entry(p.top_p, b),
+                    batch_entry(p.cand, b), p.cand_cap, batch_entry(p.n_cand, b));
 }
 
 // standalone rmsnorm (unit-test surface; the hot path fuses it into the GEMV prologue)

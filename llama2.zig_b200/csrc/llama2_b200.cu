@@ -1012,7 +1012,8 @@ int preload_kernels(l2b_ctx *ctx) {
     if (pick_attn_wo(ctx->head_size, &smem)) L2B_CUDA(ctx, cudaFuncGetAttributes(&fa, (const void *)pick_attn_wo(ctx->head_size, &smem)));
     const void *others[] = {(const void *)attention_kernel, (const void *)advance_kernel,
                             (const void *)batch_advance_kernel, (const void *)gather_logits_kernel,
-                            (const void *)resid_add_kernel, (const void *)sample_prep_kernel, (const void *)synth_fill_kernel};
+                            (const void *)resid_add_kernel, (const void *)sample_prep_kernel,
+                            (const void *)sample_prep_batch_kernel, (const void *)synth_fill_kernel};
     for (const void *f : others) L2B_CUDA(ctx, cudaFuncGetAttributes(&fa, f));
     return L2B_OK;
 }
@@ -1530,6 +1531,23 @@ int run_step(l2b_ctx *lead, int token, int pos, int which, float temperature, fl
     return L2B_OK;
 }
 
+// The output of a sampling step, from ctx's pinned buffers: its probabilities to host_probs (if not
+// NULL and not the pinned buffer itself), and with the candidate filter on its candidates and their
+// count to cand / *n_cand, or minus their number when more passed than fit (the host then filters the
+// probabilities itself).  Without the filter *n_cand = 0.
+void copy_sample_out(l2b_ctx *ctx, bool filter, float *host_probs, l2b_prob_index *cand, int cand_cap, int32_t *n_cand) {
+    const int V = ctx->cfg.vocab_size;
+    if (host_probs && host_probs != ctx->h_logits) memcpy(host_probs, ctx->h_logits, (size_t)V * sizeof(float));
+    if (n_cand) *n_cand = 0;
+    if (filter) {
+        const int n = ctx->h_ints[2];
+        if (n > kCandCap || n > cand_cap) { *n_cand = -n; return; }   // too many: filter host_probs on the host
+        static_assert(sizeof(l2b_prob_index) == sizeof(ProbIndex), "candidate layout");
+        memcpy(cand, ctx->h_cand, (size_t)n * sizeof(ProbIndex));
+        *n_cand = n;
+    }
+}
+
 }  // namespace
 
 // ---------------------------------------------------------------------------------------
@@ -1660,16 +1678,7 @@ int32_t l2b_forward_sample(l2b_ctx *ctx, int32_t token, int32_t pos, float tempe
     if (filter && (!cand || !n_cand || cand_cap <= 0)) return fail(ctx, L2B_ERR_INVALID_ARG, "candidate buffer missing");
     rc = run_step(ctx, token, pos, G_SAMPLE, temperature, filter ? top_p : -1.0f);
     if (rc) return rc;
-    const int V = ctx->cfg.vocab_size;
-    if (host_probs && host_probs != ctx->h_logits) memcpy(host_probs, ctx->h_logits, (size_t)V * sizeof(float));
-    if (n_cand) *n_cand = 0;
-    if (filter) {
-        const int n = ctx->h_ints[2];
-        if (n > kCandCap || n > cand_cap) { *n_cand = -n; return L2B_OK; }   // too many: filter host_probs on the host
-        static_assert(sizeof(l2b_prob_index) == sizeof(ProbIndex), "candidate layout");
-        memcpy(cand, ctx->h_cand, (size_t)n * sizeof(ProbIndex));
-        *n_cand = n;
-    }
+    copy_sample_out(ctx, filter, host_probs, cand, cand_cap, n_cand);
     return L2B_OK;
 }
 
@@ -1870,13 +1879,36 @@ static int check_batch_args(l2b_ctx *const *s, int32_t n, const int32_t *tokens,
     return L2B_OK;
 }
 
+// sample_prep_batch_kernel over the nb logits rows of a group in pf_logits, in place; vector b is session
+// s[b] (its candidates and count go to its own buffers) with temperature[b] and top_p[b] (< 0: no filter)
+static int launch_sample_prep_batch(l2b_ctx *ctx, l2b_ctx *const *s, int nb, const float *temperature,
+                                    const float *top_p) {
+    SamplePrepBatchParams p{};
+    p.ctl = ctx->ctl;
+    p.logits = ctx->pf_logits;
+    p.n = p.stride = ctx->cfg.vocab_size;
+    p.cand_cap = kCandCap;
+    for (int b = 0; b < nb; ++b) {
+        p.temperature[b] = temperature[b];
+        p.top_p[b] = top_p[b];
+        p.cand[b] = s[b]->cand;
+        p.n_cand[b] = s[b]->n_cand;
+    }
+    void *args[] = {&p};
+    return launch_small(ctx, (const void *)sample_prep_batch_kernel, dim3(nb), dim3(SAMP_THREADS), args, ctx->stream, true);
+}
+
 // One step of each of n validated sessions.  Where l2b_prefill would batch (pf_prepare on the first
 // session), PF_MAXB sessions share each pass over the weights on the first session's stream and batch
 // buffers; each session's x and logits are then copied to its own buffers (xb, hb and q are not
-// written).  Otherwise each session runs its own step in turn.  Leaves each session's logits in its
-// h_logits, or (argmax) the next token in its h_ints[0]; the call's time and launches on s[0].
-static int step_sessions(l2b_ctx *const *s, int n, const int32_t *tokens, const int32_t *pos, bool argmax) {
+// written).  Otherwise each session runs its own step in turn.  mode: MODE_LOGITS leaves each session's
+// logits in its h_logits, MODE_ARGMAX the next token in its h_ints[0], and MODE_SAMPLE (temperature[i],
+// top_p[i] < 0: no filter) its probabilities in h_logits, candidates in h_cand and their count in
+// h_ints[2], as l2b_forward_sample's step does.  The call's time and launches on s[0].
+static int step_sessions(l2b_ctx *const *s, int n, const int32_t *tokens, const int32_t *pos, StepMode mode,
+                         const float *temperature = nullptr, const float *top_p = nullptr) {
     l2b_ctx *ctx = s[0];
+    const bool argmax = (mode == MODE_ARGMAX), sample = (mode == MODE_SAMPLE);
     int rc = pf_prepare(ctx);
     if (rc) return rc;
     cudaStream_t st = ctx->stream;
@@ -1885,7 +1917,8 @@ static int step_sessions(l2b_ctx *const *s, int n, const int32_t *tokens, const 
     if (!ctx->pf_ok) {
         int launches = 0;
         for (int i = 0; i < n; ++i) {
-            rc = run_step(s[i], tokens[i], pos[i], argmax ? G_ARGMAX_ONE : G_LOGITS, 1.0f, 0.0f);
+            rc = sample ? run_step(s[i], tokens[i], pos[i], G_SAMPLE, temperature[i], top_p[i])
+                        : run_step(s[i], tokens[i], pos[i], argmax ? G_ARGMAX_ONE : G_LOGITS, 1.0f, 0.0f);
             if (rc) { ctx->err = s[i]->err; return rc; }
             launches += s[i]->last_launches;
         }
@@ -1909,6 +1942,10 @@ static int step_sessions(l2b_ctx *const *s, int n, const int32_t *tokens, const 
         if (argmax) L2B_CUDA(ctx, cudaMemsetAsync(ctx->pf_amax, 0, PF_MAXB * sizeof(unsigned long long), st));
         rc = batched_classifier(ctx, nb, argmax);
         if (rc) return rc;
+        if (sample) {   // logits -> probabilities in place, candidates to each session's own buffers
+            rc = launch_sample_prep_batch(ctx, s + g, nb, temperature + g, top_p + g);
+            if (rc) return rc;
+        }
         for (int b = 0; b < nb; ++b) {
             l2b_ctx *c = s[g + b];
             L2B_CUDA(ctx, cudaMemcpyAsync(c->X, ctx->pf_x + (size_t)b * dim, dim * sizeof(float), cudaMemcpyDeviceToDevice, st));
@@ -1917,6 +1954,10 @@ static int step_sessions(l2b_ctx *const *s, int n, const int32_t *tokens, const 
                 L2B_CUDA(ctx, cudaMemcpyAsync(c->h_ints, ctx->pf_amax + b, sizeof(int), cudaMemcpyDeviceToHost, st));
             else
                 L2B_CUDA(ctx, cudaMemcpyAsync(c->h_logits, ctx->pf_logits + (size_t)b * V, V * sizeof(float), cudaMemcpyDeviceToHost, st));
+            if (sample) {   // as the single step's G_SAMPLE graph copies them
+                L2B_CUDA(ctx, cudaMemcpyAsync(c->h_cand, c->cand, (size_t)kCandCap * sizeof(ProbIndex), cudaMemcpyDeviceToHost, st));
+                L2B_CUDA(ctx, cudaMemcpyAsync(c->h_ints + 2, c->n_cand, sizeof(int), cudaMemcpyDeviceToHost, st));
+            }
         }
     }
     L2B_CUDA(ctx, cudaEventRecord(ctx->ev1, st));
@@ -2107,7 +2148,7 @@ int32_t l2b_forward_batch(l2b_ctx *const *sessions, int32_t n, const int32_t *to
     if (!host_logits) return fail(sessions[0], L2B_ERR_INVALID_ARG, "host_logits is NULL");
     for (int i = 0; i < n; ++i)
         if (!host_logits[i]) return fail(sessions[0], L2B_ERR_INVALID_ARG, "a host_logits entry is NULL");
-    rc = step_sessions(sessions, n, tokens, pos, false);
+    rc = step_sessions(sessions, n, tokens, pos, MODE_LOGITS);
     if (rc) return rc;
     for (int i = 0; i < n; ++i)
         if (host_logits[i] != sessions[i]->h_logits)
@@ -2120,9 +2161,34 @@ int32_t l2b_forward_argmax_batch(l2b_ctx *const *sessions, int32_t n, const int3
     int rc = check_batch_args(sessions, n, tokens, pos);
     if (rc) return rc;
     if (!next) return fail(sessions[0], L2B_ERR_INVALID_ARG, "next is NULL");
-    rc = step_sessions(sessions, n, tokens, pos, true);
+    rc = step_sessions(sessions, n, tokens, pos, MODE_ARGMAX);
     if (rc) return rc;
     for (int i = 0; i < n; ++i) next[i] = sessions[i]->h_ints[0];
+    return L2B_OK;
+}
+
+int32_t l2b_forward_sample_batch(l2b_ctx *const *sessions, int32_t n, const int32_t *tokens, const int32_t *pos,
+                                 const float *temperature, const float *top_p, float *const *host_probs,
+                                 l2b_prob_index *cand, int32_t cand_cap, int32_t *n_cand) {
+    int rc = check_batch_args(sessions, n, tokens, pos);
+    if (rc) return rc;
+    l2b_ctx *s0 = sessions[0];
+    if (!temperature || !top_p) return fail(s0, L2B_ERR_INVALID_ARG, "temperature or top_p is NULL");
+    if (s0->cfg.vocab_size < 2) return fail(s0, L2B_ERR_INVALID_ARG, "sampling needs vocab_size >= 2");
+    std::vector<float> filter_p(n);   // the kernel's top-p: < 0 = no filter
+    for (int i = 0; i < n; ++i) {
+        if (!(temperature[i] > 0.0f)) return fail(s0, L2B_ERR_INVALID_ARG, "temperature must be > 0 (use l2b_forward_argmax_batch for 0)");
+        if (!(top_p[i] >= 0.0f && top_p[i] <= 1.0f)) return fail(s0, L2B_ERR_INVALID_ARG, "top_p must be in [0, 1]");
+        const bool filter = (top_p[i] != 0.0f && top_p[i] != 1.0f);   // :1009
+        if (filter && (!cand || !n_cand || cand_cap <= 0)) return fail(s0, L2B_ERR_INVALID_ARG, "candidate buffer missing");
+        filter_p[i] = filter ? top_p[i] : -1.0f;
+    }
+    rc = step_sessions(sessions, n, tokens, pos, MODE_SAMPLE, temperature, filter_p.data());
+    if (rc) return rc;
+    for (int i = 0; i < n; ++i)
+        copy_sample_out(sessions[i], filter_p[i] >= 0.0f, host_probs ? host_probs[i] : nullptr,
+                        cand && cand_cap > 0 ? cand + (size_t)i * cand_cap : nullptr, cand_cap,
+                        n_cand ? n_cand + i : nullptr);
     return L2B_OK;
 }
 

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Aggregate decode rate of n sessions on one llama2-7B model (l2b_create_session + l2b_forward_argmax_batch /
-l2b_generate_argmax_batch).
+l2b_generate_argmax_batch / l2b_forward_sample_batch).
 
   python scripts/bench_sessions.py [--sessions 1,2,4,8] [--positions 256] [--warmup 4] [--repeats 2]
 
@@ -9,12 +9,17 @@ prefilled to 61*b positions (staggered, so the sessions' attention lengths diffe
 --warmup batched steps, and then teacher-forced over --positions positions through
 l2b_forward_argmax_batch, one call per position ("batched step"), and in the same repeat through one
 l2b_generate_argmax_batch call over the same positions with the teacher tokens forced ("device loop":
-no host round trip per position).  The two alternate within each repeat.  The L2 cache is flushed (256 MiB memset) before
+no host round trip per position).  A third run in the same repeat samples at the reference CLI's
+defaults (temperature 1.0, top-p 0.9) through l2b_forward_sample_batch, one call per position
+("sampled batched step"): each session's token is drawn on the host from its candidates with its own
+seeded generator and fed back.  The three alternate within each repeat.  The L2 cache is flushed (256 MiB memset) before
 each timed run.  Per call the library brackets its work with CUDA events (l2b_last_timing); the device
 time of a run is their sum, and a host clock around the run (every call ends in a synchronise) gives
-the wall time (the device loop is one call).  The single-stream reference is the on-device loop of one context
-(l2b_generate_argmax, bench.py's headline), timed the same way.  One JSON line per measurement; the
-card's name and power limit (read-only nvidia-smi query) are printed in the same run.
+the wall time (the device loop is one call).  The single-stream references are the on-device loop of one context
+(l2b_generate_argmax, bench.py's headline), timed the same way, and a host loop of l2b_forward_sample on
+one context with the same draw (wall time only: single steps carry no events by default).  One JSON
+line per measurement; the card's name and power limit (read-only nvidia-smi query) are printed in the
+same run.
 """
 import argparse
 import json
@@ -23,15 +28,34 @@ import subprocess
 import sys
 import time
 
+import numpy as np
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 SHAPE = (4096, 11008, 32, 32, 32, -32000, 2048)     # llama2-7B, unshared classifier
 SEED = 7
+TEMPERATURE, TOP_P = 1.0, 0.9                        # the reference CLI's defaults
 
 
 def teacher(b, n, vocab):
     return [(1 + 7919 * p + 104729 * b) % vocab for p in range(n)]
+
+
+def draw(rng, probs, cand, n_cand):
+    """The host's part of top-p sampling: the candidates (or, when more passed than the device returned,
+    the host's own filter of probs) sorted by probability, cut where the cumulative probability passes
+    TOP_P, and one uniform draw walked along their CDF."""
+    if n_cand < 0:
+        idx = np.nonzero(probs >= np.float32((1.0 - TOP_P) / (probs.size - 1)))[0]
+        pr = probs[idx]
+    else:
+        idx, pr = cand["index"], cand["prob"]
+    order = np.argsort(-pr, kind="stable")
+    idx, pr = idx[order], pr[order]
+    cdf = np.cumsum(pr, dtype=np.float64)
+    last = min(int(np.searchsorted(cdf, TOP_P, side="right")), idx.size - 1)
+    return int(idx[min(int(np.searchsorted(cdf[:last + 1], rng.random() * cdf[last], side="right")), last)])
 
 
 def card():
@@ -82,6 +106,19 @@ def main():
         if r:
             print(json.dumps({"what": "single-stream device loop", "positions": P, "device_ms": round(ms, 2),
                               "tok_s": round(P / (ms / 1e3), 2), "wall_tok_s": round(P / wall, 2)}), flush=True)
+        # single stream, sampled: a host loop of forward_sample over the same number of positions
+        m.reset()
+        rng = np.random.default_rng(SEED)
+        flush()
+        t0 = time.perf_counter()
+        tok = toks[0][0]
+        for pos in range(P):
+            probs, cand, k = m.forward_sample(tok, pos, TEMPERATURE, TOP_P, with_count=True)
+            tok = draw(rng, probs, cand, k)
+        wall = time.perf_counter() - t0
+        if r:
+            print(json.dumps({"what": "single-stream sampled steps", "positions": P,
+                              "wall_tok_s": round(P / wall, 2)}), flush=True)
 
     for n in counts:
         group = sess[:n]
@@ -127,6 +164,26 @@ def main():
                                   "launches_per_step": launches // P,
                                   "ms_per_step": round(ms / P, 3),
                                   "tok_s": round(n * P / (ms / 1e3), 2),
+                                  "wall_tok_s": round(n * P / wall, 2)}), flush=True)
+            # the same positions sampled, each session's drawn token fed back, from the same state
+            prepare(group)
+            rngs = [np.random.default_rng(SEED + b) for b in range(n)]
+            tok = [toks[b][starts[b] + W] for b in range(n)]
+            flush()
+            dev_ms = 0.0
+            t0 = time.perf_counter()
+            for i in range(W, W + P):
+                pos = [starts[b] + i for b in range(n)]
+                probs, cands, counts = l2b.forward_sample_batch(group, tok, pos, [TEMPERATURE] * n, [TOP_P] * n)
+                ms, launches = group[0].last_timing()
+                dev_ms += ms
+                tok = [draw(rngs[b], probs[b], cands[b], counts[b]) for b in range(n)]
+            wall = time.perf_counter() - t0
+            if r:
+                print(json.dumps({"what": "sampled batched step", "sessions": n, "positions": P,
+                                  "launches_per_step": launches,
+                                  "ms_per_step": round(dev_ms / P, 3),
+                                  "tok_s": round(n * P / (dev_ms / 1e3), 2),
                                   "wall_tok_s": round(n * P / wall, 2)}), flush=True)
     for s in sess[1:]:
         s.close()
