@@ -192,6 +192,29 @@ int32_t l2b_generate_argmax(l2b_ctx *ctx, int32_t token, int32_t pos, int32_t n_
 int32_t l2b_prefill(l2b_ctx *ctx, const int32_t *tokens, int32_t n_tokens, int32_t pos0,
                     float *host_logits);
 
+/* Log-probabilities of a known sequence (teacher forcing: perplexity, reranking, comparing two
+ * checkpoints).  Runs tokens[i] at position pos0+i for i = 0 .. n_tokens-2 and writes, for each i,
+ *   logprob[i] = log softmax(logits at pos0+i)[tokens[i+1]]   (temperature 1, natural log)
+ *   greedy[i]  = argmax of those logits, first maximum wins (:715-726)   -- greedy may be NULL
+ * Afterwards the context has pos0 + n_tokens - 1 positions appended; the caller may continue with
+ * l2b_forward(ctx, tokens[n_tokens-1], pos0 + n_tokens - 1, ..).  Everything is checked before
+ * anything runs, so a refused call changes no KV cache: NULL ctx, tokens or logprob, n_tokens < 1,
+ * a token outside [0, vocab_size), pos0 < 0 or pos0 + n_tokens - 1 > seq_len => L2B_ERR_INVALID_ARG;
+ * pos0 past the positions appended => L2B_ERR_STATE; a tensor-parallel context (each rank holds only
+ * a slice of the vocabulary) => L2B_ERR_UNSUPPORTED.  n_tokens == 1 runs and writes nothing.  Works on
+ * any single-GPU context or session.
+ * Where l2b_prefill shares weight passes, the positions run in l2b_prefill's groups of 4 (the KV rows
+ * are those of l2b_prefill(tokens, n_tokens - 1, pos0) bit for bit) with the batched classifier after
+ * each group; the logits are the batched prefill's, within 1e-6 (relative to the largest logit) of
+ * single steps, so logprob is within 2e-6 x max|logit| + 1e-5 of the log-softmax of l2b_forward's
+ * logits.  Elsewhere each position runs l2b_forward_argmax's own decode step on the device: logprob[i]
+ * equals l2b_op_logprob of l2b_forward's logits bit for bit, and greedy[i] equals l2b_forward_argmax.
+ * Against the exact log-softmax of the same float32 logits: within 1e-5 + 1e-6 x |logprob|.
+ * Synchronous; l2b_last_timing(ctx) gives the call's device time and kernel launches.  x, xb, hb, q and
+ * logits are not defined afterwards.                                                        */
+int32_t l2b_score(l2b_ctx *ctx, const int32_t *tokens, int32_t n_tokens, int32_t pos0,
+                  float *logprob, int32_t *greedy);
+
 /* One transformer() step for each of n distinct sessions of one model (l2b_create_session; the
  * model's own context counts as one): sessions[i] runs tokens[i] at pos[i], under l2b_forward's rule
  * pos[i] <= (positions appended to that session).  host_logits[i] receives session i's logits.
@@ -338,6 +361,9 @@ int32_t l2b_op_attention_head(int32_t device, float *out, const float *q, const 
  * l2b_forward_sample); *n_cand = number that passed the filter (-1 when top_p is 0 or 1).   */
 int32_t l2b_op_sample_prep(int32_t device, float *logits_inout, int32_t n, float temperature,
                            float top_p, l2b_prob_index *cand, int32_t cand_cap, int32_t *n_cand);
+/* log softmax(logits)[target] of n host logits (l2b_score's device code, see there).  NULL pointers,
+ * n < 1 or a target outside [0, n) => L2B_ERR_INVALID_ARG.                                  */
+int32_t l2b_op_logprob(int32_t device, const float *logits, int32_t n, int32_t target, float *logprob);
 
 #ifdef __cplusplus
 }

@@ -94,6 +94,7 @@ def load_library():
     lib.l2b_forward_pinned.argtypes = [vp, C.c_int32, C.c_int32, C.POINTER(FP)]
     lib.l2b_generate_argmax.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, IP, C.c_int32, IP, IP]
     lib.l2b_prefill.argtypes = [vp, IP, C.c_int32, C.c_int32, FP]
+    lib.l2b_score.argtypes = [vp, IP, C.c_int32, C.c_int32, FP, IP]
     lib.l2b_logits_buffer.argtypes = [vp]
     lib.l2b_logits_buffer.restype = FP
     lib.l2b_forward_sample.argtypes = [vp, C.c_int32, C.c_int32, C.c_float, C.c_float, FP,
@@ -102,6 +103,7 @@ def load_library():
     lib.l2b_op_fused_matmul.argtypes = [C.c_int32, FP, FP, FP, FP, FP, C.c_int32, C.c_int32, C.c_int32]
     lib.l2b_op_sample_prep.argtypes = [C.c_int32, FP, C.c_int32, C.c_float, C.c_float,
                                        C.POINTER(L2BProbIndex), C.c_int32, IP]
+    lib.l2b_op_logprob.argtypes = [C.c_int32, FP, C.c_int32, C.c_int32, FP]
     lib.l2b_last_error.argtypes = [vp]
     lib.l2b_last_error.restype = C.c_char_p
     lib.l2b_status_string.argtypes = [C.c_int32]
@@ -277,6 +279,17 @@ class Transformer:
         _check(self.lib.l2b_prefill(self.h, toks.ctypes.data_as(IP), toks.size, int(pos0),
                                     out.ctypes.data_as(FP) if want_logits else None), self.h)
         return self._logits.copy() if want_logits else None
+
+    def score(self, tokens, pos0=0):
+        """Teacher forcing (l2b_score): tokens[i] at position pos0+i for i < n-1.  Returns (logprob float32[n-1],
+        greedy int32[n-1]): position i's natural-log probability of tokens[i+1] and its argmax token."""
+        toks = np.ascontiguousarray(tokens, dtype=np.int32)
+        n = max(toks.size - 1, 0)
+        lp = np.empty(max(n, 1), dtype=np.float32)
+        greedy = np.empty(max(n, 1), dtype=np.int32)
+        _check(self.lib.l2b_score(self.h, toks.ctypes.data_as(IP), toks.size, int(pos0), lp.ctypes.data_as(FP),
+                                  greedy.ctypes.data_as(IP)), self.h)
+        return lp[:n].copy(), greedy[:n].copy()
 
     def logits_buffer(self):
         """The library's pinned logits buffer as a numpy view (state.logits of the host, zero copy)."""
@@ -466,6 +479,14 @@ def sample_prep(logits, temperature, top_p, cand_cap=8192, device=0):
     if n.value > 0:
         arr = np.frombuffer(cand, dtype=[("prob", "<f4"), ("index", "<i4")], count=min(n.value, cand_cap)).copy()
     return probs, arr, n.value
+
+
+def logprob(logits, target, device=0):
+    """log softmax(logits)[target] on the device (l2b_op_logprob: l2b_score's kernel on one row)."""
+    logits, lp_ = _f32(logits)
+    out = C.c_float()
+    _check(load_library().l2b_op_logprob(device, lp_, logits.size, int(target), C.byref(out)))
+    return np.float32(out.value)
 
 
 def rmsnorm(o, x, w, device=0):

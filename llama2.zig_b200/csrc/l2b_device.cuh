@@ -2130,6 +2130,76 @@ __global__ void __launch_bounds__(SAMP_THREADS) sample_prep_batch_kernel(const S
                     batch_entry(p.cand, b), p.cand_cap, batch_entry(p.n_cand, b));
 }
 
+// ---------------------------------------------------------------------------------------
+// Scoring a known sequence (l2b_score): log softmax(logits)[target] at temperature 1, one CTA per row.
+// Two passes in a fixed reduction order (per-thread strided loop, warp butterfly, warps in order; no
+// atomics): the maximum m, then s = sum expf(l[i] - m); the result is (l[target] - m) - logf(s).  A
+// target outside [0, n) gives NaN and reads nothing (creation's warm-up replays the score graph with
+// the forced-token buffer at -1).  The greedy token is not recomputed: it is the classifier's argmax
+// key (EPI_ARGMAX, first maximum wins), so it is exactly what l2b_forward_argmax picks.
+// ---------------------------------------------------------------------------------------
+constexpr int LOGPROB_THREADS = 1024;
+__device__ __forceinline__ float logprob_row(const float *logits, int n, int target) {
+    __shared__ float red[LOGPROB_THREADS / 32];
+    if (target < 0 || target >= n) return __int_as_float(0x7fffffff);
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    float m = -INFINITY;
+    for (int i = tid; i < n; i += LOGPROB_THREADS) m = fmaxf(m, logits[i]);
+    m = warp_max(m);
+    if (lane == 0) red[warp] = m;
+    __syncthreads();
+    m = warp_max(red[lane]);                                 // 32 warps
+    __syncthreads();
+    float s = 0.0f;
+    for (int i = tid; i < n; i += LOGPROB_THREADS) s += expf(logits[i] - m);
+    s = warp_sum(s);
+    if (lane == 0) red[warp] = s;
+    __syncthreads();
+    s = warp_sum(red[lane]);
+    return (logits[target] - m) - logf(s);
+}
+__device__ __forceinline__ int argmax_key_index(unsigned long long key) {
+    return (int)(0xFFFFFFFFu - (unsigned int)(key & 0xFFFFFFFFull));
+}
+
+// One step of the score loop (G_SCORE_LOOP): the target is the step's forced token, the greedy token the
+// step's argmax key, which advance_kernel (launched next) zeroes.
+__global__ void __launch_bounds__(LOGPROB_THREADS) logprob_kernel(const float *logits, int n, const int *ctl,
+                                                                  const int *forced, const unsigned long long *amax,
+                                                                  float *lp, int *greedy) {
+    pdl_wait();
+    if (ctl[CTL_DONE]) return;
+    const int step = ctl[CTL_STEP];
+    const float r = logprob_row(logits, n, forced[step]);
+    if (threadIdx.x == 0) {
+        lp[step] = r;
+        greedy[step] = argmax_key_index(*amax);
+    }
+}
+
+// A group of the batched score (and l2b_op_logprob, nb = 1): CTA b scores row b of the group's logits
+// against targets[b], writes lp[b] and greedy[b] from amax[b], and zeroes amax[b] for the next group.
+struct LogprobBatchParams {
+    const int *ctl;                 // CTL_DONE
+    const float *logits;            // [nb][n]
+    int n;
+    const int *targets;             // [nb]
+    unsigned long long *amax;       // [nb] packed argmax keys of the group's classifier
+    float *lp;                      // [nb]
+    int *greedy;                    // [nb]
+};
+__global__ void __launch_bounds__(LOGPROB_THREADS) logprob_batch_kernel(const LogprobBatchParams p) {
+    pdl_wait();
+    if (p.ctl[CTL_DONE]) return;
+    const int b = blockIdx.x;
+    const float r = logprob_row(p.logits + (size_t)b * p.n, p.n, p.targets[b]);
+    if (threadIdx.x == 0) {
+        p.lp[b] = r;
+        p.greedy[b] = argmax_key_index(p.amax[b]);
+        p.amax[b] = 0ull;
+    }
+}
+
 // standalone rmsnorm (unit-test surface; the hot path fuses it into the GEMV prologue)
 __global__ void __launch_bounds__(NT) rmsnorm_kernel(float *o, const float *x, const float *w, int n) {
     __shared__ float scratch[NWARP + 1];

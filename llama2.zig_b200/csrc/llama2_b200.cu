@@ -84,7 +84,8 @@ bool nccl_load(std::string *err) {
 // Context (one rank)
 // ---------------------------------------------------------------------------------------
 enum StepMode { MODE_LOGITS = 0, MODE_ARGMAX = 1, MODE_SAMPLE = 2, MODE_NOCLS = 3 };
-enum GraphId { G_LOGITS = 0, G_ARGMAX_ONE = 1, G_ARGMAX_LOOP = 2, G_SAMPLE = 3, G_PREFILL_LOOP = 4, G_COUNT = 5 };
+enum GraphId { G_LOGITS = 0, G_ARGMAX_ONE = 1, G_ARGMAX_LOOP = 2, G_SAMPLE = 3, G_PREFILL_LOOP = 4, G_SCORE_LOOP = 5,
+               G_COUNT = 6 };
 constexpr int kCandCap = 8192;               // top-p candidates returned per step (more => host filters itself)
 
 // The device weights and RoPE tables of one loaded model (one rank's shard), shared by the context that
@@ -138,6 +139,8 @@ struct l2b_ctx {
     int *gen_forced = nullptr, *gen_out = nullptr, *gen_ndone = nullptr;
     ProbIndex *cand = nullptr;               // sampler: top-p candidates (index order)
     int *n_cand = nullptr;
+    float *score_lp = nullptr;               // l2b_score: seq_len log-probabilities and greedy tokens
+    int *score_greedy = nullptr;
     // host pinned
     float *h_logits = nullptr;               // vocab floats: logits, or probabilities after sample_prep
     int *h_ctl = nullptr;                    // [0..7] host -> device control words, [8..15] device -> host status
@@ -913,10 +916,23 @@ int launch_sample_prep(l2b_ctx *ctx, cudaStream_t st) {
     return launch_small(ctx, (const void *)sample_prep_kernel, dim3(1), dim3(SAMP_THREADS), args, st, true);
 }
 
+int launch_logprob(l2b_ctx *ctx, cudaStream_t st) {
+    const float *lg = ctx->logits;
+    int V = ctx->cfg.vocab_size;
+    const int *ctl = ctx->ctl;
+    const int *forced = ctx->gen_forced;
+    const unsigned long long *amax = ctx->amax;
+    float *lp = ctx->score_lp;
+    int *greedy = ctx->score_greedy;
+    void *args[] = {&lg, &V, &ctl, &forced, &amax, &lp, &greedy};
+    return launch_small(ctx, (const void *)logprob_kernel, dim3(1), dim3(LOGPROB_THREADS), args, st, true);
+}
+
 // everything one call needs, as it is captured into (or eagerly enqueued instead of) graph `which`
 int enqueue_call(l2b_ctx *ctx, cudaStream_t st, int which) {
     const bool sink = !ctx->leader || ctx->rank == 0;   // in-process group: only rank 0 returns data to the host
-    const bool loop = (which == G_ARGMAX_LOOP || which == G_PREFILL_LOOP);   // (token, pos) advance on the device
+    // (token, pos) advance on the device
+    const bool loop = (which == G_ARGMAX_LOOP || which == G_PREFILL_LOOP || which == G_SCORE_LOOP);
     if (!loop)
         L2B_CUDA(ctx, cudaMemcpyAsync(ctx->ctl, ctx->h_ctl, CTL_HOST_WORDS * sizeof(int), cudaMemcpyHostToDevice, st));
     const StepMode mode = (which == G_LOGITS) ? MODE_LOGITS : (which == G_SAMPLE) ? MODE_SAMPLE
@@ -946,6 +962,12 @@ int enqueue_call(l2b_ctx *ctx, cudaStream_t st, int which) {
         rc = launch_advance(ctx, st, true, false);
         if (rc) return rc;
         break;
+    case G_SCORE_LOOP:     // single GPU only (l2b_score); every next token is forced
+        rc = launch_logprob(ctx, st);
+        if (rc) return rc;
+        rc = launch_advance(ctx, st, true, false);
+        if (rc) return rc;
+        break;
     default:   // G_ARGMAX_LOOP
         rc = launch_advance(ctx, st, true, ctx->world > 1 && ctx->use_p2p);
         if (rc) return rc;
@@ -958,6 +980,7 @@ int enqueue_call(l2b_ctx *ctx, cudaStream_t st, int which) {
 
 int build_graphs(l2b_ctx *ctx) {
     for (int which = 0; which < G_COUNT; ++which) {
+        if (which == G_SCORE_LOOP && ctx->world > 1) continue;   // l2b_score refuses tensor parallel
         cudaGraph_t g = nullptr;
         L2B_CUDA(ctx, cudaStreamBeginCapture(ctx->stream, cudaStreamCaptureModeRelaxed));
         ctx->last_launches = 0;
@@ -1013,7 +1036,8 @@ int preload_kernels(l2b_ctx *ctx) {
     const void *others[] = {(const void *)attention_kernel, (const void *)advance_kernel,
                             (const void *)batch_advance_kernel, (const void *)gather_logits_kernel,
                             (const void *)resid_add_kernel, (const void *)sample_prep_kernel,
-                            (const void *)sample_prep_batch_kernel, (const void *)synth_fill_kernel};
+                            (const void *)sample_prep_batch_kernel, (const void *)logprob_kernel,
+                            (const void *)logprob_batch_kernel, (const void *)synth_fill_kernel};
     for (const void *f : others) L2B_CUDA(ctx, cudaFuncGetAttributes(&fa, f));
     return L2B_OK;
 }
@@ -1156,6 +1180,8 @@ int create_run_state(l2b_ctx *ctx) {
     L2B_TRY(dev_alloc(ctx, &ctx->gen_ndone, (size_t)1));
     L2B_TRY(dev_alloc(ctx, &ctx->cand, (size_t)kCandCap));
     L2B_TRY(dev_alloc(ctx, &ctx->n_cand, (size_t)1));
+    L2B_TRY(dev_alloc(ctx, &ctx->score_lp, S));
+    L2B_TRY(dev_alloc(ctx, &ctx->score_greedy, S));
     L2B_TRY(cuda_try(ctx, cudaMemsetAsync(ctx->ctl, 0, CTL_WORDS * sizeof(int), ctx->stream), "memset"));
     L2B_TRY(cuda_try(ctx, cudaMemsetAsync(ctx->X, 0, dim * sizeof(float), ctx->stream), "memset"));
     L2B_TRY(cuda_try(ctx, cudaMemsetAsync(ctx->amax, 0, sizeof(unsigned long long), ctx->stream), "memset"));
@@ -1252,12 +1278,13 @@ int create_run_state(l2b_ctx *ctx) {
 // all local ranks are enqueued before any is synchronised.
 int warm_up(const std::vector<l2b_ctx *> &ranks) {
     for (int which = 0; which < G_COUNT; ++which) {
+        if (which == G_SCORE_LOOP && ranks[0]->world > 1) continue;   // as build_graphs
         for (l2b_ctx *ctx : ranks) {
             L2B_TRY(cuda_try(ctx, cudaSetDevice(ctx->device), "cudaSetDevice"));
             memset(ctx->h_ctl, 0, CTL_WORDS * sizeof(int));
             ctx->h_ctl[CTL_TEMP] = 0x3f800000;   // 1.0f
             ctx->h_ctl[CTL_TOPP] = 0x3f666666;   // 0.9f
-            if (which == G_ARGMAX_LOOP || which == G_PREFILL_LOOP)
+            if (which == G_ARGMAX_LOOP || which == G_PREFILL_LOOP || which == G_SCORE_LOOP)
                 L2B_TRY(cuda_try(ctx, cudaMemcpyAsync(ctx->ctl, ctx->h_ctl, CTL_HOST_WORDS * sizeof(int), cudaMemcpyHostToDevice, ctx->stream), "ctl upload"));
             L2B_TRY(enqueue_call(ctx, ctx->stream, which));
         }
@@ -1265,7 +1292,8 @@ int warm_up(const std::vector<l2b_ctx *> &ranks) {
             L2B_TRY(cuda_try(ctx, cudaSetDevice(ctx->device), "cudaSetDevice"));
             L2B_TRY(cuda_try(ctx, cudaStreamSynchronize(ctx->stream), "warm-up step"));
             L2B_TRY(cuda_try(ctx, cudaGetLastError(), "warm-up step"));
-            if (ctx->h_ctl[CTL_WORDS + CTL_ERR] && which != G_ARGMAX_LOOP && which != G_PREFILL_LOOP) {
+            if (ctx->h_ctl[CTL_WORDS + CTL_ERR] && which != G_ARGMAX_LOOP && which != G_PREFILL_LOOP &&
+                which != G_SCORE_LOOP) {
                 ctx->err = "tensor-parallel warm-up step timed out waiting for a peer";
                 g_create_error = ctx->err;
                 return L2B_ERR_COMM;
@@ -1818,12 +1846,22 @@ static int batched_layers(l2b_ctx *ctx, l2b_ctx *const *kv, const int *pos, int 
     return L2B_OK;
 }
 
-// n_tokens positions starting at pos0, PF_MAXB per pass over the weights; KV cache filled, no logits
-static int prefill_batched(l2b_ctx *ctx, const int32_t *tokens, int n_tokens, int pos0) {
+static int batched_classifier(l2b_ctx *ctx, int nb, bool argmax);
+static int launch_logprob_batch(l2b_ctx *ctx, int nb, int done);
+
+// n_tokens positions starting at pos0, PF_MAXB per pass over the weights; KV cache filled.  Without
+// score no logits; with score (l2b_score: tokens holds n_tokens + 1 entries) each group then runs the
+// argmax classifier and logprob_batch_kernel, which leaves position i's log-probability of tokens[i + 1]
+// and its greedy token in score_lp[i] and score_greedy[i].
+static int prefill_batched(l2b_ctx *ctx, const int32_t *tokens, int n_tokens, int pos0, bool score = false) {
     cudaStream_t st = ctx->stream;
     L2B_CUDA(ctx, cudaSetDevice(ctx->device));
     for (int i = 0; i < n_tokens; ++i) ctx->h_gen[i] = tokens[i];
     L2B_CUDA(ctx, cudaMemcpyAsync(ctx->pf_tokens, ctx->h_gen, (size_t)n_tokens * sizeof(int), cudaMemcpyHostToDevice, st));
+    if (score) {   // the targets, from the caller's (pageable) array: staged before the call returns
+        L2B_CUDA(ctx, cudaMemcpyAsync(ctx->gen_forced, tokens + 1, (size_t)n_tokens * sizeof(int), cudaMemcpyHostToDevice, st));
+        L2B_CUDA(ctx, cudaMemsetAsync(ctx->pf_amax, 0, PF_MAXB * sizeof(unsigned long long), st));
+    }
     fill_ctl(ctx, tokens[0], pos0, 0, 1.0f, -1.0f);          // DONE = 0 for the attention kernel
     L2B_CUDA(ctx, cudaMemcpyAsync(ctx->ctl, ctx->h_ctl, CTL_HOST_WORDS * sizeof(int), cudaMemcpyHostToDevice, st));
     L2B_CUDA(ctx, cudaEventRecord(ctx->ev0, st));
@@ -1835,6 +1873,12 @@ static int prefill_batched(l2b_ctx *ctx, const int32_t *tokens, int n_tokens, in
         for (int b = 0; b < nb; ++b) { kv[b] = ctx; pos[b] = pos0 + done + b; }
         int rc = batched_layers(ctx, kv, pos, nb, ctx->pf_tokens + done, nullptr);
         if (rc) return rc;
+        if (score) {
+            rc = batched_classifier(ctx, nb, true);
+            if (rc) return rc;
+            rc = launch_logprob_batch(ctx, nb, done);
+            if (rc) return rc;
+        }
     }
     L2B_CUDA(ctx, cudaEventRecord(ctx->ev1, st));
     L2B_CUDA(ctx, cudaStreamSynchronize(st));
@@ -1858,6 +1902,21 @@ static int batched_classifier(l2b_ctx *ctx, int nb, bool argmax) {
     k.out0 = ctx->pf_logits;
     k.amax = ctx->pf_amax;
     return pf_launch<PF_MAXB>(ctx, argmax ? EPI_ARGMAX : EPI_STORE, k, ctx->stream);
+}
+
+// logprob_batch_kernel over the nb logits rows of a group in pf_logits: positions done .. done+nb-1 of a
+// score, their targets at gen_forced + done, their results to score_lp / score_greedy + done
+static int launch_logprob_batch(l2b_ctx *ctx, int nb, int done) {
+    LogprobBatchParams p{};
+    p.ctl = ctx->ctl;
+    p.logits = ctx->pf_logits;
+    p.n = ctx->cfg.vocab_size;
+    p.targets = ctx->gen_forced + done;
+    p.amax = ctx->pf_amax;
+    p.lp = ctx->score_lp + done;
+    p.greedy = ctx->score_greedy + done;
+    void *args[] = {&p};
+    return launch_small(ctx, (const void *)logprob_batch_kernel, dim3(nb), dim3(LOGPROB_THREADS), args, ctx->stream, true);
 }
 
 // Everything a batched step checks, before anything is launched: a refused call changes no session.
@@ -2020,7 +2079,8 @@ static int enqueue_device_loops(std::vector<DeviceLoop> &loops, int which, int s
             if (loops.size() > 1) L2B_CUDA(ctx, cudaSetDevice(c->device));
             if (c->use_graphs) {
                 L2B_CUDA(ctx, cudaGraphLaunch(c->graphs[which], c->stream));
-                d.launches += c->launches_per_step + (which == G_PREFILL_LOOP ? 0 : 1);
+                // G_LOGITS' count, minus the classifier (prefill), plus advance_kernel and logprob_kernel (score)
+                d.launches += c->launches_per_step + (which == G_PREFILL_LOOP ? 0 : which == G_SCORE_LOOP ? 2 : 1);
             } else {
                 c->last_launches = 0;
                 rc = enqueue_call(c, c->stream, which);
@@ -2138,6 +2198,41 @@ int32_t l2b_prefill(l2b_ctx *ctx, const int32_t *tokens, int32_t n_tokens, int32
         if (done != n_silent) return fail(ctx, L2B_ERR_STATE, "prefill stopped early");
     }
     if (host_logits) return l2b_forward(ctx, tokens[n_tokens - 1], pos0 + n_tokens - 1, host_logits);
+    return L2B_OK;
+}
+
+// Teacher forcing: tokens[i] at pos0 + i for i < n_tokens - 1, each position's log-probability of
+// tokens[i + 1] and its greedy token.  Where l2b_prefill batches, the same groups of PF_MAXB positions
+// as l2b_prefill(tokens, n_tokens - 1, pos0) with the argmax classifier and logprob_batch_kernel after
+// each; otherwise the device loop G_SCORE_LOOP (a decode step with the argmax classifier,
+// logprob_kernel, advance_kernel on the forced tokens tokens[1..]).
+int32_t l2b_score(l2b_ctx *ctx, const int32_t *tokens, int32_t n_tokens, int32_t pos0, float *logprob,
+                  int32_t *greedy) {
+    if (!ctx) { g_create_error = "ctx is NULL"; return L2B_ERR_INVALID_ARG; }
+    if (!tokens || !logprob || n_tokens < 1) return fail(ctx, L2B_ERR_INVALID_ARG, "bad score arguments");
+    for (int i = 0; i < n_tokens; ++i)
+        if (tokens[i] < 0 || tokens[i] >= ctx->cfg.vocab_size) return fail(ctx, L2B_ERR_INVALID_ARG, "token out of range");
+    if (pos0 < 0 || (int64_t)pos0 + n_tokens - 1 > ctx->cfg.seq_len) return fail(ctx, L2B_ERR_INVALID_ARG, "score runs past seq_len");
+    if (pos0 > ctx->n_appended) return fail(ctx, L2B_ERR_STATE, "pos0 skips ahead of the KV cache");
+    if (ctx->world > 1)
+        return fail(ctx, L2B_ERR_UNSUPPORTED, "l2b_score needs a single-GPU context (under tensor parallelism each rank holds only a slice of the vocabulary)");
+    ctx->last_ms = 0.0f;
+    ctx->last_launches = 0;
+    const int n = n_tokens - 1;                               // positions scored
+    if (n == 0) return L2B_OK;
+    int rc = pf_prepare(ctx);
+    if (rc) return rc;
+    if (ctx->pf_ok) {
+        rc = prefill_batched(ctx, tokens, n, pos0, true);
+        if (rc) return rc;
+    } else {
+        int done = 0;
+        rc = run_device_loop(ctx, G_SCORE_LOOP, tokens[0], pos0, n, tokens + 1, 0, &done);
+        if (rc) return rc;
+        if (done != n) return fail(ctx, L2B_ERR_STATE, "score stopped early");
+    }
+    L2B_CUDA(ctx, cudaMemcpy(logprob, ctx->score_lp, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost));
+    if (greedy) L2B_CUDA(ctx, cudaMemcpy(greedy, ctx->score_greedy, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost));
     return L2B_OK;
 }
 
@@ -2618,6 +2713,23 @@ int32_t l2b_op_attention_head(int32_t device, float *out, const float *q, const 
         fn<<<dim3(1, nsplit), NT, smem2>>>(a, AttnBatch{});
     }
     s.down(out, dout, head_size);
+    return s.rc;
+}
+
+// log softmax(logits)[target] alone (logprob_batch_kernel, one row) on host logits: unit-test surface
+int32_t l2b_op_logprob(int32_t device, const float *logits, int32_t n, int32_t target, float *logprob) {
+    if (!logits || !logprob || n < 1 || target < 0 || target >= n) return L2B_ERR_INVALID_ARG;
+    OpScope s(device);
+    float *dl = s.up(logits, n), *dlp = s.up(nullptr, 1);
+    int *ctl = (int *)s.up(nullptr, CTL_WORDS), *dt = (int *)s.up(nullptr, 1), *dg = (int *)s.up(nullptr, 1);
+    unsigned long long *amax = (unsigned long long *)s.up(nullptr, 2);
+    if (s.rc) return s.rc;
+    cudaMemset(ctl, 0, CTL_WORDS * sizeof(int));
+    cudaMemset(amax, 0, sizeof(unsigned long long));
+    cudaMemcpy(dt, &target, sizeof(int), cudaMemcpyHostToDevice);
+    LogprobBatchParams p{ctl, dl, n, dt, amax, dlp, dg};
+    logprob_batch_kernel<<<1, LOGPROB_THREADS>>>(p);
+    s.down(logprob, dlp, 1);
     return s.rc;
 }
 
