@@ -308,8 +308,9 @@ int32_t l2b_profile_step(l2b_ctx *ctx, int32_t token, int32_t pos, l2b_kernel_ti
 
 /* Debug: with L2B_TRACE=1 in the environment at l2b_create time, every kernel of a step stamps
  * %globaltimer at fixed points (entry, ring filled, dependency wait done, activations staged,
- * first/last stage consumed, producer done, epilogue done).  Copies the last step's table
- * [launch][512 CTAs][8 slots] (ns) to dst.                                                  */
+ * first/last stage consumed, producer done, epilogue done: slots 0..7, ns); the TMA-ring GEMV
+ * also records the SM each CTA ran on (slot 8).  Copies the last step's table
+ * [launch][512 CTAs][16 slots] to dst.                                                      */
 int32_t l2b_debug_trace(l2b_ctx *ctx, unsigned long long *dst, uint64_t cap_words, uint64_t *n_words);
 
 /* Algorithmic bytes one step at position pos must read (SURVEY.md 8d):

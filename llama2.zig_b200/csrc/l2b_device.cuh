@@ -124,13 +124,14 @@ struct SpinGuard {
     __device__ __forceinline__ bool expired();
 };
 
-// Optional in-kernel timeline (L2B_TRACE=1): %globaltimer stamps per CTA, 8 slots per CTA.
+// Optional in-kernel timeline (L2B_TRACE=1): per CTA, %globaltimer stamps in slots 0..7 and, from
+// gemv_tma_kernel, the SM the CTA ran on in slot 8.
 __device__ __forceinline__ unsigned long long global_ns() {
     unsigned long long t;
     asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
     return t;
 }
-constexpr int TRACE_SLOTS = 8, TRACE_MAX_CTAS = 512;
+constexpr int TRACE_SLOTS = 16, TRACE_MAX_CTAS = 512;
 #define L2B_STAMP(tr, slot) do { if (tr) (tr)[(size_t)blockIdx.x * TRACE_SLOTS + (slot)] = global_ns(); } while (0)
 
 // ---------------------------------------------------------------------------------------
@@ -842,8 +843,11 @@ __device__ __forceinline__ void prefetch_l2_bulk(const void *p, uint32_t bytes) 
     asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(p), "r"(bytes) : "memory");
 }
 
-constexpr int TMA_MAX_STAGES = 6;                         // ring depth is a launch parameter (GemvParams::nstage)
+constexpr int PF_MAX_STAGES = 6;                          // prefill_gemm_kernel: stages of 8 rows (32 KB)
 constexpr int TMA_STAGE_FLOATS = GEMV8_R * NT * 4;        // 8 rows x 256 float4 = 32 KB
+constexpr int TMA_SLOT_ROWS = 4;                          // gemv_tma_kernel: slots of 4 rows (16 KB)
+constexpr int TMA_MAX_STAGES = 13;                        // gemv_tma_kernel ring depth (GemvParams::nstage): 13 x 16 KB
+                                                          // is the deepest ring a whole H100 SM holds next to a 16 KB x
 constexpr int TMA_THREADS = NT + 64;                       // 8 consumer warps + producer warp + epilogue warp
 
 __device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
@@ -860,39 +864,54 @@ __device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
 // rmsnorm prologue, the fixed-order warp-partial sum and the QKV pair store below are the one
 // implementation both use, so per (row, vector) a prefilled position is summed in the decode order.
 
-// One CTA's ring: rows [r0, r1) stream as `total` (tile, column step) stages of GEMV8_R rows x NT
-// float4 through the nstage slots of `ring`.  full[s]: slot s has landed (producer -> consumers);
-// empty[s]: all NWARP consumer warps are done with it.
+// One CTA's ring: rows [r0, r1) stream as `total` (tile, column step) steps of GEMV8_R rows x NT
+// float4; each step is SUB slots of SR rows, so `total * SUB` slots pass through the nstage slots of
+// `ring`.  full[s]: slot s has landed (producer -> consumers); empty[s]: all NWARP consumer warps are
+// done with it.  The slot size only sets how finely the ring's shared memory is cut: the consumers
+// read the same columns of the same rows in the same order whatever SR is.
+template <int SR>
 struct TmaRing {
+    static constexpr int SUB = GEMV8_R / SR;                           // slots per (tile, column step)
+    static constexpr int SLOT_FLOATS = SR * NT * 4;
+    static_assert(SR * SUB == GEMV8_R, "a tile is a whole number of slots");
     float *ring;
     uint64_t *full, *empty;
     int nstage, n4, nsteps, r0, r1, total;
 };
 
 // The producer warp's place in the stream.  produce_one is executed by all 32 lanes of the warp:
-// lane r issues row r's bulk copy of the next stage, lane 0 owns the barriers.
+// lane r owns row r of the tile and issues its bulk copy into the slot that holds it, lane 0 owns
+// the barriers.  A slot past the tile's last row (a CTA's last tile can be short) lands no bytes.
 struct RingProducer {
-    int it = 0, stage = 0, tile = 0, step = 0;
+    int it = 0, stage = 0, tile = 0, step = 0, sub = 0;
     uint32_t phase = 0;
     const float *row = nullptr;                                        // this lane's row in the current tile
 
-    template <int EPI>
-    __device__ __forceinline__ void produce_one(const GemvParams &p, const TmaRing &R, int lane) {
+    template <int EPI, int SR>
+    __device__ __forceinline__ void produce_one(const GemvParams &p, const TmaRing<SR> &R, int lane) {
         const int c0 = step * NT;                                      // first float4 column
         const int cols4 = min(NT, R.n4 - c0);
         const int v0 = R.r0 + tile * GEMV8_R;
         const int rows = min(GEMV8_R, R.r1 - v0);
-        if (step == 0 && lane < rows) row = gemv_row_ptr<EPI>(p, v0 + lane);
+        // whole-tile slots (SUB == 1) skip the slot arithmetic, so the 8-row stream compiles as it did
+        // before slots could be smaller than a tile
+        constexpr bool whole = R.SUB == 1;
+        const int lo = whole ? 0 : sub * SR;                           // the slot's first row of the tile
+        const int srows = whole ? rows : max(0, min(SR, rows - lo));
+        if (step == 0 && (whole || sub == 0) && lane < rows) row = gemv_row_ptr<EPI>(p, v0 + lane);
         if (lane == 0) {
             mbar_wait(&R.empty[stage], phase ^ 1);
-            mbar_expect_tx(&R.full[stage], (uint32_t)(rows * cols4 * 16));
+            mbar_expect_tx(&R.full[stage], (uint32_t)(srows * cols4 * 16));
         }
         __syncwarp();
-        if (lane < rows)
-            tma_load_1d(R.ring + (size_t)stage * TMA_STAGE_FLOATS + lane * NT * 4, row + (size_t)c0 * 4,
+        if ((whole || lane >= lo) && lane < lo + srows)
+            tma_load_1d(R.ring + (size_t)stage * R.SLOT_FLOATS + (lane - lo) * NT * 4, row + (size_t)c0 * 4,
                         (uint32_t)(cols4 * 16), &R.full[stage]);
         ++it;
-        if (++step == R.nsteps) { step = 0; ++tile; }
+        if (whole || ++sub == R.SUB) {
+            sub = 0;
+            if (++step == R.nsteps) { step = 0; ++tile; }
+        }
         if (++stage == R.nstage) { stage = 0; phase ^= 1; }
     }
 };
@@ -973,9 +992,9 @@ __device__ __forceinline__ void tma_rmsnorm(const GemvParams &p, float *xs, cons
 // Consumer warps 0..NWARP-1: acc[b][r] += w_r . x_b over this thread's float4 columns, stage by stage
 // (one LDS.128 of each x_b serves the tile's rows; vectors b >= nb read x_0 and are never stored).
 // At a tile's end the butterfly leaves the warp's row sums in red[t & 1] for the epilogue warp.
-// trace (decode only, else nullptr): the first stage's arrival (slot 4), the last one consumed (5).
-template <int NB>
-__device__ __forceinline__ void tma_consume(const TmaRing &R, const float *xs, int nb, TileRed<NB> &red,
+// trace (decode only, else nullptr): the first slot's arrival (slot 4), the last one consumed (5).
+template <int NB, int SR>
+__device__ __forceinline__ void tma_consume(const TmaRing<SR> &R, const float *xs, int nb, TileRed<NB> &red,
                                             uint64_t *tile_full, uint64_t *tile_free, unsigned long long *trace) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const float4 *xs4 = reinterpret_cast<const float4 *>(xs);
@@ -992,25 +1011,30 @@ __device__ __forceinline__ void tma_consume(const TmaRing &R, const float *xs, i
         const int c = st * NT + tid;
         const int v0 = R.r0 + t * GEMV8_R;
         const int rows = min(GEMV8_R, R.r1 - v0);
-        mbar_wait(&R.full[c_stage], c_phase);
-        if (it == 0 && tid == 0) L2B_STAMP(trace, 4);
-        if (c < R.n4) {
-            const float4 *w4 = reinterpret_cast<const float4 *>(R.ring + (size_t)c_stage * TMA_STAGE_FLOATS) + tid;
-            float4 xv[NB];
+        float4 xv[NB];                                        // one LDS.128 of each x_b serves the step's slots
 #pragma unroll
-            for (int b = 0; b < NB; ++b) xv[b] = xs4[(size_t)(b < nb ? b : 0) * R.n4 + c];
+        for (int s = 0; s < R.SUB; ++s) {
+            mbar_wait(&R.full[c_stage], c_phase);
+            if (it == 0 && s == 0 && tid == 0) L2B_STAMP(trace, 4);
+            if (c < R.n4) {
+                const float4 *w4 = reinterpret_cast<const float4 *>(R.ring + (size_t)c_stage * R.SLOT_FLOATS) + tid;
+                if (s == 0) {
 #pragma unroll
-            for (int r = 0; r < GEMV8_R; ++r) {
-                if (r < rows) {
-                    const float4 w = w4[r * NT];
+                    for (int b = 0; b < NB; ++b) xv[b] = xs4[(size_t)(b < nb ? b : 0) * R.n4 + c];
+                }
 #pragma unroll
-                    for (int b = 0; b < NB; ++b) acc[b][r] = dot4(w, xv[b], acc[b][r]);
+                for (int r = 0; r < SR; ++r) {
+                    if (s * SR + r < rows) {
+                        const float4 w = w4[r * NT];
+#pragma unroll
+                        for (int b = 0; b < NB; ++b) acc[b][s * SR + r] = dot4(w, xv[b], acc[b][s * SR + r]);
+                    }
                 }
             }
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&R.empty[c_stage]);  // this warp is done with the slot
+            if (++c_stage == R.nstage) { c_stage = 0; c_phase ^= 1; }
         }
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&R.empty[c_stage]);      // this warp is done with the stage
-        if (++c_stage == R.nstage) { c_stage = 0; c_phase ^= 1; }
         if (it == R.total - 1 && tid == 0) L2B_STAMP(trace, 5);
         if (st != R.nsteps - 1) continue;
 #pragma unroll
@@ -1034,8 +1058,7 @@ template <int EPI>
 __global__ void __launch_bounds__(TMA_THREADS, 2) gemv_tma_kernel(const GemvParams p) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int NSTAGE = p.nstage;
-    float *ring = reinterpret_cast<float *>(smem_raw);                 // NSTAGE x 32 KB
-    float *xs = ring + (size_t)NSTAGE * TMA_STAGE_FLOATS;              // n floats
+    float *ring = reinterpret_cast<float *>(smem_raw);                 // NSTAGE x 16 KB
     __shared__ uint64_t full[TMA_MAX_STAGES], empty[TMA_MAX_STAGES], xbar, tile_full[2], tile_free[2];
     __shared__ float scratch[1][NWARP + 2];
     __shared__ TileRed<1> red;
@@ -1047,10 +1070,17 @@ __global__ void __launch_bounds__(TMA_THREADS, 2) gemv_tma_kernel(const GemvPara
     const RowSplit split = cta_row_split(p.total_rows);
     const int r0 = split.r0, r1 = split.r1, ntiles = split.ntiles;
     const int total = ntiles * nsteps;
-    const TmaRing R = {ring, full, empty, NSTAGE, n4, nsteps, r0, r1, total};
+    const TmaRing<TMA_SLOT_ROWS> R = {ring, full, empty, NSTAGE, n4, nsteps, r0, r1, total};
+    const int nslots = total * R.SUB;
+    float *xs = ring + (size_t)NSTAGE * R.SLOT_FLOATS;                 // n floats
 
     if (tid == 0) {
         L2B_STAMP(p.trace, 0);
+        if (p.trace) {
+            unsigned int smid;
+            asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
+            p.trace[(size_t)blockIdx.x * TRACE_SLOTS + 8] = smid;      // where this CTA ran
+        }
         for (int s = 0; s < NSTAGE; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], NWARP); }
         mbar_init(&xbar, 1);
         for (int s = 0; s < 2; ++s) { mbar_init(&tile_full[s], NWARP); mbar_init(&tile_free[s], 1); }
@@ -1068,14 +1098,14 @@ __global__ void __launch_bounds__(TMA_THREADS, 2) gemv_tma_kernel(const GemvPara
         // Only nprefill stages go out before the wait: the activation vector's bulk copy is issued by
         // warp 0 right after the wait and is served behind everything this SM already requested
         // (~47 GB/s of HBM per SM: a full 192 KB ring ahead of it costs 4 us).
-        while (prod.it < total && prod.it < p.nprefill) prod.produce_one<EPI>(p, R, lane);
-        if (prod.it >= total) pdl_launch_dependents();
+        while (prod.it < nslots && prod.it < p.nprefill) prod.produce_one<EPI>(p, R, lane);
+        if (prod.it >= nslots) pdl_launch_dependents();
         if (lane == 0) L2B_STAMP(p.trace, 1);
         pdl_wait();
         if (!p.ctl[CTL_DONE]) {
-            while (prod.it < total) {
+            while (prod.it < nslots) {
                 prod.produce_one<EPI>(p, R, lane);
-                if (prod.it == total) pdl_launch_dependents();   // last stage in flight
+                if (prod.it == nslots) pdl_launch_dependents();  // last slot in flight
             }
             if (lane == 0) L2B_STAMP(p.trace, 6);
             return;
@@ -1094,7 +1124,7 @@ __global__ void __launch_bounds__(TMA_THREADS, 2) gemv_tma_kernel(const GemvPara
     if (p.ctl[CTL_DONE]) {
         // generation already ended: drain the bulk copies already aimed at our shared memory
         if (tid == 0)
-            for (int s = 0; s < p.nprefill && s < total; ++s) mbar_wait(&full[s], 0);
+            for (int s = 0; s < p.nprefill && s < nslots; ++s) mbar_wait(&full[s], 0);
         __syncthreads();
         return;
     }
@@ -1175,7 +1205,7 @@ __global__ void __launch_bounds__(TMA_THREADS, 2) gemv_tma_kernel(const GemvPara
         return;
     }
 
-    tma_consume<1>(R, xs, 1, red, tile_full, tile_free, p.trace);   // warps 0..7
+    tma_consume<1, TMA_SLOT_ROWS>(R, xs, 1, red, tile_full, tile_free, p.trace);   // warps 0..7
 }
 
 // ---- batched prompt prefill (SURVEY 8f.2): NB consecutive prompt positions share one pass over the
@@ -1202,7 +1232,7 @@ __global__ void __launch_bounds__(TMA_THREADS, 1) prefill_gemm_kernel(const Gemv
     const int NSTAGE = p.nstage;
     float *ring = reinterpret_cast<float *>(smem_raw);                 // NSTAGE x 32 KB
     float *xs = ring + (size_t)NSTAGE * TMA_STAGE_FLOATS;              // NB x n floats
-    __shared__ uint64_t full[TMA_MAX_STAGES], empty[TMA_MAX_STAGES], xbar, tile_full[2], tile_free[2];
+    __shared__ uint64_t full[PF_MAX_STAGES], empty[PF_MAX_STAGES], xbar, tile_full[2], tile_free[2];
     __shared__ float scratch[NB][NWARP + 2];
     __shared__ TileRed<NB> red;
     __shared__ float rope_s[NB][2][128];                               // cos/sin rows of pos_b[0 .. NB-1]
@@ -1213,7 +1243,7 @@ __global__ void __launch_bounds__(TMA_THREADS, 1) prefill_gemm_kernel(const Gemv
     const RowSplit split = cta_row_split(p.total_rows);
     const int r0 = split.r0, r1 = split.r1, ntiles = split.ntiles;
     const int total = ntiles * nsteps;
-    const TmaRing R = {ring, full, empty, NSTAGE, n4, nsteps, r0, r1, total};
+    const TmaRing<GEMV8_R> R = {ring, full, empty, NSTAGE, n4, nsteps, r0, r1, total};
 
     if (tid == 0) {
         for (int s = 0; s < NSTAGE; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], NWARP); }
@@ -1321,7 +1351,7 @@ __global__ void __launch_bounds__(TMA_THREADS, 1) prefill_gemm_kernel(const Gemv
         return;
     }
 
-    tma_consume<NB>(R, xs, p.nb, red, tile_full, tile_free, nullptr);   // warps 0..7
+    tma_consume<NB, GEMV8_R>(R, xs, p.nb, red, tile_full, tile_free, nullptr);   // warps 0..7
 }
 
 // Scalar fallback for shapes the vector kernel cannot take (n % 4 != 0 or unaligned rows):

@@ -171,7 +171,8 @@ struct l2b_ctx {
     bool attn_flash = true;                  // flash-decoding attention (false: 3-pass kernel)
     unsigned long long *trace = nullptr;     // L2B_TRACE=1: [launch][TRACE_MAX_CTAS][TRACE_SLOTS] timeline
     int trace_launches = 0;
-    int tma_ctas_per_sm = 1;
+    int tma_ctas_per_sm = 1;                 // ring CTAs one SM's shared memory is split for (L2B_TMA_CTAS)
+    size_t smem_per_sm = 0, smem_reserved = 0;   // shared memory per SM, and reserved by the system per block
     int tma_stages = 0;                      // 0 = auto; else forced ring depth
     int tma_prefill = 0;                     // stages in flight before the dependency wait; 0 = the whole ring (L2B_TMA_PREFILL)
     bool big_kernel_tma = true;              // bandwidth-bound GEMVs: TMA-ring kernel (false: register-fed 8-row kernel)
@@ -458,12 +459,27 @@ unsigned long long *trace_slot(l2b_ctx *ctx) {
     return ctx->trace + (size_t)(ctx->last_launches % ctx->trace_launches) * TRACE_MAX_CTAS * TRACE_SLOTS;
 }
 
-// TMA-ring stages (at most TMA_MAX_STAGES) that fit next to xbytes of activation vectors under a
+// Ring slots of slot_bytes (at most max_slots) that fit next to xbytes of activation vectors under a
 // dynamic shared-memory budget.  Compared before subtracting: (budget - xbytes) in unsigned
 // arithmetic wraps once xbytes exceeds the budget.
-int tma_ring_stages(size_t budget, size_t xbytes) {
-    const int n = xbytes < budget ? (int)((budget - xbytes) / ((size_t)TMA_STAGE_FLOATS * 4)) : 0;
-    return n < TMA_MAX_STAGES ? n : TMA_MAX_STAGES;
+int tma_ring_stages(size_t budget, size_t xbytes, size_t slot_bytes, int max_slots) {
+    const int n = xbytes < budget ? (int)((budget - xbytes) / slot_bytes) : 0;
+    return n < max_slots ? n : max_slots;
+}
+// the batched-prefill kernel's ring: stages of 8 rows (32 KB)
+int pf_ring_stages(size_t budget, size_t xbytes) {
+    return tma_ring_stages(budget, xbytes, (size_t)TMA_STAGE_FLOATS * 4, PF_MAX_STAGES);
+}
+
+// Depth of gemv_tma_kernel's ring next to xbytes of x when `ctas` ring CTAs are to share one SM:
+// each gets 1/ctas of the SM's shared memory, less the per-block reservation and its static
+// shared memory, so any two ring kernels sized for the same split fit on one SM together.
+int tma_ring_slots(const l2b_ctx *ctx, int ctas, size_t static_bytes, size_t xbytes) {
+    const size_t share = ctx->smem_per_sm / (size_t)ctas;
+    const size_t used = ctx->smem_reserved + static_bytes;
+    size_t budget = share > used ? share - used : 0;
+    if (budget > (size_t)kMaxSmemOptin) budget = kMaxSmemOptin;
+    return tma_ring_stages(budget, xbytes, (size_t)TmaRing<TMA_SLOT_ROWS>::SLOT_FLOATS * 4, TMA_MAX_STAGES);
 }
 
 int launch_gemv(l2b_ctx *ctx, int epi, const GemvParams &p, cudaStream_t st, const char *name = "gemv",
@@ -479,20 +495,31 @@ int launch_gemv(l2b_ctx *ctx, int epi, const GemvParams &p, cudaStream_t st, con
                (uint64_t)p.total_rows * p.n * 4ull >= (uint64_t)ctx->gemv8_min_bytes;
     if (ctx->force_kernel == 1) big = false;
     if (ctx->force_kernel >= 2) big = true;
-    // TMA-ring kernel: only x is staged in shared memory, the rest of the SM's 227 KB is the ring
-    // (measured: 5-6 stages of 32 KB on ONE CTA per SM beat 2 x 3 stages and beat leaving half
-    // the SM to the successor kernel's pre-fill)
-    const size_t stage_bytes = (size_t)TMA_STAGE_FLOATS * 4;
+    // TMA-ring kernel: only x is staged in shared memory, the rest of the CTA's share of the SM is a
+    // ring of 16 KB slots.  The grid has one ring CTA per SM; the ring is sized for tma_ctas_per_sm
+    // CTAs per SM (L2B_TMA_CTAS).  With 2, the free place is taken by the next kernel's CTA, which
+    // fills its own ring before its dependency wait while this one drains; but a half-SM ring keeps
+    // too few bytes in flight, and on llama2-7B the whole-SM ring (13 slots) is faster (measured on
+    // an H100 SXM at 700 W: DESIGN.md §4.1).  An x too wide for a ring of 2 slots in that share
+    // takes the whole SM.
+    const size_t slot_bytes = (size_t)TmaRing<TMA_SLOT_ROWS>::SLOT_FLOATS * 4;
     const size_t xonly = (size_t)p.n * 4;
-    int nstage = tma_ring_stages(kMaxSmemOptin, xonly);
+    gemv_fn tma_fn = gemv_tma_pick(epi);
+    int nstage = 0;
+    if (big && ctx->big_kernel_tma) {
+        cudaFuncAttributes fa{};
+        L2B_CUDA(ctx, cudaFuncGetAttributes(&fa, (const void *)tma_fn));
+        nstage = tma_ring_slots(ctx, ctx->tma_ctas_per_sm, fa.sharedSizeBytes, xonly);
+        if (nstage < 2) nstage = tma_ring_slots(ctx, 1, fa.sharedSizeBytes, xonly);
+    }
     if (ctx->tma_stages > 0) nstage = ctx->tma_stages < TMA_MAX_STAGES ? ctx->tma_stages : TMA_MAX_STAGES;
     const bool fused_ok = !p.gamma || p.n <= TMA_MAXV * TMA_PRO_THREADS * 4;   // register slices of the rmsnorm gain
     if (p.parts && big) return fail(ctx, L2B_ERR_UNSUPPORTED, "partial-vector prologue is only in the latency kernel");
     bool tma = big && ctx->big_kernel_tma && nstage >= 2 && fused_ok && p.head_size <= 256 &&
-               (size_t)nstage * stage_bytes + xonly <= (size_t)kMaxSmemOptin;
+               (size_t)nstage * slot_bytes + xonly <= (size_t)kMaxSmemOptin;
     if (ctx->force_kernel == 2) tma = false;
     if (ctx->force_kernel == 3 && !tma) return fail(ctx, L2B_ERR_UNSUPPORTED, "shape does not fit the TMA-ring kernel");
-    const size_t smem = tma ? (size_t)nstage * stage_bytes + xonly : xbytes;
+    const size_t smem = tma ? (size_t)nstage * slot_bytes + xonly : xbytes;
     if (smem > (size_t)kMaxSmemOptin) return fail(ctx, L2B_ERR_UNSUPPORTED, "activation vector too large for shared memory");
     // hard invariant of the ring kernel, whatever the budget arithmetic above decided
     if (tma && nstage < 2) return fail(ctx, L2B_ERR_UNSUPPORTED, "TMA ring of fewer than 2 stages");
@@ -502,7 +529,7 @@ int launch_gemv(l2b_ctx *ctx, int epi, const GemvParams &p, cudaStream_t st, con
     while (ctx->tpr_min_tiles_per_sm > 0 && tpr > 8 &&
            (p.total_rows + (NT / (tpr / 2)) * GEMV_R - 1) / ((NT / (tpr / 2)) * GEMV_R) >= ctx->tpr_min_tiles_per_sm * ctx->num_sms)
         tpr /= 2;
-    gemv_fn fn = tma ? gemv_tma_pick(epi) : big ? gemv8_pick(epi) : gemv_pick(epi, tpr);
+    gemv_fn fn = tma ? tma_fn : big ? gemv8_pick(epi) : gemv_pick(epi, tpr);
     if (!ctx->attr_done.count((const void *)fn)) {
         L2B_CUDA(ctx, cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmemOptin));
         ctx->attr_done.insert((const void *)fn);
@@ -511,7 +538,7 @@ int launch_gemv(l2b_ctx *ctx, int epi, const GemvParams &p, cudaStream_t st, con
     int occ = 0;
     L2B_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fn, threads, smem));
     if (occ < 1) occ = 1;
-    if (tma && occ > ctx->tma_ctas_per_sm) occ = ctx->tma_ctas_per_sm;   // leave room for the next kernel's CTA
+    if (tma) occ = 1;                        // one ring CTA per SM: the other places are the successor's
     int grid = ctx->num_sms * occ;
     if (big) {
         const int npairs = (p.total_rows + 1) / 2;
@@ -1039,6 +1066,16 @@ int preload_kernels(l2b_ctx *ctx) {
                             (const void *)sample_prep_batch_kernel, (const void *)logprob_kernel,
                             (const void *)logprob_batch_kernel, (const void *)synth_fill_kernel};
     for (const void *f : others) L2B_CUDA(ctx, cudaFuncGetAttributes(&fa, f));
+    // The kernels that run next to a TMA-ring GEMV in a decode step (the ring GEMVs, attention, the
+    // token advance) all ask for the largest shared-memory carveout, so consecutive kernels never
+    // need a different L1 / shared split to share an SM: a ring kernel's successor enters while it drains.
+    const void *decode[] = {(const void *)pick_attention(ctx->head_size, true, &smem), (const void *)attention_kernel,
+                            (const void *)advance_kernel};
+    for (const void *f : decode)
+        L2B_CUDA(ctx, cudaFuncSetAttribute(f, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+    for (int epi = 0; epi < EPI_COUNT; ++epi)
+        L2B_CUDA(ctx, cudaFuncSetAttribute((const void *)gemv_tma_pick(epi), cudaFuncAttributePreferredSharedMemoryCarveout,
+                                           cudaSharedmemCarveoutMaxShared));
     return L2B_OK;
 }
 
@@ -1051,6 +1088,8 @@ int init_rank(l2b_ctx *ctx, const l2b_config *cfg, int rank, int world, int devi
     ctx->cfg = *cfg;
     ctx->rank = rank; ctx->world = world; ctx->device = device;
     ctx->num_sms = prop.multiProcessorCount;
+    ctx->smem_per_sm = prop.sharedMemPerMultiprocessor;
+    ctx->smem_reserved = prop.reservedSharedMemPerBlock;
     ctx->dim = cfg->dim; ctx->hidden = cfg->hidden_dim;
     ctx->head_size = cfg->dim / cfg->n_heads;
     ctx->kv_mul = cfg->n_heads / cfg->n_kv_heads;
@@ -1741,8 +1780,8 @@ static int pf_prepare(l2b_ctx *ctx) {
                            dim <= TMA_MAXV * TMA_PRO_THREADS * 4 && ctx->gemv8_min_bytes >= 0 &&
                            dim * dim * 4 >= (uint64_t)ctx->gemv8_min_bytes && ctx->attn_flash &&
                            pick_attention(ctx->head_size, true, &smem) != attention_kernel &&
-                           tma_ring_stages(kPfSmemBudget, PF_MAXB * dim * 4) >= 2 &&
-                           tma_ring_stages(kPfSmemBudget, 2 * hid * 4) >= 2;
+                           pf_ring_stages(kPfSmemBudget, PF_MAXB * dim * 4) >= 2 &&
+                           pf_ring_stages(kPfSmemBudget, 2 * hid * 4) >= 2;
     if (!shapes_ok) return L2B_OK;
     L2B_CUDA(ctx, cudaSetDevice(ctx->device));
     int rc;
@@ -1768,7 +1807,7 @@ static int pf_prepare(l2b_ctx *ctx) {
 template <int NB>
 static int pf_launch(l2b_ctx *ctx, int epi, GemvParams p, cudaStream_t st) {
     const size_t xbytes = (size_t)NB * p.n * 4;
-    const int nstage = tma_ring_stages(kPfSmemBudget, xbytes);
+    const int nstage = pf_ring_stages(kPfSmemBudget, xbytes);
     p.nstage = nstage;
     int grid = ctx->num_sms;
     const int npairs = (p.total_rows + 1) / 2;
@@ -2626,6 +2665,8 @@ int32_t l2b_op_fused_matmul(int32_t device, float *xout, const float *x, const f
     cudaDeviceProp prop{};
     cudaGetDeviceProperties(&prop, device);
     tmp.num_sms = prop.multiProcessorCount;
+    tmp.smem_per_sm = prop.sharedMemPerMultiprocessor;
+    tmp.smem_reserved = prop.reservedSharedMemPerBlock;
     GemvParams p{};
     p.ctl = ctl; p.n = n; p.x_in = dx; p.gamma = dg; p.w0 = dw; p.total_rows = d; p.rows0 = d; p.out0 = dout;
     int rc = launch_gemv(&tmp, resid_inout ? EPI_RESID : EPI_STORE, p, 0);

@@ -18,7 +18,7 @@ lib.l2b_debug_trace.argtypes = [C.c_void_p, C.POINTER(C.c_uint64), C.c_uint64, C
 for pos in range(40):
     t.forward_argmax((1 + 7919 * pos) % ck.vocab_size, pos)
 n_launch = 5 * ck.n_layers + 4
-buf = np.zeros(n_launch * 512 * 8, dtype=np.uint64)
+buf = np.zeros(n_launch * 512 * 16, dtype=np.uint64)
 n = C.c_uint64()
 assert lib.l2b_debug_trace(t.h, buf.ctypes.data_as(C.POINTER(C.c_uint64)), buf.size, C.byref(n)) == 0
 st = buf[:ck.n_layers * 32].reshape(ck.n_layers, 32).astype(np.int64)
