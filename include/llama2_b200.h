@@ -251,6 +251,37 @@ int32_t l2b_forward_sample_batch(l2b_ctx *const *sessions, int32_t n, const int3
                                  const int32_t *pos, const float *temperature, const float *top_p,
                                  float *const *host_probs, l2b_prob_index *cand, int32_t cand_cap,
                                  int32_t *n_cand);
+/* Several positions of a session in one call: prompt chunks and decode steps of n distinct sessions
+ * share weight passes.  Session i runs its n_tokens[i] >= 1 tokens at positions pos0[i] ..
+ * pos0[i] + n_tokens[i] - 1; tokens holds every session's tokens back to back, in session order.
+ * Each session gets one output, for its LAST position: what l2b_forward_batch, _argmax_batch or
+ * _sample_batch returns for it (host_logits[i]; next[i]; probabilities, candidates and n_cand[i] under
+ * the sample batch call's rules).  n_tokens[i] == 1 is a decode step, a larger count a prompt chunk or
+ * a whole prompt; with every n_tokens[i] == 1 each call is its *_batch call.
+ * Where l2b_prefill shares weight passes, the positions of all runs, concatenated in session order, go
+ * 4 per pass (a run may straddle passes), each on its own session's cache at its own position, and
+ * the classifier runs on a pass only when it holds some run's last position.  A position's arithmetic
+ * does not depend on the others in its pass: a run's KV rows are those of l2b_prefill of the same
+ * tokens bit for bit, its output is that of l2b_prefill of all but its last token followed by
+ * l2b_forward_batch of the last one, and a prompt gives the same bits however it is cut into chunks.
+ * Elsewhere each session runs l2b_prefill of all but its last token (no logits) and then its own
+ * single step of the last one: bit for bit those calls.
+ * Checked before anything runs, so a refused call changes no session: everything l2b_forward_batch
+ * checks, plus NULL n_tokens or pos0, n_tokens[i] < 1, pos0[i] + n_tokens[i] > seq_len, a token out of
+ * range anywhere in a run and a total token count past INT32_MAX => L2B_ERR_INVALID_ARG; pos0[i] past
+ * the session's appended count => L2B_ERR_STATE; the sample call also makes l2b_forward_sample_batch's
+ * own checks.  Errors through l2b_last_error(sessions[0]); l2b_last_timing(sessions[0]) gives the whole
+ * call's device time and kernel launches.  Afterwards session i has max(its appended count, pos0[i] +
+ * n_tokens[i]) positions appended, and l2b_read_state returns the x and logits (or probabilities) of its
+ * last position; xb, hb and q are not defined.  Synchronous.                                   */
+int32_t l2b_forward_ragged(l2b_ctx *const *sessions, int32_t n, const int32_t *n_tokens,
+                           const int32_t *tokens, const int32_t *pos0, float *const *host_logits);
+int32_t l2b_forward_argmax_ragged(l2b_ctx *const *sessions, int32_t n, const int32_t *n_tokens,
+                                  const int32_t *tokens, const int32_t *pos0, int32_t *next);
+int32_t l2b_forward_sample_ragged(l2b_ctx *const *sessions, int32_t n, const int32_t *n_tokens,
+                                  const int32_t *tokens, const int32_t *pos0,
+                                  const float *temperature, const float *top_p, float *const *host_probs,
+                                  l2b_prob_index *cand, int32_t cand_cap, int32_t *n_cand);
 /* The greedy loop of l2b_generate_argmax on n sessions in one call, with no host round trip per
  * step.  For each i it does what l2b_generate_argmax(sessions[i], tokens[i], pos[i], n_steps,
  * forced + i*n_steps, stop_on_bos, out_next + i*n_steps, &n_done[i]) does: forced (may be NULL)

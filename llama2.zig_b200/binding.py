@@ -85,6 +85,10 @@ def load_library():
     lib.l2b_forward_argmax_batch.argtypes = [C.POINTER(vp), C.c_int32, IP, IP, IP]
     lib.l2b_forward_sample_batch.argtypes = [C.POINTER(vp), C.c_int32, IP, IP, FP, FP, C.POINTER(FP),
                                              C.POINTER(L2BProbIndex), C.c_int32, IP]
+    lib.l2b_forward_ragged.argtypes = [C.POINTER(vp), C.c_int32, IP, IP, IP, C.POINTER(FP)]
+    lib.l2b_forward_argmax_ragged.argtypes = [C.POINTER(vp), C.c_int32, IP, IP, IP, IP]
+    lib.l2b_forward_sample_ragged.argtypes = [C.POINTER(vp), C.c_int32, IP, IP, IP, FP, FP, C.POINTER(FP),
+                                              C.POINTER(L2BProbIndex), C.c_int32, IP]
     lib.l2b_generate_argmax_batch.argtypes = [C.POINTER(vp), C.c_int32, IP, IP, C.c_int32, IP, C.c_int32, IP, IP]
     lib.l2b_destroy.argtypes = [vp]
     lib.l2b_destroy.restype = None
@@ -372,6 +376,19 @@ def _batch_args(sessions, tokens, positions):
     return n, hs, toks, pos
 
 
+def _ragged_args(sessions, runs, pos0):
+    """(n, sessions, n_tokens, tokens back to back, pos0) of the ragged calls; runs[i] is session i's tokens."""
+    n = len(sessions)
+    assert len(runs) == n
+    hs = (C.c_void_p * max(n, 1))(*[s.h.value for s in sessions])
+    lens = np.array([len(r) for r in runs] or [0], dtype=np.int32)[:n]
+    flat = [int(t) for r in runs for t in r]
+    toks = np.array(flat or [0], dtype=np.int32)
+    pos = np.ascontiguousarray(pos0, dtype=np.int32)
+    assert pos.size == n
+    return n, hs, lens, toks, pos
+
+
 def forward_batch(sessions, tokens, positions):
     """transformer(tokens[i], positions[i]) on sessions[i] for every i (l2b_forward_batch); returns the
     (n, vocab) logits."""
@@ -392,6 +409,20 @@ def forward_argmax_batch(sessions, tokens, positions):
     return nxt[:n].copy()
 
 
+def _sample_out(n, vocab, cand_cap):
+    probs = np.empty((n, vocab), dtype=np.float32)
+    rows = (FP * max(n, 1))(*[probs[i].ctypes.data_as(FP) for i in range(n)])
+    cand = (L2BProbIndex * (max(n, 1) * max(cand_cap, 1)))()
+    n_cand = np.zeros(max(n, 1), dtype=np.int32)
+    return probs, rows, cand, n_cand
+
+
+def _sample_result(n, probs, cand, n_cand, cand_cap):
+    flat = np.frombuffer(cand, dtype=[("prob", "<f4"), ("index", "<i4")])
+    cands = [flat[i * cand_cap:i * cand_cap + n_cand[i]].copy() if n_cand[i] > 0 else None for i in range(n)]
+    return probs, cands, n_cand[:n].copy()
+
+
 def forward_sample_batch(sessions, tokens, positions, temperature, top_p, cand_cap=8192):
     """Session i's forward_sample(tokens[i], positions[i], temperature[i], top_p[i]) for every i, in one
     call (l2b_forward_sample_batch).  Returns (probs (n, vocab), candidates, n_cand): candidates[i] is
@@ -401,16 +432,50 @@ def forward_sample_batch(sessions, tokens, positions, temperature, top_p, cand_c
     temp = np.ascontiguousarray(temperature, dtype=np.float32)
     tp = np.ascontiguousarray(top_p, dtype=np.float32)
     assert temp.size == n and tp.size == n
-    probs = np.empty((n, sessions[0].ck.vocab_size if n else 0), dtype=np.float32)
-    rows = (FP * max(n, 1))(*[probs[i].ctypes.data_as(FP) for i in range(n)])
-    cand = (L2BProbIndex * (max(n, 1) * max(cand_cap, 1)))()
-    n_cand = np.zeros(max(n, 1), dtype=np.int32)
+    probs, rows, cand, n_cand = _sample_out(n, sessions[0].ck.vocab_size if n else 0, cand_cap)
     _check(load_library().l2b_forward_sample_batch(hs, n, toks.ctypes.data_as(IP), pos.ctypes.data_as(IP),
                                                    temp.ctypes.data_as(FP), tp.ctypes.data_as(FP), rows, cand,
                                                    cand_cap, n_cand.ctypes.data_as(IP)), hs[0] if n else None)
-    flat = np.frombuffer(cand, dtype=[("prob", "<f4"), ("index", "<i4")])
-    cands = [flat[i * cand_cap:i * cand_cap + n_cand[i]].copy() if n_cand[i] > 0 else None for i in range(n)]
-    return probs, cands, n_cand[:n].copy()
+    return _sample_result(n, probs, cand, n_cand, cand_cap)
+
+
+# ---- runs of several positions per session (prompt chunks next to decode steps) ------------------
+
+def forward_ragged(sessions, runs, pos0):
+    """Session i runs the tokens runs[i] at positions pos0[i] .. (l2b_forward_ragged): a decode step
+    (one token), a prompt chunk or a whole prompt.  Returns the (n, vocab) logits of each session's last
+    position, as forward_batch does for a step."""
+    n, hs, lens, toks, pos = _ragged_args(sessions, runs, pos0)
+    out = np.empty((n, sessions[0].ck.vocab_size if n else 0), dtype=np.float32)
+    rows = (FP * max(n, 1))(*[out[i].ctypes.data_as(FP) for i in range(n)])
+    _check(load_library().l2b_forward_ragged(hs, n, lens.ctypes.data_as(IP), toks.ctypes.data_as(IP),
+                                             pos.ctypes.data_as(IP), rows), hs[0] if n else None)
+    return out
+
+
+def forward_argmax_ragged(sessions, runs, pos0):
+    """forward_ragged with the device argmax (l2b_forward_argmax_ragged); returns the n next tokens."""
+    n, hs, lens, toks, pos = _ragged_args(sessions, runs, pos0)
+    nxt = np.empty(max(n, 1), dtype=np.int32)
+    _check(load_library().l2b_forward_argmax_ragged(hs, n, lens.ctypes.data_as(IP), toks.ctypes.data_as(IP),
+                                                    pos.ctypes.data_as(IP), nxt.ctypes.data_as(IP)),
+           hs[0] if n else None)
+    return nxt[:n].copy()
+
+
+def forward_sample_ragged(sessions, runs, pos0, temperature, top_p, cand_cap=8192):
+    """forward_ragged with l2b_forward_sample's device sampler preparation on each session's last position
+    (l2b_forward_sample_ragged).  Returns (probs, candidates, n_cand) as forward_sample_batch does."""
+    n, hs, lens, toks, pos = _ragged_args(sessions, runs, pos0)
+    temp = np.ascontiguousarray(temperature, dtype=np.float32)
+    tp = np.ascontiguousarray(top_p, dtype=np.float32)
+    assert temp.size == n and tp.size == n
+    probs, rows, cand, n_cand = _sample_out(n, sessions[0].ck.vocab_size if n else 0, cand_cap)
+    _check(load_library().l2b_forward_sample_ragged(hs, n, lens.ctypes.data_as(IP), toks.ctypes.data_as(IP),
+                                                    pos.ctypes.data_as(IP), temp.ctypes.data_as(FP),
+                                                    tp.ctypes.data_as(FP), rows, cand, cand_cap,
+                                                    n_cand.ctypes.data_as(IP)), hs[0] if n else None)
+    return _sample_result(n, probs, cand, n_cand, cand_cap)
 
 
 def generate_argmax_batch(sessions, tokens, positions, n_steps, forced=None, stop_on_bos=True):

@@ -1958,19 +1958,30 @@ static int launch_logprob_batch(l2b_ctx *ctx, int nb, int done) {
     return launch_small(ctx, (const void *)logprob_batch_kernel, dim3(nb), dim3(LOGPROB_THREADS), args, ctx->stream, true);
 }
 
-// Everything a batched step checks, before anything is launched: a refused call changes no session.
-static int check_batch_args(l2b_ctx *const *s, int32_t n, const int32_t *tokens, const int32_t *pos) {
+// Everything a batched call checks, before anything is launched: a refused call changes no session.
+// ragged: session i runs n_tok[i] tokens (tokens holds the runs back to back) at pos[i] ..; otherwise
+// one token each and n_tok is ignored.
+static int check_batch_args(l2b_ctx *const *s, int32_t n, const int32_t *tokens, const int32_t *pos,
+                            bool ragged = false, const int32_t *n_tok = nullptr) {
     if (!s || n < 1 || !s[0]) { g_create_error = "sessions is NULL, n < 1 or sessions[0] is NULL"; return L2B_ERR_INVALID_ARG; }
     l2b_ctx *s0 = s[0];
     if (!tokens || !pos) return fail(s0, L2B_ERR_INVALID_ARG, "tokens or pos is NULL");
+    if (ragged && !n_tok) return fail(s0, L2B_ERR_INVALID_ARG, "n_tokens is NULL");
     std::set<const l2b_ctx *> seen;
+    int64_t off = 0;                                     // the run's first entry in tokens
     for (int i = 0; i < n; ++i) {
         const l2b_ctx *c = s[i];
         if (!c) return fail(s0, L2B_ERR_INVALID_ARG, "NULL session");
         if (!seen.insert(c).second) return fail(s0, L2B_ERR_INVALID_ARG, "the same session twice in one batch");
         if (c->weights != s0->weights) return fail(s0, L2B_ERR_INVALID_ARG, "sessions of different models");
-        if (tokens[i] < 0 || tokens[i] >= c->cfg.vocab_size) return fail(s0, L2B_ERR_INVALID_ARG, "token out of range");
+        const int64_t len = ragged ? n_tok[i] : 1;
+        if (len < 1) return fail(s0, L2B_ERR_INVALID_ARG, "n_tokens < 1");
         if (pos[i] < 0 || pos[i] >= c->cfg.seq_len) return fail(s0, L2B_ERR_INVALID_ARG, "pos out of range");
+        if (pos[i] + len > c->cfg.seq_len) return fail(s0, L2B_ERR_INVALID_ARG, "run past seq_len");
+        if (off + len > INT32_MAX) return fail(s0, L2B_ERR_INVALID_ARG, "total token count overflows int32");
+        for (int64_t j = off; j < off + len; ++j)   // the run's tokens are read only once its length is known sound
+            if (tokens[j] < 0 || tokens[j] >= c->cfg.vocab_size) return fail(s0, L2B_ERR_INVALID_ARG, "token out of range");
+        off += len;
     }
     for (int i = 0; i < n; ++i)
         if (pos[i] > s[i]->n_appended) return fail(s0, L2B_ERR_STATE, "pos skips ahead of a session's KV cache");
@@ -1996,27 +2007,59 @@ static int launch_sample_prep_batch(l2b_ctx *ctx, l2b_ctx *const *s, int nb, con
     return launch_small(ctx, (const void *)sample_prep_batch_kernel, dim3(nb), dim3(SAMP_THREADS), args, ctx->stream, true);
 }
 
-// One step of each of n validated sessions.  Where l2b_prefill would batch (pf_prepare on the first
-// session), PF_MAXB sessions share each pass over the weights on the first session's stream and batch
-// buffers; each session's x and logits are then copied to its own buffers (xb, hb and q are not
-// written).  Otherwise each session runs its own step in turn.  mode: MODE_LOGITS leaves each session's
+// One run of each of n validated sessions: session i runs its n_tok[i] tokens (tokens holds the runs
+// back to back) at positions pos[i] .. pos[i] + n_tok[i] - 1; n_tok == nullptr: one token each (the
+// batched step).  Only a run's last position has an output.
+// Where l2b_prefill would batch (pf_prepare on the first session), the runs' positions, concatenated in
+// session order, go PF_MAXB per pass over the weights on the first session's stream and batch buffers,
+// each vector on its own session's cache at its own position (a run may straddle groups).  A group
+// holding some run's last vector then runs the batched classifier, and each such vector's x and logits
+// are copied to its session's own buffers (xb, hb and q are not written); a vector that ends no run
+// writes nothing into any session.  Otherwise each session runs l2b_prefill of its run but the last
+// token (no logits), and then its own step of the last token.  mode: MODE_LOGITS leaves each session's
 // logits in its h_logits, MODE_ARGMAX the next token in its h_ints[0], and MODE_SAMPLE (temperature[i],
 // top_p[i] < 0: no filter) its probabilities in h_logits, candidates in h_cand and their count in
 // h_ints[2], as l2b_forward_sample's step does.  The call's time and launches on s[0].
-static int step_sessions(l2b_ctx *const *s, int n, const int32_t *tokens, const int32_t *pos, StepMode mode,
-                         const float *temperature = nullptr, const float *top_p = nullptr) {
+static int step_sessions(l2b_ctx *const *s, int n, const int32_t *n_tok, const int32_t *tokens, const int32_t *pos,
+                         StepMode mode, const float *temperature = nullptr, const float *top_p = nullptr) {
     l2b_ctx *ctx = s[0];
     const bool argmax = (mode == MODE_ARGMAX), sample = (mode == MODE_SAMPLE);
     int rc = pf_prepare(ctx);
     if (rc) return rc;
+    // the vectors: vector v runs token tokens[v] at vpos[v] on session vs[v]; last[v]: the session it ends, or -1
+    int total = 0;
+    for (int i = 0; i < n; ++i) total += n_tok ? n_tok[i] : 1;
+    std::vector<l2b_ctx *> vs(total);
+    std::vector<int> vpos(total), last(total, -1);
+    for (int i = 0, v = 0; i < n; ++i)
+        for (int j = 0, len = n_tok ? n_tok[i] : 1; j < len; ++j, ++v) {
+            vs[v] = s[i];
+            vpos[v] = pos[i] + j;
+            if (j == len - 1) last[v] = i;
+        }
     cudaStream_t st = ctx->stream;
     L2B_CUDA(ctx, cudaSetDevice(ctx->device));
-    L2B_CUDA(ctx, cudaEventRecord(ctx->ev0, st));
     if (!ctx->pf_ok) {
+        // a run's leading tokens first, session by session; each prefill times itself on its session's events
+        float pre_ms = 0.0f;
         int launches = 0;
-        for (int i = 0; i < n; ++i) {
-            rc = sample ? run_step(s[i], tokens[i], pos[i], G_SAMPLE, temperature[i], top_p[i])
-                        : run_step(s[i], tokens[i], pos[i], argmax ? G_ARGMAX_ONE : G_LOGITS, 1.0f, 0.0f);
+        for (int v = 0, i = 0; v < total; ++v) {
+            if (last[v] < 0) continue;
+            const int len = n_tok ? n_tok[i] : 1;
+            if (len > 1) {
+                rc = l2b_prefill(s[i], tokens + v - (len - 1), len - 1, pos[i], nullptr);
+                if (rc) { ctx->err = s[i]->err; return rc; }
+                pre_ms += s[i]->last_ms;
+                launches += s[i]->last_launches;
+            }
+            ++i;
+        }
+        L2B_CUDA(ctx, cudaEventRecord(ctx->ev0, st));
+        for (int v = 0; v < total; ++v) {
+            const int i = last[v];
+            if (i < 0) continue;
+            rc = sample ? run_step(s[i], tokens[v], vpos[v], G_SAMPLE, temperature[i], top_p[i])
+                        : run_step(s[i], tokens[v], vpos[v], argmax ? G_ARGMAX_ONE : G_LOGITS, 1.0f, 0.0f);
             if (rc) { ctx->err = s[i]->err; return rc; }
             launches += s[i]->last_launches;
         }
@@ -2024,34 +2067,58 @@ static int step_sessions(l2b_ctx *const *s, int n, const int32_t *tokens, const 
         L2B_CUDA(ctx, cudaEventRecord(ctx->ev1, s[n - 1]->stream));
         L2B_CUDA(ctx, cudaEventSynchronize(ctx->ev1));
         L2B_CUDA(ctx, cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
+        ctx->last_ms += pre_ms;
         ctx->last_launches = launches;
         return L2B_OK;
     }
     const int dim = ctx->dim, V = ctx->cfg.vocab_size;
+    L2B_CUDA(ctx, cudaEventRecord(ctx->ev0, st));
     fill_ctl(ctx, tokens[0], pos[0], 0, 1.0f, -1.0f);        // DONE = 0 for the attention kernel
     L2B_CUDA(ctx, cudaMemcpyAsync(ctx->ctl, ctx->h_ctl, CTL_HOST_WORDS * sizeof(int), cudaMemcpyHostToDevice, st));
     ctx->last_launches = 0;
-    for (int g = 0; g < n; g += PF_MAXB) {
-        const int nb = n - g < PF_MAXB ? n - g : PF_MAXB;
+    for (int g = 0; g < total; g += PF_MAXB) {
+        const int nb = total - g < PF_MAXB ? total - g : PF_MAXB;
         // from the caller's (pageable) array: staged before the call returns, ordered after the previous group
         L2B_CUDA(ctx, cudaMemcpyAsync(ctx->pf_tokens, tokens + g, (size_t)nb * sizeof(int), cudaMemcpyHostToDevice, st));
-        rc = batched_layers(ctx, s + g, pos + g, nb, ctx->pf_tokens, nullptr);
+        rc = batched_layers(ctx, vs.data() + g, vpos.data() + g, nb, ctx->pf_tokens, nullptr);
         if (rc) return rc;
+        // the group's vectors that end a run: row[k] in the group, of session ends[k]
+        int row[PF_MAXB], nl = 0;
+        l2b_ctx *ends[PF_MAXB];
+        float lt[PF_MAXB], lp[PF_MAXB];
+        for (int b = 0; b < nb; ++b) {
+            const int i = last[g + b];
+            if (i < 0) continue;
+            row[nl] = b;
+            ends[nl] = s[i];
+            if (sample) { lt[nl] = temperature[i]; lp[nl] = top_p[i]; }
+            ++nl;
+        }
+        if (nl == 0) continue;
         if (argmax) L2B_CUDA(ctx, cudaMemsetAsync(ctx->pf_amax, 0, PF_MAXB * sizeof(unsigned long long), st));
         rc = batched_classifier(ctx, nb, argmax);
         if (rc) return rc;
-        if (sample) {   // logits -> probabilities in place, candidates to each session's own buffers
-            rc = launch_sample_prep_batch(ctx, s + g, nb, temperature + g, top_p + g);
+        if (sample) {
+            // the sampler works on the first nl rows: the last rows move to the front, in row order (row k
+            // receives row[k] >= k, so every row is read before a copy writes over it); then logits ->
+            // probabilities in place, candidates to each session's own buffers
+            for (int k = 0; k < nl; ++k)
+                if (row[k] != k)
+                    L2B_CUDA(ctx, cudaMemcpyAsync(ctx->pf_logits + (size_t)k * V, ctx->pf_logits + (size_t)row[k] * V,
+                                                  V * sizeof(float), cudaMemcpyDeviceToDevice, st));
+            rc = launch_sample_prep_batch(ctx, ends, nl, lt, lp);
             if (rc) return rc;
         }
-        for (int b = 0; b < nb; ++b) {
-            l2b_ctx *c = s[g + b];
+        for (int k = 0; k < nl; ++k) {
+            l2b_ctx *c = ends[k];
+            const int b = row[k];
+            const float *lg = ctx->pf_logits + (size_t)(sample ? k : b) * V;
             L2B_CUDA(ctx, cudaMemcpyAsync(c->X, ctx->pf_x + (size_t)b * dim, dim * sizeof(float), cudaMemcpyDeviceToDevice, st));
-            L2B_CUDA(ctx, cudaMemcpyAsync(c->logits, ctx->pf_logits + (size_t)b * V, V * sizeof(float), cudaMemcpyDeviceToDevice, st));
+            L2B_CUDA(ctx, cudaMemcpyAsync(c->logits, lg, V * sizeof(float), cudaMemcpyDeviceToDevice, st));
             if (argmax)   // the key's low word (little-endian: its first 4 bytes) is 0xFFFFFFFF - index
                 L2B_CUDA(ctx, cudaMemcpyAsync(c->h_ints, ctx->pf_amax + b, sizeof(int), cudaMemcpyDeviceToHost, st));
             else
-                L2B_CUDA(ctx, cudaMemcpyAsync(c->h_logits, ctx->pf_logits + (size_t)b * V, V * sizeof(float), cudaMemcpyDeviceToHost, st));
+                L2B_CUDA(ctx, cudaMemcpyAsync(c->h_logits, lg, V * sizeof(float), cudaMemcpyDeviceToHost, st));
             if (sample) {   // as the single step's G_SAMPLE graph copies them
                 L2B_CUDA(ctx, cudaMemcpyAsync(c->h_cand, c->cand, (size_t)kCandCap * sizeof(ProbIndex), cudaMemcpyDeviceToHost, st));
                 L2B_CUDA(ctx, cudaMemcpyAsync(c->h_ints + 2, c->n_cand, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -2064,9 +2131,10 @@ static int step_sessions(l2b_ctx *const *s, int n, const int32_t *tokens, const 
     L2B_CUDA(ctx, cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
     for (int i = 0; i < n; ++i) {
         l2b_ctx *c = s[i];
+        const int end = pos[i] + (n_tok ? n_tok[i] : 1);
         c->final_X = c->X;
         if (argmax) c->h_ints[0] = (int)(0xFFFFFFFFu - (uint32_t)c->h_ints[0]);
-        if (pos[i] + 1 > c->n_appended) c->n_appended = pos[i] + 1;
+        if (end > c->n_appended) c->n_appended = end;
     }
     return L2B_OK;
 }
@@ -2275,14 +2343,18 @@ int32_t l2b_score(l2b_ctx *ctx, const int32_t *tokens, int32_t n_tokens, int32_t
     return L2B_OK;
 }
 
-int32_t l2b_forward_batch(l2b_ctx *const *sessions, int32_t n, const int32_t *tokens, const int32_t *pos,
-                          float *const *host_logits) {
-    int rc = check_batch_args(sessions, n, tokens, pos);
+}  // extern "C"
+
+// The batch and ragged calls of one mode share their body: ragged == false is the batched step (one
+// token per session, n_tok ignored).
+static int forward_runs(l2b_ctx *const *sessions, int32_t n, bool ragged, const int32_t *n_tok, const int32_t *tokens,
+                        const int32_t *pos, float *const *host_logits) {
+    int rc = check_batch_args(sessions, n, tokens, pos, ragged, n_tok);
     if (rc) return rc;
     if (!host_logits) return fail(sessions[0], L2B_ERR_INVALID_ARG, "host_logits is NULL");
     for (int i = 0; i < n; ++i)
         if (!host_logits[i]) return fail(sessions[0], L2B_ERR_INVALID_ARG, "a host_logits entry is NULL");
-    rc = step_sessions(sessions, n, tokens, pos, MODE_LOGITS);
+    rc = step_sessions(sessions, n, ragged ? n_tok : nullptr, tokens, pos, MODE_LOGITS);
     if (rc) return rc;
     for (int i = 0; i < n; ++i)
         if (host_logits[i] != sessions[i]->h_logits)
@@ -2290,21 +2362,22 @@ int32_t l2b_forward_batch(l2b_ctx *const *sessions, int32_t n, const int32_t *to
     return L2B_OK;
 }
 
-int32_t l2b_forward_argmax_batch(l2b_ctx *const *sessions, int32_t n, const int32_t *tokens, const int32_t *pos,
-                                 int32_t *next) {
-    int rc = check_batch_args(sessions, n, tokens, pos);
+static int forward_argmax_runs(l2b_ctx *const *sessions, int32_t n, bool ragged, const int32_t *n_tok,
+                               const int32_t *tokens, const int32_t *pos, int32_t *next) {
+    int rc = check_batch_args(sessions, n, tokens, pos, ragged, n_tok);
     if (rc) return rc;
     if (!next) return fail(sessions[0], L2B_ERR_INVALID_ARG, "next is NULL");
-    rc = step_sessions(sessions, n, tokens, pos, MODE_ARGMAX);
+    rc = step_sessions(sessions, n, ragged ? n_tok : nullptr, tokens, pos, MODE_ARGMAX);
     if (rc) return rc;
     for (int i = 0; i < n; ++i) next[i] = sessions[i]->h_ints[0];
     return L2B_OK;
 }
 
-int32_t l2b_forward_sample_batch(l2b_ctx *const *sessions, int32_t n, const int32_t *tokens, const int32_t *pos,
-                                 const float *temperature, const float *top_p, float *const *host_probs,
-                                 l2b_prob_index *cand, int32_t cand_cap, int32_t *n_cand) {
-    int rc = check_batch_args(sessions, n, tokens, pos);
+static int forward_sample_runs(l2b_ctx *const *sessions, int32_t n, bool ragged, const int32_t *n_tok,
+                               const int32_t *tokens, const int32_t *pos, const float *temperature,
+                               const float *top_p, float *const *host_probs, l2b_prob_index *cand,
+                               int32_t cand_cap, int32_t *n_cand) {
+    int rc = check_batch_args(sessions, n, tokens, pos, ragged, n_tok);
     if (rc) return rc;
     l2b_ctx *s0 = sessions[0];
     if (!temperature || !top_p) return fail(s0, L2B_ERR_INVALID_ARG, "temperature or top_p is NULL");
@@ -2317,13 +2390,50 @@ int32_t l2b_forward_sample_batch(l2b_ctx *const *sessions, int32_t n, const int3
         if (filter && (!cand || !n_cand || cand_cap <= 0)) return fail(s0, L2B_ERR_INVALID_ARG, "candidate buffer missing");
         filter_p[i] = filter ? top_p[i] : -1.0f;
     }
-    rc = step_sessions(sessions, n, tokens, pos, MODE_SAMPLE, temperature, filter_p.data());
+    rc = step_sessions(sessions, n, ragged ? n_tok : nullptr, tokens, pos, MODE_SAMPLE, temperature, filter_p.data());
     if (rc) return rc;
     for (int i = 0; i < n; ++i)
         copy_sample_out(sessions[i], filter_p[i] >= 0.0f, host_probs ? host_probs[i] : nullptr,
                         cand && cand_cap > 0 ? cand + (size_t)i * cand_cap : nullptr, cand_cap,
                         n_cand ? n_cand + i : nullptr);
     return L2B_OK;
+}
+
+extern "C" {
+
+int32_t l2b_forward_batch(l2b_ctx *const *sessions, int32_t n, const int32_t *tokens, const int32_t *pos,
+                          float *const *host_logits) {
+    return forward_runs(sessions, n, false, nullptr, tokens, pos, host_logits);
+}
+
+int32_t l2b_forward_argmax_batch(l2b_ctx *const *sessions, int32_t n, const int32_t *tokens, const int32_t *pos,
+                                 int32_t *next) {
+    return forward_argmax_runs(sessions, n, false, nullptr, tokens, pos, next);
+}
+
+int32_t l2b_forward_sample_batch(l2b_ctx *const *sessions, int32_t n, const int32_t *tokens, const int32_t *pos,
+                                 const float *temperature, const float *top_p, float *const *host_probs,
+                                 l2b_prob_index *cand, int32_t cand_cap, int32_t *n_cand) {
+    return forward_sample_runs(sessions, n, false, nullptr, tokens, pos, temperature, top_p, host_probs, cand,
+                               cand_cap, n_cand);
+}
+
+int32_t l2b_forward_ragged(l2b_ctx *const *sessions, int32_t n, const int32_t *n_tokens, const int32_t *tokens,
+                           const int32_t *pos0, float *const *host_logits) {
+    return forward_runs(sessions, n, true, n_tokens, tokens, pos0, host_logits);
+}
+
+int32_t l2b_forward_argmax_ragged(l2b_ctx *const *sessions, int32_t n, const int32_t *n_tokens,
+                                  const int32_t *tokens, const int32_t *pos0, int32_t *next) {
+    return forward_argmax_runs(sessions, n, true, n_tokens, tokens, pos0, next);
+}
+
+int32_t l2b_forward_sample_ragged(l2b_ctx *const *sessions, int32_t n, const int32_t *n_tokens,
+                                  const int32_t *tokens, const int32_t *pos0, const float *temperature,
+                                  const float *top_p, float *const *host_probs, l2b_prob_index *cand,
+                                  int32_t cand_cap, int32_t *n_cand) {
+    return forward_sample_runs(sessions, n, true, n_tokens, tokens, pos0, temperature, top_p, host_probs, cand,
+                               cand_cap, n_cand);
 }
 
 // l2b_generate_argmax_batch where the batched step runs (pf_ok on s[0]): every step of every group of
