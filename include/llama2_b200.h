@@ -132,6 +132,23 @@ void l2b_destroy(l2b_ctx *ctx);
  * generation per process and has no such entry point; benches need it.                     */
 int32_t l2b_reset(l2b_ctx *ctx);
 
+/* Fork a shared prompt: copies rows [0, n_pos) of src's key cache and value cache, in every layer, into
+ * each of the n_dst distinct sessions dst[i] of the same model (l2b_create_session; the model's own
+ * context counts as one).  Afterwards each dst[i] has exactly n_pos positions appended, which may be fewer
+ * than it had: a fork replaces the destination's stream.  Its rows at n_pos and beyond are not written.
+ * The caller continues each destination with l2b_forward(dst[i], token, n_pos, ..) or any batch call at
+ * pos n_pos (the last prompt token is re-run, as after l2b_prefill without logits).  src is not changed:
+ * not its caches, its appended count, its x or its logits.  x, xb, hb, q and logits of the destinations
+ * are not defined afterwards.  One pass reads each source row once and writes it to up to 8 destinations.
+ * n_pos == 0 launches nothing and sets every destination's appended count to 0.
+ * Everything is checked before anything launches, so a refused call changes no session: NULL src or dst,
+ * n_dst < 1, a NULL entry, the same destination twice, src among the destinations, a destination of another
+ * model, or n_pos < 0 => L2B_ERR_INVALID_ARG; n_pos past src's appended count => L2B_ERR_STATE; a
+ * tensor-parallel src => L2B_ERR_UNSUPPORTED.  Errors are reported through l2b_last_error(src)
+ * (l2b_last_error(NULL) when src is NULL); l2b_last_timing(src) gives the call's device time and kernel
+ * launches.  Synchronous.                                                                    */
+int32_t l2b_fork(l2b_ctx *src, int32_t n_pos, l2b_ctx *const *dst, int32_t n_dst);
+
 /* ---- the hot path ------------------------------------------------------------------- */
 
 /* transformer(token, pos, ...) of src/main.zig:285-430.  On return host_logits[0..vocab)

@@ -90,6 +90,7 @@ def load_library():
     lib.l2b_forward_sample_ragged.argtypes = [C.POINTER(vp), C.c_int32, IP, IP, IP, FP, FP, C.POINTER(FP),
                                               C.POINTER(L2BProbIndex), C.c_int32, IP]
     lib.l2b_generate_argmax_batch.argtypes = [C.POINTER(vp), C.c_int32, IP, IP, C.c_int32, IP, C.c_int32, IP, IP]
+    lib.l2b_fork.argtypes = [vp, C.c_int32, C.POINTER(vp), C.c_int32]
     lib.l2b_destroy.argtypes = [vp]
     lib.l2b_destroy.restype = None
     lib.l2b_reset.argtypes = [vp]
@@ -496,6 +497,16 @@ def generate_argmax_batch(sessions, tokens, positions, n_steps, forced=None, sto
                                                     out.ctypes.data_as(IP), done.ctypes.data_as(IP)),
            hs[0] if n else None)
     return [out[i, :done[i]].copy() for i in range(n)]
+
+
+def fork(src, dsts, n_pos):
+    """Copy rows [0, n_pos) of src's key and value caches, in every layer, into each session of dsts
+    (l2b_fork): each then has exactly n_pos positions appended and continues at position n_pos.  src is
+    not changed.  l2b_last_timing(src) gives the copy's device time and launches."""
+    n = len(dsts)
+    hs = (C.c_void_p * max(n, 1))(*[d.h.value for d in dsts])
+    sh = src.h if src is not None else None
+    _check(load_library().l2b_fork(sh, int(n_pos), hs, n), sh)
 
 
 # ---- reference-named single ops on host buffers (device = cuda:0) ---------------------------

@@ -2227,6 +2227,38 @@ __global__ void __launch_bounds__(LOGPROB_THREADS) logprob_batch_kernel(const Lo
     }
 }
 
+// ---------------------------------------------------------------------------------------
+// Forking a session (l2b_fork): rows [0, n_pos) of the source's key and value caches, in every layer,
+// into up to KV_FORK_MAXD destinations of the same model.  A cache is (L, seq_len, kv_loc), so the
+// prefix of one layer of one cache is one contiguous segment of n_pos * kv_loc floats at offset
+// l * seq_len * kv_loc, the same in every session; kv_loc is a multiple of 4 (head_size is), so every
+// segment is float4-aligned.  Each source float4 is read once and stored nd times.  The fork is never
+// launched inside a step or a graph: no pdl_wait, no CTL_DONE.
+// ---------------------------------------------------------------------------------------
+constexpr int KV_FORK_MAXD = 8;
+struct KvForkParams {
+    const float *k, *v;                           // source key / value cache
+    float *dk[KV_FORK_MAXD], *dv[KV_FORK_MAXD];   // destinations [0, nd)
+    int nd;
+    long long seg;                                // floats per segment: n_pos * kv_loc
+    long long stride;                             // floats between layers: seq_len * kv_loc
+    int L;
+};
+__global__ void __launch_bounds__(NT) kv_fork_kernel(const KvForkParams p) {
+    const long long seg4 = p.seg >> 2;
+    for (int s = blockIdx.y; s < 2 * p.L; s += gridDim.y) {   // segments 0 .. L-1: keys, L .. 2L-1: values
+        const bool val = s >= p.L;
+        const size_t off = (size_t)(val ? s - p.L : s) * p.stride;
+        const float4 *src = reinterpret_cast<const float4 *>((val ? p.v : p.k) + off);
+        for (long long i = (long long)blockIdx.x * NT + threadIdx.x; i < seg4; i += (long long)gridDim.x * NT) {
+            const float4 x = __ldg(src + i);
+#pragma unroll
+            for (int d = 0; d < KV_FORK_MAXD; ++d)   // constant indices: the pointers stay in parameter space
+                if (d < p.nd) reinterpret_cast<float4 *>((val ? p.dv[d] : p.dk[d]) + off)[i] = x;
+        }
+    }
+}
+
 // standalone rmsnorm (unit-test surface; the hot path fuses it into the GEMV prologue)
 __global__ void __launch_bounds__(NT) rmsnorm_kernel(float *o, const float *x, const float *w, int n) {
     __shared__ float scratch[NWARP + 1];

@@ -1035,7 +1035,8 @@ int preload_kernels(l2b_ctx *ctx) {
                             (const void *)batch_advance_kernel, (const void *)gather_logits_kernel,
                             (const void *)resid_add_kernel, (const void *)sample_prep_kernel,
                             (const void *)sample_prep_batch_kernel, (const void *)logprob_kernel,
-                            (const void *)logprob_batch_kernel, (const void *)synth_fill_kernel};
+                            (const void *)logprob_batch_kernel, (const void *)synth_fill_kernel,
+                            (const void *)kv_fork_kernel};
     for (const void *f : others) L2B_CUDA(ctx, cudaFuncGetAttributes(&fa, f));
     // The kernels that run next to a TMA-ring GEMV in a decode step (the ring GEMVs, attention, the
     // token advance) all ask for the largest shared-memory carveout, so consecutive kernels never
@@ -1658,6 +1659,62 @@ void l2b_destroy(l2b_ctx *ctx) { destroy_all(ctx); }
 int32_t l2b_reset(l2b_ctx *ctx) {
     if (!ctx) return L2B_ERR_INVALID_ARG;
     ctx->n_appended = 0;
+    return L2B_OK;
+}
+
+// Rows [0, n_pos) of src's caches into every destination: kv_fork_kernel, KV_FORK_MAXD destinations per
+// launch, on src's stream.  Everything is checked before anything launches.
+int32_t l2b_fork(l2b_ctx *src, int32_t n_pos, l2b_ctx *const *dst, int32_t n_dst) {
+    if (!src) { g_create_error = "src is NULL"; return L2B_ERR_INVALID_ARG; }
+    if (!dst || n_dst < 1) return fail(src, L2B_ERR_INVALID_ARG, "dst is NULL or n_dst < 1");
+    if (src->world > 1) return fail(src, L2B_ERR_UNSUPPORTED, "l2b_fork needs a single-GPU model (sessions are single-GPU only)");
+    if (n_pos < 0) return fail(src, L2B_ERR_INVALID_ARG, "n_pos < 0");
+    std::set<const l2b_ctx *> seen;
+    for (int i = 0; i < n_dst; ++i) {
+        const l2b_ctx *d = dst[i];
+        if (!d) return fail(src, L2B_ERR_INVALID_ARG, "NULL destination");
+        if (d == src) return fail(src, L2B_ERR_INVALID_ARG, "src among the destinations");
+        if (!seen.insert(d).second) return fail(src, L2B_ERR_INVALID_ARG, "the same destination twice");
+        if (d->weights != src->weights) return fail(src, L2B_ERR_INVALID_ARG, "a destination of another model");
+    }
+    if (n_pos > src->n_appended) return fail(src, L2B_ERR_STATE, "n_pos past the positions src has appended");
+    src->last_ms = 0.0f;
+    src->last_launches = 0;
+    if (n_pos > 0) {
+        // No wait across streams: every call of this library ends in a synchronise, so neither src's
+        // stream nor any destination's holds work when l2b_fork is entered, and the copy is synchronised
+        // below before any destination can run again.
+        cudaStream_t st = src->stream;
+        L2B_CUDA(src, cudaSetDevice(src->device));
+        const int L = src->cfg.n_layers;
+        KvForkParams p{};
+        p.k = src->kcache;
+        p.v = src->vcache;
+        p.seg = (long long)n_pos * src->kv_loc;
+        p.stride = (long long)src->cfg.seq_len * src->kv_loc;
+        p.L = L;
+        // One float4 per thread: on llama2-7B this grid beat one resident wave of grid-striding CTAs (8 per
+        // SM) by 5-12 % at every n_pos and destination count measured, and cudaMemcpy at one destination
+        // (DESIGN.md §4.5g).
+        const int gy = std::min(2 * L, 65535);
+        const long long chunks = ((p.seg >> 2) + NT - 1) / NT;
+        const int gx = (int)std::min(chunks, (long long)INT32_MAX);
+        L2B_CUDA(src, cudaEventRecord(src->ev0, st));
+        for (int g = 0; g < n_dst; g += KV_FORK_MAXD) {
+            p.nd = std::min(KV_FORK_MAXD, n_dst - g);
+            for (int d = 0; d < p.nd; ++d) {
+                p.dk[d] = dst[g + d]->kcache;
+                p.dv[d] = dst[g + d]->vcache;
+            }
+            void *args[] = {&p};
+            const int rc = launch_small(src, (const void *)kv_fork_kernel, dim3(gx, gy), dim3(NT), args, st, false);
+            if (rc) return rc;
+        }
+        L2B_CUDA(src, cudaEventRecord(src->ev1, st));
+        L2B_CUDA(src, cudaEventSynchronize(src->ev1));
+        L2B_CUDA(src, cudaEventElapsedTime(&src->last_ms, src->ev0, src->ev1));
+    }
+    for (int i = 0; i < n_dst; ++i) dst[i]->n_appended = n_pos;
     return L2B_OK;
 }
 
