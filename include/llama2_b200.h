@@ -317,6 +317,54 @@ int32_t l2b_generate_argmax_batch(l2b_ctx *const *sessions, int32_t n, const int
                                   const int32_t *pos, int32_t n_steps, const int32_t *forced,
                                   int32_t stop_on_bos, int32_t *out_next, int32_t *n_done);
 
+/* ---- greedy speculative decoding ------------------------------------------------------ */
+
+/* Verifies guessed ("draft") tokens of n distinct sessions in shared weight passes.  The runs are laid out
+ * as in l2b_forward_argmax_ragged: run i is [t, d_1 .. d_m] at positions pos0[i] .., m = n_tokens[i] - 1,
+ * where t is the session's last emitted token and d_j are drafts; off_i is the run's first entry in tokens.
+ *   greedy   : the layout of tokens; greedy[off_i + j] is the argmax (first maximum wins, :715-726) at
+ *              position pos0[i] + j, for j <= n_accept[i].  Entries past that are not written.
+ *   n_accept : n_accept[i] is the largest a <= m such that for every j < a, d_{j+1} == greedy[off_i + j]
+ *              and, with stop_on_bos, greedy[off_i + j] != 1.  The session emits greedy[off_i .. off_i + a]:
+ *              a + 1 tokens, exactly those of l2b_generate_argmax_batch from (t, pos0[i]), whatever the drafts.
+ * Afterwards session i has exactly pos0[i] + n_accept[i] + 1 positions appended (which may be fewer than it
+ * had, as after l2b_fork); its KV rows below that equal the greedy loop's bit for bit, its rows past it are
+ * not defined, nor are x, xb, hb, q and logits.  Where l2b_forward_ragged shares weight passes the vectors go
+ * 4 per pass with the same kernels, and after each pass's classifier verify_accept_kernel decides the runs it
+ * holds; once every run is decided the passes still queued return at once.  Elsewhere each run is a device
+ * loop of single decode steps (every position runs).  With every n_tokens[i] == 1, greedy equals
+ * l2b_forward_argmax_batch's next bit for bit.  Checked before anything runs, so a refused call changes no
+ * session: everything l2b_forward_argmax_ragged checks, plus NULL greedy or n_accept => L2B_ERR_INVALID_ARG;
+ * a tensor-parallel model => L2B_ERR_UNSUPPORTED.  Errors through l2b_last_error(sessions[0]);
+ * l2b_last_timing(sessions[0]) gives the call's device time and kernel launches.  Synchronous.         */
+int32_t l2b_verify_argmax_ragged(l2b_ctx *const *sessions, int32_t n, const int32_t *n_tokens,
+                                 const int32_t *tokens, const int32_t *pos0, int32_t stop_on_bos,
+                                 int32_t *greedy, int32_t *n_accept);
+
+/* Most drafts one round of l2b_generate_speculative proposes.                                        */
+#define L2B_SPECULATIVE_MAX_K 32
+
+/* The greedy loop of l2b_generate_argmax on `target`, a round at a time: `draft` (another context or session
+ * with the same vocabulary, of any model) proposes kk = min(k, tokens still wanted - 1, seq_len - 1 - p)
+ * tokens with its own device loop, and one l2b_verify_argmax_ragged of one run checks them on the target,
+ * which emits the accepted ones and its own next token.  The tokens (out_next[0 .. *n_done)), *n_done and the
+ * target's KV rows [0, pos + *n_done) equal those of l2b_generate_argmax_batch(&target, 1, &token, &pos,
+ * n_steps, NULL, stop_on_bos, ..) bit for bit, for any draft; a BOS stop and the seq_len limit behave as
+ * there.  The draft is kept in step: after a round that rejected a draft its rows already hold the accepted
+ * tokens; after one that accepted all, its next loop starts one position earlier, forced through the
+ * stream.  Afterwards target and draft each have exactly pos + *n_done positions appended, holding the same
+ * tokens (one l2b_prefill of the draft when the last round accepted everything), so a second call from
+ * (out_next[*n_done - 1], pos + *n_done) continues the stream.  k == 0 verifies one position per round.
+ * *n_rounds (n_rounds may be NULL) is the number of rounds.  Checked before anything runs: NULL target,
+ * draft, out_next or n_done, target == draft, k outside [0, L2B_SPECULATIVE_MAX_K], n_steps < 0, a token or
+ * pos out of range, a different vocab_size or a draft seq_len below the target's => L2B_ERR_INVALID_ARG;
+ * pos past either context's appended count => L2B_ERR_STATE; a tensor-parallel target or draft =>
+ * L2B_ERR_UNSUPPORTED.  Errors through l2b_last_error(target); l2b_last_timing(target) covers the whole
+ * call, draft included.  x, xb, hb, q and logits of both are not defined afterwards.  Synchronous.     */
+int32_t l2b_generate_speculative(l2b_ctx *target, l2b_ctx *draft, int32_t token, int32_t pos,
+                                 int32_t n_steps, int32_t k, int32_t stop_on_bos, int32_t *out_next,
+                                 int32_t *n_done, int32_t *n_rounds);
+
 /* ---- introspection ------------------------------------------------------------------- */
 
 const char *l2b_last_error(const l2b_ctx *ctx);     /* never NULL                           */

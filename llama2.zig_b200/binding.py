@@ -91,6 +91,8 @@ def load_library():
                                               C.POINTER(L2BProbIndex), C.c_int32, IP]
     lib.l2b_generate_argmax_batch.argtypes = [C.POINTER(vp), C.c_int32, IP, IP, C.c_int32, IP, C.c_int32, IP, IP]
     lib.l2b_fork.argtypes = [vp, C.c_int32, C.POINTER(vp), C.c_int32]
+    lib.l2b_verify_argmax_ragged.argtypes = [C.POINTER(vp), C.c_int32, IP, IP, IP, C.c_int32, IP, IP]
+    lib.l2b_generate_speculative.argtypes = [vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, IP, IP, IP]
     lib.l2b_destroy.argtypes = [vp]
     lib.l2b_destroy.restype = None
     lib.l2b_reset.argtypes = [vp]
@@ -336,6 +338,18 @@ class Transformer:
                                             C.byref(done)), self.h)
         return out[:done.value].copy()
 
+    def generate_speculative(self, draft, token, pos, n_steps, k, stop_on_bos=True):
+        """generate_argmax with greedy speculative decoding (l2b_generate_speculative): `draft` (a context or
+        session with this vocabulary) proposes up to k tokens a round and one verify pass on this model keeps
+        the ones it agrees with.  The tokens are exactly generate_argmax's.  Returns (tokens, n_rounds);
+        afterwards this model and the draft both have pos + len(tokens) positions appended."""
+        out = np.full(max(int(n_steps), 1), -1, dtype=np.int32)
+        done, rounds = C.c_int32(), C.c_int32()
+        _check(self.lib.l2b_generate_speculative(self.h, draft.h if draft is not None else None, int(token),
+                                                 int(pos), int(n_steps), int(k), 1 if stop_on_bos else 0,
+                                                 out.ctypes.data_as(IP), C.byref(done), C.byref(rounds)), self.h)
+        return out[:done.value].copy(), rounds.value
+
     # -- introspection
     def state(self, name):
         n = C.c_uint64()
@@ -497,6 +511,22 @@ def generate_argmax_batch(sessions, tokens, positions, n_steps, forced=None, sto
                                                     out.ctypes.data_as(IP), done.ctypes.data_as(IP)),
            hs[0] if n else None)
     return [out[i, :done[i]].copy() for i in range(n)]
+
+
+def verify_argmax_ragged(sessions, runs, pos0, stop_on_bos=False):
+    """Greedy verify of draft tokens (l2b_verify_argmax_ragged): runs[i] = [t, d_1 .. d_m] is session i's last
+    emitted token and m drafts at positions pos0[i] ..  Returns (greedy_per_run, n_accept): greedy_per_run[i]
+    holds the n_accept[i] + 1 tokens session i emits (the accepted drafts, then the model's own next
+    token); session i then has pos0[i] + n_accept[i] + 1 positions appended."""
+    n, hs, lens, toks, pos = _ragged_args(sessions, runs, pos0)
+    greedy = np.full(max(toks.size, 1), -1, dtype=np.int32)
+    acc = np.zeros(max(n, 1), dtype=np.int32)
+    _check(load_library().l2b_verify_argmax_ragged(hs, n, lens.ctypes.data_as(IP), toks.ctypes.data_as(IP),
+                                                   pos.ctypes.data_as(IP), 1 if stop_on_bos else 0,
+                                                   greedy.ctypes.data_as(IP), acc.ctypes.data_as(IP)),
+           hs[0] if n else None)
+    offs = np.concatenate([[0], np.cumsum(lens[:n])]).astype(int)
+    return [greedy[offs[i]:offs[i] + acc[i] + 1].copy() for i in range(n)], acc[:n].copy()
 
 
 def fork(src, dsts, n_pos):

@@ -2018,6 +2018,44 @@ __global__ void batch_advance_kernel(const BatchAdvanceParams p) {
     p.tokens[i] = next;
 }
 
+// Acceptance of one group of a greedy verify (l2b_verify_argmax_ragged): the group's nb vectors are
+// consecutive entries v = g0 .. g0+nb-1 of the call's runs laid back to back, run i being [t, d_1 .. d_m]
+// at consecutive positions.  One thread walks them in order, so the result does not depend on any
+// schedule.  For each vector it turns the classifier's packed key into the greedy token, zeroes the key
+// (no memset between groups) and, while the vector's run is undecided, records the token and decides the
+// run at its last position, at BOS (stop_on_bos) or when the next draft differs: n_accept[i] = the
+// vector's index j in its run.  Once no run is undecided it raises CTL_DONE on sessions[0], so the groups
+// still queued return at once.
+struct VerifyAcceptParams {
+    int *ctl;                   // sessions[0]'s control block
+    unsigned long long *amax;   // [PF_MAXB] packed argmax keys of the group's classifier
+    const int *tokens;          // [total] the runs back to back: d_{j+1} of vector v is tokens[v + 1]
+    int *greedy;                // [total]
+    int *n_accept;              // [n] -1 while undecided
+    int *live;                  // runs still undecided
+    int g0, nb, stop_on_bos;
+    int run[PF_MAXB], j[PF_MAXB], last[PF_MAXB];   // vector b: its run, its index in it, that run's m
+};
+__global__ void verify_accept_kernel(const VerifyAcceptParams p) {
+    pdl_wait();
+    if (threadIdx.x != 0 || p.ctl[CTL_DONE]) return;
+#pragma unroll
+    for (int b = 0; b < PF_MAXB; ++b) {   // constant indices: the per-vector arrays stay in parameter space
+        if (b >= p.nb) break;
+        const unsigned long long key = p.amax[b];
+        p.amax[b] = 0ull;
+        const int tok = (int)(0xFFFFFFFFu - (unsigned int)(key & 0xFFFFFFFFull));
+        const int i = p.run[b];
+        if (p.n_accept[i] >= 0) continue;
+        const int v = p.g0 + b;
+        p.greedy[v] = tok;
+        if (p.j[b] == p.last[b] || (p.stop_on_bos && tok == 1) || p.tokens[v + 1] != tok) {
+            p.n_accept[i] = p.j[b];
+            if (--*p.live == 0) p.ctl[CTL_DONE] = 1;
+        }
+    }
+}
+
 // Tensor parallel logits: every rank's classifier sent its vocab slice as LL units (EPI_XCHG with
 // row_base = rank * vocab_loc); this kernel waits for all of them and writes the dense logits
 // vector the D2H copy (and the sampler) read.  No collective launch per token.

@@ -1036,7 +1036,7 @@ int preload_kernels(l2b_ctx *ctx) {
                             (const void *)resid_add_kernel, (const void *)sample_prep_kernel,
                             (const void *)sample_prep_batch_kernel, (const void *)logprob_kernel,
                             (const void *)logprob_batch_kernel, (const void *)synth_fill_kernel,
-                            (const void *)kv_fork_kernel};
+                            (const void *)kv_fork_kernel, (const void *)verify_accept_kernel};
     for (const void *f : others) L2B_CUDA(ctx, cudaFuncGetAttributes(&fa, f));
     // The kernels that run next to a TMA-ring GEMV in a decode step (the ring GEMVs, attention, the
     // token advance) all ask for the largest shared-memory carveout, so consecutive kernels never
@@ -2457,6 +2457,22 @@ int32_t l2b_forward_sample_ragged(l2b_ctx *const *sessions, int32_t n, const int
                                cand_cap, n_cand);
 }
 
+// The per-call device ints of the batched generation and verify calls (gb_ints on s[0]): at least `total`,
+// grown on demand; the current device is ctx's.
+static int gb_reserve(l2b_ctx *ctx, size_t total) {
+    if (ctx->gb_cap >= total) return L2B_OK;
+    if (ctx->gb_ints) {
+        L2B_CUDA(ctx, cudaFree(ctx->gb_ints));
+        ctx->owned.erase(std::find(ctx->owned.begin(), ctx->owned.end(), (void *)ctx->gb_ints));
+        ctx->gb_ints = nullptr;
+        ctx->gb_cap = 0;
+    }
+    const int rc = dev_alloc(ctx, &ctx->gb_ints, total);
+    if (rc) { cudaGetLastError(); return rc; }
+    ctx->gb_cap = total;
+    return L2B_OK;
+}
+
 // l2b_generate_argmax_batch where the batched step runs (pf_ok on s[0]): every step of every group of
 // PF_MAXB sessions is enqueued up front on s[0]'s stream, with no host synchronise until the end.  The
 // positions are launch arguments (pos[i] + step, held at seq_len - 1 once session i is past its limit);
@@ -2476,17 +2492,8 @@ static int generate_batched(l2b_ctx *const *s, int n, const int32_t *tokens, con
     const size_t o_tok = 0, o_done = (size_t)n, o_ndone = 2 * (size_t)n, o_lim = 3 * (size_t)n, o_live = 4 * (size_t)n;
     const size_t o_forced = o_live + 1, o_out = o_forced + (size_t)n * stride, total = o_out + (size_t)n * stride;
     L2B_CUDA(ctx, cudaSetDevice(ctx->device));
-    if (ctx->gb_cap < total) {
-        if (ctx->gb_ints) {
-            L2B_CUDA(ctx, cudaFree(ctx->gb_ints));
-            ctx->owned.erase(std::find(ctx->owned.begin(), ctx->owned.end(), (void *)ctx->gb_ints));
-            ctx->gb_ints = nullptr;
-            ctx->gb_cap = 0;
-        }
-        const int rc = dev_alloc(ctx, &ctx->gb_ints, total);
-        if (rc) { cudaGetLastError(); return rc; }
-        ctx->gb_cap = total;
-    }
+    const int rc0 = gb_reserve(ctx, total);
+    if (rc0) return rc0;
     std::vector<int> h(o_out, -1);
     for (int i = 0; i < n; ++i) {
         h[o_tok + i] = tokens[i];
@@ -2586,6 +2593,208 @@ int32_t l2b_generate_argmax_batch(l2b_ctx *const *sessions, int32_t n, const int
     if (rc) return rc;
     if (s0->pf_ok) return generate_batched(sessions, n, tokens, pos, n_steps, forced, limit.data(), stop_on_bos, out_next, n_done);
     return generate_each(sessions, n, tokens, pos, n_steps, forced, limit.data(), stop_on_bos, out_next, n_done);
+}
+
+// l2b_verify_argmax_ragged where the batched step runs (pf_ok on s[0]): the runs' vectors, back to back, go
+// PF_MAXB per pass over the weights as in step_sessions, each on its own session's cache at its own
+// position, and after each group's argmax classifier verify_accept_kernel decides the runs it holds.  Every
+// group is enqueued up front; once every run is decided (CTL_DONE on s[0]) the groups still queued return
+// at once.  The call's device ints (gb_ints): tokens [total], greedy [total], n_accept [n] (-1: undecided)
+// and the undecided count.
+static int verify_batched(l2b_ctx *const *s, int n, const int32_t *n_tok, const int32_t *tokens, const int32_t *pos,
+                          int stop_on_bos, int32_t *greedy, int32_t *n_accept) {
+    l2b_ctx *ctx = s[0];
+    int total = 0;
+    for (int i = 0; i < n; ++i) total += n_tok[i];
+    // vector v runs tokens[v] at vpos[v] on session vs[v]; it is entry vj[v] of run vrun[v]
+    std::vector<l2b_ctx *> vs(total);
+    std::vector<int> vpos(total), vrun(total), vj(total);
+    for (int i = 0, v = 0; i < n; ++i)
+        for (int j = 0; j < n_tok[i]; ++j, ++v) {
+            vs[v] = s[i];
+            vpos[v] = pos[i] + j;
+            vrun[v] = i;
+            vj[v] = j;
+        }
+    const size_t o_tok = 0, o_greedy = (size_t)total, o_acc = 2 * (size_t)total, o_live = o_acc + n, size = o_live + 1;
+    L2B_CUDA(ctx, cudaSetDevice(ctx->device));
+    int rc = gb_reserve(ctx, size);
+    if (rc) return rc;
+    std::vector<int> h(size, -1);
+    for (int v = 0; v < total; ++v) h[o_tok + v] = tokens[v];
+    h[o_live] = n;
+    int *d = ctx->gb_ints;
+    cudaStream_t st = ctx->stream;
+    L2B_CUDA(ctx, cudaMemcpyAsync(d, h.data(), size * sizeof(int), cudaMemcpyHostToDevice, st));
+    L2B_CUDA(ctx, cudaMemsetAsync(ctx->pf_amax, 0, PF_MAXB * sizeof(unsigned long long), st));
+    fill_ctl(ctx, tokens[0], pos[0], 0, 1.0f, -1.0f);        // DONE = 0 until the last run is decided
+    L2B_CUDA(ctx, cudaMemcpyAsync(ctx->ctl, ctx->h_ctl, CTL_HOST_WORDS * sizeof(int), cudaMemcpyHostToDevice, st));
+    L2B_CUDA(ctx, cudaEventRecord(ctx->ev0, st));
+    ctx->last_launches = 0;
+    VerifyAcceptParams a{};
+    a.ctl = ctx->ctl;
+    a.amax = ctx->pf_amax;
+    a.tokens = d + o_tok; a.greedy = d + o_greedy; a.n_accept = d + o_acc; a.live = d + o_live;
+    a.stop_on_bos = stop_on_bos ? 1 : 0;
+    for (int g = 0; g < total; g += PF_MAXB) {
+        const int nb = total - g < PF_MAXB ? total - g : PF_MAXB;
+        rc = batched_layers(ctx, vs.data() + g, vpos.data() + g, nb, d + o_tok + g, nullptr);
+        if (rc) return rc;
+        rc = batched_classifier(ctx, nb, true);
+        if (rc) return rc;
+        a.g0 = g;
+        a.nb = nb;
+        for (int b = 0; b < nb; ++b) {
+            a.run[b] = vrun[g + b];
+            a.j[b] = vj[g + b];
+            a.last[b] = n_tok[vrun[g + b]] - 1;
+        }
+        void *args[] = {&a};
+        rc = launch_small(ctx, (const void *)verify_accept_kernel, dim3(1), dim3(32), args, st, true);
+        if (rc) return rc;
+    }
+    std::vector<int> back((size_t)total + n);     // greedy [total], then n_accept [n]
+    L2B_CUDA(ctx, cudaMemcpyAsync(back.data(), d + o_greedy, back.size() * sizeof(int), cudaMemcpyDeviceToHost, st));
+    L2B_CUDA(ctx, cudaEventRecord(ctx->ev1, st));
+    L2B_CUDA(ctx, cudaStreamSynchronize(st));
+    L2B_CUDA(ctx, cudaGetLastError());
+    L2B_CUDA(ctx, cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
+    for (int i = 0, off = 0; i < n; off += n_tok[i], ++i) {
+        const int acc = back[(size_t)total + i];
+        if (acc < 0) return fail(ctx, L2B_ERR_STATE, "verify: a run was left undecided");
+        n_accept[i] = acc;
+        for (int j = 0; j <= acc; ++j) greedy[off + j] = back[off + j];
+    }
+    return L2B_OK;
+}
+
+// l2b_verify_argmax_ragged elsewhere: each run is l2b_score's device loop (G_SCORE_LOOP: the decode step
+// with the argmax classifier) on its own session and stream, forced through the run's drafts and, after
+// its last position, a placeholder that nothing reads as a token; the sessions' replays are interleaved,
+// one synchronise for all.  Every position runs; the acceptance is decided on the host from score_greedy.
+static int verify_each(l2b_ctx *const *s, int n, const int32_t *n_tok, const int32_t *tokens, const int32_t *pos,
+                       int stop_on_bos, int32_t *greedy, int32_t *n_accept) {
+    std::vector<std::vector<int32_t>> forced(n);
+    std::vector<DeviceLoop> loops;
+    for (int i = 0, off = 0; i < n; off += n_tok[i], ++i) {
+        forced[i].assign(tokens + off + 1, tokens + off + n_tok[i]);
+        forced[i].push_back(tokens[off]);
+        loops.push_back(DeviceLoop{s[i], tokens[off], pos[i], n_tok[i], forced[i].data(), true});
+    }
+    int rc = enqueue_device_loops(loops, G_SCORE_LOOP, 0);
+    if (rc) return rc;
+    rc = finish_device_loops(loops);
+    if (rc) return rc;
+    int launches = 0;
+    std::vector<int32_t> gr;
+    for (int i = 0, off = 0; i < n; off += n_tok[i], ++i) {
+        l2b_ctx *c = s[i];
+        launches += loops[i].launches;
+        if (loops[i].done != n_tok[i]) return fail(s[0], L2B_ERR_STATE, "verify stopped early");
+        gr.resize(n_tok[i]);
+        L2B_CUDA(s[0], cudaSetDevice(c->device));
+        L2B_CUDA(s[0], cudaMemcpy(gr.data(), c->score_greedy, gr.size() * sizeof(int32_t), cudaMemcpyDeviceToHost));
+        int acc = 0;
+        while (acc < n_tok[i] - 1 && !(stop_on_bos && gr[acc] == 1) && tokens[off + acc + 1] == gr[acc]) ++acc;
+        n_accept[i] = acc;
+        for (int j = 0; j <= acc; ++j) greedy[off + j] = gr[j];
+    }
+    s[0]->last_launches = launches;
+    return L2B_OK;
+}
+
+int32_t l2b_verify_argmax_ragged(l2b_ctx *const *sessions, int32_t n, const int32_t *n_tokens, const int32_t *tokens,
+                                 const int32_t *pos0, int32_t stop_on_bos, int32_t *greedy, int32_t *n_accept) {
+    int rc = check_batch_args(sessions, n, tokens, pos0, true, n_tokens);
+    if (rc) return rc;
+    l2b_ctx *s0 = sessions[0];
+    if (!greedy || !n_accept) return fail(s0, L2B_ERR_INVALID_ARG, "greedy or n_accept is NULL");
+    if (s0->world > 1) return fail(s0, L2B_ERR_UNSUPPORTED, "l2b_verify_argmax_ragged needs a single-GPU model");
+    rc = pf_prepare(s0);
+    if (rc) return rc;
+    rc = s0->pf_ok ? verify_batched(sessions, n, n_tokens, tokens, pos0, stop_on_bos, greedy, n_accept)
+                   : verify_each(sessions, n, n_tokens, tokens, pos0, stop_on_bos, greedy, n_accept);
+    if (rc) return rc;
+    for (int i = 0; i < n; ++i) sessions[i]->n_appended = pos0[i] + n_accept[i] + 1;
+    return L2B_OK;
+}
+
+// Greedy speculative decoding: rounds of (the draft's device loop proposes kk tokens, one verify of
+// [token, d_1 .. d_kk] on the target).  dp counts the stream positions the draft holds rows for: after a
+// round that accepted a < kk drafts the draft's rows up to p + a hold the stream, after one that accepted
+// all it never ran d_kk, and after a round without proposals it did not run at all.  The next draft loop
+// starts at dp and is forced through the stream up to the target's token (the catch-up), then runs free.
+int32_t l2b_generate_speculative(l2b_ctx *target, l2b_ctx *draft, int32_t token, int32_t pos, int32_t n_steps,
+                                 int32_t k, int32_t stop_on_bos, int32_t *out_next, int32_t *n_done,
+                                 int32_t *n_rounds) {
+    if (!target) { g_create_error = "target is NULL"; return L2B_ERR_INVALID_ARG; }
+    if (!draft || !out_next || !n_done) return fail(target, L2B_ERR_INVALID_ARG, "draft, out_next or n_done is NULL");
+    if (draft == target) return fail(target, L2B_ERR_INVALID_ARG, "the draft is the target");
+    if (k < 0 || k > L2B_SPECULATIVE_MAX_K) return fail(target, L2B_ERR_INVALID_ARG, "k outside [0, L2B_SPECULATIVE_MAX_K]");
+    if (n_steps < 0) return fail(target, L2B_ERR_INVALID_ARG, "n_steps < 0");
+    const int S = target->cfg.seq_len;
+    if (token < 0 || token >= target->cfg.vocab_size) return fail(target, L2B_ERR_INVALID_ARG, "token out of range");
+    if (pos < 0 || pos >= S) return fail(target, L2B_ERR_INVALID_ARG, "pos out of range");
+    if (draft->cfg.vocab_size != target->cfg.vocab_size) return fail(target, L2B_ERR_INVALID_ARG, "the draft has another vocabulary size");
+    if (draft->cfg.seq_len < S) return fail(target, L2B_ERR_INVALID_ARG, "the draft's seq_len is below the target's");
+    if (target->world > 1 || draft->world > 1)
+        return fail(target, L2B_ERR_UNSUPPORTED, "l2b_generate_speculative needs single-GPU target and draft");
+    if (pos > target->n_appended || pos > draft->n_appended)
+        return fail(target, L2B_ERR_STATE, "pos skips ahead of the target's or the draft's KV cache");
+    if (n_steps > S - pos) n_steps = S - pos;                 // :992-993
+    float ms = 0.0f;
+    int launches = 0, rounds = 0, done = 0;
+    std::vector<int32_t> hist(1, token);   // hist[q - pos]: the stream's token at position q
+    std::vector<int32_t> run, forced, out(S), gr(L2B_SPECULATIVE_MAX_K + 1);
+    int p = pos, dp = pos;                 // the target's next position; the stream positions the draft holds
+    bool stopped = false;
+    while (done < n_steps && !stopped) {
+        int kk = k < n_steps - done - 1 ? k : n_steps - done - 1;
+        if (kk > S - 1 - p) kk = S - 1 - p;
+        run.assign(1, hist[p - pos]);
+        if (kk > 0) {
+            const int lag = p - dp;        // forced through the stream tokens at dp + 1 .. p, then free
+            forced.assign(hist.begin() + (dp - pos) + 1, hist.end());
+            forced.resize((size_t)lag + kk, -1);
+            int nd = 0;
+            int rc = l2b_generate_argmax(draft, hist[dp - pos], dp, lag + kk, forced.data(), 0, out.data(), &nd);
+            if (rc) return fail(target, rc, draft->err.c_str());
+            if (nd != lag + kk) return fail(target, L2B_ERR_STATE, "the draft loop stopped early");
+            ms += draft->last_ms;
+            launches += draft->last_launches;
+            run.insert(run.end(), out.begin() + lag, out.begin() + lag + kk);
+        }
+        const int32_t nt = kk + 1;
+        int32_t acc = 0;
+        int rc = l2b_verify_argmax_ragged(&target, 1, &nt, run.data(), &p, stop_on_bos, gr.data(), &acc);
+        if (rc) return rc;
+        ms += target->last_ms;
+        launches += target->last_launches;
+        ++rounds;
+        const int emit = acc + 1 < n_steps - done ? acc + 1 : n_steps - done;
+        for (int j = 0; j < emit; ++j) {
+            out_next[done + j] = gr[j];
+            hist.push_back(gr[j]);
+        }
+        if (kk > 0) dp = p + (acc + 1 < kk ? acc + 1 : kk);
+        done += emit;
+        p += emit;
+        stopped = stop_on_bos && gr[emit - 1] == 1;
+    }
+    const int end = pos + done;
+    if (dp < end) {                        // the draft's missing rows of the stream: one prefill
+        const int rc = l2b_prefill(draft, hist.data() + (dp - pos), end - dp, dp, nullptr);
+        if (rc) return fail(target, rc, draft->err.c_str());
+        ms += draft->last_ms;
+        launches += draft->last_launches;
+    }
+    target->n_appended = end;
+    draft->n_appended = end;
+    target->last_ms = ms;
+    target->last_launches = launches;
+    *n_done = done;
+    if (n_rounds) *n_rounds = rounds;
+    return L2B_OK;
 }
 
 int32_t l2b_read_state(l2b_ctx *ctx, int32_t which, float *dst, uint64_t n, uint64_t *n_out) {
