@@ -184,6 +184,9 @@ __device__ __forceinline__ unsigned long long argmax_key(float v, int idx) {
     u = (u & 0x80000000u) ? ~u : (u | 0x80000000u);
     return (static_cast<unsigned long long>(u) << 32) | (0xFFFFFFFFu - static_cast<uint32_t>(idx));
 }
+__device__ __forceinline__ int argmax_key_index(unsigned long long key) {
+    return (int)(0xFFFFFFFFu - (unsigned int)(key & 0xFFFFFFFFull));
+}
 
 // ---------------------------------------------------------------------------------------
 // Step control block (device memory, 16 ints):
@@ -1968,7 +1971,7 @@ __global__ void advance_kernel(const AdvanceParams p) {
     }
     if (tid != 0) return;
     const int step = ctl[CTL_STEP];
-    int next = (int)(0xFFFFFFFFu - (unsigned int)(key & 0xFFFFFFFFull));
+    int next = argmax_key_index(key);
     if (p.forced && p.forced[step] >= 0) next = p.forced[step];
     p.out_next[step] = next;
     *p.n_done = step + 1;
@@ -2006,7 +2009,7 @@ __global__ void batch_advance_kernel(const BatchAdvanceParams p) {
     const int i = p.g0 + b;
     if (p.done[i]) return;
     const size_t at = (size_t)i * p.stride + p.step;
-    int next = (int)(0xFFFFFFFFu - (unsigned int)(key & 0xFFFFFFFFull));
+    int next = argmax_key_index(key);
     if (p.forced && p.forced[at] >= 0) next = p.forced[at];
     p.out_next[at] = next;
     p.n_done[i] = p.step + 1;
@@ -2044,7 +2047,7 @@ __global__ void verify_accept_kernel(const VerifyAcceptParams p) {
         if (b >= p.nb) break;
         const unsigned long long key = p.amax[b];
         p.amax[b] = 0ull;
-        const int tok = (int)(0xFFFFFFFFu - (unsigned int)(key & 0xFFFFFFFFull));
+        const int tok = argmax_key_index(key);
         const int i = p.run[b];
         if (p.n_accept[i] >= 0) continue;
         const int v = p.g0 + b;
@@ -2222,9 +2225,6 @@ __device__ __forceinline__ float logprob_row(const float *logits, int n, int tar
     __syncthreads();
     s = warp_sum(red[lane]);
     return (logits[target] - m) - logf(s);
-}
-__device__ __forceinline__ int argmax_key_index(unsigned long long key) {
-    return (int)(0xFFFFFFFFu - (unsigned int)(key & 0xFFFFFFFFull));
 }
 
 // One step of the score loop (G_SCORE_LOOP): the target is the step's forced token, the greedy token the

@@ -123,10 +123,9 @@ struct l2b_ctx {
     unsigned long long *pf_amax = nullptr;                                       // [PF_MAXB] packed argmax keys
     float *pf_part_o = nullptr, *pf_part_ml = nullptr;
     unsigned int *pf_counters = nullptr;
-    int *pf_tokens = nullptr;
     bool pf_ready = false, pf_ok = false;
-    int *gb_ints = nullptr;                  // l2b_generate_argmax_batch on the batched path: its per-call
-    size_t gb_cap = 0;                       // session and token arrays (ints), grown on demand
+    int *call_ints = nullptr;                // a batched call's tokens and other per-call ints (batched_begin),
+    size_t call_ints_cap = 0;                // grown on demand
     float *delta = nullptr;                  // L2B_TP=nccl baseline only: partial rows before the NCCL all-reduce
     float *q = nullptr, *xb = nullptr, *hb = nullptr, *logits = nullptr, *logits_loc = nullptr;
     float *kcache = nullptr, *vcache = nullptr;     // (L, seq_len, kv_loc)
@@ -1501,10 +1500,14 @@ void fill_ctl(l2b_ctx *ctx, int token, int pos, int stop_on_bos, float temperatu
     memcpy(&h[CTL_TOPP], &top_p, sizeof(float));
 }
 
-int finish_call(l2b_ctx *lead, const std::vector<l2b_ctx *> &ranks) {
+// one synchronise of each rank's stream (ranks[0] is the lead, which keeps the error); with one rank
+// the current device is already its own
+int finish_call(l2b_ctx *const *ranks, size_t n) {
+    l2b_ctx *lead = ranks[0];
     int rc = L2B_OK;
-    for (l2b_ctx *c : ranks) {
-        cudaSetDevice(c->device);
+    for (size_t i = 0; i < n; ++i) {
+        l2b_ctx *c = ranks[i];
+        if (n > 1) cudaSetDevice(c->device);
         cudaError_t e = cudaStreamSynchronize(c->stream);
         if (e != cudaSuccess && rc == L2B_OK) {
             lead->err = std::string("step failed: ") + cudaGetErrorString(e);
@@ -1540,20 +1543,7 @@ int run_step(l2b_ctx *lead, int token, int pos, int which, float temperature, fl
         }
         if (ctx == lead && lead->time_steps) L2B_CUDA(lead, cudaEventRecord(ctx->ev1, ctx->stream));
     }
-    int rc = L2B_OK;
-    for (size_t i = 0; i < nranks; ++i) {
-        l2b_ctx *c = ranks[i];
-        if (nranks > 1) cudaSetDevice(c->device);
-        cudaError_t e = cudaStreamSynchronize(c->stream);
-        if (e != cudaSuccess && rc == L2B_OK) {
-            lead->err = std::string("step failed: ") + cudaGetErrorString(e);
-            rc = L2B_ERR_CUDA;
-        }
-        if (c->h_ctl[CTL_WORDS + CTL_ERR] && rc == L2B_OK) {
-            lead->err = "tensor-parallel exchange timed out: a peer rank died or fell out of lockstep";
-            rc = L2B_ERR_COMM;
-        }
-    }
+    int rc = finish_call(ranks, nranks);
     if (rc) return rc;
     if (lead->time_steps) {
         if (nranks > 1) L2B_CUDA(lead, cudaSetDevice(lead->device));
@@ -1815,7 +1805,6 @@ static int pf_prepare(l2b_ctx *ctx) {
     if ((rc = dev_alloc(ctx, &ctx->pf_part_o, (size_t)PF_MAXB * ctx->heads_loc * ctx->nsplit * ctx->head_size))) return rc;
     if ((rc = dev_alloc(ctx, &ctx->pf_part_ml, (size_t)PF_MAXB * ctx->heads_loc * ctx->nsplit * 2))) return rc;
     if ((rc = dev_alloc(ctx, &ctx->pf_counters, (size_t)PF_MAXB * ctx->heads_loc))) return rc;
-    if ((rc = dev_alloc(ctx, &ctx->pf_tokens, (size_t)ctx->cfg.seq_len))) return rc;
     L2B_CUDA(ctx, cudaMemsetAsync(ctx->pf_counters, 0, (size_t)PF_MAXB * ctx->heads_loc * sizeof(unsigned int), ctx->stream));
     for (int epi : {(int)EPI_QKV, (int)EPI_SILU, (int)EPI_RESID, (int)EPI_STORE, (int)EPI_ARGMAX}) {
         L2B_CUDA(ctx, cudaFuncSetAttribute(pf_pick<PF_MAXB>(epi), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPfSmemBudget));
@@ -1909,29 +1898,80 @@ static int batched_layers(l2b_ctx *ctx, l2b_ctx *const *kv, const int *pos, int 
 static int batched_classifier(l2b_ctx *ctx, int nb, bool argmax);
 static int launch_logprob_batch(l2b_ctx *ctx, int nb, int done);
 
-// n_tokens positions starting at pos0, PF_MAXB per pass over the weights; KV cache filled.  Without
-// score no logits; with score (l2b_score: tokens holds n_tokens + 1 entries) each group then runs the
-// argmax classifier and logprob_batch_kernel, which leaves position i's log-probability of tokens[i + 1]
-// and its greedy token in score_lp[i] and score_greedy[i].
-static int prefill_batched(l2b_ctx *ctx, const int32_t *tokens, int n_tokens, int pos0, bool score = false) {
-    cudaStream_t st = ctx->stream;
-    L2B_CUDA(ctx, cudaSetDevice(ctx->device));
-    for (int i = 0; i < n_tokens; ++i) ctx->h_gen[i] = tokens[i];
-    L2B_CUDA(ctx, cudaMemcpyAsync(ctx->pf_tokens, ctx->h_gen, (size_t)n_tokens * sizeof(int), cudaMemcpyHostToDevice, st));
-    if (score) {   // the targets, from the caller's (pageable) array: staged before the call returns
-        L2B_CUDA(ctx, cudaMemcpyAsync(ctx->gen_forced, tokens + 1, (size_t)n_tokens * sizeof(int), cudaMemcpyHostToDevice, st));
-        L2B_CUDA(ctx, cudaMemsetAsync(ctx->pf_amax, 0, PF_MAXB * sizeof(unsigned long long), st));
+// ctx->call_ints: at least `count` ints, grown on demand; the current device is ctx's
+static int call_ints_reserve(l2b_ctx *ctx, size_t count) {
+    if (ctx->call_ints_cap >= count) return L2B_OK;
+    if (ctx->call_ints) {
+        L2B_CUDA(ctx, cudaFree(ctx->call_ints));
+        ctx->owned.erase(std::find(ctx->owned.begin(), ctx->owned.end(), (void *)ctx->call_ints));
+        ctx->call_ints = nullptr;
+        ctx->call_ints_cap = 0;
     }
-    fill_ctl(ctx, tokens[0], pos0, 0, 1.0f, -1.0f);          // DONE = 0 for the attention kernel
+    const int rc = dev_alloc(ctx, &ctx->call_ints, count);
+    if (rc) { cudaGetLastError(); return rc; }
+    ctx->call_ints_cap = count;
+    return L2B_OK;
+}
+
+// The prologue of a batched call on ctx (the current device): the call's `count` ints, its tokens among
+// them, to call_ints in one copy (from pageable memory: staged before this returns), the argmax keys
+// zeroed, the control block with DONE = 0 (for the attention kernel, and until an early exit raises
+// it), then ev0.  Everything enqueued from here to batched_end is the call's timed work.
+static int batched_begin(l2b_ctx *ctx, const int32_t *ints, size_t count, int token0, int pos0) {
+    cudaStream_t st = ctx->stream;
+    int rc = call_ints_reserve(ctx, count);
+    if (rc) return rc;
+    L2B_CUDA(ctx, cudaMemcpyAsync(ctx->call_ints, ints, count * sizeof(int), cudaMemcpyHostToDevice, st));
+    L2B_CUDA(ctx, cudaMemsetAsync(ctx->pf_amax, 0, PF_MAXB * sizeof(unsigned long long), st));
+    fill_ctl(ctx, token0, pos0, 0, 1.0f, -1.0f);
     L2B_CUDA(ctx, cudaMemcpyAsync(ctx->ctl, ctx->h_ctl, CTL_HOST_WORDS * sizeof(int), cudaMemcpyHostToDevice, st));
     L2B_CUDA(ctx, cudaEventRecord(ctx->ev0, st));
     ctx->last_launches = 0;
+    return L2B_OK;
+}
+
+// The epilogue: with back, `count` result ints from call_ints + from to back; then ev1, one synchronise,
+// and the call's device time in last_ms.
+static int batched_end(l2b_ctx *ctx, int *back, size_t from, size_t count) {
+    cudaStream_t st = ctx->stream;
+    if (back) L2B_CUDA(ctx, cudaMemcpyAsync(back, ctx->call_ints + from, count * sizeof(int), cudaMemcpyDeviceToHost, st));
+    L2B_CUDA(ctx, cudaEventRecord(ctx->ev1, st));
+    L2B_CUDA(ctx, cudaStreamSynchronize(st));
+    L2B_CUDA(ctx, cudaGetLastError());
+    L2B_CUDA(ctx, cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
+    return L2B_OK;
+}
+
+// The vectors of n runs laid back to back: run i is n_tok[i] vectors (n_tok == nullptr: one each) on
+// session s[i] from pos[i] on, and vector v runs at pos[v] on the cache of kv[v], entry j[v] of run run[v].
+struct RunVectors {
+    std::vector<l2b_ctx *> kv;
+    std::vector<int> pos, run, j;
+};
+static RunVectors expand_runs(l2b_ctx *const *s, int n, const int32_t *n_tok, const int32_t *pos) {
+    RunVectors r;
+    for (int i = 0; i < n; ++i)
+        for (int j = 0, len = n_tok ? n_tok[i] : 1; j < len; ++j) {
+            r.kv.push_back(s[i]);
+            r.pos.push_back(pos[i] + j);
+            r.run.push_back(i);
+            r.j.push_back(j);
+        }
+    return r;
+}
+
+// n_tokens positions starting at pos0, PF_MAXB per pass over the weights; KV cache filled.  Without
+// score no logits; with score (l2b_score: tokens holds n_tokens + 1 entries, all staged) each group then
+// runs the argmax classifier and logprob_batch_kernel, which leaves position i's log-probability of
+// tokens[i + 1] and its greedy token in score_lp[i] and score_greedy[i].
+static int prefill_batched(l2b_ctx *ctx, const int32_t *tokens, int n_tokens, int pos0, bool score = false) {
+    L2B_CUDA(ctx, cudaSetDevice(ctx->device));
+    const RunVectors r = expand_runs(&ctx, 1, &n_tokens, &pos0);
+    int rc = batched_begin(ctx, tokens, (size_t)n_tokens + (score ? 1 : 0), tokens[0], pos0);
+    if (rc) return rc;
     for (int done = 0; done < n_tokens; done += PF_MAXB) {
         const int nb = n_tokens - done < PF_MAXB ? n_tokens - done : PF_MAXB;
-        l2b_ctx *kv[PF_MAXB];
-        int pos[PF_MAXB];
-        for (int b = 0; b < nb; ++b) { kv[b] = ctx; pos[b] = pos0 + done + b; }
-        int rc = batched_layers(ctx, kv, pos, nb, ctx->pf_tokens + done, nullptr);
+        rc = batched_layers(ctx, r.kv.data() + done, r.pos.data() + done, nb, ctx->call_ints + done, nullptr);
         if (rc) return rc;
         if (score) {
             rc = batched_classifier(ctx, nb, true);
@@ -1940,10 +1980,8 @@ static int prefill_batched(l2b_ctx *ctx, const int32_t *tokens, int n_tokens, in
             if (rc) return rc;
         }
     }
-    L2B_CUDA(ctx, cudaEventRecord(ctx->ev1, st));
-    L2B_CUDA(ctx, cudaStreamSynchronize(st));
-    L2B_CUDA(ctx, cudaGetLastError());
-    L2B_CUDA(ctx, cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
+    rc = batched_end(ctx, nullptr, 0, 0);
+    if (rc) return rc;
     if (pos0 + n_tokens > ctx->n_appended) ctx->n_appended = pos0 + n_tokens;
     return L2B_OK;
 }
@@ -1965,13 +2003,13 @@ static int batched_classifier(l2b_ctx *ctx, int nb, bool argmax) {
 }
 
 // logprob_batch_kernel over the nb logits rows of a group in pf_logits: positions done .. done+nb-1 of a
-// score, their targets at gen_forced + done, their results to score_lp / score_greedy + done
+// score, their targets the staged tokens at call_ints + 1 + done, their results to score_lp / score_greedy + done
 static int launch_logprob_batch(l2b_ctx *ctx, int nb, int done) {
     LogprobBatchParams p{};
     p.ctl = ctx->ctl;
     p.logits = ctx->pf_logits;
     p.n = ctx->cfg.vocab_size;
-    p.targets = ctx->gen_forced + done;
+    p.targets = ctx->call_ints + 1 + done;
     p.amax = ctx->pf_amax;
     p.lp = ctx->score_lp + done;
     p.greedy = ctx->score_greedy + done;
@@ -2047,17 +2085,10 @@ static int step_sessions(l2b_ctx *const *s, int n, const int32_t *n_tok, const i
     const bool argmax = (mode == MODE_ARGMAX), sample = (mode == MODE_SAMPLE);
     int rc = pf_prepare(ctx);
     if (rc) return rc;
-    // the vectors: vector v runs token tokens[v] at vpos[v] on session vs[v]; last[v]: the session it ends, or -1
-    int total = 0;
-    for (int i = 0; i < n; ++i) total += n_tok ? n_tok[i] : 1;
-    std::vector<l2b_ctx *> vs(total);
-    std::vector<int> vpos(total), last(total, -1);
-    for (int i = 0, v = 0; i < n; ++i)
-        for (int j = 0, len = n_tok ? n_tok[i] : 1; j < len; ++j, ++v) {
-            vs[v] = s[i];
-            vpos[v] = pos[i] + j;
-            if (j == len - 1) last[v] = i;
-        }
+    // the vectors: vector v runs token tokens[v]; last(v): the session it ends, or -1
+    const RunVectors r = expand_runs(s, n, n_tok, pos);
+    const int total = (int)r.kv.size();
+    auto last = [&](int v) { return r.j[v] == (n_tok ? n_tok[r.run[v]] : 1) - 1 ? r.run[v] : -1; };
     cudaStream_t st = ctx->stream;
     L2B_CUDA(ctx, cudaSetDevice(ctx->device));
     if (!ctx->pf_ok) {
@@ -2065,7 +2096,7 @@ static int step_sessions(l2b_ctx *const *s, int n, const int32_t *n_tok, const i
         float pre_ms = 0.0f;
         int launches = 0;
         for (int v = 0, i = 0; v < total; ++v) {
-            if (last[v] < 0) continue;
+            if (last(v) < 0) continue;
             const int len = n_tok ? n_tok[i] : 1;
             if (len > 1) {
                 rc = l2b_prefill(s[i], tokens + v - (len - 1), len - 1, pos[i], nullptr);
@@ -2077,10 +2108,10 @@ static int step_sessions(l2b_ctx *const *s, int n, const int32_t *n_tok, const i
         }
         L2B_CUDA(ctx, cudaEventRecord(ctx->ev0, st));
         for (int v = 0; v < total; ++v) {
-            const int i = last[v];
+            const int i = last(v);
             if (i < 0) continue;
-            rc = sample ? run_step(s[i], tokens[v], vpos[v], G_SAMPLE, temperature[i], top_p[i])
-                        : run_step(s[i], tokens[v], vpos[v], argmax ? G_ARGMAX_ONE : G_LOGITS, 1.0f, 0.0f);
+            rc = sample ? run_step(s[i], tokens[v], r.pos[v], G_SAMPLE, temperature[i], top_p[i])
+                        : run_step(s[i], tokens[v], r.pos[v], argmax ? G_ARGMAX_ONE : G_LOGITS, 1.0f, 0.0f);
             if (rc) { ctx->err = s[i]->err; return rc; }
             launches += s[i]->last_launches;
         }
@@ -2093,22 +2124,18 @@ static int step_sessions(l2b_ctx *const *s, int n, const int32_t *n_tok, const i
         return L2B_OK;
     }
     const int dim = ctx->dim, V = ctx->cfg.vocab_size;
-    L2B_CUDA(ctx, cudaEventRecord(ctx->ev0, st));
-    fill_ctl(ctx, tokens[0], pos[0], 0, 1.0f, -1.0f);        // DONE = 0 for the attention kernel
-    L2B_CUDA(ctx, cudaMemcpyAsync(ctx->ctl, ctx->h_ctl, CTL_HOST_WORDS * sizeof(int), cudaMemcpyHostToDevice, st));
-    ctx->last_launches = 0;
+    rc = batched_begin(ctx, tokens, total, tokens[0], pos[0]);
+    if (rc) return rc;
     for (int g = 0; g < total; g += PF_MAXB) {
         const int nb = total - g < PF_MAXB ? total - g : PF_MAXB;
-        // from the caller's (pageable) array: staged before the call returns, ordered after the previous group
-        L2B_CUDA(ctx, cudaMemcpyAsync(ctx->pf_tokens, tokens + g, (size_t)nb * sizeof(int), cudaMemcpyHostToDevice, st));
-        rc = batched_layers(ctx, vs.data() + g, vpos.data() + g, nb, ctx->pf_tokens, nullptr);
+        rc = batched_layers(ctx, r.kv.data() + g, r.pos.data() + g, nb, ctx->call_ints + g, nullptr);
         if (rc) return rc;
         // the group's vectors that end a run: row[k] in the group, of session ends[k]
         int row[PF_MAXB], nl = 0;
         l2b_ctx *ends[PF_MAXB];
         float lt[PF_MAXB], lp[PF_MAXB];
         for (int b = 0; b < nb; ++b) {
-            const int i = last[g + b];
+            const int i = last(g + b);
             if (i < 0) continue;
             row[nl] = b;
             ends[nl] = s[i];
@@ -2146,10 +2173,8 @@ static int step_sessions(l2b_ctx *const *s, int n, const int32_t *n_tok, const i
             }
         }
     }
-    L2B_CUDA(ctx, cudaEventRecord(ctx->ev1, st));
-    L2B_CUDA(ctx, cudaStreamSynchronize(st));
-    L2B_CUDA(ctx, cudaGetLastError());
-    L2B_CUDA(ctx, cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
+    rc = batched_end(ctx, nullptr, 0, 0);
+    if (rc) return rc;
     for (int i = 0; i < n; ++i) {
         l2b_ctx *c = s[i];
         const int end = pos[i] + (n_tok ? n_tok[i] : 1);
@@ -2243,7 +2268,7 @@ static int finish_device_loops(std::vector<DeviceLoop> &loops) {
     l2b_ctx *ctx = loops[0].c;
     std::vector<l2b_ctx *> cs;
     for (const DeviceLoop &d : loops) cs.push_back(d.c);
-    int rc = finish_call(ctx, cs);
+    int rc = finish_call(cs.data(), cs.size());
     if (rc) return rc;
     L2B_CUDA(ctx, cudaSetDevice(ctx->device));
     L2B_CUDA(ctx, cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
@@ -2457,22 +2482,6 @@ int32_t l2b_forward_sample_ragged(l2b_ctx *const *sessions, int32_t n, const int
                                cand_cap, n_cand);
 }
 
-// The per-call device ints of the batched generation and verify calls (gb_ints on s[0]): at least `total`,
-// grown on demand; the current device is ctx's.
-static int gb_reserve(l2b_ctx *ctx, size_t total) {
-    if (ctx->gb_cap >= total) return L2B_OK;
-    if (ctx->gb_ints) {
-        L2B_CUDA(ctx, cudaFree(ctx->gb_ints));
-        ctx->owned.erase(std::find(ctx->owned.begin(), ctx->owned.end(), (void *)ctx->gb_ints));
-        ctx->gb_ints = nullptr;
-        ctx->gb_cap = 0;
-    }
-    const int rc = dev_alloc(ctx, &ctx->gb_ints, total);
-    if (rc) { cudaGetLastError(); return rc; }
-    ctx->gb_cap = total;
-    return L2B_OK;
-}
-
 // l2b_generate_argmax_batch where the batched step runs (pf_ok on s[0]): every step of every group of
 // PF_MAXB sessions is enqueued up front on s[0]'s stream, with no host synchronise until the end.  The
 // positions are launch arguments (pos[i] + step, held at seq_len - 1 once session i is past its limit);
@@ -2487,14 +2496,12 @@ static int generate_batched(l2b_ctx *const *s, int n, const int32_t *tokens, con
     const int S = ctx->cfg.seq_len;
     int stride = 0;                          // steps of the longest-running session
     for (int i = 0; i < n; ++i) stride = limit[i] > stride ? limit[i] : stride;
-    // the call's device ints: tokens, done flags, n_done, limits [n] each, the live count, then forced
-    // and out_next [n][stride]
-    const size_t o_tok = 0, o_done = (size_t)n, o_ndone = 2 * (size_t)n, o_lim = 3 * (size_t)n, o_live = 4 * (size_t)n;
-    const size_t o_forced = o_live + 1, o_out = o_forced + (size_t)n * stride, total = o_out + (size_t)n * stride;
+    // the call's device ints: tokens, done flags, limits [n] each, the live count, forced [n][stride], then
+    // the results: n_done [n] and out_next [n][stride]
+    const size_t o_tok = 0, o_done = (size_t)n, o_lim = 2 * (size_t)n, o_live = 3 * (size_t)n;
+    const size_t o_forced = o_live + 1, o_ndone = o_forced + (size_t)n * stride, o_out = o_ndone + n;
     L2B_CUDA(ctx, cudaSetDevice(ctx->device));
-    const int rc0 = gb_reserve(ctx, total);
-    if (rc0) return rc0;
-    std::vector<int> h(o_out, -1);
+    std::vector<int> h(o_out + (size_t)n * stride, -1);
     for (int i = 0; i < n; ++i) {
         h[o_tok + i] = tokens[i];
         h[o_done + i] = 0;
@@ -2504,14 +2511,9 @@ static int generate_batched(l2b_ctx *const *s, int n, const int32_t *tokens, con
             for (int k = 0; k < limit[i]; ++k) h[o_forced + (size_t)i * stride + k] = forced[(size_t)i * n_steps + k];
     }
     h[o_live] = n;
-    int *d = ctx->gb_ints;
-    cudaStream_t st = ctx->stream;
-    L2B_CUDA(ctx, cudaMemcpyAsync(d, h.data(), o_out * sizeof(int), cudaMemcpyHostToDevice, st));
-    L2B_CUDA(ctx, cudaMemsetAsync(ctx->pf_amax, 0, PF_MAXB * sizeof(unsigned long long), st));
-    fill_ctl(ctx, tokens[0], pos[0], 0, 1.0f, -1.0f);        // DONE = 0 until the last session stops
-    L2B_CUDA(ctx, cudaMemcpyAsync(ctx->ctl, ctx->h_ctl, CTL_HOST_WORDS * sizeof(int), cudaMemcpyHostToDevice, st));
-    L2B_CUDA(ctx, cudaEventRecord(ctx->ev0, st));
-    ctx->last_launches = 0;
+    int rc = batched_begin(ctx, h.data(), h.size(), tokens[0], pos[0]);
+    if (rc) return rc;
+    int *d = ctx->call_ints;
     BatchAdvanceParams a{};
     a.ctl = ctx->ctl;
     a.amax = ctx->pf_amax;
@@ -2526,23 +2528,19 @@ static int generate_batched(l2b_ctx *const *s, int n, const int32_t *tokens, con
             const int nb = n - g < PF_MAXB ? n - g : PF_MAXB;
             int p[PF_MAXB];
             for (int b = 0; b < nb; ++b) p[b] = pos[g + b] + step < S ? pos[g + b] + step : S - 1;
-            int rc = batched_layers(ctx, s + g, p, nb, d + o_tok + g, d + o_done + g);
+            rc = batched_layers(ctx, s + g, p, nb, d + o_tok + g, d + o_done + g);
             if (rc) return rc;
             rc = batched_classifier(ctx, nb, true);
             if (rc) return rc;
             a.g0 = g; a.nb = nb; a.step = step;
             void *args[] = {&a};
-            rc = launch_small(ctx, (const void *)batch_advance_kernel, dim3(1), dim3(PF_MAXB), args, st, true);
+            rc = launch_small(ctx, (const void *)batch_advance_kernel, dim3(1), dim3(PF_MAXB), args, ctx->stream, true);
             if (rc) return rc;
         }
     }
-    std::vector<int> back((size_t)n * stride + n);
-    L2B_CUDA(ctx, cudaMemcpyAsync(back.data(), d + o_ndone, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost, st));
-    L2B_CUDA(ctx, cudaMemcpyAsync(back.data() + n, d + o_out, (size_t)n * stride * sizeof(int), cudaMemcpyDeviceToHost, st));
-    L2B_CUDA(ctx, cudaEventRecord(ctx->ev1, st));
-    L2B_CUDA(ctx, cudaStreamSynchronize(st));
-    L2B_CUDA(ctx, cudaGetLastError());
-    L2B_CUDA(ctx, cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
+    std::vector<int> back(h.size() - o_ndone);     // n_done [n], then out_next [n][stride]
+    rc = batched_end(ctx, back.data(), o_ndone, back.size());
+    if (rc) return rc;
     for (int i = 0; i < n; ++i) {
         n_done[i] = back[i];
         for (int k = 0; k < n_done[i]; ++k) out_next[(size_t)i * n_steps + k] = back[n + (size_t)i * stride + k];
@@ -2599,38 +2597,21 @@ int32_t l2b_generate_argmax_batch(l2b_ctx *const *sessions, int32_t n, const int
 // PF_MAXB per pass over the weights as in step_sessions, each on its own session's cache at its own
 // position, and after each group's argmax classifier verify_accept_kernel decides the runs it holds.  Every
 // group is enqueued up front; once every run is decided (CTL_DONE on s[0]) the groups still queued return
-// at once.  The call's device ints (gb_ints): tokens [total], greedy [total], n_accept [n] (-1: undecided)
-// and the undecided count.
+// at once.  The call's device ints: tokens [total], greedy [total], n_accept [n] (-1: undecided) and the
+// undecided count.
 static int verify_batched(l2b_ctx *const *s, int n, const int32_t *n_tok, const int32_t *tokens, const int32_t *pos,
                           int stop_on_bos, int32_t *greedy, int32_t *n_accept) {
     l2b_ctx *ctx = s[0];
-    int total = 0;
-    for (int i = 0; i < n; ++i) total += n_tok[i];
-    // vector v runs tokens[v] at vpos[v] on session vs[v]; it is entry vj[v] of run vrun[v]
-    std::vector<l2b_ctx *> vs(total);
-    std::vector<int> vpos(total), vrun(total), vj(total);
-    for (int i = 0, v = 0; i < n; ++i)
-        for (int j = 0; j < n_tok[i]; ++j, ++v) {
-            vs[v] = s[i];
-            vpos[v] = pos[i] + j;
-            vrun[v] = i;
-            vj[v] = j;
-        }
+    const RunVectors r = expand_runs(s, n, n_tok, pos);   // vector v runs tokens[v]
+    const int total = (int)r.kv.size();
     const size_t o_tok = 0, o_greedy = (size_t)total, o_acc = 2 * (size_t)total, o_live = o_acc + n, size = o_live + 1;
     L2B_CUDA(ctx, cudaSetDevice(ctx->device));
-    int rc = gb_reserve(ctx, size);
-    if (rc) return rc;
     std::vector<int> h(size, -1);
     for (int v = 0; v < total; ++v) h[o_tok + v] = tokens[v];
     h[o_live] = n;
-    int *d = ctx->gb_ints;
-    cudaStream_t st = ctx->stream;
-    L2B_CUDA(ctx, cudaMemcpyAsync(d, h.data(), size * sizeof(int), cudaMemcpyHostToDevice, st));
-    L2B_CUDA(ctx, cudaMemsetAsync(ctx->pf_amax, 0, PF_MAXB * sizeof(unsigned long long), st));
-    fill_ctl(ctx, tokens[0], pos[0], 0, 1.0f, -1.0f);        // DONE = 0 until the last run is decided
-    L2B_CUDA(ctx, cudaMemcpyAsync(ctx->ctl, ctx->h_ctl, CTL_HOST_WORDS * sizeof(int), cudaMemcpyHostToDevice, st));
-    L2B_CUDA(ctx, cudaEventRecord(ctx->ev0, st));
-    ctx->last_launches = 0;
+    int rc = batched_begin(ctx, h.data(), size, tokens[0], pos[0]);
+    if (rc) return rc;
+    int *d = ctx->call_ints;
     VerifyAcceptParams a{};
     a.ctl = ctx->ctl;
     a.amax = ctx->pf_amax;
@@ -2638,27 +2619,24 @@ static int verify_batched(l2b_ctx *const *s, int n, const int32_t *n_tok, const 
     a.stop_on_bos = stop_on_bos ? 1 : 0;
     for (int g = 0; g < total; g += PF_MAXB) {
         const int nb = total - g < PF_MAXB ? total - g : PF_MAXB;
-        rc = batched_layers(ctx, vs.data() + g, vpos.data() + g, nb, d + o_tok + g, nullptr);
+        rc = batched_layers(ctx, r.kv.data() + g, r.pos.data() + g, nb, d + o_tok + g, nullptr);
         if (rc) return rc;
         rc = batched_classifier(ctx, nb, true);
         if (rc) return rc;
         a.g0 = g;
         a.nb = nb;
         for (int b = 0; b < nb; ++b) {
-            a.run[b] = vrun[g + b];
-            a.j[b] = vj[g + b];
-            a.last[b] = n_tok[vrun[g + b]] - 1;
+            a.run[b] = r.run[g + b];
+            a.j[b] = r.j[g + b];
+            a.last[b] = n_tok[r.run[g + b]] - 1;
         }
         void *args[] = {&a};
-        rc = launch_small(ctx, (const void *)verify_accept_kernel, dim3(1), dim3(32), args, st, true);
+        rc = launch_small(ctx, (const void *)verify_accept_kernel, dim3(1), dim3(32), args, ctx->stream, true);
         if (rc) return rc;
     }
     std::vector<int> back((size_t)total + n);     // greedy [total], then n_accept [n]
-    L2B_CUDA(ctx, cudaMemcpyAsync(back.data(), d + o_greedy, back.size() * sizeof(int), cudaMemcpyDeviceToHost, st));
-    L2B_CUDA(ctx, cudaEventRecord(ctx->ev1, st));
-    L2B_CUDA(ctx, cudaStreamSynchronize(st));
-    L2B_CUDA(ctx, cudaGetLastError());
-    L2B_CUDA(ctx, cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
+    rc = batched_end(ctx, back.data(), o_greedy, back.size());
+    if (rc) return rc;
     for (int i = 0, off = 0; i < n; off += n_tok[i], ++i) {
         const int acc = back[(size_t)total + i];
         if (acc < 0) return fail(ctx, L2B_ERR_STATE, "verify: a run was left undecided");
@@ -2861,7 +2839,7 @@ int32_t l2b_profile_step(l2b_ctx *ctx, int32_t token, int32_t pos, l2b_kernel_ti
     }
     ctx->n_appended = saved_appended;
     {
-        int r2 = finish_call(ctx, ranks);
+        int r2 = finish_call(ranks.data(), ranks.size());
         if (rc == L2B_OK) rc = r2;
     }
     cudaSetDevice(ctx->device);
