@@ -344,6 +344,41 @@ int32_t l2b_verify_argmax_ragged(l2b_ctx *const *sessions, int32_t n, const int3
 /* Most drafts one round of l2b_generate_speculative proposes.                                        */
 #define L2B_SPECULATIVE_MAX_K 32
 
+/* ---- sampled speculative decoding ------------------------------------------------------ */
+
+/* The positions one l2b_verify_sample_ragged call may run.  Every position's output crosses to the host
+ * through one pinned staging area of the call: vocab_size probabilities and 8192 candidates, 4 * vocab_size
+ * + 65536 bytes a position (193,536 at vocab_size 32000).  The staging may hold L2B_VERIFY_SAMPLE_STAGE_BYTES,
+ * so the cap on sum(n_tokens) is
+ *     max(n * (L2B_SPECULATIVE_MAX_K + 1), L2B_VERIFY_SAMPLE_STAGE_BYTES / (4 * vocab_size + 65536))
+ * which is 346 positions at vocab_size 32000, and never less than a full round for every session.         */
+#define L2B_VERIFY_SAMPLE_STAGE_BYTES (64 << 20)
+
+/* The sampler preparation of l2b_forward_sample_ragged at EVERY position of the runs, for sampled speculative
+ * decoding: the host walks the positions with its own sampler and coins (PRNG draws) and accepts drafts while
+ * the sampled token equals the next draft.  The runs are laid out as in l2b_forward_sample_ragged (run i is
+ * n_tokens[i] tokens at positions pos0[i] ..; total = sum(n_tokens)), and position v of that layout gets
+ *   host_probs + v * vocab_size : its probabilities (host_probs may be NULL: none are copied),
+ *   cand + v * cand_cap, n_cand[v] : its candidates and their count under l2b_forward_sample's rules (the
+ *                  count; minus the number that passed when more than min(cand_cap, 8192) did; 0 when the
+ *                  session does not filter).  cand and n_cand may be NULL when no session filters,
+ * exactly what l2b_forward_sample_ragged returns for a run ending at that position.  Where l2b_forward_ragged
+ * shares weight passes, every pass runs the classifier and sample_prep_batch_kernel over all its rows: a
+ * position's arithmetic does not depend on its pass, so its outputs equal l2b_forward_sample_ragged's bit for
+ * bit.  Elsewhere each position runs l2b_forward_sample's own step: bit for bit that call.
+ * Afterwards session i has max(its appended count, pos0[i] + n_tokens[i]) positions appended, as after the
+ * ragged call.  A host that accepts fewer positions continues at its accepted position (pos <= appended allows
+ * it); the rows past that position are stale until they are overwritten.  x, xb, hb, q and logits are not
+ * defined afterwards.  Checked before anything runs, so a refused call changes no session: everything
+ * l2b_forward_sample_ragged checks, and a total above the cap of L2B_VERIFY_SAMPLE_STAGE_BYTES =>
+ * L2B_ERR_INVALID_ARG; a tensor-parallel model => L2B_ERR_UNSUPPORTED.  Errors through
+ * l2b_last_error(sessions[0]); l2b_last_timing(sessions[0]) gives the call's device time and kernel
+ * launches.  Synchronous.                                                                               */
+int32_t l2b_verify_sample_ragged(l2b_ctx *const *sessions, int32_t n, const int32_t *n_tokens,
+                                 const int32_t *tokens, const int32_t *pos0,
+                                 const float *temperature, const float *top_p, float *host_probs,
+                                 l2b_prob_index *cand, int32_t cand_cap, int32_t *n_cand);
+
 /* The greedy loop of l2b_generate_argmax on `target`, a round at a time: `draft` (another context or session
  * with the same vocabulary, of any model) proposes kk = min(k, tokens still wanted - 1, seq_len - 1 - p)
  * tokens with its own device loop, and one l2b_verify_argmax_ragged of one run checks them on the target,

@@ -92,6 +92,8 @@ def load_library():
     lib.l2b_generate_argmax_batch.argtypes = [C.POINTER(vp), C.c_int32, IP, IP, C.c_int32, IP, C.c_int32, IP, IP]
     lib.l2b_fork.argtypes = [vp, C.c_int32, C.POINTER(vp), C.c_int32]
     lib.l2b_verify_argmax_ragged.argtypes = [C.POINTER(vp), C.c_int32, IP, IP, IP, C.c_int32, IP, IP]
+    lib.l2b_verify_sample_ragged.argtypes = [C.POINTER(vp), C.c_int32, IP, IP, IP, FP, FP, FP,
+                                             C.POINTER(L2BProbIndex), C.c_int32, IP]
     lib.l2b_generate_speculative.argtypes = [vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, IP, IP, IP]
     lib.l2b_destroy.argtypes = [vp]
     lib.l2b_destroy.restype = None
@@ -527,6 +529,28 @@ def verify_argmax_ragged(sessions, runs, pos0, stop_on_bos=False):
            hs[0] if n else None)
     offs = np.concatenate([[0], np.cumsum(lens[:n])]).astype(int)
     return [greedy[offs[i]:offs[i] + acc[i] + 1].copy() for i in range(n)], acc[:n].copy()
+
+
+def verify_sample_ragged(sessions, runs, pos0, temperature, top_p, cand_cap=8192):
+    """The device sampler preparation at every position of the runs (l2b_verify_sample_ragged): runs[i] =
+    [t, d_1 .. d_m] are session i's tokens at positions pos0[i] ..  Returns (probs (total, vocab), candidates,
+    n_cand (total,)) in the layout of the runs back to back: row v is what forward_sample_ragged returns for a
+    run ending at that position (candidates[v] is None when n_cand[v] <= 0).  Session i then has
+    max(its appended count, pos0[i] + len(runs[i])) positions appended."""
+    n, hs, lens, toks, pos = _ragged_args(sessions, runs, pos0)
+    temp = np.ascontiguousarray(temperature, dtype=np.float32)
+    tp = np.ascontiguousarray(top_p, dtype=np.float32)
+    assert temp.size == n and tp.size == n
+    total = int(lens[:n].sum()) if n else 0
+    probs = np.empty((max(total, 1), sessions[0].ck.vocab_size if n else 1), dtype=np.float32)
+    cand = (L2BProbIndex * (max(total, 1) * max(cand_cap, 1)))()
+    n_cand = np.zeros(max(total, 1), dtype=np.int32)
+    _check(load_library().l2b_verify_sample_ragged(hs, n, lens.ctypes.data_as(IP), toks.ctypes.data_as(IP),
+                                                   pos.ctypes.data_as(IP), temp.ctypes.data_as(FP),
+                                                   tp.ctypes.data_as(FP), probs.ctypes.data_as(FP), cand, cand_cap,
+                                                   n_cand.ctypes.data_as(IP)), hs[0] if n else None)
+    probs, cands, n_cand = _sample_result(total, probs, cand, n_cand, cand_cap)
+    return probs[:total], cands, n_cand
 
 
 def fork(src, dsts, n_pos):

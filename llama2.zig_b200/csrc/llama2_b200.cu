@@ -126,6 +126,10 @@ struct l2b_ctx {
     bool pf_ready = false, pf_ok = false;
     int *call_ints = nullptr;                // a batched call's tokens and other per-call ints (batched_begin),
     size_t call_ints_cap = 0;                // grown on demand
+    ProbIndex *call_cand = nullptr;          // l2b_verify_sample_ragged: kCandCap candidates per position,
+    size_t call_cand_cap = 0;                // grown on demand
+    unsigned char *h_call = nullptr;         // ... and its pinned D2H staging (probabilities, candidates)
+    size_t h_call_bytes = 0;
     float *delta = nullptr;                  // L2B_TP=nccl baseline only: partial rows before the NCCL all-reduce
     float *q = nullptr, *xb = nullptr, *hb = nullptr, *logits = nullptr, *logits_loc = nullptr;
     float *kcache = nullptr, *vcache = nullptr;     // (L, seq_len, kv_loc)
@@ -1397,6 +1401,7 @@ void destroy_rank(l2b_ctx *ctx) {
     if (ctx->h_ints) cudaFreeHost(ctx->h_ints);
     if (ctx->h_gen) cudaFreeHost(ctx->h_gen);
     if (ctx->h_cand) cudaFreeHost(ctx->h_cand);
+    if (ctx->h_call) cudaFreeHost(ctx->h_call);
     if (ctx->ev0) cudaEventDestroy(ctx->ev0);
     if (ctx->ev1) cudaEventDestroy(ctx->ev1);
     if (ctx->stream) cudaStreamDestroy(ctx->stream);
@@ -1553,21 +1558,24 @@ int run_step(l2b_ctx *lead, int token, int pos, int which, float temperature, fl
     return L2B_OK;
 }
 
-// The output of a sampling step, from ctx's pinned buffers: its probabilities to host_probs (if not
-// NULL and not the pinned buffer itself), and with the candidate filter on its candidates and their
-// count to cand / *n_cand, or minus their number when more passed than fit (the host then filters the
-// probabilities itself).  Without the filter *n_cand = 0.
-void copy_sample_out(l2b_ctx *ctx, bool filter, float *host_probs, l2b_prob_index *cand, int cand_cap, int32_t *n_cand) {
-    const int V = ctx->cfg.vocab_size;
-    if (host_probs && host_probs != ctx->h_logits) memcpy(host_probs, ctx->h_logits, (size_t)V * sizeof(float));
+// The output of a sampling step, from the pinned buffers it was copied to (V probabilities probs, the
+// candidates h_cand and their count): the probabilities to host_probs (if not NULL and not probs itself),
+// and with the candidate filter the candidates and their count to cand / *n_cand, or minus their number
+// when more passed than fit (the host then filters the probabilities itself).  Without the filter *n_cand = 0.
+void copy_sample_out(int V, const float *probs, const ProbIndex *h_cand, int count, bool filter, float *host_probs,
+                     l2b_prob_index *cand, int cand_cap, int32_t *n_cand) {
+    if (host_probs && host_probs != probs) memcpy(host_probs, probs, (size_t)V * sizeof(float));
     if (n_cand) *n_cand = 0;
     if (filter) {
-        const int n = ctx->h_ints[2];
-        if (n > kCandCap || n > cand_cap) { *n_cand = -n; return; }   // too many: filter host_probs on the host
+        if (count > kCandCap || count > cand_cap) { *n_cand = -count; return; }   // too many: filter host_probs on the host
         static_assert(sizeof(l2b_prob_index) == sizeof(ProbIndex), "candidate layout");
-        memcpy(cand, ctx->h_cand, (size_t)n * sizeof(ProbIndex));
-        *n_cand = n;
+        memcpy(cand, h_cand, (size_t)count * sizeof(ProbIndex));
+        *n_cand = count;
     }
+}
+// the output of ctx's last single sampling step (G_SAMPLE), from its own pinned buffers
+void copy_step_sample_out(l2b_ctx *ctx, bool filter, float *host_probs, l2b_prob_index *cand, int cand_cap, int32_t *n_cand) {
+    copy_sample_out(ctx->cfg.vocab_size, ctx->h_logits, ctx->h_cand, ctx->h_ints[2], filter, host_probs, cand, cand_cap, n_cand);
 }
 
 }  // namespace
@@ -1756,7 +1764,7 @@ int32_t l2b_forward_sample(l2b_ctx *ctx, int32_t token, int32_t pos, float tempe
     if (filter && (!cand || !n_cand || cand_cap <= 0)) return fail(ctx, L2B_ERR_INVALID_ARG, "candidate buffer missing");
     rc = run_step(ctx, token, pos, G_SAMPLE, temperature, filter ? top_p : -1.0f);
     if (rc) return rc;
-    copy_sample_out(ctx, filter, host_probs, cand, cand_cap, n_cand);
+    copy_step_sample_out(ctx, filter, host_probs, cand, cand_cap, n_cand);
     return L2B_OK;
 }
 
@@ -1898,18 +1906,20 @@ static int batched_layers(l2b_ctx *ctx, l2b_ctx *const *kv, const int *pos, int 
 static int batched_classifier(l2b_ctx *ctx, int nb, bool argmax);
 static int launch_logprob_batch(l2b_ctx *ctx, int nb, int done);
 
-// ctx->call_ints: at least `count` ints, grown on demand; the current device is ctx's
-static int call_ints_reserve(l2b_ctx *ctx, size_t count) {
-    if (ctx->call_ints_cap >= count) return L2B_OK;
-    if (ctx->call_ints) {
-        L2B_CUDA(ctx, cudaFree(ctx->call_ints));
-        ctx->owned.erase(std::find(ctx->owned.begin(), ctx->owned.end(), (void *)ctx->call_ints));
-        ctx->call_ints = nullptr;
-        ctx->call_ints_cap = 0;
+// a per-call device buffer of ctx (call_ints, call_cand): at least `count` entries, grown on demand; the
+// current device is ctx's
+template <typename T>
+static int call_buf_reserve(l2b_ctx *ctx, T *&buf, size_t &cap, size_t count) {
+    if (cap >= count) return L2B_OK;
+    if (buf) {
+        L2B_CUDA(ctx, cudaFree(buf));
+        ctx->owned.erase(std::find(ctx->owned.begin(), ctx->owned.end(), (void *)buf));
+        buf = nullptr;
+        cap = 0;
     }
-    const int rc = dev_alloc(ctx, &ctx->call_ints, count);
+    const int rc = dev_alloc(ctx, &buf, count);
     if (rc) { cudaGetLastError(); return rc; }
-    ctx->call_ints_cap = count;
+    cap = count;
     return L2B_OK;
 }
 
@@ -1919,7 +1929,7 @@ static int call_ints_reserve(l2b_ctx *ctx, size_t count) {
 // it), then ev0.  Everything enqueued from here to batched_end is the call's timed work.
 static int batched_begin(l2b_ctx *ctx, const int32_t *ints, size_t count, int token0, int pos0) {
     cudaStream_t st = ctx->stream;
-    int rc = call_ints_reserve(ctx, count);
+    int rc = call_buf_reserve(ctx, ctx->call_ints, ctx->call_ints_cap, count);
     if (rc) return rc;
     L2B_CUDA(ctx, cudaMemcpyAsync(ctx->call_ints, ints, count * sizeof(int), cudaMemcpyHostToDevice, st));
     L2B_CUDA(ctx, cudaMemsetAsync(ctx->pf_amax, 0, PF_MAXB * sizeof(unsigned long long), st));
@@ -2047,10 +2057,10 @@ static int check_batch_args(l2b_ctx *const *s, int32_t n, const int32_t *tokens,
     return L2B_OK;
 }
 
-// sample_prep_batch_kernel over the nb logits rows of a group in pf_logits, in place; vector b is session
-// s[b] (its candidates and count go to its own buffers) with temperature[b] and top_p[b] (< 0: no filter)
-static int launch_sample_prep_batch(l2b_ctx *ctx, l2b_ctx *const *s, int nb, const float *temperature,
-                                    const float *top_p) {
+// sample_prep_batch_kernel over the nb logits rows of a group in pf_logits, in place; row b with
+// temperature[b] and top_p[b] (< 0: no filter), its kCandCap candidates to cand[b] and their count to n_cand[b]
+static int launch_sample_prep_batch(l2b_ctx *ctx, int nb, const float *temperature, const float *top_p,
+                                    ProbIndex *const *cand, int *const *n_cand) {
     SamplePrepBatchParams p{};
     p.ctl = ctx->ctl;
     p.logits = ctx->pf_logits;
@@ -2059,8 +2069,8 @@ static int launch_sample_prep_batch(l2b_ctx *ctx, l2b_ctx *const *s, int nb, con
     for (int b = 0; b < nb; ++b) {
         p.temperature[b] = temperature[b];
         p.top_p[b] = top_p[b];
-        p.cand[b] = s[b]->cand;
-        p.n_cand[b] = s[b]->n_cand;
+        p.cand[b] = cand[b];
+        p.n_cand[b] = n_cand[b];
     }
     void *args[] = {&p};
     return launch_small(ctx, (const void *)sample_prep_batch_kernel, dim3(nb), dim3(SAMP_THREADS), args, ctx->stream, true);
@@ -2134,12 +2144,14 @@ static int step_sessions(l2b_ctx *const *s, int n, const int32_t *n_tok, const i
         int row[PF_MAXB], nl = 0;
         l2b_ctx *ends[PF_MAXB];
         float lt[PF_MAXB], lp[PF_MAXB];
+        ProbIndex *lc[PF_MAXB];
+        int *ln[PF_MAXB];
         for (int b = 0; b < nb; ++b) {
             const int i = last(g + b);
             if (i < 0) continue;
             row[nl] = b;
             ends[nl] = s[i];
-            if (sample) { lt[nl] = temperature[i]; lp[nl] = top_p[i]; }
+            if (sample) { lt[nl] = temperature[i]; lp[nl] = top_p[i]; lc[nl] = s[i]->cand; ln[nl] = s[i]->n_cand; }
             ++nl;
         }
         if (nl == 0) continue;
@@ -2154,7 +2166,7 @@ static int step_sessions(l2b_ctx *const *s, int n, const int32_t *n_tok, const i
                 if (row[k] != k)
                     L2B_CUDA(ctx, cudaMemcpyAsync(ctx->pf_logits + (size_t)k * V, ctx->pf_logits + (size_t)row[k] * V,
                                                   V * sizeof(float), cudaMemcpyDeviceToDevice, st));
-            rc = launch_sample_prep_batch(ctx, ends, nl, lt, lp);
+            rc = launch_sample_prep_batch(ctx, nl, lt, lp, lc, ln);
             if (rc) return rc;
         }
         for (int k = 0; k < nl; ++k) {
@@ -2419,16 +2431,14 @@ static int forward_argmax_runs(l2b_ctx *const *sessions, int32_t n, bool ragged,
     return L2B_OK;
 }
 
-static int forward_sample_runs(l2b_ctx *const *sessions, int32_t n, bool ragged, const int32_t *n_tok,
-                               const int32_t *tokens, const int32_t *pos, const float *temperature,
-                               const float *top_p, float *const *host_probs, l2b_prob_index *cand,
-                               int32_t cand_cap, int32_t *n_cand) {
-    int rc = check_batch_args(sessions, n, tokens, pos, ragged, n_tok);
-    if (rc) return rc;
-    l2b_ctx *s0 = sessions[0];
+// The sampler arguments of the batch, ragged and verify sample calls, checked before anything runs; on
+// success filter_p[i] is session i's top-p as the kernels take it (< 0: no filter).
+static int check_sample_args(l2b_ctx *s0, int32_t n, const float *temperature, const float *top_p,
+                             const l2b_prob_index *cand, int32_t cand_cap, const int32_t *n_cand,
+                             std::vector<float> &filter_p) {
     if (!temperature || !top_p) return fail(s0, L2B_ERR_INVALID_ARG, "temperature or top_p is NULL");
     if (s0->cfg.vocab_size < 2) return fail(s0, L2B_ERR_INVALID_ARG, "sampling needs vocab_size >= 2");
-    std::vector<float> filter_p(n);   // the kernel's top-p: < 0 = no filter
+    filter_p.assign(n, -1.0f);
     for (int i = 0; i < n; ++i) {
         if (!(temperature[i] > 0.0f)) return fail(s0, L2B_ERR_INVALID_ARG, "temperature must be > 0 (use l2b_forward_argmax_batch for 0)");
         if (!(top_p[i] >= 0.0f && top_p[i] <= 1.0f)) return fail(s0, L2B_ERR_INVALID_ARG, "top_p must be in [0, 1]");
@@ -2436,10 +2446,22 @@ static int forward_sample_runs(l2b_ctx *const *sessions, int32_t n, bool ragged,
         if (filter && (!cand || !n_cand || cand_cap <= 0)) return fail(s0, L2B_ERR_INVALID_ARG, "candidate buffer missing");
         filter_p[i] = filter ? top_p[i] : -1.0f;
     }
+    return L2B_OK;
+}
+
+static int forward_sample_runs(l2b_ctx *const *sessions, int32_t n, bool ragged, const int32_t *n_tok,
+                               const int32_t *tokens, const int32_t *pos, const float *temperature,
+                               const float *top_p, float *const *host_probs, l2b_prob_index *cand,
+                               int32_t cand_cap, int32_t *n_cand) {
+    int rc = check_batch_args(sessions, n, tokens, pos, ragged, n_tok);
+    if (rc) return rc;
+    std::vector<float> filter_p;
+    rc = check_sample_args(sessions[0], n, temperature, top_p, cand, cand_cap, n_cand, filter_p);
+    if (rc) return rc;
     rc = step_sessions(sessions, n, ragged ? n_tok : nullptr, tokens, pos, MODE_SAMPLE, temperature, filter_p.data());
     if (rc) return rc;
     for (int i = 0; i < n; ++i)
-        copy_sample_out(sessions[i], filter_p[i] >= 0.0f, host_probs ? host_probs[i] : nullptr,
+        copy_step_sample_out(sessions[i], filter_p[i] >= 0.0f, host_probs ? host_probs[i] : nullptr,
                         cand && cand_cap > 0 ? cand + (size_t)i * cand_cap : nullptr, cand_cap,
                         n_cand ? n_cand + i : nullptr);
     return L2B_OK;
@@ -2773,6 +2795,131 @@ int32_t l2b_generate_speculative(l2b_ctx *target, l2b_ctx *draft, int32_t token,
     *n_done = done;
     if (n_rounds) *n_rounds = rounds;
     return L2B_OK;
+}
+
+// l2b_verify_sample_ragged where the batched step runs (pf_ok on s[0]): the runs' vectors go PF_MAXB per pass
+// as in step_sessions, and every vector is an output: each pass runs the classifier and sample_prep_batch_kernel
+// over all its rows, row v's candidates to call_cand + v * kCandCap and its count to the call's ints.  The
+// probabilities of each pass (when wanted) and, at the end, every position's candidates (when some session
+// filters) go to the pinned staging h_call in one copy each; the counts come back through batched_end.  The
+// call's device ints: tokens [total], then counts [total].
+static int verify_sample_batched(l2b_ctx *const *s, int n, const int32_t *n_tok, const int32_t *tokens, const int32_t *pos,
+                                 const float *temperature, const float *filter_p, float *host_probs,
+                                 l2b_prob_index *cand, int32_t cand_cap, int32_t *n_cand) {
+    l2b_ctx *ctx = s[0];
+    const RunVectors r = expand_runs(s, n, n_tok, pos);   // vector v runs tokens[v]
+    const int total = (int)r.kv.size(), V = ctx->cfg.vocab_size;
+    bool want_cand = false;
+    for (int i = 0; i < n; ++i) want_cand |= filter_p[i] >= 0.0f;
+    const size_t probs_bytes = host_probs ? (size_t)total * V * sizeof(float) : 0;
+    const size_t bytes = probs_bytes + (want_cand ? (size_t)total * kCandCap * sizeof(ProbIndex) : 0);
+    L2B_CUDA(ctx, cudaSetDevice(ctx->device));
+    if (ctx->h_call_bytes < bytes) {
+        if (ctx->h_call) L2B_CUDA(ctx, cudaFreeHost(ctx->h_call));
+        ctx->h_call = nullptr;
+        ctx->h_call_bytes = 0;
+        if (cudaHostAlloc((void **)&ctx->h_call, bytes, cudaHostAllocDefault) != cudaSuccess) {
+            cudaGetLastError();
+            ctx->h_call = nullptr;
+            return fail(ctx, L2B_ERR_OOM, "cudaHostAlloc of the verify staging failed");
+        }
+        ctx->h_call_bytes = bytes;
+    }
+    float *h_probs = reinterpret_cast<float *>(ctx->h_call);
+    ProbIndex *h_cand = reinterpret_cast<ProbIndex *>(ctx->h_call + probs_bytes);
+    int rc = want_cand ? call_buf_reserve(ctx, ctx->call_cand, ctx->call_cand_cap, (size_t)total * kCandCap) : L2B_OK;
+    if (rc) return rc;
+    std::vector<int> h(2 * (size_t)total, 0);
+    std::copy(tokens, tokens + total, h.begin());
+    rc = batched_begin(ctx, h.data(), h.size(), tokens[0], pos[0]);
+    if (rc) return rc;
+    int *d = ctx->call_ints;
+    cudaStream_t st = ctx->stream;
+    for (int g = 0; g < total; g += PF_MAXB) {
+        const int nb = total - g < PF_MAXB ? total - g : PF_MAXB;
+        rc = batched_layers(ctx, r.kv.data() + g, r.pos.data() + g, nb, d + g, nullptr);
+        if (rc) return rc;
+        rc = batched_classifier(ctx, nb, false);
+        if (rc) return rc;
+        float lt[PF_MAXB], lp[PF_MAXB];
+        ProbIndex *lc[PF_MAXB];
+        int *ln[PF_MAXB];
+        for (int b = 0; b < nb; ++b) {
+            const int v = g + b, i = r.run[v];
+            lt[b] = temperature[i];
+            lp[b] = filter_p[i];
+            lc[b] = want_cand ? ctx->call_cand + (size_t)v * kCandCap : nullptr;   // not read without the filter
+            ln[b] = d + total + v;
+        }
+        rc = launch_sample_prep_batch(ctx, nb, lt, lp, lc, ln);
+        if (rc) return rc;
+        if (host_probs)
+            L2B_CUDA(ctx, cudaMemcpyAsync(h_probs + (size_t)g * V, ctx->pf_logits, (size_t)nb * V * sizeof(float),
+                                          cudaMemcpyDeviceToHost, st));
+    }
+    if (want_cand)
+        L2B_CUDA(ctx, cudaMemcpyAsync(h_cand, ctx->call_cand, (size_t)total * kCandCap * sizeof(ProbIndex),
+                                      cudaMemcpyDeviceToHost, st));
+    std::vector<int> counts(total);
+    rc = batched_end(ctx, counts.data(), total, total);
+    if (rc) return rc;
+    for (int v = 0; v < total; ++v)
+        copy_sample_out(V, h_probs + (size_t)v * V, h_cand + (size_t)v * kCandCap, counts[v], filter_p[r.run[v]] >= 0.0f,
+                        host_probs ? host_probs + (size_t)v * V : nullptr,
+                        cand && cand_cap > 0 ? cand + (size_t)v * cand_cap : nullptr, cand_cap, n_cand ? n_cand + v : nullptr);
+    for (int i = 0; i < n; ++i)
+        if (pos[i] + n_tok[i] > s[i]->n_appended) s[i]->n_appended = pos[i] + n_tok[i];
+    return L2B_OK;
+}
+
+// l2b_verify_sample_ragged elsewhere: every position is l2b_forward_sample's own step (G_SAMPLE) on its
+// session, and its output is copied out as that call copies it.  Each step ends in a synchronise: ev0 .. ev1
+// spans them all.
+static int verify_sample_each(l2b_ctx *const *s, int n, const int32_t *n_tok, const int32_t *tokens, const int32_t *pos,
+                              const float *temperature, const float *filter_p, float *host_probs,
+                              l2b_prob_index *cand, int32_t cand_cap, int32_t *n_cand) {
+    l2b_ctx *ctx = s[0];
+    const int V = ctx->cfg.vocab_size;
+    L2B_CUDA(ctx, cudaSetDevice(ctx->device));
+    L2B_CUDA(ctx, cudaEventRecord(ctx->ev0, ctx->stream));
+    int launches = 0;
+    for (int i = 0, v = 0; i < n; ++i)
+        for (int j = 0; j < n_tok[i]; ++j, ++v) {
+            int rc = run_step(s[i], tokens[v], pos[i] + j, G_SAMPLE, temperature[i], filter_p[i]);
+            if (rc) { ctx->err = s[i]->err; return rc; }
+            launches += s[i]->last_launches;
+            copy_step_sample_out(s[i], filter_p[i] >= 0.0f, host_probs ? host_probs + (size_t)v * V : nullptr,
+                                 cand && cand_cap > 0 ? cand + (size_t)v * cand_cap : nullptr, cand_cap,
+                                 n_cand ? n_cand + v : nullptr);
+        }
+    L2B_CUDA(ctx, cudaEventRecord(ctx->ev1, s[n - 1]->stream));
+    L2B_CUDA(ctx, cudaEventSynchronize(ctx->ev1));
+    L2B_CUDA(ctx, cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
+    ctx->last_launches = launches;
+    return L2B_OK;
+}
+
+int32_t l2b_verify_sample_ragged(l2b_ctx *const *sessions, int32_t n, const int32_t *n_tokens, const int32_t *tokens,
+                                 const int32_t *pos0, const float *temperature, const float *top_p, float *host_probs,
+                                 l2b_prob_index *cand, int32_t cand_cap, int32_t *n_cand) {
+    int rc = check_batch_args(sessions, n, tokens, pos0, true, n_tokens);
+    if (rc) return rc;
+    l2b_ctx *s0 = sessions[0];
+    std::vector<float> filter_p;
+    rc = check_sample_args(s0, n, temperature, top_p, cand, cand_cap, n_cand, filter_p);
+    if (rc) return rc;
+    int64_t total = 0;
+    for (int i = 0; i < n; ++i) total += n_tokens[i];
+    const int64_t per_pos = 4ll * s0->cfg.vocab_size + (int64_t)kCandCap * sizeof(ProbIndex);
+    const int64_t cap = std::max<int64_t>((int64_t)n * (L2B_SPECULATIVE_MAX_K + 1), L2B_VERIFY_SAMPLE_STAGE_BYTES / per_pos);
+    if (total > cap) return fail(s0, L2B_ERR_INVALID_ARG, "more positions than the verify staging holds (see L2B_VERIFY_SAMPLE_STAGE_BYTES)");
+    if (s0->world > 1) return fail(s0, L2B_ERR_UNSUPPORTED, "l2b_verify_sample_ragged needs a single-GPU model");
+    rc = pf_prepare(s0);
+    if (rc) return rc;
+    return s0->pf_ok ? verify_sample_batched(sessions, n, n_tokens, tokens, pos0, temperature, filter_p.data(), host_probs,
+                                             cand, cand_cap, n_cand)
+                     : verify_sample_each(sessions, n, n_tokens, tokens, pos0, temperature, filter_p.data(), host_probs,
+                                          cand, cand_cap, n_cand);
 }
 
 int32_t l2b_read_state(l2b_ctx *ctx, int32_t which, float *dst, uint64_t n, uint64_t *n_out) {

@@ -10,6 +10,7 @@
 
 #include <algorithm>
 #include <chrono>
+#include <deque>
 #include <string>
 #include <unordered_map>
 #include <vector>
@@ -193,8 +194,22 @@ static uint64_t next_u64() {
     g_s[3] = rotl(g_s[3], 45);
     return result;
 }
-static float next_f32() { return (float)(next_u64() >> 40) * (1.0f / 16777216.0f); }
+static float draw_f32() { return (float)(next_u64() >> 40) * (1.0f / 16777216.0f); }
+// Coins drawn ahead of their turn (peek_f32) wait here and are handed out in order before any new draw, so
+// peeking never changes which coin a sampled token gets.
+static std::deque<float> g_queued;
+static float next_f32() {
+    if (g_queued.empty()) return draw_f32();
+    const float r = g_queued.front();
+    g_queued.pop_front();
+    return r;
+}
+static float peek_f32(size_t ahead) {   // the coin next_f32 returns after `ahead` more calls
+    while (g_queued.size() <= ahead) g_queued.push_back(draw_f32());
+    return g_queued[ahead];
+}
 extern "C" void l2h_seed(uint64_t seed) {
+    g_queued.clear();
     for (int i = 0; i < 4; ++i) {
         seed += 0x9E3779B97F4A7C15ull;
         uint64_t z = seed;
@@ -204,8 +219,8 @@ extern "C" void l2h_seed(uint64_t seed) {
     }
 }
 
-extern "C" int32_t l2h_sample(const float *x, int32_t n) {
-    const float r = next_f32();
+extern "C" int32_t l2h_sample(const float *x, int32_t n) { return l2h_sample_r(x, n, next_f32()); }
+extern "C" int32_t l2h_sample_r(const float *x, int32_t n, float r) {
     float cdf = 0.0f;
     for (int32_t i = 0; i < n; ++i) { cdf += x[i]; if (r < cdf) return i; }
     return n - 1;
@@ -214,6 +229,12 @@ extern "C" int32_t l2h_sample(const float *x, int32_t n) {
 struct IndexedF32 { uint32_t index; float value; };   // :743-750
 
 extern "C" int32_t l2h_sample_top_p(const float *logits, int32_t n, float p, void *scratch) {
+    const float cutoff = (1.0f - p) / ((float)n - 1.0f);                    // :761
+    for (int32_t i = 0; i < n; ++i)   // a coin only when some entry passes the cutoff
+        if (logits[i] >= cutoff) return l2h_sample_top_p_r(logits, n, p, scratch, next_f32());
+    return l2h_argmax(logits, n);
+}
+extern "C" int32_t l2h_sample_top_p_r(const float *logits, int32_t n, float p, void *scratch, float coin) {
     IndexedF32 *idx = (IndexedF32 *)scratch;
     const float cutoff = (1.0f - p) / ((float)n - 1.0f);                    // :761
     int32_t m = 0;
@@ -224,18 +245,21 @@ extern "C" int32_t l2h_sample_top_p(const float *logits, int32_t n, float p, voi
     float cumulative = 0.0f;
     int32_t cutoff_index = m - 1;
     for (int32_t i = 0; i < m; ++i) { cumulative += idx[i].value; if (cumulative > p) { cutoff_index = i; break; } }
-    const float r = next_f32() * cumulative;
+    const float r = coin * cumulative;
     float cdf = 0.0f;
     for (int32_t i = 0; i <= cutoff_index; ++i) { cdf += idx[i].value; if (r < cdf) return (int32_t)idx[i].index; }
     return (int32_t)idx[cutoff_index].index;
 }
 
 extern "C" int32_t l2h_sample_top_p_candidates(l2b_prob_index *cand, int32_t m, float p) {
+    return l2h_sample_top_p_candidates_r(cand, m, p, next_f32());
+}
+extern "C" int32_t l2h_sample_top_p_candidates_r(l2b_prob_index *cand, int32_t m, float p, float coin) {
     std::sort(cand, cand + m, [](const l2b_prob_index &a, const l2b_prob_index &b) { return a.prob > b.prob; });   // :771
     float cumulative = 0.0f;
     int32_t cutoff_index = m - 1;
     for (int32_t i = 0; i < m; ++i) { cumulative += cand[i].prob; if (cumulative > p) { cutoff_index = i; break; } }   // :774-781
-    const float r = next_f32() * cumulative;                                                                        // :785
+    const float r = coin * cumulative;                                                                              // :785
     float cdf = 0.0f;
     for (int32_t i = 0; i <= cutoff_index; ++i) { cdf += cand[i].prob; if (r < cdf) return cand[i].index; }
     return cand[cutoff_index].index;
@@ -255,6 +279,16 @@ static int raw_byte(const char *s, int len) {
     }
     if ((byte >= 32 && byte < 127) || byte == ' ' || (byte >= 9 && byte <= 13)) return byte;
     return -1;
+}
+
+extern "C" void l2h_print_token(const l2h_tokenizer *tk, int32_t token, int32_t next) {
+    int32_t len = 0;
+    const char *s = l2h_tokenizer_token(tk, next, &len);          // :1022-1034
+    if (s) {
+        if (token == 1 && len > 0 && s[0] == ' ') { ++s; --len; }
+        const int b = raw_byte(s, len);
+        if (b >= 0) fputc(b, stdout); else fwrite(s, 1, len, stdout);
+    }
 }
 
 // ---------------------------------------------------------------------------------------
@@ -282,17 +316,7 @@ extern "C" int32_t l2h_generate(l2b_ctx *ctx, const l2b_config *cfg, const l2h_g
     const clk::time_point t_begin = clk::now();
     int pos = 0;
     std::vector<l2b_prob_index> cand(8192);
-    auto print_token = [&](int32_t nx) {
-        if (tk) {                                                 // :1022-1034
-            int32_t len = 0;
-            const char *s = l2h_tokenizer_token(tk, nx, &len);
-            if (s) {
-                if (token == 1 && len > 0 && s[0] == ' ') { ++s; --len; }
-                const int b = raw_byte(s, len);
-                if (b >= 0) fputc(b, stdout); else fwrite(s, 1, len, stdout);
-            }
-        }
-    };
+    auto print_token = [&](int32_t nx) { if (tk) l2h_print_token(tk, token, nx); };
     if (opt->use_prefill && n_prompt > 0 && n_prompt < seq_len) {
         // positions 0 .. n_prompt-1 hold BOS, prompt[0 .. n_prompt-2]; their logits are never read (:999-1000)
         std::vector<int32_t> toks(n_prompt);
@@ -357,15 +381,7 @@ extern "C" int32_t l2h_generate(l2b_ctx *ctx, const l2b_config *cfg, const l2h_g
         }
         if (out_tokens && res->n_tokens < cap) out_tokens[res->n_tokens++] = next;
         if (opt->stop_on_bos && next == 1) break;                 // :1017-1019
-        if (tk) {                                                 // :1022-1034
-            int32_t len = 0;
-            const char *s = l2h_tokenizer_token(tk, next, &len);
-            if (s) {
-                if (token == 1 && len > 0 && s[0] == ' ') { ++s; --len; }
-                const int b = raw_byte(s, len);
-                if (b >= 0) fputc(b, stdout); else fwrite(s, 1, len, stdout);
-            }
-        }
+        print_token(next);
         token = next;
         if (!timer_started) { timer_started = true; t_first = clk::now(); }   // :1038-1041
     }
@@ -373,5 +389,86 @@ extern "C" int32_t l2h_generate(l2b_ctx *ctx, const l2b_config *cfg, const l2h_g
     res->secs_total = std::chrono::duration<double>(t_end - t_begin).count();
     res->secs_after_first = timer_started ? std::chrono::duration<double>(t_end - t_first).count() : 0.0;
     if (tk) fflush(stdout);
+    return L2B_OK;
+}
+
+// ---------------------------------------------------------------------------------------
+// sampled speculative decoding: the device-sampler loop of l2h_generate, a round at a time
+// ---------------------------------------------------------------------------------------
+// One sampled token from the output of l2b_forward_sample (or a row of l2b_verify_sample_ragged) with the
+// given coin, as the device-sampler loop picks it (:1009-1012).  *used: whether the token consumes the coin;
+// it does not when top-p filtering leaves no candidate (then the argmax, as l2h_sample_top_p).
+static int32_t sample_prepared(const float *probs, int32_t V, float top_p, l2b_prob_index *cand, int32_t n_cand,
+                               IndexedF32 *scratch, float coin, bool *used) {
+    *used = true;
+    if (top_p == 0.0f || top_p == 1.0f) return l2h_sample_r(probs, V, coin);
+    if (n_cand > 0) return l2h_sample_top_p_candidates_r(cand, n_cand, top_p, coin);
+    *used = n_cand < 0;                 // < 0: more candidates than fit, the host filters the probabilities
+    return l2h_sample_top_p_r(probs, V, top_p, scratch, coin);
+}
+
+// p: the target's next position, whose token is hist[p - pos]; dp: the stream positions the draft holds
+// rows for (as in l2b_generate_speculative: after a round that accepted every draft, the draft never ran
+// d_kk, so its next round first runs it at dp = p - 1).
+extern "C" int32_t l2h_generate_speculative_sample(l2b_ctx *target, const l2b_config *cfg, l2b_ctx *draft,
+                                                   const l2b_config *draft_cfg, int32_t token, int32_t pos,
+                                                   int32_t n_steps, int32_t k, float temperature, float top_p,
+                                                   int32_t stop_on_bos, int32_t *out_next, int32_t *n_done,
+                                                   int32_t *n_rounds) {
+    if (!target || !cfg || !draft || !draft_cfg || !out_next || !n_done || target == draft) return L2B_ERR_INVALID_ARG;
+    if (k < 0 || k > L2B_SPECULATIVE_MAX_K || n_steps < 0) return L2B_ERR_INVALID_ARG;
+    if (!(temperature > 0.0f) || !(top_p >= 0.0f && top_p <= 1.0f)) return L2B_ERR_INVALID_ARG;   // 0: l2b_generate_speculative
+    const int V = cfg->vocab_size, S = cfg->seq_len;
+    if (draft_cfg->vocab_size != V || draft_cfg->seq_len < S) return L2B_ERR_INVALID_ARG;
+    if (token < 0 || token >= V || pos < 0 || pos >= S) return L2B_ERR_INVALID_ARG;
+    if (n_steps > S - pos) n_steps = S - pos;                    // :992-993
+    constexpr int kCap = 8192, kRun = L2B_SPECULATIVE_MAX_K + 1;
+    std::vector<float> probs((size_t)kRun * V), dprobs(V);
+    std::vector<l2b_prob_index> cand((size_t)kRun * kCap), dcand(kCap);
+    std::vector<int32_t> n_cand(kRun), run, hist(1, token);
+    std::vector<IndexedF32> scratch(V);
+    int p = pos, dp = pos, done = 0, rounds = 0;
+    bool stopped = false, used = false;
+    int32_t rc;
+    while (done < n_steps && !stopped) {
+        const int kk = std::min(std::min(k, n_steps - done - 1), S - 1 - p);
+        run.assign(1, hist[p - pos]);
+        if (kk > 0) {
+            if (dp < p && (rc = l2b_prefill(draft, hist.data() + (dp - pos), p - dp, dp, nullptr))) return rc;
+            // draft token j takes the coin the stream's token at p + j + 1 would take if every draft before
+            // it is accepted; the coins stay queued for the target's walk
+            size_t ahead = 0;
+            for (int j = 0; j < kk; ++j) {
+                int32_t dn = 0;
+                rc = l2b_forward_sample(draft, run.back(), p + j, temperature, top_p, dprobs.data(), dcand.data(), kCap, &dn);
+                if (rc) return rc;
+                run.push_back(sample_prepared(dprobs.data(), V, top_p, dcand.data(), dn, scratch.data(), peek_f32(ahead), &used));
+                ahead += used;
+            }
+        }
+        const int32_t nt = kk + 1;
+        rc = l2b_verify_sample_ragged(&target, 1, &nt, run.data(), &p, &temperature, &top_p, probs.data(), cand.data(),
+                                      kCap, n_cand.data());
+        if (rc) return rc;
+        ++rounds;
+        // the plain loop's tokens: the target's own sampler and coins, in order, while it agrees with the drafts
+        int emit = 0;
+        for (int j = 0; j <= kk; ++j) {
+            const int32_t g = sample_prepared(probs.data() + (size_t)j * V, V, top_p, cand.data() + (size_t)j * kCap,
+                                              n_cand[j], scratch.data(), peek_f32(0), &used);
+            if (used) next_f32();
+            out_next[done + emit++] = g;
+            hist.push_back(g);
+            if (stop_on_bos && g == 1) { stopped = true; break; }   // :1017-1019
+            if (j == kk || run[j + 1] != g) break;
+        }
+        if (kk > 0) dp = p + std::min(emit, kk);
+        done += emit;
+        p += emit;
+    }
+    const int end = pos + done;
+    if (dp < end && (rc = l2b_prefill(draft, hist.data() + (dp - pos), end - dp, dp, nullptr))) return rc;
+    *n_done = done;
+    if (n_rounds) *n_rounds = rounds;
     return L2B_OK;
 }

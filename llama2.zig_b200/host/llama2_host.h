@@ -46,6 +46,14 @@ int32_t l2h_sample(const float *probs, int32_t n);                              
 int32_t l2h_sample_top_p(const float *probs, int32_t n, float p, void *scratch_2n_words);  /* :754-798 */
 /* :770-797 on a candidate list that already passed the cutoff of :761-768 (sorted here)      */
 int32_t l2h_sample_top_p_candidates(l2b_prob_index *cand, int32_t n_cand, float p);
+/* The same three with the uniform draw ("coin", in [0, 1)) passed in: each of the above draws one coin
+ * from the PRNG and calls its _r form, except that l2h_sample_top_p draws nothing (and returns the argmax)
+ * when no entry passes the cutoff; l2h_sample_top_p_r then does not read the coin either.              */
+int32_t l2h_sample_r(const float *probs, int32_t n, float coin);
+int32_t l2h_sample_top_p_r(const float *probs, int32_t n, float p, void *scratch_2n_words, float coin);
+int32_t l2h_sample_top_p_candidates_r(l2b_prob_index *cand, int32_t n_cand, float p, float coin);
+/* Prints token `next` as the reference does after `token` (:1022-1034).                       */
+void l2h_print_token(const l2h_tokenizer *t, int32_t token, int32_t next);
 
 typedef struct l2h_gen_options {
     float temperature;      /* :840, 0 => argmax                                             */
@@ -75,6 +83,28 @@ typedef struct l2h_gen_result {
 int32_t l2h_generate(l2b_ctx *ctx, const l2b_config *cfg, const l2h_gen_options *opt,
                      const int32_t *prompt, int32_t n_prompt, const l2h_tokenizer *print_tok,
                      int32_t *out_tokens, int32_t cap, l2h_gen_result *res);
+
+/* Sampled speculative decoding: the device-sampler loop of l2h_generate (l2b_forward_sample on the target,
+ * then l2h_sample / l2h_sample_top_p_candidates / l2h_sample_top_p with the PRNG of l2h_seed) from `token` at
+ * `pos`, a round at a time.  Each round the draft (another context or session with the same vocabulary and a
+ * seq_len at least the target's) proposes kk = min(k, tokens still wanted - 1, seq_len - 1 - p) tokens, each
+ * one l2b_forward_sample and the _r sampler with the coin the target would use for that token if every
+ * earlier proposal is accepted (peeked, not drawn).  One l2b_verify_sample_ragged then gives the target's
+ * sampler output at every position of [t, d_1 .. d_kk]; the host walks them with the same sampler, consuming
+ * coins exactly as the plain loop does, and emits tokens up to the first that differs from the next draft (or
+ * BOS, with stop_on_bos).  Coins peeked and not consumed stay queued for the tokens they belong to.  So
+ * out_next[0 .. *n_done), *n_done and the target's KV rows [0, pos + *n_done) are those of the plain loop with
+ * the same seed, bit for bit, whatever the draft, and the PRNG is left where that loop leaves it.  Afterwards
+ * target and draft both hold the stream's rows [0, pos + *n_done) (rows past it are stale), so a second call
+ * from (out_next[*n_done - 1], pos + *n_done) continues the stream.  *n_rounds (n_rounds may be NULL) counts
+ * rounds.  cfg and draft_cfg are the two models' configs.  NULL pointers, target == draft, k outside [0,
+ * L2B_SPECULATIVE_MAX_K], n_steps < 0, temperature not > 0 (greedy: l2b_generate_speculative), top_p outside
+ * [0, 1], another vocab_size, a smaller draft seq_len, or token / pos out of range => L2B_ERR_INVALID_ARG
+ * before anything runs; a library error is returned as is (see l2b_last_error of target or draft).       */
+int32_t l2h_generate_speculative_sample(l2b_ctx *target, const l2b_config *cfg, l2b_ctx *draft,
+                                        const l2b_config *draft_cfg, int32_t token, int32_t pos, int32_t n_steps,
+                                        int32_t k, float temperature, float top_p, int32_t stop_on_bos,
+                                        int32_t *out_next, int32_t *n_done, int32_t *n_rounds);
 
 #ifdef __cplusplus
 }

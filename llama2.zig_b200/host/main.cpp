@@ -5,6 +5,7 @@
 #include <string.h>
 #include <time.h>
 
+#include <chrono>
 #include <string>
 #include <vector>
 
@@ -25,13 +26,55 @@ static const char *usage_text =
     "     --device-argmax       with -t 0: argmax on the GPU, only the token id crosses PCIe\n"
     "     --device-sampler      with -t > 0: logits/T, softmax and the top-p prefilter on the GPU\n"
     "     --prefill             prompt positions run on the GPU back to back (no logits, no host round trip)\n"
-    "     --gpus <1|2|4|8>      tensor-parallel over that many GPUs (llama2-7B class models)\n";
+    "     --gpus <1|2|4|8>      tensor-parallel over that many GPUs (llama2-7B class models)\n"
+    "     --draft <checkpoint>  speculative decoding with this draft model (same vocabulary); same tokens\n"
+    "     --draft-k <int>       tokens the draft proposes per round, default 3, at most 32\n";
+
+// Generation with a draft model: the prompt positions are prefilled on target and draft, then
+// l2b_generate_speculative (-t 0) or l2h_generate_speculative_sample (-t > 0) runs the rest.  The tokens
+// are those of the --device-argmax / --device-sampler loops with the same seed, whatever the draft.
+static int generate_with_draft(l2b_ctx *ctx, const l2b_config &c, l2b_ctx *draft, const l2b_config &dc, int k,
+                               const l2h_gen_options &opt, const std::vector<int32_t> &prompt, const l2h_tokenizer *tk,
+                               bool verbose) {
+    int seq_len = opt.n_steps == 0 ? c.seq_len : opt.n_steps;   // :992-993
+    seq_len = seq_len < 1 ? 1 : seq_len > c.seq_len ? c.seq_len : seq_len;
+    const int n_prompt = (int)prompt.size() < seq_len ? (int)prompt.size() : seq_len;
+    int32_t token = 1, rc;                                      // :988 BOS
+    if (n_prompt > 0 && n_prompt < seq_len) {   // positions 0 .. n_prompt-1 hold BOS, prompt[0 .. n_prompt-2] (:999-1000)
+        std::vector<int32_t> toks(1, token);
+        toks.insert(toks.end(), prompt.begin(), prompt.begin() + n_prompt - 1);
+        for (l2b_ctx *t : {ctx, draft})
+            if ((rc = l2b_prefill(t, toks.data(), n_prompt, 0, nullptr))) return rc;
+    }
+    for (int i = 0; i < n_prompt; ++i) { l2h_print_token(tk, token, prompt[i]); token = prompt[i]; }
+    if (n_prompt == seq_len) return L2B_OK;
+    std::vector<int32_t> out(seq_len);
+    int32_t done = 0, rounds = 0;
+    const auto t0 = std::chrono::steady_clock::now();
+    rc = opt.temperature == 0.0f
+             ? l2b_generate_speculative(ctx, draft, token, n_prompt, seq_len - n_prompt, k, opt.stop_on_bos,
+                                        out.data(), &done, &rounds)
+             : l2h_generate_speculative_sample(ctx, &c, draft, &dc, token, n_prompt, seq_len - n_prompt, k,
+                                               opt.temperature, opt.top_p, opt.stop_on_bos, out.data(), &done, &rounds);
+    if (rc) return rc;
+    const double secs = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+    for (int i = 0; i < done; ++i) {
+        if (opt.stop_on_bos && out[i] == 1) break;              // :1017-1019
+        l2h_print_token(tk, token, out[i]);
+        token = out[i];
+    }
+    fflush(stdout);
+    if (verbose && secs > 0)
+        fprintf(stderr, "\n\n%d tokens in %d rounds, %d tokens per second\n", done, rounds, (int)(done / secs));
+    return L2B_OK;
+}
 
 int main(int argc, char **argv) {
     if (argc < 2) { fputs(usage_text, stdout); return 0; }
     const char *bin_path = nullptr, *input = nullptr, *tokenizer_path = "tokenizer.bin";
     l2h_gen_options opt{1.0f, 0.9f, 0, 1, 0, 0, 0};
-    int n_gpus = 1;
+    int n_gpus = 1, draft_k = 3;
+    const char *draft_path = nullptr;
     bool verbose = false;
     l2h_seed((uint64_t)time(nullptr));
     for (int i = 1; i < argc; ++i) {
@@ -55,6 +98,8 @@ int main(int argc, char **argv) {
         else if (a == "--device-sampler") opt.use_device_sampler = 1;
         else if (a == "--prefill") opt.use_prefill = 1;
         else if (a == "--gpus") n_gpus = atoi(need("gpus"));
+        else if (a == "--draft") draft_path = need("draft");
+        else if (a == "--draft-k") draft_k = atoi(need("draft-k"));
         else { fprintf(stderr, "error: unknown argument '%s'\n", argv[i]); fputs(usage_text, stdout); return 0; }
     }
     if (!bin_path) { fputs(usage_text, stdout); return 0; }
@@ -71,6 +116,21 @@ int main(int argc, char **argv) {
     int32_t rc = l2b_create(&ctx, &c, ck.data, ck.n_floats, nullptr, nullptr, n_gpus);   // after :967
     if (rc) { fprintf(stderr, "error: l2b_create: %s (%s)\n", l2b_status_string(rc), l2b_last_error(nullptr)); return 1; }
     l2h_free_checkpoint(&ck);   // host copy no longer needed: weights live in HBM
+    l2b_ctx *draft = nullptr;
+    l2b_config dc{};
+    if (draft_path) {
+        l2h_checkpoint dck;
+        if (l2h_load_checkpoint(draft_path, &dck) != L2B_OK) { fprintf(stderr, "error: cannot read draft checkpoint %s\n", draft_path); return 1; }
+        dc = dck.config;
+        if (dc.vocab_size != c.vocab_size || dc.seq_len < c.seq_len) {
+            fprintf(stderr, "error: the draft needs the target's vocab_size (%d) and a seq_len of at least %d\n", c.vocab_size, c.seq_len);
+            return 1;
+        }
+        if (draft_k < 0 || draft_k > L2B_SPECULATIVE_MAX_K) { fprintf(stderr, "error: --draft-k must be in [0, %d]\n", L2B_SPECULATIVE_MAX_K); return 1; }
+        rc = l2b_create(&draft, &dc, dck.data, dck.n_floats, nullptr, nullptr, 1);
+        if (rc) { fprintf(stderr, "error: l2b_create (draft): %s (%s)\n", l2b_status_string(rc), l2b_last_error(nullptr)); return 1; }
+        l2h_free_checkpoint(&dck);
+    }
 
     l2h_tokenizer *tk = nullptr;
     if (l2h_tokenizer_load(tokenizer_path, c.vocab_size, &tk) != L2B_OK) { fprintf(stderr, "error: cannot read tokenizer %s\n", tokenizer_path); return 1; }
@@ -81,12 +141,18 @@ int main(int argc, char **argv) {
         if (n < 0) { fprintf(stderr, "error: cannot encode prompt\n"); return 1; }
         prompt.resize(n);
     }
-    l2h_gen_result res;
-    rc = l2h_generate(ctx, &c, &opt, prompt.data(), (int32_t)prompt.size(), tk, nullptr, 0, &res);
-    if (rc) { fprintf(stderr, "\nerror: %s (%s)\n", l2b_status_string(rc), l2b_last_error(ctx)); return 1; }
-    if (verbose && res.secs_after_first > 0)   // :1043-1050: (pos - 1) / elapsed since the first token
-        fprintf(stderr, "\n\n%d tokens per second\n", (int)((res.n_forward - 1) / res.secs_after_first));
+    if (draft) {
+        rc = generate_with_draft(ctx, c, draft, dc, draft_k, opt, prompt, tk, verbose);
+        if (rc) { fprintf(stderr, "\nerror: %s (%s / %s)\n", l2b_status_string(rc), l2b_last_error(ctx), l2b_last_error(draft)); return 1; }
+    } else {
+        l2h_gen_result res;
+        rc = l2h_generate(ctx, &c, &opt, prompt.data(), (int32_t)prompt.size(), tk, nullptr, 0, &res);
+        if (rc) { fprintf(stderr, "\nerror: %s (%s)\n", l2b_status_string(rc), l2b_last_error(ctx)); return 1; }
+        if (verbose && res.secs_after_first > 0)   // :1043-1050: (pos - 1) / elapsed since the first token
+            fprintf(stderr, "\n\n%d tokens per second\n", (int)((res.n_forward - 1) / res.secs_after_first));
+    }
     l2h_tokenizer_free(tk);
+    l2b_destroy(draft);
     l2b_destroy(ctx);
     return 0;
 }
