@@ -497,6 +497,39 @@ int32_t l2b_op_sample_prep(int32_t device, float *logits_inout, int32_t n, float
  * n < 1 or a target outside [0, n) => L2B_ERR_INVALID_ARG.                                  */
 int32_t l2b_op_logprob(int32_t device, const float *logits, int32_t n, int32_t target, float *logprob);
 
+/* ---- device weight format ------------------------------------------------------------------
+ * Which tensors: the token embedding, wq wk wv wo w1 w2 w3 and an unshared wcls are stored in the
+ * format; the RMSNorm gains, RoPE tables, KV cache and all run state stay fp32.
+ * Rounding (L2B_WEIGHTS_BF16): each fp32 weight becomes the nearest bf16, ties to even.  +-inf stays
+ * +-inf, finite values above the bf16 maximum become +-inf, subnormals are rounded (not flushed), NaN
+ * stays NaN.  For every non-NaN value this is bitwise torch's float32 -> bfloat16 -> float32 round
+ * trip.  The host upload, l2b_round_bf16_host and the synthetic generator share this one rounding.
+ * Contract: for every payload P and every entry point, a bf16 context of P (and its sessions) returns
+ * exactly what an fp32 context of round_bf16(P) (P with those tensors rounded) returns: logits, probabilities, candidates,
+ * log-probabilities, tokens, n_accept, n_done, and l2b_read_state of x, the KV cache and the logits.
+ * Each bf16 kernel is the fp32 kernel the same shape selects, reading bf16 and widening it exactly.
+ * Device rows of a bf16 matrix are padded to a multiple of 8 elements (16 bytes) with zeros.
+ * l2b_load_stats, l2b_step_bytes and the bytes of l2b_profile_step count 2 bytes per bf16 element
+ * stored, padding included.
+ * Sessions (l2b_create_session) of a bf16 model are bf16; l2b_create_sharded stays fp32.          */
+typedef enum l2b_weight_format { L2B_WEIGHTS_F32 = 0, L2B_WEIGHTS_BF16 = 1 } l2b_weight_format;
+
+/* l2b_create with a device weight format.  L2B_WEIGHTS_F32 is exactly l2b_create.  Checked before
+ * any device is touched: an unknown format => L2B_ERR_INVALID_ARG; L2B_WEIGHTS_BF16 with n_gpus > 1
+ * => L2B_ERR_UNSUPPORTED (tensor parallel is fp32 only); every other check is l2b_create's.         */
+int32_t l2b_create_format(l2b_ctx **out, const l2b_config *cfg, const float *host_weights, uint64_t n_floats,
+                          const float *rope_cos, const float *rope_sin, int32_t n_gpus, int32_t weight_format);
+/* l2b_create_synthetic (single GPU, device 0) with a device weight format.  The bf16 matrices are
+ * exactly those of l2b_synth_checkpoint_host's payload passed through l2b_round_bf16_host.          */
+int32_t l2b_create_synthetic_format(l2b_ctx **out, const l2b_config *cfg, uint64_t seed, int32_t weight_format);
+/* Format of ctx's model, and how many matrix weights rounding changed (their bit pattern differs
+ * from the fp32 value; 0: every output equals that of an fp32 context of the same payload).  Counted
+ * during the upload, or on the device for synthetic weights.                                      */
+int32_t l2b_weight_info(const l2b_ctx *ctx, int32_t *weight_format, uint64_t *n_rounded);
+/* In place: each value -> the nearest bf16 (ties to even), widened back to fp32.  The library's own
+ * rounding (see above).                                                                            */
+void l2b_round_bf16_host(float *data, uint64_t n);
+
 #ifdef __cplusplus
 }
 #endif

@@ -25,6 +25,8 @@ from .binding import (  # noqa: F401
     rmsnorm,
     softmax,
     synth_checkpoint_host,
+    round_bf16_host,
+    WEIGHT_FORMATS,
     vector_weighted_sum_rows,
     attention_head,
     fused_matmul,
@@ -46,7 +48,7 @@ from .checkpoint import Checkpoint, read_checkpoint, MODEL_SHAPES  # noqa: F401
 
 __all__ = [
     "L2BError", "L2BConfig", "L2BShard", "Transformer", "checkpoint_floats", "comm_unique_id",
-    "lib_path", "load_library", "matmul", "rmsnorm", "softmax", "synth_checkpoint_host",
+    "lib_path", "load_library", "matmul", "rmsnorm", "softmax", "synth_checkpoint_host", "round_bf16_host", "WEIGHT_FORMATS",
     "vector_weighted_sum_rows", "attention_head", "fused_matmul", "sample_prep", "logprob", "exported_symbols", "forward_batch", "forward_argmax_batch", "forward_sample_batch", "generate_argmax_batch", "forward_ragged", "forward_argmax_ragged", "forward_sample_ragged", "fork", "verify_argmax_ragged", "verify_sample_ragged", "Checkpoint",
     "read_checkpoint", "MODEL_SHAPES",
 ]

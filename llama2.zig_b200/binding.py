@@ -134,6 +134,12 @@ def load_library():
     lib.l2b_op_softmax.argtypes = [C.c_int32, FP, C.c_int32]
     lib.l2b_op_weighted_sum_rows.argtypes = [C.c_int32, FP, C.c_int32, FP, C.c_int32, FP, C.c_int32]
     lib.l2b_op_attention_head.argtypes = [C.c_int32, FP, FP, FP, FP, C.c_int32, C.c_int32, C.c_int32]
+    lib.l2b_create_format.argtypes = [C.POINTER(vp), C.POINTER(L2BConfig), FP, C.c_uint64, FP, FP, C.c_int32,
+                                      C.c_int32]
+    lib.l2b_create_synthetic_format.argtypes = [C.POINTER(vp), C.POINTER(L2BConfig), C.c_uint64, C.c_int32]
+    lib.l2b_weight_info.argtypes = [vp, IP, U64P]
+    lib.l2b_round_bf16_host.argtypes = [FP, C.c_uint64]
+    lib.l2b_round_bf16_host.restype = None
     _lib = lib
     return lib
 
@@ -166,6 +172,18 @@ def comm_unique_id():
     return bytes(buf)
 
 
+WEIGHT_FORMATS = {"f32": 0, "bf16": 1}   # l2b_weight_format
+
+
+def round_bf16_host(a):
+    """In place on a C-contiguous float32 array: each value -> the nearest bf16 (ties to even), widened
+    back to fp32 (l2b_round_bf16_host, the rounding a bf16 context applies to its weights).  Returns a."""
+    if not (isinstance(a, np.ndarray) and a.dtype == np.float32 and a.flags["C_CONTIGUOUS"]):
+        raise TypeError("round_bf16_host needs a C-contiguous float32 array")
+    load_library().l2b_round_bf16_host(a.ctypes.data_as(FP), a.size)
+    return a
+
+
 def synth_checkpoint_host(ck, seed):
     """Host copy of the synthetic payload l2b_create_synthetic puts on the device."""
     lib = load_library()
@@ -184,13 +202,19 @@ class Transformer:
 
     `ck` is a checkpoint.Checkpoint.  With `ck.data` set the payload is uploaded
     (l2b_create / l2b_create_sharded); with `synthetic_seed` the weights are generated on the
-    device (l2b_create_synthetic).
+    device (l2b_create_synthetic).  weight_format="bf16" keeps the matrix weights in bf16 on the
+    device (l2b_create_format / l2b_create_synthetic_format; single GPU, device 0).
     """
 
     def __init__(self, ck, synthetic_seed=None, rank=0, world_size=1, device=0, comm_id=None,
-                 rope_cos=None, rope_sin=None, n_gpus=1):
+                 rope_cos=None, rope_sin=None, n_gpus=1, weight_format="f32"):
         """n_gpus > 1: ONE process drives n_gpus GPUs (l2b_create(.., n_gpus)); rank/world_size:
         one process per GPU (l2b_create_sharded)."""
+        if weight_format not in WEIGHT_FORMATS:
+            raise ValueError(f"weight_format must be one of {sorted(WEIGHT_FORMATS)}")
+        fmt = WEIGHT_FORMATS[weight_format]
+        if fmt and (world_size > 1 or device != 0 or rank != 0 or n_gpus != 1):
+            raise ValueError("bf16 weights are single-GPU on device 0")
         self.lib = load_library()
         self.ck = ck
         self.cfg = make_config(ck)
@@ -201,7 +225,9 @@ class Transformer:
             shard = L2BShard(rank, world_size, device, 0)
             if comm_id is not None:
                 C.memmove(shard.comm_id, comm_id, 128)
-        if synthetic_seed is not None and n_gpus > 1:
+        if synthetic_seed is not None and fmt:
+            rc = self.lib.l2b_create_synthetic_format(C.byref(self.h), C.byref(self.cfg), synthetic_seed, fmt)
+        elif synthetic_seed is not None and n_gpus > 1:
             rc = self.lib.l2b_create_synthetic_group(C.byref(self.h), C.byref(self.cfg), synthetic_seed, n_gpus)
         elif synthetic_seed is not None:
             rc = self.lib.l2b_create_synthetic(C.byref(self.h), C.byref(self.cfg), synthetic_seed,
@@ -218,7 +244,10 @@ class Transformer:
             if rope_cos is not None:
                 self._rc, rcos = _f32(rope_cos)
                 self._rs, rsin = _f32(rope_sin)
-            if shard is None:
+            if fmt:
+                rc = self.lib.l2b_create_format(C.byref(self.h), C.byref(self.cfg), cp, data.size, rcos, rsin,
+                                                n_gpus, fmt)
+            elif shard is None:
                 rc = self.lib.l2b_create(C.byref(self.h), C.byref(self.cfg), cp, data.size, rcos, rsin, n_gpus)
             else:
                 rc = self.lib.l2b_create_sharded(C.byref(self.h), C.byref(self.cfg), cp, data.size, rcos,
@@ -320,6 +349,14 @@ class Transformer:
         if n.value > 0:
             arr = np.frombuffer(cand, dtype=[("prob", "<f4"), ("index", "<i4")], count=n.value).copy()
         return (probs, arr, n.value) if with_count else (probs, arr)
+
+    def weight_info(self):
+        """(weight_format name, n_rounded): the device format of the model's matrix weights and how many
+        of them the bf16 rounding changed (l2b_weight_info)."""
+        fmt = C.c_int32()
+        n = C.c_uint64()
+        _check(self.lib.l2b_weight_info(self.h, C.byref(fmt), C.byref(n)), self.h)
+        return {v: k for k, v in WEIGHT_FORMATS.items()}[fmt.value], n.value
 
     def load_stats(self):
         ms = C.c_double()

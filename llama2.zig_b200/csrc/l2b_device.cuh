@@ -9,6 +9,7 @@
 #pragma once
 
 #include <cooperative_groups.h>
+#include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -177,6 +178,61 @@ __device__ __forceinline__ float dot4(const float4 a, const float4 b, float acc)
     return acc;
 }
 
+// ---------------------------------------------------------------------------------------
+// Weight element type.  Matrix weights live on the device as fp32 (W = float) or bf16 (W = bf16).
+// Every kernel that reads weights takes W as a template parameter; a thread owns the same float4
+// column groups in both (a bf16 group is 4 elements, 8 bytes) and widens each weight exactly, so a
+// bf16 kernel computes exactly what its fp32 twin computes on the rounded weights.  bf16 rows are
+// padded to a multiple of 8 elements (16 bytes, the TMA bulk-copy granule) with zeros no consumer
+// multiplies; fp32 rows are dense.
+// ---------------------------------------------------------------------------------------
+typedef __nv_bfloat16 bf16;
+
+template <typename W>
+__host__ __device__ __forceinline__ constexpr int w_pitch(int n) {
+    return sizeof(W) == 4 ? n : (n + 7) & ~7;
+}
+
+// nearest bf16, ties to even; +-inf stays, finite values past the bf16 maximum become +-inf, subnormals
+// are rounded (not flushed), NaN stays NaN (quietened).  The one rounding of the library: the host
+// upload, l2b_round_bf16_host and synth_fill_kernel all use it.
+__host__ __device__ __forceinline__ uint16_t bf16_round_bits(uint32_t u) {
+    if ((u & 0x7FFFFFFFu) > 0x7F800000u) return (uint16_t)((u >> 16) | 0x0040u);
+    return (uint16_t)((u + 0x7FFFu + ((u >> 16) & 1u)) >> 16);
+}
+
+__device__ __forceinline__ float4 widen_bf16x4(uint2 u) {
+    return make_float4(__uint_as_float(u.x << 16), __uint_as_float(u.x & 0xFFFF0000u),
+                       __uint_as_float(u.y << 16), __uint_as_float(u.y & 0xFFFF0000u));
+}
+
+// float4 column group c of a weight row in global memory (streaming, no L1 allocation)
+template <typename W>
+__device__ __forceinline__ float4 ldg_w4(const W *row, int c);
+template <>
+__device__ __forceinline__ float4 ldg_w4<float>(const float *row, int c) {
+    return ldg_stream(reinterpret_cast<const float4 *>(row) + c);
+}
+template <>
+__device__ __forceinline__ float4 ldg_w4<bf16>(const bf16 *row, int c) {
+    uint2 u;
+    asm("ld.global.nc.L1::no_allocate.v2.u32 {%0,%1}, [%2];"
+        : "=r"(u.x), "=r"(u.y)
+        : "l"(reinterpret_cast<const uint2 *>(row) + c));
+    return widen_bf16x4(u);
+}
+// float4 column group c of a weight row in shared memory
+template <typename W>
+__device__ __forceinline__ float4 lds_w4(const W *row, int c);
+template <>
+__device__ __forceinline__ float4 lds_w4<float>(const float *row, int c) {
+    return reinterpret_cast<const float4 *>(row)[c];
+}
+template <>
+__device__ __forceinline__ float4 lds_w4<bf16>(const bf16 *row, int c) {
+    return widen_bf16x4(reinterpret_cast<const uint2 *>(row)[c]);
+}
+
 // Orderable key for a device-side argmax with the reference's tie rule (src/main.zig:715-726:
 // strict '>' so the FIRST maximum wins): larger value wins, then smaller index.
 __device__ __forceinline__ unsigned long long argmax_key(float v, int idx) {
@@ -248,7 +304,7 @@ constexpr int PF_MAXB = 4;   // input vectors per weight pass of the batched ker
 struct GemvParams {
     // ---- input vector / prologue
     const float *x_in;      // n floats; when emb != nullptr: row `token` of emb is used instead
-    const float *emb;       // token embedding table (layer 0: x = emb[token], :295-296) or nullptr
+    const void *emb;        // token embedding table, element type W (layer 0: x = emb[token], :295-296) or nullptr
     const float *gamma;     // rmsnorm gain (n floats) => fused rmsnorm, or nullptr => plain staging
     float *x_out;           // CTA 0 writes the staged (un-normalised) x here: layer 0 (x = embedding row) and
                             // kernels that fold `parts` in (x_out must then differ from x_in)
@@ -257,8 +313,8 @@ struct GemvParams {
     const int *ctl;         // control block (token, pos, done, epoch, error)
     int n;                  // columns (multiple of 4)
     // ---- matrices (virtual row space depends on the epilogue)
-    const float *w0, *w1, *w2;
-    int rows0, rows1, rows2;  // EPI_QKV: q/k/v rows.  EPI_SILU: rows0 = hidden (virtual rows = 2*hidden)
+    const void *w0, *w1, *w2;   // element type W, rows w_pitch<W>(n) elements apart
+    int rows0, rows1, rows2; // EPI_QKV: q/k/v rows.  EPI_SILU: rows0 = hidden (virtual rows = 2*hidden)
     int total_rows;           // virtual rows
     // ---- outputs
     float *out0;            // STORE: out; QKV: q; SILU: hb; RESID: the residual stream x (read-modify-write)
@@ -297,19 +353,29 @@ struct GemvParams {
     const int *skip_b;
 };
 
-template <int EPI>
-__device__ __forceinline__ const float *gemv_row_ptr(const GemvParams &p, int v) {
+template <int EPI, typename W>
+__device__ __forceinline__ const W *gemv_row_ptr(const GemvParams &p, int v) {
+    const int ld = w_pitch<W>(p.n);
+    const W *w0 = static_cast<const W *>(p.w0), *w1 = static_cast<const W *>(p.w1), *w2 = static_cast<const W *>(p.w2);
     if (EPI == EPI_QKV) {
-        if (v < p.rows0) return p.w0 + (size_t)v * p.n;
+        if (v < p.rows0) return w0 + (size_t)v * ld;
         v -= p.rows0;
-        if (v < p.rows1) return p.w1 + (size_t)v * p.n;
+        if (v < p.rows1) return w1 + (size_t)v * ld;
         v -= p.rows1;
-        return p.w2 + (size_t)v * p.n;
+        return w2 + (size_t)v * ld;
     } else if (EPI == EPI_SILU) {
-        return ((v & 1) ? p.w1 : p.w0) + (size_t)(v >> 1) * p.n;
+        return ((v & 1) ? w1 : w0) + (size_t)(v >> 1) * ld;
     } else {
-        return p.w0 + (size_t)v * p.n;
+        return w0 + (size_t)v * ld;
     }
+}
+
+// bf16 only: row `token` of the embedding table, widened into the n floats at xs by the threads
+// idx = 0 .. nthreads-1 (a bulk copy cannot widen).  The caller orders it before the readers of xs.
+__device__ __forceinline__ void widen_emb_row(const GemvParams &p, int token, float *xs, int idx, int nthreads) {
+    const bf16 *row = static_cast<const bf16 *>(p.emb) + (size_t)token * w_pitch<bf16>(p.n);
+    for (int i = idx; i < (p.n >> 2); i += nthreads)
+        reinterpret_cast<float4 *>(xs)[i] = widen_bf16x4(__ldg(reinterpret_cast<const uint2 *>(row) + i));
 }
 
 // EPI_QKV, rows (v, v+1): an adjacent pair of q, k or v (segment sizes are even).  q and k pairs are
@@ -404,19 +470,24 @@ __device__ __forceinline__ void tp_reduce_tail(const GemvParams &p, unsigned int
 
 // ---- shared prologue: stage the activation vector (+ rmsnorm) into shared memory.
 // Must be called by all NT threads after pdl_wait(); thread 0 has already initialised `bar`.
+template <typename W>
 __device__ __forceinline__ void gemv_stage_input(const GemvParams &p, float *xs, float *aux,
                                                  uint64_t *bar, float *scratch) {
     const int tid = threadIdx.x;
     const int n4 = p.n >> 2;
-    const float *xsrc = p.emb ? p.emb + (size_t)p.ctl[CTL_TOKEN] * p.n : p.x_in;
+    const bool widen = sizeof(W) == 2 && p.emb;          // a bf16 embedding row is widened, not bulk-copied
     float *gs = aux;
     float *ps = p.gamma ? aux + p.n : aux;               // sum of the partial vectors (when p.parts)
     if (tid == 0) {
         const uint32_t bytes = (uint32_t)p.n * 4u;
-        mbar_expect_tx(bar, bytes * (1u + (p.gamma ? 1u : 0u)));
-        tma_load_1d(xs, xsrc, bytes, bar);
+        mbar_expect_tx(bar, bytes * ((widen ? 0u : 1u) + (p.gamma ? 1u : 0u)));
+        if (!widen) {
+            const float *xsrc = p.emb ? static_cast<const float *>(p.emb) + (size_t)p.ctl[CTL_TOKEN] * p.n : p.x_in;
+            tma_load_1d(xs, xsrc, bytes, bar);
+        }
         if (p.gamma) tma_load_1d(gs, p.gamma, bytes, bar);
     }
+    if (widen) widen_emb_row(p, p.ctl[CTL_TOKEN], xs, tid, NT);
     if (p.parts) {
         // the wo / w2 product arrives split into nparts partial vectors (by head / by hidden slice):
         // complete it in fixed order while the bulk copies are in flight
@@ -539,7 +610,7 @@ __device__ __forceinline__ void gemv_finish_argmax(const GemvParams &p, unsigned
 }
 
 // ---- v1: small / latency-bound shapes.  TPR threads per pair of rows, tiles strided over CTAs.
-template <int TPR, int EPI>
+template <int TPR, int EPI, typename W = float>
 __global__ void __launch_bounds__(NT) gemv_kernel(const GemvParams p) {
     constexpr int GROUPS = NT / TPR;           // row groups per CTA
     constexpr int TILE_ROWS = GROUPS * GEMV_R;
@@ -568,12 +639,11 @@ __global__ void __launch_bounds__(NT) gemv_kernel(const GemvParams p) {
         for (int r = 0; r < GEMV_R; ++r) {
             const int v = v0 + r;
             const bool rok = v < p.total_rows;
-            const float4 *wr =
-                reinterpret_cast<const float4 *>(gemv_row_ptr<EPI>(p, rok ? v : 0));
+            const W *wr = gemv_row_ptr<EPI, W>(p, rok ? v : 0);
 #pragma unroll
             for (int u = 0; u < GEMV_U; ++u) {
                 const int c = (ch * GEMV_U + u) * TPR + sub;
-                wv[r][u] = (rok && c < n4) ? ldg_stream(wr + c) : make_float4(0.f, 0.f, 0.f, 0.f);
+                wv[r][u] = (rok && c < n4) ? ldg_w4<W>(wr, c) : make_float4(0.f, 0.f, 0.f, 0.f);
             }
         }
     };
@@ -594,7 +664,7 @@ __global__ void __launch_bounds__(NT) gemv_kernel(const GemvParams p) {
     if (p.ctl[CTL_DONE]) return;  // generation loop already ended (BOS)
     if (p.bump_epoch && blockIdx.x == 0 && tid == 0) const_cast<int *>(p.ctl)[CTL_EPOCH] += 1;
     if (tid == 0) L2B_STAMP(p.trace, 2);
-    gemv_stage_input(p, xs, aux, &bar, scratch);
+    gemv_stage_input<W>(p, xs, aux, &bar, scratch);
     if (tid == 0) L2B_STAMP(p.trace, 3);
 
     const float4 *xs4 = reinterpret_cast<const float4 *>(xs);
@@ -738,7 +808,7 @@ __device__ __forceinline__ float2 sum_warp_partials(const float (&red)[NWARP][GE
     return make_float2(s0, s1);
 }
 
-template <int EPI>
+template <int EPI, typename W = float>
 __global__ void __launch_bounds__(NT, 2) gemv8_kernel(const GemvParams p) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     float *xs = reinterpret_cast<float *>(smem_raw);
@@ -764,8 +834,8 @@ __global__ void __launch_bounds__(NT, 2) gemv8_kernel(const GemvParams p) {
         for (int r = 0; r < GEMV8_R; ++r) {
             const int v = v0 + r;
             const bool ok = (v < r1) && (c < n4);
-            const float4 *wr = reinterpret_cast<const float4 *>(gemv_row_ptr<EPI>(p, ok ? v : 0));
-            w[r] = ok ? ldg_stream(wr + c) : make_float4(0.f, 0.f, 0.f, 0.f);
+            const W *wr = gemv_row_ptr<EPI, W>(p, ok ? v : 0);
+            w[r] = ok ? ldg_w4<W>(wr, c) : make_float4(0.f, 0.f, 0.f, 0.f);
         }
     };
     if (0 < total) issue(wa, 0);
@@ -780,7 +850,7 @@ __global__ void __launch_bounds__(NT, 2) gemv8_kernel(const GemvParams p) {
     pdl_wait();
     if (p.ctl[CTL_DONE]) return;
     if (p.bump_epoch && blockIdx.x == 0 && tid == 0) const_cast<int *>(p.ctl)[CTL_EPOCH] += 1;
-    gemv_stage_input(p, xs, aux, &bar, scratch);
+    gemv_stage_input<W>(p, xs, aux, &bar, scratch);
 
     const float4 *xs4 = reinterpret_cast<const float4 *>(xs);
     const int pos = p.ctl[CTL_POS];
@@ -869,15 +939,27 @@ __device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
 // `ring`.  full[s]: slot s has landed (producer -> consumers); empty[s]: all NWARP consumer warps are
 // done with it.  The slot size only sets how finely the ring's shared memory is cut: the consumers
 // read the same columns of the same rows in the same order whatever SR is.
-template <int SR>
+// W: the weight element type.  A row's part of a slot is NT float4 column groups whatever W is, so a
+// bf16 slot of SR rows is half the bytes of an fp32 one.  A bf16 row's last chunk is copied whole to
+// its 16-byte end (a row of n = 4 mod 8 columns ends on its zero padding).
+template <int SR, typename W = float>
 struct TmaRing {
     static constexpr int SUB = GEMV8_R / SR;                           // slots per (tile, column step)
-    static constexpr int SLOT_FLOATS = SR * NT * 4;
+    static constexpr int SLOT_ELEMS = SR * NT * 4;
+    static constexpr int SLOT_BYTES = SLOT_ELEMS * (int)sizeof(W);
     static_assert(SR * SUB == GEMV8_R, "a tile is a whole number of slots");
-    float *ring;
+    static __device__ __forceinline__ uint32_t chunk_bytes(int cols4) {
+        return sizeof(W) == 4 ? (uint32_t)(cols4 * 16) : (uint32_t)((cols4 * 8 + 15) & ~15);
+    }
+    W *ring;
     uint64_t *full, *empty;
     int nstage, n4, nsteps, r0, r1, total;
 };
+// gemv_tma_kernel's slot: 4 fp32 rows or 8 bf16 rows, 16 KB either way
+template <typename W>
+__host__ __device__ constexpr int tma_slot_rows() { return sizeof(W) == 4 ? TMA_SLOT_ROWS : GEMV8_R; }
+static_assert(TmaRing<TMA_SLOT_ROWS, float>::SLOT_BYTES == TmaRing<tma_slot_rows<bf16>(), bf16>::SLOT_BYTES,
+              "both formats' decode rings have the same slot size");
 
 // The producer warp's place in the stream.  produce_one is executed by all 32 lanes of the warp:
 // lane r owns row r of the tile and issues its bulk copy into the slot that holds it, lane 0 owns
@@ -885,10 +967,10 @@ struct TmaRing {
 struct RingProducer {
     int it = 0, stage = 0, tile = 0, step = 0, sub = 0;
     uint32_t phase = 0;
-    const float *row = nullptr;                                        // this lane's row in the current tile
+    const void *row = nullptr;                                         // this lane's row in the current tile
 
-    template <int EPI, int SR>
-    __device__ __forceinline__ void produce_one(const GemvParams &p, const TmaRing<SR> &R, int lane) {
+    template <int EPI, int SR, typename W>
+    __device__ __forceinline__ void produce_one(const GemvParams &p, const TmaRing<SR, W> &R, int lane) {
         const int c0 = step * NT;                                      // first float4 column
         const int cols4 = min(NT, R.n4 - c0);
         const int v0 = R.r0 + tile * GEMV8_R;
@@ -898,15 +980,16 @@ struct RingProducer {
         constexpr bool whole = R.SUB == 1;
         const int lo = whole ? 0 : sub * SR;                           // the slot's first row of the tile
         const int srows = whole ? rows : max(0, min(SR, rows - lo));
-        if (step == 0 && (whole || sub == 0) && lane < rows) row = gemv_row_ptr<EPI>(p, v0 + lane);
+        if (step == 0 && (whole || sub == 0) && lane < rows) row = gemv_row_ptr<EPI, W>(p, v0 + lane);
+        const uint32_t bytes = R.chunk_bytes(cols4);
         if (lane == 0) {
             mbar_wait(&R.empty[stage], phase ^ 1);
-            mbar_expect_tx(&R.full[stage], (uint32_t)(srows * cols4 * 16));
+            mbar_expect_tx(&R.full[stage], (uint32_t)srows * bytes);
         }
         __syncwarp();
         if ((whole || lane >= lo) && lane < lo + srows)
-            tma_load_1d(R.ring + (size_t)stage * R.SLOT_FLOATS + (lane - lo) * NT * 4, row + (size_t)c0 * 4,
-                        (uint32_t)(cols4 * 16), &R.full[stage]);
+            tma_load_1d(R.ring + (size_t)stage * R.SLOT_ELEMS + (lane - lo) * NT * 4, static_cast<const W *>(row) + (size_t)c0 * 4,
+                        bytes, &R.full[stage]);
         ++it;
         if (whole || ++sub == R.SUB) {
             sub = 0;
@@ -993,8 +1076,8 @@ __device__ __forceinline__ void tma_rmsnorm(const GemvParams &p, float *xs, cons
 // (one LDS.128 of each x_b serves the tile's rows; vectors b >= nb read x_0 and are never stored).
 // At a tile's end the butterfly leaves the warp's row sums in red[t & 1] for the epilogue warp.
 // trace (decode only, else nullptr): the first slot's arrival (slot 4), the last one consumed (5).
-template <int NB, int SR>
-__device__ __forceinline__ void tma_consume(const TmaRing<SR> &R, const float *xs, int nb, TileRed<NB> &red,
+template <int NB, int SR, typename W>
+__device__ __forceinline__ void tma_consume(const TmaRing<SR, W> &R, const float *xs, int nb, TileRed<NB> &red,
                                             uint64_t *tile_full, uint64_t *tile_free, unsigned long long *trace) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const float4 *xs4 = reinterpret_cast<const float4 *>(xs);
@@ -1017,7 +1100,7 @@ __device__ __forceinline__ void tma_consume(const TmaRing<SR> &R, const float *x
             mbar_wait(&R.full[c_stage], c_phase);
             if (it == 0 && s == 0 && tid == 0) L2B_STAMP(trace, 4);
             if (c < R.n4) {
-                const float4 *w4 = reinterpret_cast<const float4 *>(R.ring + (size_t)c_stage * R.SLOT_FLOATS) + tid;
+                const W *slot = R.ring + (size_t)c_stage * R.SLOT_ELEMS;
                 if (s == 0) {
 #pragma unroll
                     for (int b = 0; b < NB; ++b) xv[b] = xs4[(size_t)(b < nb ? b : 0) * R.n4 + c];
@@ -1025,7 +1108,7 @@ __device__ __forceinline__ void tma_consume(const TmaRing<SR> &R, const float *x
 #pragma unroll
                 for (int r = 0; r < SR; ++r) {
                     if (s * SR + r < rows) {
-                        const float4 w = w4[r * NT];
+                        const float4 w = lds_w4<W>(slot, r * NT + tid);
 #pragma unroll
                         for (int b = 0; b < NB; ++b) acc[b][s * SR + r] = dot4(w, xv[b], acc[b][s * SR + r]);
                     }
@@ -1054,11 +1137,11 @@ __device__ __forceinline__ void tma_consume(const TmaRing<SR> &R, const float *x
     }
 }
 
-template <int EPI>
+template <int EPI, typename W = float>
 __global__ void __launch_bounds__(TMA_THREADS, 2) gemv_tma_kernel(const GemvParams p) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int NSTAGE = p.nstage;
-    float *ring = reinterpret_cast<float *>(smem_raw);                 // NSTAGE x 16 KB
+    W *ring = reinterpret_cast<W *>(smem_raw);                         // NSTAGE x 16 KB
     __shared__ uint64_t full[TMA_MAX_STAGES], empty[TMA_MAX_STAGES], xbar, tile_full[2], tile_free[2];
     __shared__ float scratch[1][NWARP + 2];
     __shared__ TileRed<1> red;
@@ -1070,9 +1153,9 @@ __global__ void __launch_bounds__(TMA_THREADS, 2) gemv_tma_kernel(const GemvPara
     const RowSplit split = cta_row_split(p.total_rows);
     const int r0 = split.r0, r1 = split.r1, ntiles = split.ntiles;
     const int total = ntiles * nsteps;
-    const TmaRing<TMA_SLOT_ROWS> R = {ring, full, empty, NSTAGE, n4, nsteps, r0, r1, total};
+    const TmaRing<tma_slot_rows<W>(), W> R = {ring, full, empty, NSTAGE, n4, nsteps, r0, r1, total};
     const int nslots = total * R.SUB;
-    float *xs = ring + (size_t)NSTAGE * R.SLOT_FLOATS;                 // n floats
+    float *xs = reinterpret_cast<float *>(smem_raw + (size_t)NSTAGE * R.SLOT_BYTES);   // n floats
 
     if (tid == 0) {
         L2B_STAMP(p.trace, 0);
@@ -1134,11 +1217,18 @@ __global__ void __launch_bounds__(TMA_THREADS, 2) gemv_tma_kernel(const GemvPara
 
     // stage the activation vector (consumer warps + epilogue warp; barrier 1 is theirs)
     {
-        const float *xsrc = p.emb ? p.emb + (size_t)p.ctl[CTL_TOKEN] * p.n : p.x_in;
+        const bool widen = sizeof(W) == 2 && p.emb;                    // a bf16 embedding row is widened, not bulk-copied
         if (tid == 0) {
             const uint32_t bytes = (uint32_t)p.n * 4u;
-            mbar_expect_tx(&xbar, bytes);
-            tma_load_1d(xs, xsrc, bytes, &xbar);
+            mbar_expect_tx(&xbar, widen ? 0u : bytes);
+            if (!widen) {
+                const float *xsrc = p.emb ? static_cast<const float *>(p.emb) + (size_t)p.ctl[CTL_TOKEN] * p.n : p.x_in;
+                tma_load_1d(xs, xsrc, bytes, &xbar);
+            }
+        }
+        if (widen) {
+            widen_emb_row(p, p.ctl[CTL_TOKEN], xs, ptid, TMA_PRO_THREADS);
+            named_bar_sync(1, TMA_PRO_THREADS);
         }
         // epilogue warp: this position's RoPE row.  The table row comes from DRAM on big models (the
         // weight stream evicts it), so it is only FETCHED here, into registers; it is parked in shared
@@ -1205,7 +1295,7 @@ __global__ void __launch_bounds__(TMA_THREADS, 2) gemv_tma_kernel(const GemvPara
         return;
     }
 
-    tma_consume<1, TMA_SLOT_ROWS>(R, xs, 1, red, tile_full, tile_free, p.trace);   // warps 0..7
+    tma_consume<1>(R, xs, 1, red, tile_full, tile_free, p.trace);   // warps 0..7
 }
 
 // ---- batched prompt prefill (SURVEY 8f.2): NB consecutive prompt positions share one pass over the
@@ -1226,13 +1316,16 @@ __global__ void __launch_bounds__(TMA_THREADS, 2) gemv_tma_kernel(const GemvPara
 // (l2b_generate_argmax_batch) skip_b keeps a stopped session's vector from appending KV rows, and once
 // every session has stopped (CTL_DONE) the launches still queued return at once.  Prefill and the
 // batched step clear CTL_DONE before they launch.
-template <int EPI, int NB>
+// bf16 (W = bf16): stages of 8 rows are 16 KB, so the same ring bytes hold twice as many stages
+// (the host passes nstage doubled).
+template <int EPI, int NB, typename W = float>
 __global__ void __launch_bounds__(TMA_THREADS, 1) prefill_gemm_kernel(const GemvParams p) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
+    constexpr int MAX_STAGES = PF_MAX_STAGES * (4 / (int)sizeof(W));
     const int NSTAGE = p.nstage;
-    float *ring = reinterpret_cast<float *>(smem_raw);                 // NSTAGE x 32 KB
-    float *xs = ring + (size_t)NSTAGE * TMA_STAGE_FLOATS;              // NB x n floats
-    __shared__ uint64_t full[PF_MAX_STAGES], empty[PF_MAX_STAGES], xbar, tile_full[2], tile_free[2];
+    W *ring = reinterpret_cast<W *>(smem_raw);                         // NSTAGE x 32 KB (fp32) or 16 KB (bf16)
+    float *xs = reinterpret_cast<float *>(smem_raw + (size_t)NSTAGE * TmaRing<GEMV8_R, W>::SLOT_BYTES);   // NB x n floats
+    __shared__ uint64_t full[MAX_STAGES], empty[MAX_STAGES], xbar, tile_full[2], tile_free[2];
     __shared__ float scratch[NB][NWARP + 2];
     __shared__ TileRed<NB> red;
     __shared__ float rope_s[NB][2][128];                               // cos/sin rows of pos_b[0 .. NB-1]
@@ -1243,7 +1336,7 @@ __global__ void __launch_bounds__(TMA_THREADS, 1) prefill_gemm_kernel(const Gemv
     const RowSplit split = cta_row_split(p.total_rows);
     const int r0 = split.r0, r1 = split.r1, ntiles = split.ntiles;
     const int total = ntiles * nsteps;
-    const TmaRing<GEMV8_R> R = {ring, full, empty, NSTAGE, n4, nsteps, r0, r1, total};
+    const TmaRing<GEMV8_R, W> R = {ring, full, empty, NSTAGE, n4, nsteps, r0, r1, total};
 
     if (tid == 0) {
         for (int s = 0; s < NSTAGE; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], NWARP); }
@@ -1274,15 +1367,20 @@ __global__ void __launch_bounds__(TMA_THREADS, 1) prefill_gemm_kernel(const Gemv
     if (p.gamma) tma_fetch_gain(p, gv, ptid, n4);
     pdl_wait();
     const bool done = p.ctl[CTL_DONE] != 0;                            // read while x is staged below
+    const bool widen = sizeof(W) == 2 && p.emb;                        // bf16 embedding rows are widened, not bulk-copied
     if (tid == 0) {
         const uint32_t bytes = (uint32_t)p.n * 4u;
-        mbar_expect_tx(&xbar, bytes * (uint32_t)p.nb);
+        mbar_expect_tx(&xbar, widen ? 0u : bytes * (uint32_t)p.nb);
         if (p.emb) {
-            for (int b = 0; b < p.nb; ++b)                              // x[b] = token_embedding_table[tokens[b]], :295-296
-                tma_load_1d(xs + (size_t)b * p.n, p.emb + (size_t)p.tokens[b] * p.n, bytes, &xbar);
+            for (int b = 0; b < p.nb && !widen; ++b)                    // x[b] = token_embedding_table[tokens[b]], :295-296
+                tma_load_1d(xs + (size_t)b * p.n, static_cast<const float *>(p.emb) + (size_t)p.tokens[b] * p.n, bytes, &xbar);
         } else {
             tma_load_1d(xs, p.x_in, bytes * (uint32_t)p.nb, &xbar);
         }
+    }
+    if (widen) {
+        for (int b = 0; b < p.nb; ++b) widen_emb_row(p, p.tokens[b], xs + (size_t)b * p.n, ptid, TMA_PRO_THREADS);
+        named_bar_sync(1, TMA_PRO_THREADS);
     }
     if (EPI == EPI_QKV && tid >= NT + 32) {                            // epilogue warp: RoPE rows of the vectors' positions
         const int half = p.head_size >> 1;
@@ -1351,7 +1449,7 @@ __global__ void __launch_bounds__(TMA_THREADS, 1) prefill_gemm_kernel(const Gemv
         return;
     }
 
-    tma_consume<NB, GEMV8_R>(R, xs, p.nb, red, tile_full, tile_free, nullptr);   // warps 0..7
+    tma_consume<NB>(R, xs, p.nb, red, tile_full, tile_free, nullptr);   // warps 0..7
 }
 
 // Scalar fallback for shapes the vector kernel cannot take (n % 4 != 0 or unaligned rows):
@@ -1776,12 +1874,12 @@ __global__ void __launch_bounds__(NT) attention_flash_kernel(const AttnParams p,
 // ---------------------------------------------------------------------------------------
 struct AttnWoParams {
     AttnParams a;
-    const float *wo;        // this layer's (dim, q_dim) row-major
+    const void *wo;         // this layer's (dim, q_dim) row-major, element type W, rows w_pitch<W>(q_dim) apart
     float *parts;           // (n_heads, dim)
     int dim, q_dim;
 };
 
-template <int NF>   // float4 per lane per row: head_size = 4 * NF * LPR
+template <int NF, typename W = float>   // float4 per lane per row: head_size = 4 * NF * LPR
 __global__ void __launch_bounds__(NT) attn_wo_kernel(const AttnWoParams q) {
     namespace cg = cooperative_groups;
     cg::cluster_group cluster = cg::this_cluster();
@@ -1801,14 +1899,14 @@ __global__ void __launch_bounds__(NT) attn_wo_kernel(const AttnWoParams q) {
     // rows of the wo slice this CTA produces; the first pass of weights is immutable: fetch it now
     const int rows_per = (q.dim + R - 1) / R;
     const int r0 = s * rows_per, r1 = min(q.dim, r0 + rows_per);
-    const float4 *wo4 = reinterpret_cast<const float4 *>(q.wo) + (size_t)h * hs4;
-    const int q4 = q.q_dim >> 2;
+    const W *woh = static_cast<const W *>(q.wo) + (size_t)h * hs;     // column h * hs of row 0
+    const int ld = w_pitch<W>(q.q_dim);
     float4 wpre[NF];
     {
         const int row = r0 + warp * RPW + rw;
 #pragma unroll
         for (int f = 0; f < NF; ++f)
-            wpre[f] = (row < r1) ? ldg_stream(wo4 + (size_t)row * q4 + lr + f * LPR) : make_float4(0.f, 0.f, 0.f, 0.f);
+            wpre[f] = (row < r1) ? ldg_w4<W>(woh + (size_t)row * ld, lr + f * LPR) : make_float4(0.f, 0.f, 0.f, 0.f);
     }
     pdl_launch_dependents();
     pdl_wait();
@@ -1917,7 +2015,7 @@ __global__ void __launch_bounds__(NT) attn_wo_kernel(const AttnWoParams q) {
 #pragma unroll
         for (int f = 0; f < NF; ++f) {
             const float4 w = first ? wpre[f]
-                                   : (valid ? ldg_stream(wo4 + (size_t)row * q4 + lr + f * LPR) : make_float4(0.f, 0.f, 0.f, 0.f));
+                                   : (valid ? ldg_w4<W>(woh + (size_t)row * ld, lr + f * LPR) : make_float4(0.f, 0.f, 0.f, 0.f));
             a = dot4(w, xb4[lr + f * LPR], a);
         }
         first = false;
@@ -2350,6 +2448,13 @@ __host__ __device__ __forceinline__ int32_t synth_irwin_hall(uint64_t tensor_see
     return (int32_t)((h & 0xFFFF) + ((h >> 16) & 0xFFFF) + ((h >> 32) & 0xFFFF) + ((h >> 48) & 0xFFFF)) -
            131070;
 }
+// element i of a tensor: the value both device generators write (l2b_synth_fill_host mirrors it)
+__device__ __forceinline__ float synth_value(uint64_t tensor_seed, uint64_t i, double mean, double scale, float lo,
+                                             float hi) {
+    const int32_t s = synth_irwin_hall(tensor_seed, i);
+    const float v = (float)__dadd_rn(__dmul_rn((double)s, scale), mean);
+    return fminf(fmaxf(v, lo), hi);
+}
 // rows x cols window of a (.., src_cols) tensor starting at element `first`, written densely
 __global__ void synth_fill_kernel(float *dst, uint64_t rows, uint64_t cols, uint64_t first,
                                   uint64_t src_cols, uint64_t tensor_seed, double mean, double scale,
@@ -2359,11 +2464,29 @@ __global__ void synth_fill_kernel(float *dst, uint64_t rows, uint64_t cols, uint
          j += (uint64_t)gridDim.x * blockDim.x) {
         const uint64_t r = j / cols, c = j - r * cols;
         const uint64_t i = first + r * src_cols + c;
-        const int32_t s = synth_irwin_hall(tensor_seed, i);
-        float v = (float)__dadd_rn(__dmul_rn((double)s, scale), mean);
-        v = fminf(fmaxf(v, lo), hi);
+        const float v = synth_value(tensor_seed, i, mean, scale, lo, hi);
         dst[j] = v;
     }
+}
+// The same values rounded to bf16 (bf16_round_bits), rows w_pitch<bf16>(cols) apart (the padding is
+// the caller's zeros); the weights the rounding changed are added to *n_rounded.
+__global__ void synth_fill_bf16_kernel(uint16_t *dst, uint64_t rows, uint64_t cols, uint64_t first,
+                                       uint64_t src_cols, uint64_t tensor_seed, double mean, double scale,
+                                       float lo, float hi, unsigned long long *n_rounded) {
+    const uint64_t total = rows * cols, ld = (uint64_t)w_pitch<bf16>((int)cols);
+    unsigned long long changed = 0;
+    for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < total;
+         j += (uint64_t)gridDim.x * blockDim.x) {
+        const uint64_t r = j / cols, c = j - r * cols;
+        const uint64_t i = first + r * src_cols + c;
+        const float v = synth_value(tensor_seed, i, mean, scale, lo, hi);
+        const uint32_t u = __float_as_uint(v);
+        const uint16_t b = bf16_round_bits(u);
+        changed += ((uint32_t)b << 16) != u;
+        dst[r * ld + c] = b;
+    }
+    changed = __reduce_add_sync(0xffffffffu, (unsigned int)changed);
+    if ((threadIdx.x & 31) == 0 && changed) atomicAdd(n_rounded, changed);
 }
 
 }  // namespace l2b

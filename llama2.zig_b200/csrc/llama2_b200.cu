@@ -107,9 +107,15 @@ struct l2b_ctx {
     int q_loc = 0, kv_loc = 0, hid_loc = 0, heads_loc = 0, vocab_loc = 0;
     // device weights (Weights, src/main.zig:53-71), this rank's slices, owned by `weights`
     SharedWeights *weights = nullptr;
-    float *emb = nullptr, *rms_att = nullptr, *rms_ffn = nullptr, *rms_final = nullptr;
-    float *wq = nullptr, *wk = nullptr, *wv = nullptr, *wo = nullptr;
-    float *w1 = nullptr, *w2 = nullptr, *w3 = nullptr, *wcls = nullptr;
+    float *rms_att = nullptr, *rms_ffn = nullptr, *rms_final = nullptr;
+    // matrix weights in the device format `wfmt` (l2b_weight_format): fp32, or bf16 with rows padded to
+    // w_pitch<bf16>(cols) elements; address them with wrow()
+    int wfmt = L2B_WEIGHTS_F32;
+    uint64_t n_rounded = 0;                  // matrix weights the bf16 rounding changed (l2b_weight_info)
+    unsigned long long *d_rounded = nullptr; // ... counted on the device while synthetic weights are generated
+    void *emb = nullptr;
+    void *wq = nullptr, *wk = nullptr, *wv = nullptr, *wo = nullptr;
+    void *w1 = nullptr, *w2 = nullptr, *w3 = nullptr, *wcls = nullptr;
     // device run state (RunState, :119-135)
     float *X = nullptr;                      // residual stream x; wo / w2 add into it (:395, :422)
     float *Xalt = nullptr;                   // second copy: kernels that fold partial vectors in write the new x here (ping-pong)
@@ -253,6 +259,15 @@ int dev_alloc(l2b_ctx *ctx, T **p, size_t count, std::vector<void *> *owner = nu
     return L2B_OK;
 }
 
+// ---- device weight format ----
+bool is_bf16(const l2b_ctx *ctx) { return ctx->wfmt == L2B_WEIGHTS_BF16; }
+size_t w_elem(const l2b_ctx *ctx) { return is_bf16(ctx) ? 2 : 4; }
+uint64_t w_ld(const l2b_ctx *ctx, uint64_t cols) { return is_bf16(ctx) ? (uint64_t)w_pitch<bf16>((int)cols) : cols; }
+// row `row` of a matrix of `cols` columns that starts at base
+const void *wrow(const l2b_ctx *ctx, const void *base, uint64_t row, uint64_t cols) {
+    return static_cast<const unsigned char *>(base) + row * w_ld(ctx, cols) * w_elem(ctx);
+}
+
 // ---- shape validation (the reference's asserts, src/main.zig:433-434,:534-540,:658-661) ----
 int validate_config(const l2b_config *c, int world, std::string *why) {
     auto bad = [&](const char *m) { *why = m; return L2B_ERR_UNSUPPORTED; };
@@ -301,7 +316,7 @@ struct Source {
 // in chunks through two pinned buffers: while chunk k is in flight on the copy engine, the host
 // is already filling the other buffer with chunk k+1 (for column-sharded tensors the host-side
 // fill also compacts the strided window, so the DMA is always a dense 1-D copy).
-int upload(l2b_ctx *ctx, float *dst, const float *src, uint64_t rows, uint64_t cols, uint64_t src_pitch) {
+int upload(l2b_ctx *ctx, void *dst, const float *src, uint64_t rows, uint64_t cols, uint64_t src_pitch, bool bf16w) {
     if (!ctx->stage[0]) {
         size_t want = 32ull << 20;
         const char *env = getenv("L2B_STAGE_MB");
@@ -312,8 +327,11 @@ int upload(l2b_ctx *ctx, float *dst, const float *src, uint64_t rows, uint64_t c
             L2B_CUDA(ctx, cudaEventCreateWithFlags(&ctx->stage_ev[i], cudaEventDisableTiming));
         }
     }
-    const uint64_t row_bytes = cols * sizeof(float);
-    const bool dense = (src_pitch == cols);
+    // bf16: each row is rounded (bf16_round_bits) and padded with zeros to w_ld elements while it is
+    // packed into the stage, so the DMA moves dense bf16 rows
+    const uint64_t ld = bf16w ? (uint64_t)w_pitch<bf16>((int)cols) : cols;
+    const uint64_t row_bytes = bf16w ? ld * 2 : cols * sizeof(float);
+    const bool dense = (src_pitch == cols) && !bf16w;
     const uint64_t total = rows * row_bytes;
     uint64_t done = 0;                       // bytes of the dense destination already issued
     while (done < total) {
@@ -321,7 +339,26 @@ int upload(l2b_ctx *ctx, float *dst, const float *src, uint64_t rows, uint64_t c
         ctx->stage_next ^= 1;
         L2B_CUDA(ctx, cudaEventSynchronize(ctx->stage_ev[b]));   // previous DMA out of this buffer finished
         uint64_t chunk = total - done < ctx->stage_bytes ? total - done : ctx->stage_bytes;
-        if (!dense) {
+        if (bf16w) {
+            const uint64_t r = chunk / row_bytes;
+            if (r == 0) return fail(ctx, L2B_ERR_UNSUPPORTED, "row larger than the upload staging buffer");
+            chunk = r * row_bytes;
+            const uint64_t row0 = done / row_bytes;
+            uint16_t *o = reinterpret_cast<uint16_t *>(ctx->stage[b]);
+            uint64_t changed = 0;
+            for (uint64_t i = 0; i < r; ++i) {
+                const float *s = src + (row0 + i) * src_pitch;
+                uint16_t *d = o + i * ld;
+                for (uint64_t c = 0; c < cols; ++c) {
+                    uint32_t u;
+                    memcpy(&u, s + c, 4);
+                    d[c] = bf16_round_bits(u);
+                    changed += ((uint32_t)d[c] << 16) != u;
+                }
+                for (uint64_t c = cols; c < ld; ++c) d[c] = 0;
+            }
+            ctx->n_rounded += changed;
+        } else if (!dense) {
             // whole rows only (a chunk never splits a row of a sharded window)
             uint64_t r = chunk / row_bytes;
             if (r == 0) return fail(ctx, L2B_ERR_UNSUPPORTED, "row larger than the upload staging buffer");
@@ -341,24 +378,33 @@ int upload(l2b_ctx *ctx, float *dst, const float *src, uint64_t rows, uint64_t c
     return L2B_OK;
 }
 
-int materialize(l2b_ctx *ctx, float **dptr, const Source &src, uint64_t payload_off, int tensor_id,
-                uint64_t L, uint64_t rows, uint64_t cols, ShardMode mode, Dist dist) {
+// matrix: a weight matrix, stored in the context's format (wfmt); otherwise fp32 (RMSNorm gains).
+// A bf16 matrix is only ever whole (single GPU).
+int materialize(l2b_ctx *ctx, void **dptr, const Source &src, uint64_t payload_off, int tensor_id,
+                uint64_t L, uint64_t rows, uint64_t cols, ShardMode mode, Dist dist, bool matrix) {
     const uint64_t g = ctx->world, r = ctx->rank;
     const uint64_t rows_loc = (mode == SH_ROWS) ? rows / g : rows;
     const uint64_t cols_loc = (mode == SH_COLS) ? cols / g : cols;
     const uint64_t row0 = (mode == SH_ROWS) ? r * rows_loc : 0;
     const uint64_t col0 = (mode == SH_COLS) ? r * cols_loc : 0;
-    int rc = dev_alloc(ctx, dptr, L * rows_loc * cols_loc, &ctx->weights->owned);
+    const bool bf16w = matrix && is_bf16(ctx);
+    const uint64_t ld = bf16w ? (uint64_t)w_pitch<bf16>((int)cols_loc) : cols_loc;
+    const size_t esize = bf16w ? 2 : 4;
+    unsigned char *base = nullptr;
+    int rc = dev_alloc(ctx, &base, L * rows_loc * ld * esize, &ctx->weights->owned);
     if (rc) return rc;
+    *dptr = base;
     const uint64_t tensor_seed = mix64(src.seed * 1000003ull + (uint64_t)tensor_id);
     const bool whole = (rows_loc == rows && cols_loc == cols);
     const uint64_t nl = whole ? 1 : L;            // one shot when nothing is cut
     const uint64_t rr = whole ? L * rows : rows_loc;
+    if (bf16w && !src.host)     // the row padding; the upload writes its own zeros
+        L2B_CUDA(ctx, cudaMemsetAsync(base, 0, L * rows_loc * ld * esize, ctx->stream));
     for (uint64_t l = 0; l < nl; ++l) {
-        float *dst = *dptr + l * rows_loc * cols_loc;
+        void *dst = base + l * rows_loc * ld * esize;
         const uint64_t first = l * rows * cols + row0 * cols + col0;
         if (src.host) {
-            rc = upload(ctx, dst, src.host + payload_off + first, rr, cols_loc, cols);
+            rc = upload(ctx, dst, src.host + payload_off + first, rr, cols_loc, cols, bf16w);
             if (rc) return rc;
         } else {
             const uint64_t total = rr * cols_loc;
@@ -366,37 +412,52 @@ int materialize(l2b_ctx *ctx, float **dptr, const Source &src, uint64_t payload_
                                    ? (total + 255) / 256
                                    : (uint64_t)(ctx->num_sms * 16));
             if (blocks < 1) blocks = 1;
-            synth_fill_kernel<<<blocks, 256, 0, ctx->stream>>>(dst, rr, cols_loc, first, cols, tensor_seed,
-                                                               dist.mean, dist.sigma * kSynthInvStd,
-                                                               dist.lo, dist.hi);
+            if (bf16w)
+                synth_fill_bf16_kernel<<<blocks, 256, 0, ctx->stream>>>(
+                    static_cast<uint16_t *>(dst), rr, cols_loc, first, cols, tensor_seed, dist.mean,
+                    dist.sigma * kSynthInvStd, dist.lo, dist.hi, ctx->d_rounded);
+            else
+                synth_fill_kernel<<<blocks, 256, 0, ctx->stream>>>(static_cast<float *>(dst), rr, cols_loc, first, cols,
+                                                                   tensor_seed, dist.mean, dist.sigma * kSynthInvStd,
+                                                                   dist.lo, dist.hi);
             L2B_CUDA(ctx, cudaGetLastError());
         }
     }
     return L2B_OK;
 }
+int materialize(l2b_ctx *ctx, float **dptr, const Source &src, uint64_t payload_off, int tensor_id,
+                uint64_t L, uint64_t rows, uint64_t cols, ShardMode mode, Dist dist) {
+    void *p = nullptr;
+    const int rc = materialize(ctx, &p, src, payload_off, tensor_id, L, rows, cols, mode, dist, false);
+    *dptr = static_cast<float *>(p);
+    return rc;
+}
 
 // ---- GEMV launch ---------------------------------------------------------------------------
 typedef void (*gemv_fn)(const GemvParams);
 
-template <int EPI>
+// Kernel instantiations by weight element type W.  EPI_XCHG (tensor parallel) has fp32 kernels only:
+// bf16 weights are single-GPU.
+template <int EPI, typename W>
 gemv_fn gemv_pick(int tpr) {
     switch (tpr) {
-    case 8: return gemv_kernel<8, EPI>;
-    case 16: return gemv_kernel<16, EPI>;
-    case 32: return gemv_kernel<32, EPI>;
-    case 64: return gemv_kernel<64, EPI>;
-    case 128: return gemv_kernel<128, EPI>;
-    default: return gemv_kernel<256, EPI>;
+    case 8: return gemv_kernel<8, EPI, W>;
+    case 16: return gemv_kernel<16, EPI, W>;
+    case 32: return gemv_kernel<32, EPI, W>;
+    case 64: return gemv_kernel<64, EPI, W>;
+    case 128: return gemv_kernel<128, EPI, W>;
+    default: return gemv_kernel<256, EPI, W>;
     }
 }
+template <typename W>
 gemv_fn gemv_pick(int epi, int tpr) {
     switch (epi) {
-    case EPI_XCHG: return gemv_pick<EPI_XCHG>(tpr);
-    case EPI_RESID: return gemv_pick<EPI_RESID>(tpr);
-    case EPI_STORE: return gemv_pick<EPI_STORE>(tpr);
-    case EPI_ARGMAX: return gemv_pick<EPI_ARGMAX>(tpr);
-    case EPI_QKV: return gemv_pick<EPI_QKV>(tpr);
-    default: return gemv_pick<EPI_SILU>(tpr);
+    case EPI_XCHG: return sizeof(W) == 4 ? gemv_pick<EPI_XCHG, float>(tpr) : nullptr;
+    case EPI_RESID: return gemv_pick<EPI_RESID, W>(tpr);
+    case EPI_STORE: return gemv_pick<EPI_STORE, W>(tpr);
+    case EPI_ARGMAX: return gemv_pick<EPI_ARGMAX, W>(tpr);
+    case EPI_QKV: return gemv_pick<EPI_QKV, W>(tpr);
+    default: return gemv_pick<EPI_SILU, W>(tpr);
     }
 }
 
@@ -424,26 +485,43 @@ int prof_mark(l2b_ctx *ctx, const char *name, int layer, uint64_t bytes, cudaStr
     return L2B_OK;
 }
 
+template <typename W>
 gemv_fn gemv_tma_pick(int epi) {
     switch (epi) {
-    case EPI_XCHG: return gemv_tma_kernel<EPI_XCHG>;
-    case EPI_RESID: return gemv_tma_kernel<EPI_RESID>;
-    case EPI_STORE: return gemv_tma_kernel<EPI_STORE>;
-    case EPI_ARGMAX: return gemv_tma_kernel<EPI_ARGMAX>;
-    case EPI_QKV: return gemv_tma_kernel<EPI_QKV>;
-    default: return gemv_tma_kernel<EPI_SILU>;
+    case EPI_XCHG: return sizeof(W) == 4 ? gemv_tma_kernel<EPI_XCHG, float> : nullptr;
+    case EPI_RESID: return gemv_tma_kernel<EPI_RESID, W>;
+    case EPI_STORE: return gemv_tma_kernel<EPI_STORE, W>;
+    case EPI_ARGMAX: return gemv_tma_kernel<EPI_ARGMAX, W>;
+    case EPI_QKV: return gemv_tma_kernel<EPI_QKV, W>;
+    default: return gemv_tma_kernel<EPI_SILU, W>;
     }
 }
 
+template <typename W>
 gemv_fn gemv8_pick(int epi) {
     switch (epi) {
-    case EPI_XCHG: return gemv8_kernel<EPI_XCHG>;
-    case EPI_RESID: return gemv8_kernel<EPI_RESID>;
-    case EPI_STORE: return gemv8_kernel<EPI_STORE>;
-    case EPI_ARGMAX: return gemv8_kernel<EPI_ARGMAX>;
-    case EPI_QKV: return gemv8_kernel<EPI_QKV>;
-    default: return gemv8_kernel<EPI_SILU>;
+    case EPI_XCHG: return sizeof(W) == 4 ? gemv8_kernel<EPI_XCHG, float> : nullptr;
+    case EPI_RESID: return gemv8_kernel<EPI_RESID, W>;
+    case EPI_STORE: return gemv8_kernel<EPI_STORE, W>;
+    case EPI_ARGMAX: return gemv8_kernel<EPI_ARGMAX, W>;
+    case EPI_QKV: return gemv8_kernel<EPI_QKV, W>;
+    default: return gemv8_kernel<EPI_SILU, W>;
     }
+}
+
+// GEMV kernel families: the latency kernel (gemv_kernel, tpr threads per row pair), the register-fed
+// 8-row kernel and the TMA ring
+enum GemvKind { GK_LATENCY, GK_ROWS8, GK_TMA };
+
+// the formats an epilogue has kernels in: EPI_XCHG (tensor parallel) is fp32 only
+bool has_kernel(const l2b_ctx *ctx, int epi) { return !(is_bf16(ctx) && epi == EPI_XCHG); }
+
+// The one place a GEMV kernel is chosen for the context's weight format.  The shape rules that pick
+// `kind` are the same for both formats (computed at 4 bytes per weight).
+gemv_fn pick_gemv(const l2b_ctx *ctx, GemvKind kind, int epi, int tpr) {
+    if (is_bf16(ctx))
+        return kind == GK_TMA ? gemv_tma_pick<bf16>(epi) : kind == GK_ROWS8 ? gemv8_pick<bf16>(epi) : gemv_pick<bf16>(epi, tpr);
+    return kind == GK_TMA ? gemv_tma_pick<float>(epi) : kind == GK_ROWS8 ? gemv8_pick<float>(epi) : gemv_pick<float>(epi, tpr);
 }
 
 cudaLaunchAttribute pdl_attr() {
@@ -473,12 +551,12 @@ int pf_ring_stages(size_t budget, size_t xbytes) {
 int launch_gemv(l2b_ctx *ctx, int epi, const GemvParams &p, cudaStream_t st, const char *name = "gemv",
                 int layer = -1) {
     {
-        int prc = prof_mark(ctx, name, layer, (uint64_t)p.total_rows * p.n * 4ull, st);
+        int prc = prof_mark(ctx, name, layer, (uint64_t)p.total_rows * w_ld(ctx, p.n) * w_elem(ctx), st);
         if (prc) return prc;
     }
     const size_t xbytes = (size_t)p.n * 4 * (1 + (p.gamma ? 1 : 0) + (p.parts ? 1 : 0));
     const size_t xonly = (size_t)p.n * 4;
-    const size_t slot_bytes = (size_t)TmaRing<TMA_SLOT_ROWS>::SLOT_FLOATS * 4;
+    const size_t slot_bytes = (size_t)TmaRing<TMA_SLOT_ROWS>::SLOT_BYTES;   // = TmaRing<GEMV8_R, bf16>::SLOT_BYTES
     // Decision from the shape.  Bandwidth-bound shapes take the TMA-ring kernel, latency-bound ones
     // the fine-grained kernel.  The ring kernel stages only x in shared memory; the rest of the
     // opt-in limit is its ring of 16 KB slots (13 next to a 16 KB x; DESIGN.md §4.1).
@@ -501,7 +579,8 @@ int launch_gemv(l2b_ctx *ctx, int epi, const GemvParams &p, cudaStream_t st, con
     if (smem > (size_t)kMaxSmemOptin) return fail(ctx, L2B_ERR_UNSUPPORTED, "activation vector too large for shared memory");
     if (tma && nstage < 2) return fail(ctx, L2B_ERR_UNSUPPORTED, "TMA ring of fewer than 2 stages");
     const int tpr = gemv_tpr(p.n);
-    gemv_fn fn = tma ? gemv_tma_pick(epi) : big ? gemv8_pick(epi) : gemv_pick(epi, tpr);
+    if (!has_kernel(ctx, epi)) return fail(ctx, L2B_ERR_UNSUPPORTED, "no kernel for this epilogue in the context's weight format");
+    gemv_fn fn = pick_gemv(ctx, tma ? GK_TMA : big ? GK_ROWS8 : GK_LATENCY, epi, tpr);
     if (!ctx->attr_done.count((const void *)fn)) {
         L2B_CUDA(ctx, cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmemOptin));
         ctx->attr_done.insert((const void *)fn);
@@ -566,22 +645,27 @@ attn_fn pick_attention(int head_size, bool flash, size_t *smem) {
 }
 
 typedef void (*attn_wo_fn)(const AttnWoParams);
-attn_wo_fn pick_attn_wo(int head_size, size_t *smem) {
+template <typename W>
+attn_wo_fn attn_wo_pick(int nf) {
+    switch (nf) {
+    case 1: return attn_wo_kernel<1, W>;
+    case 2: return attn_wo_kernel<2, W>;
+    case 3: return attn_wo_kernel<3, W>;
+    case 4: return attn_wo_kernel<4, W>;
+    case 5: return attn_wo_kernel<5, W>;
+    case 6: return attn_wo_kernel<6, W>;
+    case 8: return attn_wo_kernel<8, W>;
+    default: return nullptr;
+    }
+}
+// the attention + wo kernel for head_size in weight format wfmt (whether one exists does not depend on it)
+attn_wo_fn pick_attn_wo(int head_size, size_t *smem, int wfmt = L2B_WEIGHTS_F32) {
     const int hs4 = head_size / 4;
     const int lpr = (hs4 % 8 == 0) ? 8 : (hs4 % 4 == 0) ? 4 : (hs4 % 2 == 0) ? 2 : 1;
     const int nf = hs4 / lpr;
     const int ng = NWARP * (32 / lpr);
     *smem = ((size_t)ng * head_size + 3 * (size_t)ng + 2 * (size_t)head_size + 4) * sizeof(float);
-    switch (nf) {
-    case 1: return attn_wo_kernel<1>;
-    case 2: return attn_wo_kernel<2>;
-    case 3: return attn_wo_kernel<3>;
-    case 4: return attn_wo_kernel<4>;
-    case 5: return attn_wo_kernel<5>;
-    case 6: return attn_wo_kernel<6>;
-    case 8: return attn_wo_kernel<8>;
-    default: return nullptr;
-    }
+    return wfmt == L2B_WEIGHTS_BF16 ? attn_wo_pick<bf16>(nf) : attn_wo_pick<float>(nf);
 }
 
 constexpr int kAttnClusterCtas = 8;   // CTAs per head cluster of attn_wo_kernel; 4 and 2 measured slower (DESIGN.md §4.6)
@@ -604,12 +688,12 @@ int launch_attn_wo(l2b_ctx *ctx, int layer, cudaStream_t st) {
     a.kv_dim = ctx->kv_loc;
     a.kv_mul = ctx->kv_mul;
     a.trace = nullptr;
-    q.wo = ctx->wo + (size_t)layer * ctx->dim * ctx->q_loc;
+    q.wo = wrow(ctx, ctx->wo, (uint64_t)layer * ctx->dim, ctx->q_loc);
     q.parts = ctx->attn_parts;
     q.dim = ctx->dim;
     q.q_dim = ctx->q_loc;
     size_t smem = 0;
-    attn_wo_fn fn = pick_attn_wo(ctx->head_size, &smem);
+    attn_wo_fn fn = pick_attn_wo(ctx->head_size, &smem, ctx->wfmt);
     cudaLaunchConfig_t lc{};
     lc.gridDim = dim3(ctx->heads_loc, kAttnClusterCtas);
     lc.blockDim = dim3(NT);
@@ -730,9 +814,9 @@ LayerGemvs layer_gemvs(const l2b_ctx *ctx, int l) {
     p.ctl = ctx->ctl;
     p.n = dim;
     p.gamma = ctx->rms_att + (size_t)l * dim;
-    p.w0 = ctx->wq + (size_t)l * ctx->q_loc * dim;
-    p.w1 = ctx->wk + (size_t)l * ctx->kv_loc * dim;
-    p.w2 = ctx->wv + (size_t)l * ctx->kv_loc * dim;
+    p.w0 = wrow(ctx, ctx->wq, (uint64_t)l * ctx->q_loc, dim);
+    p.w1 = wrow(ctx, ctx->wk, (uint64_t)l * ctx->kv_loc, dim);
+    p.w2 = wrow(ctx, ctx->wv, (uint64_t)l * ctx->kv_loc, dim);
     p.rows0 = ctx->q_loc; p.rows1 = ctx->kv_loc; p.rows2 = ctx->kv_loc;
     p.total_rows = ctx->q_loc + 2 * ctx->kv_loc;
     const size_t loff = (size_t)l * ctx->cfg.seq_len * ctx->kv_loc;
@@ -743,20 +827,20 @@ LayerGemvs layer_gemvs(const l2b_ctx *ctx, int l) {
     // wo, whose result is added to the residual stream (:392-395)
     g.wo.ctl = ctx->ctl;
     g.wo.n = ctx->q_loc;
-    g.wo.w0 = ctx->wo + (size_t)l * dim * ctx->q_loc;
+    g.wo.w0 = wrow(ctx, ctx->wo, (uint64_t)l * dim, ctx->q_loc);
     g.wo.total_rows = dim; g.wo.rows0 = dim;
     // rmsnorm + w1,w3 + SiLU*mul (:398-416)
     g.w13.ctl = ctx->ctl;
     g.w13.n = dim;
     g.w13.gamma = ctx->rms_ffn + (size_t)l * dim;
-    g.w13.w0 = ctx->w1 + (size_t)l * ctx->hid_loc * dim;
-    g.w13.w1 = ctx->w3 + (size_t)l * ctx->hid_loc * dim;
+    g.w13.w0 = wrow(ctx, ctx->w1, (uint64_t)l * ctx->hid_loc, dim);
+    g.w13.w1 = wrow(ctx, ctx->w3, (uint64_t)l * ctx->hid_loc, dim);
     g.w13.rows0 = ctx->hid_loc;
     g.w13.total_rows = 2 * ctx->hid_loc;
     // w2, added to the residual stream (:419-422)
     g.w2.ctl = ctx->ctl;
     g.w2.n = ctx->hid_loc;
-    g.w2.w0 = ctx->w2 + (size_t)l * dim * ctx->hid_loc;
+    g.w2.w0 = wrow(ctx, ctx->w2, (uint64_t)l * dim, ctx->hid_loc);
     g.w2.total_rows = dim; g.w2.rows0 = dim;
     return g;
 }
@@ -1027,18 +1111,20 @@ int preload_kernels(l2b_ctx *ctx) {
     cudaFuncAttributes fa;
     const int tprs[] = {8, 16, 32, 64, 128, 256};
     for (int epi = 0; epi < EPI_COUNT; ++epi) {
-        for (int tpr : tprs) L2B_CUDA(ctx, cudaFuncGetAttributes(&fa, (const void *)gemv_pick(epi, tpr)));
-        L2B_CUDA(ctx, cudaFuncGetAttributes(&fa, (const void *)gemv8_pick(epi)));
-        L2B_CUDA(ctx, cudaFuncGetAttributes(&fa, (const void *)gemv_tma_pick(epi)));
+        if (!has_kernel(ctx, epi)) continue;
+        for (int tpr : tprs) L2B_CUDA(ctx, cudaFuncGetAttributes(&fa, (const void *)pick_gemv(ctx, GK_LATENCY, epi, tpr)));
+        L2B_CUDA(ctx, cudaFuncGetAttributes(&fa, (const void *)pick_gemv(ctx, GK_ROWS8, epi, 0)));
+        L2B_CUDA(ctx, cudaFuncGetAttributes(&fa, (const void *)pick_gemv(ctx, GK_TMA, epi, 0)));
     }
     size_t smem = 0;
     L2B_CUDA(ctx, cudaFuncGetAttributes(&fa, (const void *)pick_attention(ctx->head_size, true, &smem)));
-    if (pick_attn_wo(ctx->head_size, &smem)) L2B_CUDA(ctx, cudaFuncGetAttributes(&fa, (const void *)pick_attn_wo(ctx->head_size, &smem)));
+    if (attn_wo_fn aw = pick_attn_wo(ctx->head_size, &smem, ctx->wfmt)) L2B_CUDA(ctx, cudaFuncGetAttributes(&fa, (const void *)aw));
     const void *others[] = {(const void *)attention_kernel, (const void *)advance_kernel,
                             (const void *)batch_advance_kernel, (const void *)gather_logits_kernel,
                             (const void *)resid_add_kernel, (const void *)sample_prep_kernel,
                             (const void *)sample_prep_batch_kernel, (const void *)logprob_kernel,
                             (const void *)logprob_batch_kernel, (const void *)synth_fill_kernel,
+                            (const void *)synth_fill_bf16_kernel,
                             (const void *)kv_fork_kernel, (const void *)verify_accept_kernel};
     for (const void *f : others) L2B_CUDA(ctx, cudaFuncGetAttributes(&fa, f));
     // The kernels that run next to a TMA-ring GEMV in a decode step (the ring GEMVs, attention, the
@@ -1050,8 +1136,9 @@ int preload_kernels(l2b_ctx *ctx) {
     for (const void *f : decode)
         L2B_CUDA(ctx, cudaFuncSetAttribute(f, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
     for (int epi = 0; epi < EPI_COUNT; ++epi)
-        L2B_CUDA(ctx, cudaFuncSetAttribute((const void *)gemv_tma_pick(epi), cudaFuncAttributePreferredSharedMemoryCarveout,
-                                           cudaSharedmemCarveoutMaxShared));
+        if (has_kernel(ctx, epi))
+            L2B_CUDA(ctx, cudaFuncSetAttribute((const void *)pick_gemv(ctx, GK_TMA, epi, 0),
+                                               cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
     return L2B_OK;
 }
 
@@ -1109,21 +1196,31 @@ int create_rank(l2b_ctx *ctx, const l2b_config *cfg, const Source &src, const fl
     const uint64_t o_wcls = off;
 
     const auto t_load0 = std::chrono::steady_clock::now();
-    L2B_TRY(materialize(ctx, &ctx->emb, src, o_emb, 1, 1, V, dim, SH_NONE, {0.0, 0.04, -BIG, BIG}));
+    if (is_bf16(ctx) && !src.host) {
+        L2B_TRY(dev_alloc(ctx, &ctx->d_rounded, 1));
+        L2B_TRY(cuda_try(ctx, cudaMemsetAsync(ctx->d_rounded, 0, sizeof(unsigned long long), ctx->stream), "memset"));
+    }
+    L2B_TRY(materialize(ctx, &ctx->emb, src, o_emb, 1, 1, V, dim, SH_NONE, {0.0, 0.04, -BIG, BIG}, true));
     L2B_TRY(materialize(ctx, &ctx->rms_att, src, o_ratt, 2, 1, L, dim, SH_NONE, {1.35, 0.35, 0.25f, 2.4f}));
-    L2B_TRY(materialize(ctx, &ctx->wq, src, o_wq, 3, L, dim, dim, SH_ROWS, {0.0, 0.04 * sd, -BIG, BIG}));
-    L2B_TRY(materialize(ctx, &ctx->wk, src, o_wk, 4, L, kvd, dim, SH_ROWS, {0.0, 0.04 * sd, -BIG, BIG}));
-    L2B_TRY(materialize(ctx, &ctx->wv, src, o_wv, 5, L, kvd, dim, SH_ROWS, {0.0, 0.02 * sd, -BIG, BIG}));
-    L2B_TRY(materialize(ctx, &ctx->wo, src, o_wo, 6, L, dim, dim, SH_COLS, {0.0, 0.02 * sd, -BIG, BIG}));
+    L2B_TRY(materialize(ctx, &ctx->wq, src, o_wq, 3, L, dim, dim, SH_ROWS, {0.0, 0.04 * sd, -BIG, BIG}, true));
+    L2B_TRY(materialize(ctx, &ctx->wk, src, o_wk, 4, L, kvd, dim, SH_ROWS, {0.0, 0.04 * sd, -BIG, BIG}, true));
+    L2B_TRY(materialize(ctx, &ctx->wv, src, o_wv, 5, L, kvd, dim, SH_ROWS, {0.0, 0.02 * sd, -BIG, BIG}, true));
+    L2B_TRY(materialize(ctx, &ctx->wo, src, o_wo, 6, L, dim, dim, SH_COLS, {0.0, 0.02 * sd, -BIG, BIG}, true));
     L2B_TRY(materialize(ctx, &ctx->rms_ffn, src, o_rffn, 7, 1, L, dim, SH_NONE, {1.35, 0.35, 0.25f, 2.4f}));
-    L2B_TRY(materialize(ctx, &ctx->w1, src, o_w1, 8, L, hid, dim, SH_ROWS, {0.0, 0.026 * sd, -BIG, BIG}));
-    L2B_TRY(materialize(ctx, &ctx->w2, src, o_w2, 9, L, dim, hid, SH_COLS, {0.0, 0.026 * sh, -BIG, BIG}));
-    L2B_TRY(materialize(ctx, &ctx->w3, src, o_w3, 10, L, hid, dim, SH_ROWS, {0.0, 0.026 * sd, -BIG, BIG}));
+    L2B_TRY(materialize(ctx, &ctx->w1, src, o_w1, 8, L, hid, dim, SH_ROWS, {0.0, 0.026 * sd, -BIG, BIG}, true));
+    L2B_TRY(materialize(ctx, &ctx->w2, src, o_w2, 9, L, dim, hid, SH_COLS, {0.0, 0.026 * sh, -BIG, BIG}, true));
+    L2B_TRY(materialize(ctx, &ctx->w3, src, o_w3, 10, L, hid, dim, SH_ROWS, {0.0, 0.026 * sd, -BIG, BIG}, true));
     L2B_TRY(materialize(ctx, &ctx->rms_final, src, o_rfin, 11, 1, 1, dim, SH_NONE, {7.1, 0.6, 3.0f, 10.0f}));
     if (cfg->shared_weights) {
-        ctx->wcls = ctx->emb + (size_t)rank * ctx->vocab_loc * dim;   // :112
+        ctx->wcls = const_cast<void *>(wrow(ctx, ctx->emb, (uint64_t)rank * ctx->vocab_loc, dim));   // :112
     } else {
-        L2B_TRY(materialize(ctx, &ctx->wcls, src, o_wcls, 14, 1, V, dim, SH_ROWS, {0.0, 0.04, -BIG, BIG}));
+        L2B_TRY(materialize(ctx, &ctx->wcls, src, o_wcls, 14, 1, V, dim, SH_ROWS, {0.0, 0.04, -BIG, BIG}, true));
+    }
+    if (ctx->d_rounded) {
+        unsigned long long n = 0;
+        L2B_TRY(cuda_try(ctx, cudaMemcpyAsync(&n, ctx->d_rounded, sizeof n, cudaMemcpyDeviceToHost, ctx->stream), "rounding count"));
+        L2B_TRY(cuda_try(ctx, cudaStreamSynchronize(ctx->stream), "weight upload"));
+        ctx->n_rounded = n;
     }
     L2B_TRY(cuda_try(ctx, cudaStreamSynchronize(ctx->stream), "weight upload"));
     ctx->load_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_load0).count();
@@ -1417,7 +1514,8 @@ void destroy_all(l2b_ctx *ctx) {
 }
 
 int common_create(l2b_ctx **out, const l2b_config *cfg, const Source &src, uint64_t n_floats,
-                  const float *rope_cos, const float *rope_sin, const l2b_shard *shard, int n_gpus) {
+                  const float *rope_cos, const float *rope_sin, const l2b_shard *shard, int n_gpus,
+                  int wfmt = L2B_WEIGHTS_F32) {
     if (!out || !cfg) { g_create_error = "NULL argument"; return L2B_ERR_INVALID_ARG; }
     *out = nullptr;
     const bool in_process = n_gpus > 1;
@@ -1449,6 +1547,7 @@ int common_create(l2b_ctx **out, const l2b_config *cfg, const Source &src, uint6
     for (int i = 0; i < nlocal; ++i) {
         l2b_ctx *ctx = new l2b_ctx();
         ranks.push_back(ctx);
+        ctx->wfmt = wfmt;
         const int rank = in_process ? i : (shard ? shard->rank : 0);
         const int device = in_process ? i : device0;
         rc = create_rank(ctx, cfg, src, rope_cos, rope_sin, rank, world, device);
@@ -1484,6 +1583,8 @@ int common_create(l2b_ctx **out, const l2b_config *cfg, const Source &src, uint6
 
 // a context on the weights of `model` (single GPU): its own run state, caches, stream and graphs
 int create_session(l2b_ctx *ctx, const l2b_ctx *model) {
+    ctx->wfmt = model->wfmt;
+    ctx->n_rounded = model->n_rounded;
     L2B_TRY(init_rank(ctx, &model->cfg, 0, 1, model->device));
     ctx->weights = model->weights;
     ++ctx->weights->refs;
@@ -1641,6 +1742,45 @@ int32_t l2b_create_synthetic_group(l2b_ctx **out, const l2b_config *cfg, uint64_
     return common_create(out, cfg, s, 0, nullptr, nullptr, nullptr, n_gpus);
 }
 
+int32_t l2b_create_format(l2b_ctx **out, const l2b_config *cfg, const float *host_weights, uint64_t n_floats,
+                          const float *rope_cos, const float *rope_sin, int32_t n_gpus, int32_t weight_format) {
+    if (weight_format != L2B_WEIGHTS_F32 && weight_format != L2B_WEIGHTS_BF16) {
+        g_create_error = "unknown weight format";
+        return L2B_ERR_INVALID_ARG;
+    }
+    if (weight_format == L2B_WEIGHTS_F32) return l2b_create(out, cfg, host_weights, n_floats, rope_cos, rope_sin, n_gpus);
+    if (!host_weights) { g_create_error = "host_weights is NULL"; return L2B_ERR_INVALID_ARG; }
+    if (n_gpus != 1) { g_create_error = "bf16 weights are single-GPU (n_gpus must be 1)"; return L2B_ERR_UNSUPPORTED; }
+    Source s; s.host = host_weights;
+    return common_create(out, cfg, s, n_floats, rope_cos, rope_sin, nullptr, 1, weight_format);
+}
+
+int32_t l2b_create_synthetic_format(l2b_ctx **out, const l2b_config *cfg, uint64_t seed, int32_t weight_format) {
+    if (weight_format != L2B_WEIGHTS_F32 && weight_format != L2B_WEIGHTS_BF16) {
+        g_create_error = "unknown weight format";
+        return L2B_ERR_INVALID_ARG;
+    }
+    Source s; s.host = nullptr; s.seed = seed;
+    return common_create(out, cfg, s, 0, nullptr, nullptr, nullptr, 1, weight_format);
+}
+
+int32_t l2b_weight_info(const l2b_ctx *ctx, int32_t *weight_format, uint64_t *n_rounded) {
+    if (!ctx) return L2B_ERR_INVALID_ARG;
+    if (weight_format) *weight_format = ctx->wfmt;
+    if (n_rounded) *n_rounded = ctx->n_rounded;
+    return L2B_OK;
+}
+
+void l2b_round_bf16_host(float *data, uint64_t n) {
+    if (!data) return;
+    for (uint64_t i = 0; i < n; ++i) {
+        uint32_t u;
+        memcpy(&u, data + i, 4);
+        u = (uint32_t)bf16_round_bits(u) << 16;
+        memcpy(data + i, &u, 4);
+    }
+}
+
 int32_t l2b_create_session(l2b_ctx **out, l2b_ctx *model) {
     if (!out || !model) { g_create_error = "NULL argument"; return L2B_ERR_INVALID_ARG; }
     *out = nullptr;
@@ -1771,15 +1911,19 @@ int32_t l2b_forward_sample(l2b_ctx *ctx, int32_t token, int32_t pos, float tempe
 }  // extern "C" (templates below)
 
 // ---- batched prompt prefill (prefill_gemm_kernel in l2b_device.cuh) -----------------------------
-template <int NB>
+template <int NB, typename W>
 gemv_fn pf_pick(int epi) {
     switch (epi) {
-    case EPI_QKV: return prefill_gemm_kernel<EPI_QKV, NB>;
-    case EPI_SILU: return prefill_gemm_kernel<EPI_SILU, NB>;
-    case EPI_STORE: return prefill_gemm_kernel<EPI_STORE, NB>;
-    case EPI_ARGMAX: return prefill_gemm_kernel<EPI_ARGMAX, NB>;
-    default: return prefill_gemm_kernel<EPI_RESID, NB>;
+    case EPI_QKV: return prefill_gemm_kernel<EPI_QKV, NB, W>;
+    case EPI_SILU: return prefill_gemm_kernel<EPI_SILU, NB, W>;
+    case EPI_STORE: return prefill_gemm_kernel<EPI_STORE, NB, W>;
+    case EPI_ARGMAX: return prefill_gemm_kernel<EPI_ARGMAX, NB, W>;
+    default: return prefill_gemm_kernel<EPI_RESID, NB, W>;
     }
+}
+template <int NB>
+gemv_fn pf_pick(const l2b_ctx *ctx, int epi) {
+    return is_bf16(ctx) ? pf_pick<NB, bf16>(epi) : pf_pick<NB, float>(epi);
 }
 constexpr size_t kPfSmemBudget = 227 * 1024 - 8192;   // the prefill kernels keep ~6.5 KB of static shared memory
 
@@ -1815,8 +1959,8 @@ static int pf_prepare(l2b_ctx *ctx) {
     if ((rc = dev_alloc(ctx, &ctx->pf_counters, (size_t)PF_MAXB * ctx->heads_loc))) return rc;
     L2B_CUDA(ctx, cudaMemsetAsync(ctx->pf_counters, 0, (size_t)PF_MAXB * ctx->heads_loc * sizeof(unsigned int), ctx->stream));
     for (int epi : {(int)EPI_QKV, (int)EPI_SILU, (int)EPI_RESID, (int)EPI_STORE, (int)EPI_ARGMAX}) {
-        L2B_CUDA(ctx, cudaFuncSetAttribute(pf_pick<PF_MAXB>(epi), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPfSmemBudget));
-        L2B_CUDA(ctx, cudaFuncSetAttribute(pf_pick<2>(epi), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPfSmemBudget));
+        L2B_CUDA(ctx, cudaFuncSetAttribute(pf_pick<PF_MAXB>(ctx, epi), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPfSmemBudget));
+        L2B_CUDA(ctx, cudaFuncSetAttribute(pf_pick<2>(ctx, epi), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPfSmemBudget));
     }
     ctx->pf_ok = true;
     return L2B_OK;
@@ -1826,7 +1970,7 @@ template <int NB>
 static int pf_launch(l2b_ctx *ctx, int epi, GemvParams p, cudaStream_t st) {
     const size_t xbytes = (size_t)NB * p.n * 4;
     const int nstage = pf_ring_stages(kPfSmemBudget, xbytes);
-    p.nstage = nstage;
+    p.nstage = is_bf16(ctx) ? 2 * nstage : nstage;   // the same ring bytes in 16 KB bf16 stages
     int grid = ctx->num_sms;
     const int npairs = (p.total_rows + 1) / 2;
     if (grid > npairs) grid = npairs;
@@ -1841,7 +1985,7 @@ static int pf_launch(l2b_ctx *ctx, int epi, GemvParams p, cudaStream_t st) {
     cudaLaunchAttribute at[1] = {pdl_attr()};
     lc.attrs = at;
     lc.numAttrs = ctx->use_pdl ? 1 : 0;
-    L2B_CUDA(ctx, cudaLaunchKernelEx(&lc, pf_pick<NB>(epi), p));
+    L2B_CUDA(ctx, cudaLaunchKernelEx(&lc, pf_pick<NB>(ctx, epi), p));
     ++ctx->last_launches;
     return L2B_OK;
 }
@@ -3022,11 +3166,13 @@ int32_t l2b_debug_trace(l2b_ctx *ctx, unsigned long long *dst, uint64_t cap_word
 int32_t l2b_step_bytes(const l2b_ctx *ctx, int32_t pos, uint64_t *weight_bytes, uint64_t *kv_bytes) {
     if (!ctx) return L2B_ERR_INVALID_ARG;
     const uint64_t dim = ctx->dim, L = ctx->cfg.n_layers;
-    // SURVEY.md 8d: every weight touched once per token (+ the embedding row), this rank's shard
-    uint64_t w = L * ((uint64_t)ctx->q_loc * dim + 2ull * ctx->kv_loc * dim + dim * ctx->q_loc +
-                      3ull * ctx->hid_loc * dim + 2 * dim) +
-                 dim + (uint64_t)ctx->vocab_loc * dim;
-    if (weight_bytes) *weight_bytes = 4 * w;
+    // SURVEY.md 8d: every weight touched once per token (+ the embedding row), this rank's shard.
+    // Matrices count w_elem bytes per stored element (bf16 rows with their padding), gains 4.
+    const uint64_t ld_dim = w_ld(ctx, dim), ld_q = w_ld(ctx, ctx->q_loc), ld_hid = w_ld(ctx, ctx->hid_loc);
+    const uint64_t mat = L * ((uint64_t)ctx->q_loc * ld_dim + 2ull * ctx->kv_loc * ld_dim + dim * ld_q +
+                              2ull * ctx->hid_loc * ld_dim + dim * ld_hid) +
+                         ld_dim + (uint64_t)ctx->vocab_loc * ld_dim;
+    if (weight_bytes) *weight_bytes = w_elem(ctx) * mat + 4 * (L * 2 * dim);
     if (kv_bytes) *kv_bytes = 4ull * L * 2 * ctx->kv_loc * (uint64_t)(pos + 1);
     return L2B_OK;
 }

@@ -28,7 +28,9 @@ static const char *usage_text =
     "     --prefill             prompt positions run on the GPU back to back (no logits, no host round trip)\n"
     "     --gpus <1|2|4|8>      tensor-parallel over that many GPUs (llama2-7B class models)\n"
     "     --draft <checkpoint>  speculative decoding with this draft model (same vocabulary); same tokens\n"
-    "     --draft-k <int>       tokens the draft proposes per round, default 3, at most 32\n";
+    "     --draft-k <int>       tokens the draft proposes per round, default 3, at most 32\n"
+    "     --bf16                keep the matrix weights (and the draft's) in bf16 on the GPU: half the memory and\n"
+    "                           bytes per step; outputs equal an fp32 run of the bf16-rounded checkpoint (1 GPU)\n";
 
 // Generation with a draft model: the prompt positions are prefilled on target and draft, then
 // l2b_generate_speculative (-t 0) or l2h_generate_speculative_sample (-t > 0) runs the rest.  The tokens
@@ -76,6 +78,7 @@ int main(int argc, char **argv) {
     int n_gpus = 1, draft_k = 3;
     const char *draft_path = nullptr;
     bool verbose = false;
+    int32_t weight_format = L2B_WEIGHTS_F32;
     l2h_seed((uint64_t)time(nullptr));
     for (int i = 1; i < argc; ++i) {
         std::string a = argv[i];
@@ -100,6 +103,7 @@ int main(int argc, char **argv) {
         else if (a == "--gpus") n_gpus = atoi(need("gpus"));
         else if (a == "--draft") draft_path = need("draft");
         else if (a == "--draft-k") draft_k = atoi(need("draft-k"));
+        else if (a == "--bf16") weight_format = L2B_WEIGHTS_BF16;
         else { fprintf(stderr, "error: unknown argument '%s'\n", argv[i]); fputs(usage_text, stdout); return 0; }
     }
     if (!bin_path) { fputs(usage_text, stdout); return 0; }
@@ -113,8 +117,15 @@ int main(int argc, char **argv) {
         fprintf(stderr, "shared weights: %s\ntemperature: %g\ntop-p: %g\n\n", c.shared_weights ? "true" : "false", opt.temperature, opt.top_p);
     }
     l2b_ctx *ctx = nullptr;
-    int32_t rc = l2b_create(&ctx, &c, ck.data, ck.n_floats, nullptr, nullptr, n_gpus);   // after :967
+    int32_t rc = l2b_create_format(&ctx, &c, ck.data, ck.n_floats, nullptr, nullptr, n_gpus, weight_format);   // after :967
     if (rc) { fprintf(stderr, "error: l2b_create: %s (%s)\n", l2b_status_string(rc), l2b_last_error(nullptr)); return 1; }
+    if (verbose) {
+        int32_t fmt = 0;
+        uint64_t n_rounded = 0;
+        l2b_weight_info(ctx, &fmt, &n_rounded);
+        fprintf(stderr, "weights: %s on the GPU, %llu matrix weights changed by rounding\n\n",
+                fmt == L2B_WEIGHTS_BF16 ? "bf16" : "fp32", (unsigned long long)n_rounded);
+    }
     l2h_free_checkpoint(&ck);   // host copy no longer needed: weights live in HBM
     l2b_ctx *draft = nullptr;
     l2b_config dc{};
@@ -127,7 +138,7 @@ int main(int argc, char **argv) {
             return 1;
         }
         if (draft_k < 0 || draft_k > L2B_SPECULATIVE_MAX_K) { fprintf(stderr, "error: --draft-k must be in [0, %d]\n", L2B_SPECULATIVE_MAX_K); return 1; }
-        rc = l2b_create(&draft, &dc, dck.data, dck.n_floats, nullptr, nullptr, 1);
+        rc = l2b_create_format(&draft, &dc, dck.data, dck.n_floats, nullptr, nullptr, 1, weight_format);
         if (rc) { fprintf(stderr, "error: l2b_create (draft): %s (%s)\n", l2b_status_string(rc), l2b_last_error(nullptr)); return 1; }
         l2h_free_checkpoint(&dck);
     }
