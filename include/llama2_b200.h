@@ -511,24 +511,47 @@ int32_t l2b_op_logprob(int32_t device, const float *logits, int32_t n, int32_t t
  * Device rows of a bf16 matrix are padded to a multiple of 8 elements (16 bytes) with zeros.
  * l2b_load_stats, l2b_step_bytes and the bytes of l2b_profile_step count 2 bytes per bf16 element
  * stored, padding included.
- * Sessions (l2b_create_session) of a bf16 model are bf16; l2b_create_sharded stays fp32.          */
-typedef enum l2b_weight_format { L2B_WEIGHTS_F32 = 0, L2B_WEIGHTS_BF16 = 1 } l2b_weight_format;
+ * Quantization (L2B_WEIGHTS_Q8): row r of a matrix of n columns is cut into groups of L2B_Q8_GROUP
+ * weights, [64g, min(n, 64g + 64)) (the last group of a row may be short; no group spans two rows).
+ * In fp32, with IEEE division and no contraction: a = max |w| over the group, s = a / 127.0f; a == 0
+ * gives s = 0 and every q = 0, otherwise q = clamp(rint(w / s), -127, 127) with rint to nearest even
+ * (0 / 0, when s underflows to 0, gives q = 0).  The dequantized weight is w' = fl((float)q * s), the
+ * only value any kernel multiplies.  A non-finite matrix weight has no group scale and is refused with
+ * L2B_ERR_INVALID_ARG (by an upload as it quantizes: the context is freed and *out stays NULL).  The
+ * host upload, l2b_round_q8_host and the synthetic generator share this one quantizer.
+ * Contract, as for bf16: a q8 context of P returns exactly what an fp32 context of dq(P) (P with
+ * every matrix weight replaced by w') returns, for every entry point.  Each q8 kernel is the fp32
+ * kernel the same shape selects; every thread rebuilds the weights of its fp32 columns as w' and adds
+ * in the fp32 order.  A q8 row is stored as its n int8 codes zero-padded to 16 bytes, followed by its
+ * ceil(n / 64) fp32 scales zero-padded to 16 bytes; l2b_load_stats, l2b_step_bytes and the bytes of
+ * l2b_profile_step count 1 byte per stored code and 4 per stored scale, padding included.
+ * Sessions (l2b_create_session) of a bf16 or q8 model share its format; l2b_create_sharded stays fp32. */
+/* 2 is not a format: it stays an unknown format (L2B_ERR_INVALID_ARG), as it was before q8 existed.   */
+typedef enum l2b_weight_format { L2B_WEIGHTS_F32 = 0, L2B_WEIGHTS_BF16 = 1, L2B_WEIGHTS_Q8 = 3 } l2b_weight_format;
+#define L2B_Q8_GROUP 64
 
 /* l2b_create with a device weight format.  L2B_WEIGHTS_F32 is exactly l2b_create.  Checked before
- * any device is touched: an unknown format => L2B_ERR_INVALID_ARG; L2B_WEIGHTS_BF16 with n_gpus > 1
- * => L2B_ERR_UNSUPPORTED (tensor parallel is fp32 only); every other check is l2b_create's.         */
+ * any device is touched: an unknown format => L2B_ERR_INVALID_ARG; L2B_WEIGHTS_BF16 or L2B_WEIGHTS_Q8
+ * with n_gpus > 1 => L2B_ERR_UNSUPPORTED (tensor parallel is fp32 only); every other check is
+ * l2b_create's, plus (q8) a non-finite matrix weight => L2B_ERR_INVALID_ARG.                        */
 int32_t l2b_create_format(l2b_ctx **out, const l2b_config *cfg, const float *host_weights, uint64_t n_floats,
                           const float *rope_cos, const float *rope_sin, int32_t n_gpus, int32_t weight_format);
 /* l2b_create_synthetic (single GPU, device 0) with a device weight format.  The bf16 matrices are
- * exactly those of l2b_synth_checkpoint_host's payload passed through l2b_round_bf16_host.          */
+ * exactly those of l2b_synth_checkpoint_host's payload passed through l2b_round_bf16_host, the q8
+ * ones exactly a q8 upload of that payload.                                                         */
 int32_t l2b_create_synthetic_format(l2b_ctx **out, const l2b_config *cfg, uint64_t seed, int32_t weight_format);
-/* Format of ctx's model, and how many matrix weights rounding changed (their bit pattern differs
- * from the fp32 value; 0: every output equals that of an fp32 context of the same payload).  Counted
- * during the upload, or on the device for synthetic weights.                                      */
+/* Format of ctx's model, and how many matrix weights rounding (bf16) or quantization (q8) changed
+ * (their bit pattern differs from the fp32 value; 0: every output equals that of an fp32 context of
+ * the same payload).  Counted during the upload, or on the device for synthetic weights.           */
 int32_t l2b_weight_info(const l2b_ctx *ctx, int32_t *weight_format, uint64_t *n_rounded);
 /* In place: each value -> the nearest bf16 (ties to even), widened back to fp32.  The library's own
  * rounding (see above).                                                                            */
 void l2b_round_bf16_host(float *data, uint64_t n);
+/* In place on a rows x cols row-major matrix: each weight -> its q8 dequantized value w' (see above);
+ * *n_changed (if not NULL) = how many weights changed bitwise.  A stacked [L][rows][cols] tensor is
+ * L * rows rows.  NULL data, cols == 0, cols > 2^30 or a non-finite value => L2B_ERR_INVALID_ARG with
+ * data untouched (every value is checked before any is written).                                   */
+int32_t l2b_round_q8_host(float *data, uint64_t rows, uint64_t cols, uint64_t *n_changed);
 
 #ifdef __cplusplus
 }

@@ -140,6 +140,7 @@ def load_library():
     lib.l2b_weight_info.argtypes = [vp, IP, U64P]
     lib.l2b_round_bf16_host.argtypes = [FP, C.c_uint64]
     lib.l2b_round_bf16_host.restype = None
+    lib.l2b_round_q8_host.argtypes = [FP, C.c_uint64, C.c_uint64, U64P]
     _lib = lib
     return lib
 
@@ -172,7 +173,10 @@ def comm_unique_id():
     return bytes(buf)
 
 
-WEIGHT_FORMATS = {"f32": 0, "bf16": 1}   # l2b_weight_format
+WEIGHT_FORMATS = {"f32": 0, "bf16": 1}   # l2b_weight_format: one stored element per weight
+QUANT_FORMATS = {"q8": 3}                # l2b_weight_format: codes plus a scale per group of weights
+_FORMATS = {**WEIGHT_FORMATS, **QUANT_FORMATS}
+Q8_GROUP = 64   # L2B_Q8_GROUP
 
 
 def round_bf16_host(a):
@@ -182,6 +186,18 @@ def round_bf16_host(a):
         raise TypeError("round_bf16_host needs a C-contiguous float32 array")
     load_library().l2b_round_bf16_host(a.ctypes.data_as(FP), a.size)
     return a
+
+
+def round_q8_host(a):
+    """In place on a C-contiguous 2-D float32 array (rows x cols): each weight -> its q8 dequantized
+    value, quantized in groups of Q8_GROUP weights of a row (l2b_round_q8_host, what a q8 context
+    multiplies).  Returns the number of weights that changed bitwise.  Raises L2BError(INVALID_ARG),
+    with `a` untouched, on a non-finite value."""
+    if not (isinstance(a, np.ndarray) and a.dtype == np.float32 and a.flags["C_CONTIGUOUS"] and a.ndim == 2):
+        raise TypeError("round_q8_host needs a C-contiguous 2-D float32 array")
+    n = C.c_uint64()
+    _check(load_library().l2b_round_q8_host(a.ctypes.data_as(FP), a.shape[0], a.shape[1], C.byref(n)))
+    return n.value
 
 
 def synth_checkpoint_host(ck, seed):
@@ -203,18 +219,19 @@ class Transformer:
     `ck` is a checkpoint.Checkpoint.  With `ck.data` set the payload is uploaded
     (l2b_create / l2b_create_sharded); with `synthetic_seed` the weights are generated on the
     device (l2b_create_synthetic).  weight_format="bf16" keeps the matrix weights in bf16 on the
-    device (l2b_create_format / l2b_create_synthetic_format; single GPU, device 0).
+    device, "q8" as int8 with one fp32 scale per 64 weights of a row (l2b_create_format /
+    l2b_create_synthetic_format; single GPU, device 0).
     """
 
     def __init__(self, ck, synthetic_seed=None, rank=0, world_size=1, device=0, comm_id=None,
                  rope_cos=None, rope_sin=None, n_gpus=1, weight_format="f32"):
         """n_gpus > 1: ONE process drives n_gpus GPUs (l2b_create(.., n_gpus)); rank/world_size:
         one process per GPU (l2b_create_sharded)."""
-        if weight_format not in WEIGHT_FORMATS:
-            raise ValueError(f"weight_format must be one of {sorted(WEIGHT_FORMATS)}")
-        fmt = WEIGHT_FORMATS[weight_format]
+        if weight_format not in _FORMATS:
+            raise ValueError(f"weight_format must be one of {sorted(_FORMATS)}")
+        fmt = _FORMATS[weight_format]
         if fmt and (world_size > 1 or device != 0 or rank != 0 or n_gpus != 1):
-            raise ValueError("bf16 weights are single-GPU on device 0")
+            raise ValueError(f"{weight_format} weights are single-GPU on device 0")
         self.lib = load_library()
         self.ck = ck
         self.cfg = make_config(ck)
@@ -352,11 +369,11 @@ class Transformer:
 
     def weight_info(self):
         """(weight_format name, n_rounded): the device format of the model's matrix weights and how many
-        of them the bf16 rounding changed (l2b_weight_info)."""
+        of them the bf16 rounding or q8 quantization changed (l2b_weight_info)."""
         fmt = C.c_int32()
         n = C.c_uint64()
         _check(self.lib.l2b_weight_info(self.h, C.byref(fmt), C.byref(n)), self.h)
-        return {v: k for k, v in WEIGHT_FORMATS.items()}[fmt.value], n.value
+        return {v: k for k, v in _FORMATS.items()}[fmt.value], n.value
 
     def load_stats(self):
         ms = C.c_double()

@@ -179,18 +179,65 @@ __device__ __forceinline__ float dot4(const float4 a, const float4 b, float acc)
 }
 
 // ---------------------------------------------------------------------------------------
-// Weight element type.  Matrix weights live on the device as fp32 (W = float) or bf16 (W = bf16).
-// Every kernel that reads weights takes W as a template parameter; a thread owns the same float4
-// column groups in both (a bf16 group is 4 elements, 8 bytes) and widens each weight exactly, so a
-// bf16 kernel computes exactly what its fp32 twin computes on the rounded weights.  bf16 rows are
+// Weight element type.  Matrix weights live on the device as fp32 (W = float), bf16 (W = bf16) or
+// int8 with group scales (W = q8).  Every kernel that reads weights takes W as a template parameter; a
+// thread owns the same float4 column groups in all three (a bf16 group is 4 elements, 8 bytes; a q8
+// group 4 bytes and its group's scale) and rebuilds each weight exactly, so a bf16 or q8 kernel
+// computes exactly what its fp32 twin computes on the rounded or dequantized weights.  bf16 rows are
 // padded to a multiple of 8 elements (16 bytes, the TMA bulk-copy granule) with zeros no consumer
 // multiplies; fp32 rows are dense.
 // ---------------------------------------------------------------------------------------
 typedef __nv_bfloat16 bf16;
 
+// q8 (W = q8): int8 weights with one fp32 scale per group of Q8_GROUP consecutive weights of a row
+// (the last group of a row may be short; a group never spans two rows).  A row is one record of
+// w_pitch<q8>(n) bytes: its n int8 codes, zero-padded to 16 bytes, then its ceil(n / 64) fp32 scales,
+// zero-padded to 16 bytes.  The weight every kernel multiplies is q8_dequant(q, s) = fl(q * s), so a
+// q8 kernel computes exactly what its fp32 twin computes on the dequantized weights.
+struct q8 { int8_t v; };
+constexpr int Q8_GROUP = 64;
+static_assert(sizeof(q8) == 1, "a q8 element is one byte");
+__host__ __device__ __forceinline__ constexpr int q8_groups(int n) { return (n + Q8_GROUP - 1) / Q8_GROUP; }
+// byte offset of a q8 row's scales from the row's start
+__host__ __device__ __forceinline__ constexpr int q8_scale_off(int n) { return (n + 15) & ~15; }
+
+// elements of W from one row of an n-column matrix to the next (q8: bytes of a row record)
 template <typename W>
 __host__ __device__ __forceinline__ constexpr int w_pitch(int n) {
-    return sizeof(W) == 4 ? n : (n + 7) & ~7;
+    return sizeof(W) == 4 ? n : sizeof(W) == 2 ? (n + 7) & ~7 : q8_scale_off(n) + ((4 * q8_groups(n) + 15) & ~15);
+}
+
+// The quantizer (host upload, l2b_round_q8_host and synth_fill_q8_kernel): a group of absolute maximum
+// a (finite) has scale s = a / 127 and codes q = clamp(rint(w / s), -127, 127), rint to nearest even;
+// a == 0 gives s = 0 and q = 0 (and 0 / 0, when s underflows to 0, gives q = 0).  IEEE division and
+// multiplication, no contraction.
+__host__ __device__ __forceinline__ float q8_scale(float a) {
+#ifdef __CUDA_ARCH__
+    return __fdiv_rn(a, 127.0f);
+#else
+    return a / 127.0f;
+#endif
+}
+__host__ __device__ __forceinline__ int8_t q8_code(float w, float a, float s) {
+    if (a == 0.0f) return 0;
+#ifdef __CUDA_ARCH__
+    const float t = rintf(__fdiv_rn(w, s));
+#else
+    const float t = rintf(w / s);
+#endif
+    return t >= 127.0f ? (int8_t)127 : t <= -127.0f ? (int8_t)-127 : t == t ? (int8_t)t : (int8_t)0;
+}
+__host__ __device__ __forceinline__ float q8_dequant(int q, float s) {
+#ifdef __CUDA_ARCH__
+    return __fmul_rn((float)q, s);
+#else
+    return (float)q * s;
+#endif
+}
+// the four codes of a 32-bit word (little-endian: code 0 in the low byte) times s
+__device__ __forceinline__ float4 dequant_q8x4(uint32_t u, float s) {
+    return make_float4(q8_dequant((int8_t)(u & 0xFFu), s), q8_dequant((int8_t)((u >> 8) & 0xFFu), s),
+                       q8_dequant((int8_t)((u >> 16) & 0xFFu), s), q8_dequant((int8_t)(u >> 24), s));
 }
 
 // nearest bf16, ties to even; +-inf stays, finite values past the bf16 maximum become +-inf, subnormals
@@ -206,20 +253,28 @@ __device__ __forceinline__ float4 widen_bf16x4(uint2 u) {
                        __uint_as_float(u.y << 16), __uint_as_float(u.y & 0xFFFF0000u));
 }
 
-// float4 column group c of a weight row in global memory (streaming, no L1 allocation)
+// float4 column group c of a weight row of n columns in global memory (streaming, no L1 allocation;
+// a q8 scale, shared by 16 neighbouring groups, is read through L1)
 template <typename W>
-__device__ __forceinline__ float4 ldg_w4(const W *row, int c);
+__device__ __forceinline__ float4 ldg_w4(const W *row, int c, int n);
 template <>
-__device__ __forceinline__ float4 ldg_w4<float>(const float *row, int c) {
+__device__ __forceinline__ float4 ldg_w4<float>(const float *row, int c, int) {
     return ldg_stream(reinterpret_cast<const float4 *>(row) + c);
 }
 template <>
-__device__ __forceinline__ float4 ldg_w4<bf16>(const bf16 *row, int c) {
+__device__ __forceinline__ float4 ldg_w4<bf16>(const bf16 *row, int c, int) {
     uint2 u;
     asm("ld.global.nc.L1::no_allocate.v2.u32 {%0,%1}, [%2];"
         : "=r"(u.x), "=r"(u.y)
         : "l"(reinterpret_cast<const uint2 *>(row) + c));
     return widen_bf16x4(u);
+}
+template <>
+__device__ __forceinline__ float4 ldg_w4<q8>(const q8 *row, int c, int n) {
+    uint32_t u;
+    asm("ld.global.nc.L1::no_allocate.u32 %0, [%1];" : "=r"(u) : "l"(reinterpret_cast<const uint32_t *>(row) + c));
+    const float s = __ldg(reinterpret_cast<const float *>(row + q8_scale_off(n)) + (c >> 4));
+    return dequant_q8x4(u, s);
 }
 // float4 column group c of a weight row in shared memory
 template <typename W>
@@ -370,12 +425,20 @@ __device__ __forceinline__ const W *gemv_row_ptr(const GemvParams &p, int v) {
     }
 }
 
-// bf16 only: row `token` of the embedding table, widened into the n floats at xs by the threads
-// idx = 0 .. nthreads-1 (a bulk copy cannot widen).  The caller orders it before the readers of xs.
+// bf16 and q8 only: row `token` of the embedding table, widened (bf16) or dequantized (q8) into the n
+// floats at xs by the threads idx = 0 .. nthreads-1 (a bulk copy cannot convert).  The caller orders it
+// before the readers of xs.
+template <typename W>
 __device__ __forceinline__ void widen_emb_row(const GemvParams &p, int token, float *xs, int idx, int nthreads) {
-    const bf16 *row = static_cast<const bf16 *>(p.emb) + (size_t)token * w_pitch<bf16>(p.n);
-    for (int i = idx; i < (p.n >> 2); i += nthreads)
-        reinterpret_cast<float4 *>(xs)[i] = widen_bf16x4(__ldg(reinterpret_cast<const uint2 *>(row) + i));
+    const W *row = static_cast<const W *>(p.emb) + (size_t)token * w_pitch<W>(p.n);
+    for (int i = idx; i < (p.n >> 2); i += nthreads) {
+        if constexpr (sizeof(W) == 2) {
+            reinterpret_cast<float4 *>(xs)[i] = widen_bf16x4(__ldg(reinterpret_cast<const uint2 *>(row) + i));
+        } else {
+            const float s = __ldg(reinterpret_cast<const float *>(row + q8_scale_off(p.n)) + (i >> 4));
+            reinterpret_cast<float4 *>(xs)[i] = dequant_q8x4(__ldg(reinterpret_cast<const unsigned int *>(row) + i), s);
+        }
+    }
 }
 
 // EPI_QKV, rows (v, v+1): an adjacent pair of q, k or v (segment sizes are even).  q and k pairs are
@@ -475,7 +538,7 @@ __device__ __forceinline__ void gemv_stage_input(const GemvParams &p, float *xs,
                                                  uint64_t *bar, float *scratch) {
     const int tid = threadIdx.x;
     const int n4 = p.n >> 2;
-    const bool widen = sizeof(W) == 2 && p.emb;          // a bf16 embedding row is widened, not bulk-copied
+    const bool widen = sizeof(W) != 4 && p.emb;          // a bf16 / q8 embedding row is converted, not bulk-copied
     float *gs = aux;
     float *ps = p.gamma ? aux + p.n : aux;               // sum of the partial vectors (when p.parts)
     if (tid == 0) {
@@ -487,7 +550,7 @@ __device__ __forceinline__ void gemv_stage_input(const GemvParams &p, float *xs,
         }
         if (p.gamma) tma_load_1d(gs, p.gamma, bytes, bar);
     }
-    if (widen) widen_emb_row(p, p.ctl[CTL_TOKEN], xs, tid, NT);
+    if (widen) widen_emb_row<W>(p, p.ctl[CTL_TOKEN], xs, tid, NT);
     if (p.parts) {
         // the wo / w2 product arrives split into nparts partial vectors (by head / by hidden slice):
         // complete it in fixed order while the bulk copies are in flight
@@ -643,7 +706,7 @@ __global__ void __launch_bounds__(NT) gemv_kernel(const GemvParams p) {
 #pragma unroll
             for (int u = 0; u < GEMV_U; ++u) {
                 const int c = (ch * GEMV_U + u) * TPR + sub;
-                wv[r][u] = (rok && c < n4) ? ldg_w4<W>(wr, c) : make_float4(0.f, 0.f, 0.f, 0.f);
+                wv[r][u] = (rok && c < n4) ? ldg_w4<W>(wr, c, p.n) : make_float4(0.f, 0.f, 0.f, 0.f);
             }
         }
     };
@@ -835,7 +898,7 @@ __global__ void __launch_bounds__(NT, 2) gemv8_kernel(const GemvParams p) {
             const int v = v0 + r;
             const bool ok = (v < r1) && (c < n4);
             const W *wr = gemv_row_ptr<EPI, W>(p, ok ? v : 0);
-            w[r] = ok ? ldg_w4<W>(wr, c) : make_float4(0.f, 0.f, 0.f, 0.f);
+            w[r] = ok ? ldg_w4<W>(wr, c, p.n) : make_float4(0.f, 0.f, 0.f, 0.f);
         }
     };
     if (0 < total) issue(wa, 0);
@@ -939,27 +1002,62 @@ __device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
 // `ring`.  full[s]: slot s has landed (producer -> consumers); empty[s]: all NWARP consumer warps are
 // done with it.  The slot size only sets how finely the ring's shared memory is cut: the consumers
 // read the same columns of the same rows in the same order whatever SR is.
-// W: the weight element type.  A row's part of a slot is NT float4 column groups whatever W is, so a
-// bf16 slot of SR rows is half the bytes of an fp32 one.  A bf16 row's last chunk is copied whole to
-// its 16-byte end (a row of n = 4 mod 8 columns ends on its zero padding).
-template <int SR, typename W = float>
+// W: the weight element type.  A row's part of a slot is KS * NT float4 column groups whatever W is,
+// so a bf16 slot of SR rows is half the bytes of an fp32 one.  A bf16 row's last chunk is copied whole
+// to its 16-byte end (a row of n = 4 mod 8 columns ends on its zero padding).
+// KS > 1 (q8): a slot holds KS consecutive column steps of its SR rows, each row's codes in one bulk
+// copy and their scales in a second one; the scales of the slot's rows follow the codes.  The
+// consumers still walk the columns step by step, so the order of every sum is the KS = 1 order.
+template <int SR, typename W = float, int KS = 1>
 struct TmaRing {
-    static constexpr int SUB = GEMV8_R / SR;                           // slots per (tile, column step)
-    static constexpr int SLOT_ELEMS = SR * NT * 4;
-    static constexpr int SLOT_BYTES = SLOT_ELEMS * (int)sizeof(W);
+    static constexpr int SUB = GEMV8_R / SR;                           // slots per (tile, column step group)
+    static constexpr int SLOT_ELEMS = SR * KS * NT * 4;                // weights (codes) of a slot
+    static constexpr int ROW_SCALES = KS * NT * 4 / Q8_GROUP;          // q8: scales of a row's part
+    static constexpr int SLOT_BYTES = SLOT_ELEMS * (int)sizeof(W) + (sizeof(W) == 1 ? SR * ROW_SCALES * 4 : 0);
     static_assert(SR * SUB == GEMV8_R, "a tile is a whole number of slots");
+    static_assert(KS == 1 || sizeof(W) == 1, "only q8 slots hold several column steps");
+    static_assert(SLOT_BYTES % 16 == 0, "slots keep the bulk-copy alignment");
     static __device__ __forceinline__ uint32_t chunk_bytes(int cols4) {
-        return sizeof(W) == 4 ? (uint32_t)(cols4 * 16) : (uint32_t)((cols4 * 8 + 15) & ~15);
+        return sizeof(W) == 4 ? (uint32_t)(cols4 * 16) : (uint32_t)((cols4 * 4 * (int)sizeof(W) + 15) & ~15);
     }
     W *ring;
     uint64_t *full, *empty;
     int nstage, n4, nsteps, r0, r1, total;
+
+    __device__ __forceinline__ W *slot(int stage) const {
+        return reinterpret_cast<W *>(reinterpret_cast<unsigned char *>(ring) + (size_t)stage * SLOT_BYTES);
+    }
+    // slots the CTA's `total` (tile, column step) steps pass through the ring in
+    __device__ __forceinline__ int nslots() const {
+        return KS == 1 ? total * SUB : (total / nsteps) * ((nsteps + KS - 1) / KS) * SUB;
+    }
+    // float4 column group `tid` of column step k of row r of a slot
+    __device__ __forceinline__ float4 w4(const W *s, int r, int k, int tid) const {
+        if constexpr (sizeof(W) == 1) {
+            const uint32_t u = reinterpret_cast<const uint32_t *>(s)[(r * KS + k) * NT + tid];
+            const float sc = reinterpret_cast<const float *>(s + SLOT_ELEMS)[r * ROW_SCALES + ((k * NT + tid) >> 4)];
+            return dequant_q8x4(u, sc);
+        } else {
+            return lds_w4<W>(s, r * NT + tid);
+        }
+    }
 };
-// gemv_tma_kernel's slot: 4 fp32 rows or 8 bf16 rows, 16 KB either way
+// The slot shapes (rows, column steps): fp32 4 x 1 and bf16 8 x 1 (16 KB) in the decode ring, 8 x 1 in
+// the prefill ring (32 KB fp32, 16 KB bf16); q8 4 x 4 in both (16 KB of codes + 1 KB of scales, and
+// 8 bulk copies per slot, as many as a bf16 slot)
 template <typename W>
-__host__ __device__ constexpr int tma_slot_rows() { return sizeof(W) == 4 ? TMA_SLOT_ROWS : GEMV8_R; }
-static_assert(TmaRing<TMA_SLOT_ROWS, float>::SLOT_BYTES == TmaRing<tma_slot_rows<bf16>(), bf16>::SLOT_BYTES,
-              "both formats' decode rings have the same slot size");
+__host__ __device__ constexpr int tma_slot_rows() { return sizeof(W) == 2 ? GEMV8_R : TMA_SLOT_ROWS; }
+template <typename W>
+__host__ __device__ constexpr int pf_slot_rows() { return sizeof(W) == 1 ? TMA_SLOT_ROWS : GEMV8_R; }
+template <typename W>
+__host__ __device__ constexpr int ring_steps() { return sizeof(W) == 1 ? 4 : 1; }
+template <typename W>
+using DecodeRing = TmaRing<tma_slot_rows<W>(), W, ring_steps<W>()>;
+template <typename W>
+using PrefillRing = TmaRing<pf_slot_rows<W>(), W, ring_steps<W>()>;
+static_assert(DecodeRing<float>::SLOT_BYTES == DecodeRing<bf16>::SLOT_BYTES,
+              "the fp32 and bf16 decode rings have the same slot size");
+static_assert(DecodeRing<q8>::SLOT_BYTES == 16384 + 1024, "a q8 slot is 16 KB of codes and 1 KB of scales");
 
 // The producer warp's place in the stream.  produce_one is executed by all 32 lanes of the warp:
 // lane r owns row r of the tile and issues its bulk copy into the slot that holds it, lane 0 owns
@@ -969,10 +1067,10 @@ struct RingProducer {
     uint32_t phase = 0;
     const void *row = nullptr;                                         // this lane's row in the current tile
 
-    template <int EPI, int SR, typename W>
-    __device__ __forceinline__ void produce_one(const GemvParams &p, const TmaRing<SR, W> &R, int lane) {
+    template <int EPI, int SR, typename W, int KS>
+    __device__ __forceinline__ void produce_one(const GemvParams &p, const TmaRing<SR, W, KS> &R, int lane) {
         const int c0 = step * NT;                                      // first float4 column
-        const int cols4 = min(NT, R.n4 - c0);
+        const int cols4 = min(KS * NT, R.n4 - c0);
         const int v0 = R.r0 + tile * GEMV8_R;
         const int rows = min(GEMV8_R, R.r1 - v0);
         // whole-tile slots (SUB == 1) skip the slot arithmetic, so the 8-row stream compiles as it did
@@ -982,18 +1080,26 @@ struct RingProducer {
         const int srows = whole ? rows : max(0, min(SR, rows - lo));
         if (step == 0 && (whole || sub == 0) && lane < rows) row = gemv_row_ptr<EPI, W>(p, v0 + lane);
         const uint32_t bytes = R.chunk_bytes(cols4);
+        // q8: the scales of the chunk's groups (c0 is a multiple of 16 float4 columns, one group)
+        const uint32_t sbytes = sizeof(W) == 1 ? (uint32_t)((((cols4 + 15) >> 4) * 4 + 15) & ~15) : 0u;
         if (lane == 0) {
             mbar_wait(&R.empty[stage], phase ^ 1);
-            mbar_expect_tx(&R.full[stage], (uint32_t)srows * bytes);
+            mbar_expect_tx(&R.full[stage], (uint32_t)srows * (bytes + sbytes));
         }
         __syncwarp();
-        if ((whole || lane >= lo) && lane < lo + srows)
-            tma_load_1d(R.ring + (size_t)stage * R.SLOT_ELEMS + (lane - lo) * NT * 4, static_cast<const W *>(row) + (size_t)c0 * 4,
-                        bytes, &R.full[stage]);
+        if ((whole || lane >= lo) && lane < lo + srows) {
+            W *dst = R.slot(stage);
+            const W *src = static_cast<const W *>(row);
+            tma_load_1d(dst + (lane - lo) * KS * NT * 4, src + (size_t)c0 * 4, bytes, &R.full[stage]);
+            if (sizeof(W) == 1)
+                tma_load_1d(reinterpret_cast<float *>(dst + R.SLOT_ELEMS) + (lane - lo) * R.ROW_SCALES,
+                            reinterpret_cast<const float *>(src + q8_scale_off(R.n4 * 4)) + (c0 >> 4), sbytes, &R.full[stage]);
+        }
         ++it;
         if (whole || ++sub == R.SUB) {
             sub = 0;
-            if (++step == R.nsteps) { step = 0; ++tile; }
+            step += KS;
+            if (step >= R.nsteps) { step = 0; ++tile; }
         }
         if (++stage == R.nstage) { stage = 0; phase ^= 1; }
     }
@@ -1076,8 +1182,8 @@ __device__ __forceinline__ void tma_rmsnorm(const GemvParams &p, float *xs, cons
 // (one LDS.128 of each x_b serves the tile's rows; vectors b >= nb read x_0 and are never stored).
 // At a tile's end the butterfly leaves the warp's row sums in red[t & 1] for the epilogue warp.
 // trace (decode only, else nullptr): the first slot's arrival (slot 4), the last one consumed (5).
-template <int NB, int SR, typename W>
-__device__ __forceinline__ void tma_consume(const TmaRing<SR, W> &R, const float *xs, int nb, TileRed<NB> &red,
+template <int NB, int SR, typename W, int KS>
+__device__ __forceinline__ void tma_consume(const TmaRing<SR, W, KS> &R, const float *xs, int nb, TileRed<NB> &red,
                                             uint64_t *tile_full, uint64_t *tile_free, unsigned long long *trace) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const float4 *xs4 = reinterpret_cast<const float4 *>(xs);
@@ -1089,34 +1195,75 @@ __device__ __forceinline__ void tma_consume(const TmaRing<SR, W> &R, const float
     int c_stage = 0;
     uint32_t c_phase = 0;
     int t = 0, st = 0;
+    int k = 0;                                                // KS > 1: the step's place in its slots
     for (int it = 0; it < R.total; ++it, ++st) {
         if (st == R.nsteps) { st = 0; ++t; }
         const int c = st * NT + tid;
         const int v0 = R.r0 + t * GEMV8_R;
         const int rows = min(GEMV8_R, R.r1 - v0);
         float4 xv[NB];                                        // one LDS.128 of each x_b serves the step's slots
+        if constexpr (KS == 1) {
 #pragma unroll
-        for (int s = 0; s < R.SUB; ++s) {
-            mbar_wait(&R.full[c_stage], c_phase);
-            if (it == 0 && s == 0 && tid == 0) L2B_STAMP(trace, 4);
-            if (c < R.n4) {
-                const W *slot = R.ring + (size_t)c_stage * R.SLOT_ELEMS;
-                if (s == 0) {
+            for (int s = 0; s < R.SUB; ++s) {
+                mbar_wait(&R.full[c_stage], c_phase);
+                if (it == 0 && s == 0 && tid == 0) L2B_STAMP(trace, 4);
+                if (c < R.n4) {
+                    const W *slot = R.slot(c_stage);
+                    if (s == 0) {
 #pragma unroll
-                    for (int b = 0; b < NB; ++b) xv[b] = xs4[(size_t)(b < nb ? b : 0) * R.n4 + c];
-                }
+                        for (int b = 0; b < NB; ++b) xv[b] = xs4[(size_t)(b < nb ? b : 0) * R.n4 + c];
+                    }
 #pragma unroll
-                for (int r = 0; r < SR; ++r) {
-                    if (s * SR + r < rows) {
-                        const float4 w = lds_w4<W>(slot, r * NT + tid);
+                    for (int r = 0; r < SR; ++r) {
+                        if (s * SR + r < rows) {
+                            const float4 w = R.w4(slot, r, 0, tid);
 #pragma unroll
-                        for (int b = 0; b < NB; ++b) acc[b][s * SR + r] = dot4(w, xv[b], acc[b][s * SR + r]);
+                            for (int b = 0; b < NB; ++b) acc[b][s * SR + r] = dot4(w, xv[b], acc[b][s * SR + r]);
+                        }
                     }
                 }
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&R.empty[c_stage]);  // this warp is done with the slot
+                if (++c_stage == R.nstage) { c_stage = 0; c_phase ^= 1; }
             }
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&R.empty[c_stage]);  // this warp is done with the slot
-            if (++c_stage == R.nstage) { c_stage = 0; c_phase ^= 1; }
+        } else {
+            // the SUB slots of this step's group (stages c_stage, c_stage + 1, ..) hold KS column steps;
+            // they are waited for at the group's first step and released after its last one
+            const bool last = k == KS - 1 || st == R.nsteps - 1;
+#pragma unroll
+            for (int s = 0; s < R.SUB; ++s) {
+                int stage = c_stage + s;
+                uint32_t phase = c_phase;
+                if (stage >= R.nstage) { stage -= R.nstage; phase ^= 1; }
+                if (k == 0) mbar_wait(&R.full[stage], phase);
+                if (it == 0 && s == 0 && tid == 0) L2B_STAMP(trace, 4);
+                if (c < R.n4) {
+                    const W *slot = R.slot(stage);
+                    if (s == 0) {
+#pragma unroll
+                        for (int b = 0; b < NB; ++b) xv[b] = xs4[(size_t)(b < nb ? b : 0) * R.n4 + c];
+                    }
+#pragma unroll
+                    for (int r = 0; r < SR; ++r) {
+                        if (s * SR + r < rows) {
+                            const float4 w = R.w4(slot, r, k, tid);
+#pragma unroll
+                            for (int b = 0; b < NB; ++b) acc[b][s * SR + r] = dot4(w, xv[b], acc[b][s * SR + r]);
+                        }
+                    }
+                }
+                if (last) {
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(&R.empty[stage]);  // this warp is done with the slot
+                }
+            }
+            if (last) {
+                k = 0;
+                c_stage += R.SUB;
+                if (c_stage >= R.nstage) { c_stage -= R.nstage; c_phase ^= 1; }
+            } else {
+                ++k;
+            }
         }
         if (it == R.total - 1 && tid == 0) L2B_STAMP(trace, 5);
         if (st != R.nsteps - 1) continue;
@@ -1141,7 +1288,7 @@ template <int EPI, typename W = float>
 __global__ void __launch_bounds__(TMA_THREADS, 2) gemv_tma_kernel(const GemvParams p) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int NSTAGE = p.nstage;
-    W *ring = reinterpret_cast<W *>(smem_raw);                         // NSTAGE x 16 KB
+    W *ring = reinterpret_cast<W *>(smem_raw);                         // NSTAGE x 16 KB (q8: 17 KB)
     __shared__ uint64_t full[TMA_MAX_STAGES], empty[TMA_MAX_STAGES], xbar, tile_full[2], tile_free[2];
     __shared__ float scratch[1][NWARP + 2];
     __shared__ TileRed<1> red;
@@ -1153,8 +1300,8 @@ __global__ void __launch_bounds__(TMA_THREADS, 2) gemv_tma_kernel(const GemvPara
     const RowSplit split = cta_row_split(p.total_rows);
     const int r0 = split.r0, r1 = split.r1, ntiles = split.ntiles;
     const int total = ntiles * nsteps;
-    const TmaRing<tma_slot_rows<W>(), W> R = {ring, full, empty, NSTAGE, n4, nsteps, r0, r1, total};
-    const int nslots = total * R.SUB;
+    const DecodeRing<W> R = {ring, full, empty, NSTAGE, n4, nsteps, r0, r1, total};
+    const int nslots = R.nslots();
     float *xs = reinterpret_cast<float *>(smem_raw + (size_t)NSTAGE * R.SLOT_BYTES);   // n floats
 
     if (tid == 0) {
@@ -1217,7 +1364,7 @@ __global__ void __launch_bounds__(TMA_THREADS, 2) gemv_tma_kernel(const GemvPara
 
     // stage the activation vector (consumer warps + epilogue warp; barrier 1 is theirs)
     {
-        const bool widen = sizeof(W) == 2 && p.emb;                    // a bf16 embedding row is widened, not bulk-copied
+        const bool widen = sizeof(W) != 4 && p.emb;                    // a bf16 / q8 embedding row is converted, not bulk-copied
         if (tid == 0) {
             const uint32_t bytes = (uint32_t)p.n * 4u;
             mbar_expect_tx(&xbar, widen ? 0u : bytes);
@@ -1227,7 +1374,7 @@ __global__ void __launch_bounds__(TMA_THREADS, 2) gemv_tma_kernel(const GemvPara
             }
         }
         if (widen) {
-            widen_emb_row(p, p.ctl[CTL_TOKEN], xs, ptid, TMA_PRO_THREADS);
+            widen_emb_row<W>(p, p.ctl[CTL_TOKEN], xs, ptid, TMA_PRO_THREADS);
             named_bar_sync(1, TMA_PRO_THREADS);
         }
         // epilogue warp: this position's RoPE row.  The table row comes from DRAM on big models (the
@@ -1316,15 +1463,19 @@ __global__ void __launch_bounds__(TMA_THREADS, 2) gemv_tma_kernel(const GemvPara
 // (l2b_generate_argmax_batch) skip_b keeps a stopped session's vector from appending KV rows, and once
 // every session has stopped (CTL_DONE) the launches still queued return at once.  Prefill and the
 // batched step clear CTL_DONE before they launch.
-// bf16 (W = bf16): stages of 8 rows are 16 KB, so the same ring bytes hold twice as many stages
-// (the host passes nstage doubled).
+// bf16 (W = bf16): stages of 8 rows are 16 KB, so the same ring bytes hold twice as many stages; q8
+// stages are 17 KB (pf_stages: the host passes the stages of the format that fit the fp32 ring's bytes).
+template <typename W>
+__host__ __device__ constexpr int pf_stages(int fp32_stages) {
+    return (int)((size_t)fp32_stages * TMA_STAGE_FLOATS * 4 / PrefillRing<W>::SLOT_BYTES);
+}
 template <int EPI, int NB, typename W = float>
 __global__ void __launch_bounds__(TMA_THREADS, 1) prefill_gemm_kernel(const GemvParams p) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
-    constexpr int MAX_STAGES = PF_MAX_STAGES * (4 / (int)sizeof(W));
+    constexpr int MAX_STAGES = pf_stages<W>(PF_MAX_STAGES);
     const int NSTAGE = p.nstage;
-    W *ring = reinterpret_cast<W *>(smem_raw);                         // NSTAGE x 32 KB (fp32) or 16 KB (bf16)
-    float *xs = reinterpret_cast<float *>(smem_raw + (size_t)NSTAGE * TmaRing<GEMV8_R, W>::SLOT_BYTES);   // NB x n floats
+    W *ring = reinterpret_cast<W *>(smem_raw);                         // NSTAGE x 32 KB (fp32), 16 KB (bf16) or 17 KB (q8)
+    float *xs = reinterpret_cast<float *>(smem_raw + (size_t)NSTAGE * PrefillRing<W>::SLOT_BYTES);   // NB x n floats
     __shared__ uint64_t full[MAX_STAGES], empty[MAX_STAGES], xbar, tile_full[2], tile_free[2];
     __shared__ float scratch[NB][NWARP + 2];
     __shared__ TileRed<NB> red;
@@ -1336,7 +1487,8 @@ __global__ void __launch_bounds__(TMA_THREADS, 1) prefill_gemm_kernel(const Gemv
     const RowSplit split = cta_row_split(p.total_rows);
     const int r0 = split.r0, r1 = split.r1, ntiles = split.ntiles;
     const int total = ntiles * nsteps;
-    const TmaRing<GEMV8_R, W> R = {ring, full, empty, NSTAGE, n4, nsteps, r0, r1, total};
+    const PrefillRing<W> R = {ring, full, empty, NSTAGE, n4, nsteps, r0, r1, total};
+    const int nslots = R.nslots();
 
     if (tid == 0) {
         for (int s = 0; s < NSTAGE; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], NWARP); }
@@ -1350,14 +1502,14 @@ __global__ void __launch_bounds__(TMA_THREADS, 1) prefill_gemm_kernel(const Gemv
         // the ring is filled before the dependency wait (weights are immutable); the rest of the stream
         // only while the batched generation loop is running (CTL_DONE, as in gemv_tma_kernel)
         RingProducer prod;
-        while (prod.it < total && prod.it < NSTAGE) prod.produce_one<EPI>(p, R, lane);
+        while (prod.it < nslots && prod.it < NSTAGE) prod.produce_one<EPI>(p, R, lane);
         pdl_wait();
         if (p.ctl[CTL_DONE]) {   // the loop has ended: drain the bulk copies already aimed at shared memory
             if (lane == 0)
                 for (int s = 0; s < prod.it; ++s) mbar_wait(&full[s], 0);
             return;
         }
-        while (prod.it < total) prod.produce_one<EPI>(p, R, lane);
+        while (prod.it < nslots) prod.produce_one<EPI>(p, R, lane);
         pdl_launch_dependents();
         return;
     }
@@ -1367,7 +1519,7 @@ __global__ void __launch_bounds__(TMA_THREADS, 1) prefill_gemm_kernel(const Gemv
     if (p.gamma) tma_fetch_gain(p, gv, ptid, n4);
     pdl_wait();
     const bool done = p.ctl[CTL_DONE] != 0;                            // read while x is staged below
-    const bool widen = sizeof(W) == 2 && p.emb;                        // bf16 embedding rows are widened, not bulk-copied
+    const bool widen = sizeof(W) != 4 && p.emb;                        // bf16 / q8 embedding rows are converted, not bulk-copied
     if (tid == 0) {
         const uint32_t bytes = (uint32_t)p.n * 4u;
         mbar_expect_tx(&xbar, widen ? 0u : bytes * (uint32_t)p.nb);
@@ -1379,7 +1531,7 @@ __global__ void __launch_bounds__(TMA_THREADS, 1) prefill_gemm_kernel(const Gemv
         }
     }
     if (widen) {
-        for (int b = 0; b < p.nb; ++b) widen_emb_row(p, p.tokens[b], xs + (size_t)b * p.n, ptid, TMA_PRO_THREADS);
+        for (int b = 0; b < p.nb; ++b) widen_emb_row<W>(p, p.tokens[b], xs + (size_t)b * p.n, ptid, TMA_PRO_THREADS);
         named_bar_sync(1, TMA_PRO_THREADS);
     }
     if (EPI == EPI_QKV && tid >= NT + 32) {                            // epilogue warp: RoPE rows of the vectors' positions
@@ -1901,12 +2053,19 @@ __global__ void __launch_bounds__(NT) attn_wo_kernel(const AttnWoParams q) {
     const int r0 = s * rows_per, r1 = min(q.dim, r0 + rows_per);
     const W *woh = static_cast<const W *>(q.wo) + (size_t)h * hs;     // column h * hs of row 0
     const int ld = w_pitch<W>(q.q_dim);
+    // float4 column group c of the head's columns of a row (q8: the scale index counts from the row's start)
+    auto wload = [&](int row, int c) -> float4 {
+        if constexpr (sizeof(W) == 1)
+            return ldg_w4<W>(static_cast<const W *>(q.wo) + (size_t)row * ld, h * hs4 + c, q.q_dim);
+        else
+            return ldg_w4<W>(woh + (size_t)row * ld, c, q.q_dim);
+    };
     float4 wpre[NF];
     {
         const int row = r0 + warp * RPW + rw;
 #pragma unroll
         for (int f = 0; f < NF; ++f)
-            wpre[f] = (row < r1) ? ldg_w4<W>(woh + (size_t)row * ld, lr + f * LPR) : make_float4(0.f, 0.f, 0.f, 0.f);
+            wpre[f] = (row < r1) ? wload(row, lr + f * LPR) : make_float4(0.f, 0.f, 0.f, 0.f);
     }
     pdl_launch_dependents();
     pdl_wait();
@@ -2015,7 +2174,7 @@ __global__ void __launch_bounds__(NT) attn_wo_kernel(const AttnWoParams q) {
 #pragma unroll
         for (int f = 0; f < NF; ++f) {
             const float4 w = first ? wpre[f]
-                                   : (valid ? ldg_w4<W>(woh + (size_t)row * ld, lr + f * LPR) : make_float4(0.f, 0.f, 0.f, 0.f));
+                                   : (valid ? wload(row, lr + f * LPR) : make_float4(0.f, 0.f, 0.f, 0.f));
             a = dot4(w, xb4[lr + f * LPR], a);
         }
         first = false;
@@ -2484,6 +2643,35 @@ __global__ void synth_fill_bf16_kernel(uint16_t *dst, uint64_t rows, uint64_t co
         const uint16_t b = bf16_round_bits(u);
         changed += ((uint32_t)b << 16) != u;
         dst[r * ld + c] = b;
+    }
+    changed = __reduce_add_sync(0xffffffffu, (unsigned int)changed);
+    if ((threadIdx.x & 31) == 0 && changed) atomicAdd(n_rounded, changed);
+}
+// The same values quantized to q8 (q8_scale / q8_code), one thread per group, into row records of
+// w_pitch<q8>(cols) bytes (the padding is the caller's zeros); the weights whose dequantized value
+// differs from the generated one are added to *n_rounded.  The values are generated twice (absolute
+// maximum, then codes) rather than held.
+__global__ void synth_fill_q8_kernel(unsigned char *dst, uint64_t rows, uint64_t cols, uint64_t first,
+                                     uint64_t src_cols, uint64_t tensor_seed, double mean, double scale,
+                                     float lo, float hi, unsigned long long *n_rounded) {
+    const uint64_t ng = (uint64_t)q8_groups((int)cols), total = rows * ng, ld = (uint64_t)w_pitch<q8>((int)cols);
+    unsigned long long changed = 0;
+    for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < total;
+         j += (uint64_t)gridDim.x * blockDim.x) {
+        const uint64_t r = j / ng, g = j - r * ng;
+        const uint64_t c0 = g * Q8_GROUP, c1 = min(cols, c0 + Q8_GROUP);
+        const uint64_t i0 = first + r * src_cols;
+        float a = 0.0f;
+        for (uint64_t c = c0; c < c1; ++c) a = fmaxf(a, fabsf(synth_value(tensor_seed, i0 + c, mean, scale, lo, hi)));
+        const float s = q8_scale(a);
+        unsigned char *row = dst + r * ld;
+        for (uint64_t c = c0; c < c1; ++c) {
+            const float v = synth_value(tensor_seed, i0 + c, mean, scale, lo, hi);
+            const int8_t q = q8_code(v, a, s);
+            changed += __float_as_uint(q8_dequant(q, s)) != __float_as_uint(v);
+            row[c] = (unsigned char)q;
+        }
+        reinterpret_cast<float *>(row + q8_scale_off((int)cols))[g] = s;
     }
     changed = __reduce_add_sync(0xffffffffu, (unsigned int)changed);
     if ((threadIdx.x & 31) == 0 && changed) atomicAdd(n_rounded, changed);

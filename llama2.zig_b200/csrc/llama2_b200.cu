@@ -16,6 +16,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <cmath>
 #include <chrono>
 #include <set>
 #include <string>
@@ -108,10 +109,10 @@ struct l2b_ctx {
     // device weights (Weights, src/main.zig:53-71), this rank's slices, owned by `weights`
     SharedWeights *weights = nullptr;
     float *rms_att = nullptr, *rms_ffn = nullptr, *rms_final = nullptr;
-    // matrix weights in the device format `wfmt` (l2b_weight_format): fp32, or bf16 with rows padded to
-    // w_pitch<bf16>(cols) elements; address them with wrow()
+    // matrix weights in the device format `wfmt` (l2b_weight_format): fp32, bf16 with rows padded to
+    // w_pitch<bf16>(cols) elements, or q8 row records of w_pitch<q8>(cols) bytes; address them with wrow()
     int wfmt = L2B_WEIGHTS_F32;
-    uint64_t n_rounded = 0;                  // matrix weights the bf16 rounding changed (l2b_weight_info)
+    uint64_t n_rounded = 0;                  // matrix weights the bf16 rounding / q8 quantization changed (l2b_weight_info)
     unsigned long long *d_rounded = nullptr; // ... counted on the device while synthetic weights are generated
     void *emb = nullptr;
     void *wq = nullptr, *wk = nullptr, *wv = nullptr, *wo = nullptr;
@@ -261,8 +262,15 @@ int dev_alloc(l2b_ctx *ctx, T **p, size_t count, std::vector<void *> *owner = nu
 
 // ---- device weight format ----
 bool is_bf16(const l2b_ctx *ctx) { return ctx->wfmt == L2B_WEIGHTS_BF16; }
-size_t w_elem(const l2b_ctx *ctx) { return is_bf16(ctx) ? 2 : 4; }
-uint64_t w_ld(const l2b_ctx *ctx, uint64_t cols) { return is_bf16(ctx) ? (uint64_t)w_pitch<bf16>((int)cols) : cols; }
+bool is_q8(const l2b_ctx *ctx) { return ctx->wfmt == L2B_WEIGHTS_Q8; }
+// bytes of a stored element and elements from one row to the next, of a matrix in format fmt
+size_t fmt_elem(int fmt) { return fmt == L2B_WEIGHTS_BF16 ? 2 : fmt == L2B_WEIGHTS_Q8 ? 1 : 4; }
+uint64_t fmt_ld(int fmt, uint64_t cols) {
+    return fmt == L2B_WEIGHTS_BF16 ? (uint64_t)w_pitch<bf16>((int)cols)
+           : fmt == L2B_WEIGHTS_Q8 ? (uint64_t)w_pitch<q8>((int)cols) : cols;
+}
+size_t w_elem(const l2b_ctx *ctx) { return fmt_elem(ctx->wfmt); }
+uint64_t w_ld(const l2b_ctx *ctx, uint64_t cols) { return fmt_ld(ctx->wfmt, cols); }
 // row `row` of a matrix of `cols` columns that starts at base
 const void *wrow(const l2b_ctx *ctx, const void *base, uint64_t row, uint64_t cols) {
     return static_cast<const unsigned char *>(base) + row * w_ld(ctx, cols) * w_elem(ctx);
@@ -316,7 +324,33 @@ struct Source {
 // in chunks through two pinned buffers: while chunk k is in flight on the copy engine, the host
 // is already filling the other buffer with chunk k+1 (for column-sharded tensors the host-side
 // fill also compacts the strided window, so the DMA is always a dense 1-D copy).
-int upload(l2b_ctx *ctx, void *dst, const float *src, uint64_t rows, uint64_t cols, uint64_t src_pitch, bool bf16w) {
+// Quantizes one row of cols fp32 weights into a q8 row record (w_pitch<q8>(cols) bytes, padding zeroed);
+// returns how many weights the quantization changed, or -1 when the row holds a non-finite value.
+int64_t quantize_q8_row(const float *w, uint64_t cols, unsigned char *rec) {
+    const int ng = q8_groups((int)cols), so = q8_scale_off((int)cols);
+    float *scales = reinterpret_cast<float *>(rec + so);
+    memset(rec, 0, (size_t)w_pitch<q8>((int)cols));
+    int64_t changed = 0;
+    for (int g = 0; g < ng; ++g) {
+        const uint64_t c0 = (uint64_t)g * Q8_GROUP, c1 = std::min<uint64_t>(cols, c0 + Q8_GROUP);
+        float a = 0.0f;
+        for (uint64_t c = c0; c < c1; ++c) {
+            if (!std::isfinite(w[c])) return -1;
+            a = std::max(a, std::fabs(w[c]));
+        }
+        const float s = q8_scale(a);
+        for (uint64_t c = c0; c < c1; ++c) {
+            const int8_t q = q8_code(w[c], a, s);
+            const float d = q8_dequant(q, s);
+            changed += memcmp(&d, w + c, 4) != 0;
+            rec[c] = (unsigned char)q;
+        }
+        memcpy(scales + g, &s, 4);
+    }
+    return changed;
+}
+
+int upload(l2b_ctx *ctx, void *dst, const float *src, uint64_t rows, uint64_t cols, uint64_t src_pitch, int fmt) {
     if (!ctx->stage[0]) {
         size_t want = 32ull << 20;
         const char *env = getenv("L2B_STAGE_MB");
@@ -328,10 +362,12 @@ int upload(l2b_ctx *ctx, void *dst, const float *src, uint64_t rows, uint64_t co
         }
     }
     // bf16: each row is rounded (bf16_round_bits) and padded with zeros to w_ld elements while it is
-    // packed into the stage, so the DMA moves dense bf16 rows
-    const uint64_t ld = bf16w ? (uint64_t)w_pitch<bf16>((int)cols) : cols;
-    const uint64_t row_bytes = bf16w ? ld * 2 : cols * sizeof(float);
-    const bool dense = (src_pitch == cols) && !bf16w;
+    // packed into the stage, so the DMA moves dense bf16 rows.  q8: each row is quantized into its row
+    // record (quantize_q8_row).
+    const bool bf16w = fmt == L2B_WEIGHTS_BF16, q8w = fmt == L2B_WEIGHTS_Q8;
+    const uint64_t ld = fmt_ld(fmt, cols);
+    const uint64_t row_bytes = ld * fmt_elem(fmt);
+    const bool dense = (src_pitch == cols) && fmt == L2B_WEIGHTS_F32;
     const uint64_t total = rows * row_bytes;
     uint64_t done = 0;                       // bytes of the dense destination already issued
     while (done < total) {
@@ -358,6 +394,16 @@ int upload(l2b_ctx *ctx, void *dst, const float *src, uint64_t rows, uint64_t co
                 for (uint64_t c = cols; c < ld; ++c) d[c] = 0;
             }
             ctx->n_rounded += changed;
+        } else if (q8w) {
+            const uint64_t r = chunk / row_bytes;
+            if (r == 0) return fail(ctx, L2B_ERR_UNSUPPORTED, "row larger than the upload staging buffer");
+            chunk = r * row_bytes;
+            const uint64_t row0 = done / row_bytes;
+            for (uint64_t i = 0; i < r; ++i) {
+                const int64_t changed = quantize_q8_row(src + (row0 + i) * src_pitch, cols, ctx->stage[b] + i * row_bytes);
+                if (changed < 0) return fail(ctx, L2B_ERR_INVALID_ARG, "non-finite matrix weight in a q8 payload");
+                ctx->n_rounded += (uint64_t)changed;
+            }
         } else if (!dense) {
             // whole rows only (a chunk never splits a row of a sharded window)
             uint64_t r = chunk / row_bytes;
@@ -379,7 +425,7 @@ int upload(l2b_ctx *ctx, void *dst, const float *src, uint64_t rows, uint64_t co
 }
 
 // matrix: a weight matrix, stored in the context's format (wfmt); otherwise fp32 (RMSNorm gains).
-// A bf16 matrix is only ever whole (single GPU).
+// A bf16 or q8 matrix is only ever whole (single GPU).
 int materialize(l2b_ctx *ctx, void **dptr, const Source &src, uint64_t payload_off, int tensor_id,
                 uint64_t L, uint64_t rows, uint64_t cols, ShardMode mode, Dist dist, bool matrix) {
     const uint64_t g = ctx->world, r = ctx->rank;
@@ -387,9 +433,9 @@ int materialize(l2b_ctx *ctx, void **dptr, const Source &src, uint64_t payload_o
     const uint64_t cols_loc = (mode == SH_COLS) ? cols / g : cols;
     const uint64_t row0 = (mode == SH_ROWS) ? r * rows_loc : 0;
     const uint64_t col0 = (mode == SH_COLS) ? r * cols_loc : 0;
-    const bool bf16w = matrix && is_bf16(ctx);
-    const uint64_t ld = bf16w ? (uint64_t)w_pitch<bf16>((int)cols_loc) : cols_loc;
-    const size_t esize = bf16w ? 2 : 4;
+    const int fmt = matrix ? ctx->wfmt : L2B_WEIGHTS_F32;
+    const uint64_t ld = fmt_ld(fmt, cols_loc);
+    const size_t esize = fmt_elem(fmt);
     unsigned char *base = nullptr;
     int rc = dev_alloc(ctx, &base, L * rows_loc * ld * esize, &ctx->weights->owned);
     if (rc) return rc;
@@ -398,13 +444,13 @@ int materialize(l2b_ctx *ctx, void **dptr, const Source &src, uint64_t payload_o
     const bool whole = (rows_loc == rows && cols_loc == cols);
     const uint64_t nl = whole ? 1 : L;            // one shot when nothing is cut
     const uint64_t rr = whole ? L * rows : rows_loc;
-    if (bf16w && !src.host)     // the row padding; the upload writes its own zeros
+    if (fmt != L2B_WEIGHTS_F32 && !src.host)     // the row padding; the upload writes its own zeros
         L2B_CUDA(ctx, cudaMemsetAsync(base, 0, L * rows_loc * ld * esize, ctx->stream));
     for (uint64_t l = 0; l < nl; ++l) {
         void *dst = base + l * rows_loc * ld * esize;
         const uint64_t first = l * rows * cols + row0 * cols + col0;
         if (src.host) {
-            rc = upload(ctx, dst, src.host + payload_off + first, rr, cols_loc, cols, bf16w);
+            rc = upload(ctx, dst, src.host + payload_off + first, rr, cols_loc, cols, fmt);
             if (rc) return rc;
         } else {
             const uint64_t total = rr * cols_loc;
@@ -412,7 +458,13 @@ int materialize(l2b_ctx *ctx, void **dptr, const Source &src, uint64_t payload_o
                                    ? (total + 255) / 256
                                    : (uint64_t)(ctx->num_sms * 16));
             if (blocks < 1) blocks = 1;
-            if (bf16w)
+            if (fmt == L2B_WEIGHTS_Q8) {
+                const uint64_t groups = rr * (uint64_t)q8_groups((int)cols_loc);   // one thread per group
+                const int gblocks = (int)std::min<uint64_t>((groups + 255) / 256, (uint64_t)ctx->num_sms * 16);
+                synth_fill_q8_kernel<<<gblocks < 1 ? 1 : gblocks, 256, 0, ctx->stream>>>(
+                    static_cast<unsigned char *>(dst), rr, cols_loc, first, cols, tensor_seed, dist.mean,
+                    dist.sigma * kSynthInvStd, dist.lo, dist.hi, ctx->d_rounded);
+            } else if (fmt == L2B_WEIGHTS_BF16)
                 synth_fill_bf16_kernel<<<blocks, 256, 0, ctx->stream>>>(
                     static_cast<uint16_t *>(dst), rr, cols_loc, first, cols, tensor_seed, dist.mean,
                     dist.sigma * kSynthInvStd, dist.lo, dist.hi, ctx->d_rounded);
@@ -437,7 +489,7 @@ int materialize(l2b_ctx *ctx, float **dptr, const Source &src, uint64_t payload_
 typedef void (*gemv_fn)(const GemvParams);
 
 // Kernel instantiations by weight element type W.  EPI_XCHG (tensor parallel) has fp32 kernels only:
-// bf16 weights are single-GPU.
+// bf16 and q8 weights are single-GPU.
 template <int EPI, typename W>
 gemv_fn gemv_pick(int tpr) {
     switch (tpr) {
@@ -514,11 +566,13 @@ gemv_fn gemv8_pick(int epi) {
 enum GemvKind { GK_LATENCY, GK_ROWS8, GK_TMA };
 
 // the formats an epilogue has kernels in: EPI_XCHG (tensor parallel) is fp32 only
-bool has_kernel(const l2b_ctx *ctx, int epi) { return !(is_bf16(ctx) && epi == EPI_XCHG); }
+bool has_kernel(const l2b_ctx *ctx, int epi) { return !(ctx->wfmt != L2B_WEIGHTS_F32 && epi == EPI_XCHG); }
 
 // The one place a GEMV kernel is chosen for the context's weight format.  The shape rules that pick
-// `kind` are the same for both formats (computed at 4 bytes per weight).
+// `kind` are the same for every format (computed at 4 bytes per weight).
 gemv_fn pick_gemv(const l2b_ctx *ctx, GemvKind kind, int epi, int tpr) {
+    if (is_q8(ctx))
+        return kind == GK_TMA ? gemv_tma_pick<q8>(epi) : kind == GK_ROWS8 ? gemv8_pick<q8>(epi) : gemv_pick<q8>(epi, tpr);
     if (is_bf16(ctx))
         return kind == GK_TMA ? gemv_tma_pick<bf16>(epi) : kind == GK_ROWS8 ? gemv8_pick<bf16>(epi) : gemv_pick<bf16>(epi, tpr);
     return kind == GK_TMA ? gemv_tma_pick<float>(epi) : kind == GK_ROWS8 ? gemv8_pick<float>(epi) : gemv_pick<float>(epi, tpr);
@@ -556,7 +610,7 @@ int launch_gemv(l2b_ctx *ctx, int epi, const GemvParams &p, cudaStream_t st, con
     }
     const size_t xbytes = (size_t)p.n * 4 * (1 + (p.gamma ? 1 : 0) + (p.parts ? 1 : 0));
     const size_t xonly = (size_t)p.n * 4;
-    const size_t slot_bytes = (size_t)TmaRing<TMA_SLOT_ROWS>::SLOT_BYTES;   // = TmaRing<GEMV8_R, bf16>::SLOT_BYTES
+    const size_t slot_bytes = is_q8(ctx) ? (size_t)DecodeRing<q8>::SLOT_BYTES : (size_t)DecodeRing<float>::SLOT_BYTES;   // = DecodeRing<bf16>'s
     // Decision from the shape.  Bandwidth-bound shapes take the TMA-ring kernel, latency-bound ones
     // the fine-grained kernel.  The ring kernel stages only x in shared memory; the rest of the
     // opt-in limit is its ring of 16 KB slots (13 next to a 16 KB x; DESIGN.md §4.1).
@@ -665,7 +719,7 @@ attn_wo_fn pick_attn_wo(int head_size, size_t *smem, int wfmt = L2B_WEIGHTS_F32)
     const int nf = hs4 / lpr;
     const int ng = NWARP * (32 / lpr);
     *smem = ((size_t)ng * head_size + 3 * (size_t)ng + 2 * (size_t)head_size + 4) * sizeof(float);
-    return wfmt == L2B_WEIGHTS_BF16 ? attn_wo_pick<bf16>(nf) : attn_wo_pick<float>(nf);
+    return wfmt == L2B_WEIGHTS_BF16 ? attn_wo_pick<bf16>(nf) : wfmt == L2B_WEIGHTS_Q8 ? attn_wo_pick<q8>(nf) : attn_wo_pick<float>(nf);
 }
 
 constexpr int kAttnClusterCtas = 8;   // CTAs per head cluster of attn_wo_kernel; 4 and 2 measured slower (DESIGN.md §4.6)
@@ -674,7 +728,7 @@ constexpr int kAttnClusterCtas = 8;   // CTAs per head cluster of attn_wo_kernel
 int launch_attn_wo(l2b_ctx *ctx, int layer, cudaStream_t st) {
     if (ctx->profiling) {
         const int hpos = ctx->n_appended > 0 ? ctx->n_appended - 1 : 0;
-        int prc = prof_mark(ctx, "attn_wo", layer, 2ull * (uint64_t)(hpos + 1) * ctx->kv_loc * 4ull + (uint64_t)ctx->dim * ctx->q_loc * 4ull, st);
+        int prc = prof_mark(ctx, "attn_wo", layer, 2ull * (uint64_t)(hpos + 1) * ctx->kv_loc * 4ull + (uint64_t)ctx->dim * w_ld(ctx, ctx->q_loc) * w_elem(ctx), st);
         if (prc) return prc;
     }
     AttnWoParams q{};
@@ -1124,7 +1178,7 @@ int preload_kernels(l2b_ctx *ctx) {
                             (const void *)resid_add_kernel, (const void *)sample_prep_kernel,
                             (const void *)sample_prep_batch_kernel, (const void *)logprob_kernel,
                             (const void *)logprob_batch_kernel, (const void *)synth_fill_kernel,
-                            (const void *)synth_fill_bf16_kernel,
+                            (const void *)synth_fill_bf16_kernel, (const void *)synth_fill_q8_kernel,
                             (const void *)kv_fork_kernel, (const void *)verify_accept_kernel};
     for (const void *f : others) L2B_CUDA(ctx, cudaFuncGetAttributes(&fa, f));
     // The kernels that run next to a TMA-ring GEMV in a decode step (the ring GEMVs, attention, the
@@ -1196,7 +1250,7 @@ int create_rank(l2b_ctx *ctx, const l2b_config *cfg, const Source &src, const fl
     const uint64_t o_wcls = off;
 
     const auto t_load0 = std::chrono::steady_clock::now();
-    if (is_bf16(ctx) && !src.host) {
+    if (ctx->wfmt != L2B_WEIGHTS_F32 && !src.host) {
         L2B_TRY(dev_alloc(ctx, &ctx->d_rounded, 1));
         L2B_TRY(cuda_try(ctx, cudaMemsetAsync(ctx->d_rounded, 0, sizeof(unsigned long long), ctx->stream), "memset"));
     }
@@ -1744,19 +1798,19 @@ int32_t l2b_create_synthetic_group(l2b_ctx **out, const l2b_config *cfg, uint64_
 
 int32_t l2b_create_format(l2b_ctx **out, const l2b_config *cfg, const float *host_weights, uint64_t n_floats,
                           const float *rope_cos, const float *rope_sin, int32_t n_gpus, int32_t weight_format) {
-    if (weight_format != L2B_WEIGHTS_F32 && weight_format != L2B_WEIGHTS_BF16) {
+    if (weight_format != L2B_WEIGHTS_F32 && weight_format != L2B_WEIGHTS_BF16 && weight_format != L2B_WEIGHTS_Q8) {
         g_create_error = "unknown weight format";
         return L2B_ERR_INVALID_ARG;
     }
     if (weight_format == L2B_WEIGHTS_F32) return l2b_create(out, cfg, host_weights, n_floats, rope_cos, rope_sin, n_gpus);
     if (!host_weights) { g_create_error = "host_weights is NULL"; return L2B_ERR_INVALID_ARG; }
-    if (n_gpus != 1) { g_create_error = "bf16 weights are single-GPU (n_gpus must be 1)"; return L2B_ERR_UNSUPPORTED; }
+    if (n_gpus != 1) { g_create_error = "bf16 and q8 weights are single-GPU (n_gpus must be 1)"; return L2B_ERR_UNSUPPORTED; }
     Source s; s.host = host_weights;
     return common_create(out, cfg, s, n_floats, rope_cos, rope_sin, nullptr, 1, weight_format);
 }
 
 int32_t l2b_create_synthetic_format(l2b_ctx **out, const l2b_config *cfg, uint64_t seed, int32_t weight_format) {
-    if (weight_format != L2B_WEIGHTS_F32 && weight_format != L2B_WEIGHTS_BF16) {
+    if (weight_format != L2B_WEIGHTS_F32 && weight_format != L2B_WEIGHTS_BF16 && weight_format != L2B_WEIGHTS_Q8) {
         g_create_error = "unknown weight format";
         return L2B_ERR_INVALID_ARG;
     }
@@ -1779,6 +1833,26 @@ void l2b_round_bf16_host(float *data, uint64_t n) {
         u = (uint32_t)bf16_round_bits(u) << 16;
         memcpy(data + i, &u, 4);
     }
+}
+
+int32_t l2b_round_q8_host(float *data, uint64_t rows, uint64_t cols, uint64_t *n_changed) {
+    if (!data || cols == 0 || cols > (1ull << 30)) return L2B_ERR_INVALID_ARG;
+    for (uint64_t i = 0; i < rows * cols; ++i)   // refuse before anything is written
+        if (!std::isfinite(data[i])) return L2B_ERR_INVALID_ARG;
+    std::vector<unsigned char> rec((size_t)w_pitch<q8>((int)cols));
+    const int so = q8_scale_off((int)cols);
+    uint64_t changed = 0;
+    for (uint64_t r = 0; r < rows; ++r) {
+        float *w = data + r * cols;
+        changed += (uint64_t)quantize_q8_row(w, cols, rec.data());
+        for (uint64_t c = 0; c < cols; ++c) {
+            float s;
+            memcpy(&s, rec.data() + so + (c / Q8_GROUP) * 4, 4);
+            w[c] = q8_dequant((int8_t)rec[c], s);
+        }
+    }
+    if (n_changed) *n_changed = changed;
+    return L2B_OK;
 }
 
 int32_t l2b_create_session(l2b_ctx **out, l2b_ctx *model) {
@@ -1923,7 +1997,7 @@ gemv_fn pf_pick(int epi) {
 }
 template <int NB>
 gemv_fn pf_pick(const l2b_ctx *ctx, int epi) {
-    return is_bf16(ctx) ? pf_pick<NB, bf16>(epi) : pf_pick<NB, float>(epi);
+    return is_q8(ctx) ? pf_pick<NB, q8>(epi) : is_bf16(ctx) ? pf_pick<NB, bf16>(epi) : pf_pick<NB, float>(epi);
 }
 constexpr size_t kPfSmemBudget = 227 * 1024 - 8192;   // the prefill kernels keep ~6.5 KB of static shared memory
 
@@ -1970,7 +2044,8 @@ template <int NB>
 static int pf_launch(l2b_ctx *ctx, int epi, GemvParams p, cudaStream_t st) {
     const size_t xbytes = (size_t)NB * p.n * 4;
     const int nstage = pf_ring_stages(kPfSmemBudget, xbytes);
-    p.nstage = is_bf16(ctx) ? 2 * nstage : nstage;   // the same ring bytes in 16 KB bf16 stages
+    // the same ring bytes in the format's stages: 32 KB fp32, 16 KB bf16, 17 KB q8
+    p.nstage = is_q8(ctx) ? pf_stages<q8>(nstage) : is_bf16(ctx) ? pf_stages<bf16>(nstage) : nstage;
     int grid = ctx->num_sms;
     const int npairs = (p.total_rows + 1) / 2;
     if (grid > npairs) grid = npairs;

@@ -30,7 +30,9 @@ static const char *usage_text =
     "     --draft <checkpoint>  speculative decoding with this draft model (same vocabulary); same tokens\n"
     "     --draft-k <int>       tokens the draft proposes per round, default 3, at most 32\n"
     "     --bf16                keep the matrix weights (and the draft's) in bf16 on the GPU: half the memory and\n"
-    "                           bytes per step; outputs equal an fp32 run of the bf16-rounded checkpoint (1 GPU)\n";
+    "                           bytes per step; outputs equal an fp32 run of the bf16-rounded checkpoint (1 GPU)\n"
+    "     --q8                  keep the matrix weights (and the draft's) as int8 with one scale per 64 weights: 0.53x\n"
+    "                           the bf16 bytes per step; outputs equal an fp32 run of the dequantized checkpoint (1 GPU)\n";
 
 // Generation with a draft model: the prompt positions are prefilled on target and draft, then
 // l2b_generate_speculative (-t 0) or l2h_generate_speculative_sample (-t > 0) runs the rest.  The tokens
@@ -104,6 +106,7 @@ int main(int argc, char **argv) {
         else if (a == "--draft") draft_path = need("draft");
         else if (a == "--draft-k") draft_k = atoi(need("draft-k"));
         else if (a == "--bf16") weight_format = L2B_WEIGHTS_BF16;
+        else if (a == "--q8") weight_format = L2B_WEIGHTS_Q8;
         else { fprintf(stderr, "error: unknown argument '%s'\n", argv[i]); fputs(usage_text, stdout); return 0; }
     }
     if (!bin_path) { fputs(usage_text, stdout); return 0; }
@@ -123,8 +126,8 @@ int main(int argc, char **argv) {
         int32_t fmt = 0;
         uint64_t n_rounded = 0;
         l2b_weight_info(ctx, &fmt, &n_rounded);
-        fprintf(stderr, "weights: %s on the GPU, %llu matrix weights changed by rounding\n\n",
-                fmt == L2B_WEIGHTS_BF16 ? "bf16" : "fp32", (unsigned long long)n_rounded);
+        fprintf(stderr, "weights: %s on the GPU, %llu matrix weights changed by rounding or quantization\n\n",
+                fmt == L2B_WEIGHTS_BF16 ? "bf16" : fmt == L2B_WEIGHTS_Q8 ? "q8" : "fp32", (unsigned long long)n_rounded);
     }
     l2h_free_checkpoint(&ck);   // host copy no longer needed: weights live in HBM
     l2b_ctx *draft = nullptr;
