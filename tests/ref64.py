@@ -64,7 +64,11 @@ def rope_angles(positions, head_size):
     """(n, head_size/2) float64 cos and sin of the reference's f32 angle pos * freq (:336-342); pair j
     of a head is dims (2j, 2j+1) of that head, its head_dim is 2j."""
     hd = np.arange(0, head_size, 2, dtype=np.float32)
-    freq = np.float32(1.0) / np.power(np.float32(10000.0), hd / np.float32(head_size))
+    # the correctly rounded f32 power (libm's powf gives it at every head size here); numpy's float32
+    # power is 1 ulp off at 11 of head size 128's 64 pairs, which turns the angle at position 8191 by
+    # 2.4e-4 rad
+    power = np.power(np.float64(10000.0), (hd / np.float32(head_size)).astype(np.float64)).astype(np.float32)
+    freq = np.float32(1.0) / power
     val = np.asarray(positions, dtype=np.float32)[:, None] * freq[None, :]
     val = val.astype(np.float64)
     return np.cos(val), np.sin(val)
@@ -100,10 +104,12 @@ class Run:
       every requested position p; key_cache, value_cache: (layers, seq_len, kv_dim) float64 with
       rows 0..n-1 filled, as state.key_cache / value_cache (:151-152, :353-358); probs[l][p]:
       (heads, p+1) attention weights of layer l at the requested positions, and scores[l][p] the
-      scaled scores they come from (:367-378)."""
+      scaled scores they come from (:367-378); q[l][p]: (heads, hs) the rotated query, att[l][p]:
+      (heads, hs) the attention output (:381-388)."""
 
     def __init__(self):
         self.logits, self.x, self.resid, self.probs, self.scores = {}, {}, {}, {}, {}
+        self.q, self.att = {}, {}
         self.key_cache = self.value_cache = None
 
 
@@ -143,18 +149,26 @@ def forward(shape, data, tokens, want, block=1 << 22):
         vals = r.value_cache[l, :n].reshape(n, KV, hs)
         att_out = np.empty((len(rows), H, hs))
         step = max(1, block // (H * n))
+        keys_t = np.ascontiguousarray(keys.transpose(1, 2, 0))                     # (KV, hs, n)
+        vals_g = np.ascontiguousarray(vals.transpose(1, 0, 2))                     # (KV, n, hs)
         for b in range(0, len(rows), step):                                        # :361-389
             qb = q[b:b + step].reshape(-1, KV, kv_mul, hs)                         # head h reads kv head h / kv_mul
-            sc = np.einsum("qgmd,tgd->qgmt", qb, keys) / np.sqrt(hs)                # :367-375
+            nb = qb.shape[0]
+            # one batched matmul per kv head over all its query heads and rows: (KV, nb*kv_mul, n)
+            sc = np.matmul(qb.transpose(1, 0, 2, 3).reshape(KV, nb * kv_mul, hs), keys_t) / np.sqrt(hs)   # :367-375
+            sc = sc.reshape(KV, nb, kv_mul, n).transpose(1, 0, 2, 3)               # (nb, KV, kv_mul, n)
             pos = rows[b:b + step]
             sc = np.where(np.arange(n)[None, None, None, :] <= pos[:, None, None, None], sc, -np.inf)
             p = np.exp(sc - sc.max(axis=-1, keepdims=True))                        # :378, :687-706
             p /= p.sum(axis=-1, keepdims=True)
-            att_out[b:b + step] = np.einsum("qgmt,tgd->qgmd", p, vals).reshape(-1, H, hs)   # :381-388
+            pg = np.ascontiguousarray(p.transpose(1, 0, 2, 3)).reshape(KV, nb * kv_mul, n)
+            att_out[b:b + step] = np.matmul(pg, vals_g).reshape(KV, nb, kv_mul, hs).transpose(1, 0, 2, 3).reshape(nb, H, hs)   # :381-388
             for i, ps in enumerate(pos):
                 if ps in want:
                     r.scores.setdefault(l, {})[int(ps)] = sc[i].reshape(H, n)[:, :ps + 1].copy()
                     r.probs.setdefault(l, {})[int(ps)] = p[i].reshape(H, n)[:, :ps + 1].copy()
+                    r.q.setdefault(l, {})[int(ps)] = q[b + i].copy()
+                    r.att.setdefault(l, {})[int(ps)] = att_out[b + i].copy()
         x = x + matmul(att_out.reshape(len(rows), dim), w["wo"][l])               # :392-395
         xb = rmsnorm(x, w["rms_ffn_weight"][l].astype(np.float64))                # :398
         h1, h3 = matmul(xb, w["w1"][l]), matmul(xb, w["w3"][l])                    # :405-408
