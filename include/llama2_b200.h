@@ -530,7 +530,8 @@ int32_t l2b_op_logprob(int32_t device, const float *logits, int32_t n, int32_t t
 typedef enum l2b_weight_format { L2B_WEIGHTS_F32 = 0, L2B_WEIGHTS_BF16 = 1, L2B_WEIGHTS_Q8 = 3 } l2b_weight_format;
 #define L2B_Q8_GROUP 64
 
-/* l2b_create with a device weight format.  L2B_WEIGHTS_F32 is exactly l2b_create.  Checked before
+/* l2b_create with a device weight format (and optionally L2B_KV_BF16, see below).  L2B_WEIGHTS_F32 is
+ * exactly l2b_create.  Checked before
  * any device is touched: an unknown format => L2B_ERR_INVALID_ARG; L2B_WEIGHTS_BF16 or L2B_WEIGHTS_Q8
  * with n_gpus > 1 => L2B_ERR_UNSUPPORTED (tensor parallel is fp32 only); every other check is
  * l2b_create's, plus (q8) a non-finite matrix weight => L2B_ERR_INVALID_ARG.                        */
@@ -552,6 +553,35 @@ void l2b_round_bf16_host(float *data, uint64_t n);
  * L * rows rows.  NULL data, cols == 0, cols > 2^30 or a non-finite value => L2B_ERR_INVALID_ARG with
  * data untouched (every value is checked before any is written).                                   */
 int32_t l2b_round_q8_host(float *data, uint64_t rows, uint64_t cols, uint64_t *n_changed);
+
+/* ---- KV-cache format ------------------------------------------------------------------------
+ * L2B_KV_BF16, or'd into the weight_format of l2b_create_format / l2b_create_synthetic_format (with any
+ * weight format, e.g. L2B_WEIGHTS_Q8 | L2B_KV_BF16), keeps the context's key and value caches in bf16:
+ * half the cache memory and half the cache bytes attention reads per step.  Any other bit outside the
+ * weight formats => L2B_ERR_INVALID_ARG; L2B_KV_BF16 with n_gpus > 1 => L2B_ERR_UNSUPPORTED (tensor
+ * parallel is fp32 only), both checked before any device is touched.  Sessions (l2b_create_session)
+ * take their model's KV format, so every batched call and every l2b_fork is of one format.
+ * Rounding: every K value (after RoPE) and every V value is rounded to the nearest bf16, ties to even,
+ * as it is appended (the weights' rounding above: NaN stays NaN, overflow goes to +-inf, subnormals are
+ * rounded).  Attention widens each stored value exactly; q, scores, softmax, partials and all run state
+ * stay fp32.
+ * Contract: a bf16-KV context returns, on every entry point, exactly what an fp32-KV context of the same
+ * payload and weight format returns when it rounds every appended K/V value to bf16 before storing it
+ * (an L2B_KV_ROUND_BF16 context, below): logits,
+ * probabilities, candidates, log-probabilities, tokens, n_accept, n_done, and l2b_read_state of x, the
+ * KV cache and the logits.  Each bf16-KV kernel is the fp32 kernel the same shape selects.
+ * l2b_read_state(4 / 5) returns the caches widened to fp32 (the same count of floats); l2b_step_bytes'
+ * kv_bytes and the attention / attn_wo bytes of l2b_profile_step count 2 bytes per stored element.     */
+#define L2B_KV_BF16 0x100
+/* The reference of that contract, for tests: an fp32 cache that rounds every appended K/V value to bf16
+ * and stores it widened; attention runs the fp32 kernels.  It is not a format to serve with: it costs the
+ * fp32 cache's memory and bytes and the bf16 cache's accuracy.  Or'd in like L2B_KV_BF16, with the same
+ * checks; both flags together => L2B_ERR_INVALID_ARG.                                                  */
+#define L2B_KV_ROUND_BF16 0x200
+/* The KV format of ctx (0: fp32, L2B_KV_BF16, L2B_KV_ROUND_BF16) and the bytes of its key and value caches
+ * together: 2 * n_layers * seq_len * kv_dim * (2 for L2B_KV_BF16, else 4).  l2b_weight_info reports the
+ * weight format alone.                                                                                 */
+int32_t l2b_kv_info(const l2b_ctx *ctx, int32_t *kv_format, uint64_t *cache_bytes);
 
 #ifdef __cplusplus
 }

@@ -138,6 +138,7 @@ def load_library():
                                       C.c_int32]
     lib.l2b_create_synthetic_format.argtypes = [C.POINTER(vp), C.POINTER(L2BConfig), C.c_uint64, C.c_int32]
     lib.l2b_weight_info.argtypes = [vp, IP, U64P]
+    lib.l2b_kv_info.argtypes = [vp, IP, U64P]
     lib.l2b_round_bf16_host.argtypes = [FP, C.c_uint64]
     lib.l2b_round_bf16_host.restype = None
     lib.l2b_round_q8_host.argtypes = [FP, C.c_uint64, C.c_uint64, U64P]
@@ -177,6 +178,9 @@ WEIGHT_FORMATS = {"f32": 0, "bf16": 1}   # l2b_weight_format: one stored element
 QUANT_FORMATS = {"q8": 3}                # l2b_weight_format: codes plus a scale per group of weights
 _FORMATS = {**WEIGHT_FORMATS, **QUANT_FORMATS}
 Q8_GROUP = 64   # L2B_Q8_GROUP
+KV_BF16 = 0x100                          # L2B_KV_BF16: or'd into the weight format of l2b_create_format
+KV_ROUND_BF16 = 0x200                    # L2B_KV_ROUND_BF16: fp32 cache of bf16-rounded values (the reference)
+KV_FORMATS = {"f32": 0, "bf16": KV_BF16, "f32-round-bf16": KV_ROUND_BF16}   # l2b_kv_info's kv_format
 
 
 def round_bf16_host(a):
@@ -219,19 +223,23 @@ class Transformer:
     `ck` is a checkpoint.Checkpoint.  With `ck.data` set the payload is uploaded
     (l2b_create / l2b_create_sharded); with `synthetic_seed` the weights are generated on the
     device (l2b_create_synthetic).  weight_format="bf16" keeps the matrix weights in bf16 on the
-    device, "q8" as int8 with one fp32 scale per 64 weights of a row (l2b_create_format /
-    l2b_create_synthetic_format; single GPU, device 0).
+    device, "q8" as int8 with one fp32 scale per 64 weights of a row; kv_format="bf16" keeps the KV
+    cache in bf16, "f32-round-bf16" in fp32 holding bf16-rounded values, the bf16 cache's bitwise reference
+    (l2b_create_format / l2b_create_synthetic_format; single GPU, device 0).  Sessions take the model's
+    formats.
     """
 
     def __init__(self, ck, synthetic_seed=None, rank=0, world_size=1, device=0, comm_id=None,
-                 rope_cos=None, rope_sin=None, n_gpus=1, weight_format="f32"):
+                 rope_cos=None, rope_sin=None, n_gpus=1, weight_format="f32", kv_format="f32"):
         """n_gpus > 1: ONE process drives n_gpus GPUs (l2b_create(.., n_gpus)); rank/world_size:
         one process per GPU (l2b_create_sharded)."""
         if weight_format not in _FORMATS:
             raise ValueError(f"weight_format must be one of {sorted(_FORMATS)}")
-        fmt = _FORMATS[weight_format]
+        if kv_format not in KV_FORMATS:
+            raise ValueError(f"kv_format must be one of {sorted(KV_FORMATS)}")
+        fmt = _FORMATS[weight_format] | KV_FORMATS[kv_format]
         if fmt and (world_size > 1 or device != 0 or rank != 0 or n_gpus != 1):
-            raise ValueError(f"{weight_format} weights are single-GPU on device 0")
+            raise ValueError(f"{weight_format} weights with a {kv_format} KV cache are single-GPU on device 0")
         self.lib = load_library()
         self.ck = ck
         self.cfg = make_config(ck)
@@ -374,6 +382,14 @@ class Transformer:
         n = C.c_uint64()
         _check(self.lib.l2b_weight_info(self.h, C.byref(fmt), C.byref(n)), self.h)
         return {v: k for k, v in _FORMATS.items()}[fmt.value], n.value
+
+    def kv_info(self):
+        """(kv_format name, cache_bytes): the format of this context's KV cache (a KV_FORMATS key) and the
+        bytes of its key and value caches together (l2b_kv_info)."""
+        fmt = C.c_int32()
+        n = C.c_uint64()
+        _check(self.lib.l2b_kv_info(self.h, C.byref(fmt), C.byref(n)), self.h)
+        return {v: k for k, v in KV_FORMATS.items()}[fmt.value], n.value
 
     def load_stats(self):
         ms = C.c_double()

@@ -12,6 +12,7 @@
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <type_traits>
 
 namespace l2b {
 
@@ -253,6 +254,38 @@ __device__ __forceinline__ float4 widen_bf16x4(uint2 u) {
                        __uint_as_float(u.y << 16), __uint_as_float(u.y & 0xFFFF0000u));
 }
 
+// ---- KV-cache element types.  KV is a template parameter of every kernel that writes or reads the cache:
+//   float       the fp32 cache;
+//   bf16        the bf16 cache (L2B_KV_BF16): each appended value rounded by bf16_round_bits, widened on load;
+//   kv_f32_bf16 an fp32 cache whose appended values are rounded to bf16 and stored widened (the
+//               L2B_KV_ROUND_BF16 reference).  Only the writers have it; its readers are the fp32 kernels.
+struct kv_f32_bf16 { float v; };
+template <typename KV>
+__device__ __forceinline__ float kv_value(float x) {
+    return std::is_same<KV, float>::value ? x : __uint_as_float((uint32_t)bf16_round_bits(__float_as_uint(x)) << 16);
+}
+// the cache pair (dst[0], dst[1]) = (a0, a1) as KV elements: one 64-bit store (fp32) or one 32-bit store (bf16)
+template <typename KV>
+__device__ __forceinline__ void kv_store2(KV *dst, float a0, float a1) {
+    if constexpr (sizeof(KV) == 2)
+        *reinterpret_cast<uint32_t *>(dst) = (uint32_t)bf16_round_bits(__float_as_uint(a0)) |
+                                             ((uint32_t)bf16_round_bits(__float_as_uint(a1)) << 16);
+    else
+        *reinterpret_cast<float2 *>(dst) = make_float2(kv_value<KV>(a0), kv_value<KV>(a1));
+}
+// float4 group j (ldg_kv4) or lr + k (ldcg_kv4) of a cache row, through the read-only path (ldg) or L2 only
+// (ldcg), widened exactly
+template <typename KV>
+__device__ __forceinline__ float4 ldcg_kv4(const KV *row, int lr, int k) {
+    if constexpr (sizeof(KV) == 2) return widen_bf16x4(__ldcg(reinterpret_cast<const uint2 *>(row) + lr + k));
+    else return __ldcg(reinterpret_cast<const float4 *>(row) + lr + k);
+}
+template <typename KV>
+__device__ __forceinline__ float4 ldg_kv4(const KV *row, int j) {
+    if constexpr (sizeof(KV) == 2) return widen_bf16x4(__ldg(reinterpret_cast<const uint2 *>(row) + j));
+    else return __ldg(reinterpret_cast<const float4 *>(row) + j);
+}
+
 // float4 column group c of a weight row of n columns in global memory (streaming, no L1 allocation;
 // a q8 scale, shared by 16 neighbouring groups, is read through L1)
 template <typename W>
@@ -373,7 +406,7 @@ struct GemvParams {
     int total_rows;           // virtual rows
     // ---- outputs
     float *out0;            // STORE: out; QKV: q; SILU: hb; RESID: the residual stream x (read-modify-write)
-    float *kcache, *vcache; // QKV: this layer's (seq_len, kv_dim) caches
+    void *kcache, *vcache;  // QKV: this layer's (seq_len, kv_dim) caches, element type KV
     const float *rope_cos, *rope_sin;  // (seq_len, head_size/2)
     int head_size, kv_dim;
     unsigned long long *amax;  // ARGMAX: packed running maximum (must be 0 before the launch)
@@ -402,7 +435,7 @@ struct GemvParams {
     const int *tokens;
     int nb;
     int pos_b[PF_MAXB];
-    float *kcache_b[PF_MAXB], *vcache_b[PF_MAXB];
+    void *kcache_b[PF_MAXB], *vcache_b[PF_MAXB];
     // EPI_QKV of the batched kernels: vector b appends no KV row when skip_b[b] != 0 (a session that has
     // stopped in the batched generation loop), or nullptr: every vector appends
     const int *skip_b;
@@ -443,9 +476,12 @@ __device__ __forceinline__ void widen_emb_row(const GemvParams &p, int token, fl
 
 // EPI_QKV, rows (v, v+1): an adjacent pair of q, k or v (segment sizes are even).  q and k pairs are
 // rotated by the RoPE row (rc, rs) of position `pos`; q goes to `q`, k and v to row `pos` of the caches
-// kc / vc.  The ring kernels' epilogue warps use it with the RoPE rows they staged in shared memory.
-__device__ __forceinline__ void qkv_store_pair(const GemvParams &p, float *q, float *kc, float *vc, int pos,
+// kc / vc as KV elements.  The ring kernels' epilogue warps use it with the RoPE rows they staged in shared
+// memory.
+template <typename KV>
+__device__ __forceinline__ void qkv_store_pair(const GemvParams &p, float *q, void *kcv, void *vcv, int pos,
                                                const float *rc, const float *rs, int v, float a0, float a1) {
+    KV *kc = static_cast<KV *>(kcv), *vc = static_cast<KV *>(vcv);
     if (v < p.rows0 + p.rows1) {
         const bool is_q = v < p.rows0;
         const int i = is_q ? v : v - p.rows0;            // index within q / k
@@ -454,17 +490,22 @@ __device__ __forceinline__ void qkv_store_pair(const GemvParams &p, float *q, fl
         // :348-349, evaluated without FMA contraction like the reference
         const float r0 = __fsub_rn(__fmul_rn(a0, fcr), __fmul_rn(a1, fci));
         const float r1 = __fadd_rn(__fmul_rn(a0, fci), __fmul_rn(a1, fcr));
-        float *dst = is_q ? q + i : kc + (size_t)pos * p.kv_dim + i;   // :355,:357
-        *reinterpret_cast<float2 *>(dst) = make_float2(r0, r1);
+        if (sizeof(KV) == 4 || is_q) {                   // 4-byte caches: q and k share one 64-bit store
+            float *dst = is_q ? q + i : reinterpret_cast<float *>(kc + (size_t)pos * p.kv_dim + i);   // :355,:357
+            *reinterpret_cast<float2 *>(dst) = is_q ? make_float2(r0, r1) : make_float2(kv_value<KV>(r0), kv_value<KV>(r1));
+        } else {
+            kv_store2(kc + (size_t)pos * p.kv_dim + i, r0, r1);
+        }
     } else {
         const int i = v - p.rows0 - p.rows1;
-        *reinterpret_cast<float2 *>(vc + (size_t)pos * p.kv_dim + i) = make_float2(a0, a1);  // :356,:358
+        kv_store2(vc + (size_t)pos * p.kv_dim + i, a0, a1);  // :356,:358
     }
 }
 // the decode step's form: the layer's caches of the launch
+template <typename KV>
 __device__ __forceinline__ void qkv_store_pair(const GemvParams &p, float *q, int pos, const float *rc,
                                                const float *rs, int v, float a0, float a1) {
-    qkv_store_pair(p, q, p.kcache, p.vcache, pos, rc, rs, v, a0, a1);
+    qkv_store_pair<KV>(p, q, p.kcache, p.vcache, pos, rc, rs, v, a0, a1);
 }
 
 // ---- tensor-parallel all-reduce, second half, run by ONE warp of a wo / w2 CTA after that CTA has
@@ -601,8 +642,9 @@ __device__ __forceinline__ void gemv_stage_input(const GemvParams &p, float *xs,
 }
 
 // ---- shared epilogue for one adjacent pair of virtual rows (v0 even).  `xr` is the pair of
-// residual-stream values the caller prefetched for EPI_RESID (ignored otherwise).
-template <int EPI>
+// residual-stream values the caller prefetched for EPI_RESID (ignored otherwise).  KV: the cache element
+// type (EPI_QKV).
+template <int EPI, typename KV = float>
 __device__ __forceinline__ void gemv_epilogue_pair(const GemvParams &p, int v0, float a0, float a1,
                                                    int pos, unsigned long long &best, unsigned int epoch,
                                                    float2 xr) {
@@ -628,7 +670,10 @@ __device__ __forceinline__ void gemv_epilogue_pair(const GemvParams &p, int v0, 
         }
     } else if (EPI == EPI_QKV) {
         // rows (v0, v0+1) are an adjacent pair of q, k or v (segment sizes are even)
-        if (v0 < p.rows0 + p.rows1) {
+        if constexpr (!std::is_same<KV, float>::value) {
+            const size_t ro = (size_t)pos * (p.head_size >> 1);
+            qkv_store_pair<KV>(p, p.out0, pos, p.rope_cos + ro, p.rope_sin + ro, v0, a0, a1);
+        } else if (v0 < p.rows0 + p.rows1) {
             const bool is_q = v0 < p.rows0;
             const int i = is_q ? v0 : v0 - p.rows0;       // index within q / k
             const int pr = (i % p.head_size) >> 1;          // :338 (i % head_size)
@@ -637,11 +682,11 @@ __device__ __forceinline__ void gemv_epilogue_pair(const GemvParams &p, int v0, 
             // :348-349, evaluated without FMA contraction like the reference
             const float r0 = __fsub_rn(__fmul_rn(a0, fcr), __fmul_rn(a1, fci));
             const float r1 = __fadd_rn(__fmul_rn(a0, fci), __fmul_rn(a1, fcr));
-            float *dst = is_q ? p.out0 + i : p.kcache + (size_t)pos * p.kv_dim + i;   // :355,:357
+            float *dst = is_q ? p.out0 + i : static_cast<float *>(p.kcache) + (size_t)pos * p.kv_dim + i;   // :355,:357
             *reinterpret_cast<float2 *>(dst) = make_float2(r0, r1);
         } else {
             const int i = v0 - p.rows0 - p.rows1;
-            *reinterpret_cast<float2 *>(p.vcache + (size_t)pos * p.kv_dim + i) = make_float2(a0, a1);  // :356,:358
+            *reinterpret_cast<float2 *>(static_cast<float *>(p.vcache) + (size_t)pos * p.kv_dim + i) = make_float2(a0, a1);  // :356,:358
         }
     } else {  // EPI_SILU
         const float sg = __fmul_rn(a0, __fdiv_rn(1.0f, __fadd_rn(1.0f, expf(-a0))));   // :412
@@ -673,7 +718,7 @@ __device__ __forceinline__ void gemv_finish_argmax(const GemvParams &p, unsigned
 }
 
 // ---- v1: small / latency-bound shapes.  TPR threads per pair of rows, tiles strided over CTAs.
-template <int TPR, int EPI, typename W = float>
+template <int TPR, int EPI, typename W = float, typename KV = float>
 __global__ void __launch_bounds__(NT) gemv_kernel(const GemvParams p) {
     constexpr int GROUPS = NT / TPR;           // row groups per CTA
     constexpr int TILE_ROWS = GROUPS * GEMV_R;
@@ -792,7 +837,7 @@ __global__ void __launch_bounds__(NT) gemv_kernel(const GemvParams p) {
                 }
             }
             if (sub == 0)
-                gemv_epilogue_pair<EPI>(p, tile * TILE_ROWS + grp * GEMV_R, acc[0], acc[1], pos, best, epoch, xr);
+                gemv_epilogue_pair<EPI, KV>(p, tile * TILE_ROWS + grp * GEMV_R, acc[0], acc[1], pos, best, epoch, xr);
 #pragma unroll
             for (int r = 0; r < GEMV_R; ++r) acc[r] = 0.0f;
         }
@@ -871,7 +916,7 @@ __device__ __forceinline__ float2 sum_warp_partials(const float (&red)[NWARP][GE
     return make_float2(s0, s1);
 }
 
-template <int EPI, typename W = float>
+template <int EPI, typename W = float, typename KV = float>
 __global__ void __launch_bounds__(NT, 2) gemv8_kernel(const GemvParams p) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     float *xs = reinterpret_cast<float *>(smem_raw);
@@ -942,7 +987,7 @@ __global__ void __launch_bounds__(NT, 2) gemv8_kernel(const GemvParams p) {
         if (tid < GEMV8_R / 2) {
             const float2 s = sum_warp_partials<1>(red[par], tid, 0);
             const int v0 = r0 + t * GEMV8_R + 2 * tid;
-            if (v0 < r1) gemv_epilogue_pair<EPI>(p, v0, s.x, s.y, pos, best, epoch, xr);
+            if (v0 < r1) gemv_epilogue_pair<EPI, KV>(p, v0, s.x, s.y, pos, best, epoch, xr);
         }
 #pragma unroll
         for (int r = 0; r < GEMV8_R; ++r) acc[r] = 0.0f;
@@ -1284,7 +1329,7 @@ __device__ __forceinline__ void tma_consume(const TmaRing<SR, W, KS> &R, const f
     }
 }
 
-template <int EPI, typename W = float>
+template <int EPI, typename W = float, typename KV = float>
 __global__ void __launch_bounds__(TMA_THREADS, 2) gemv_tma_kernel(const GemvParams p) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int NSTAGE = p.nstage;
@@ -1425,7 +1470,7 @@ __global__ void __launch_bounds__(TMA_THREADS, 2) gemv_tma_kernel(const GemvPara
             if (lane == 0) mbar_arrive(&tile_free[par]);  // consumers may overwrite red[par]
             const int vp = r0 + t * GEMV8_R + 2 * lane;
             if (lane < GEMV8_R / 2 && vp < r1) {
-                if (EPI == EPI_QKV) qkv_store_pair(p, p.out0, pos, rope_s[0], rope_s[1], vp, s.x, s.y);
+                if (EPI == EPI_QKV) qkv_store_pair<KV>(p, p.out0, pos, rope_s[0], rope_s[1], vp, s.x, s.y);
                 else gemv_epilogue_pair<EPI>(p, vp, s.x, s.y, pos, best, epoch, xr);
             }
         }
@@ -1469,7 +1514,7 @@ template <typename W>
 __host__ __device__ constexpr int pf_stages(int fp32_stages) {
     return (int)((size_t)fp32_stages * TMA_STAGE_FLOATS * 4 / PrefillRing<W>::SLOT_BYTES);
 }
-template <int EPI, int NB, typename W = float>
+template <int EPI, int NB, typename W = float, typename KV = float>
 __global__ void __launch_bounds__(TMA_THREADS, 1) prefill_gemm_kernel(const GemvParams p) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     constexpr int MAX_STAGES = pf_stages<W>(PF_MAX_STAGES);
@@ -1562,7 +1607,7 @@ __global__ void __launch_bounds__(TMA_THREADS, 1) prefill_gemm_kernel(const Gemv
             if (!active || vp >= r1) continue;
             if (EPI == EPI_QKV) {
                 if (append || vp < p.rows0)                            // q rows always; k / v rows are the KV append
-                    qkv_store_pair(p, p.out0 + (size_t)eb * p.rows0, p.kcache_b[eb], p.vcache_b[eb], p.pos_b[eb],
+                    qkv_store_pair<KV>(p, p.out0 + (size_t)eb * p.rows0, p.kcache_b[eb], p.vcache_b[eb], p.pos_b[eb],
                                    rope_s[eb][0], rope_s[eb][1], vp, s.x, s.y);
             } else if (EPI == EPI_STORE || EPI == EPI_ARGMAX) {   // logits[b][row] (:429), as gemv_epilogue_pair
                 float *dst = p.out0 + (size_t)eb * p.total_rows;
@@ -1633,8 +1678,8 @@ __global__ void __launch_bounds__(NT) gemv_scalar_kernel(float *out, const float
 struct AttnParams {
     const int *ctl;
     const float *q;        // (n_heads * head_size)
-    const float *kcache;   // this layer: (seq_len, kv_dim)
-    const float *vcache;
+    const void *kcache;    // this layer: (seq_len, kv_dim), element type KV
+    const void *vcache;
     float *xb;             // (n_heads * head_size)
     float *part_o;         // (n_heads, nsplit, head_size)
     float *part_ml;        // (n_heads, nsplit, 2)
@@ -1651,7 +1696,7 @@ struct AttnParams {
 // Query z of a batched launch: position pos[z] over this layer's caches kcache[z] / vcache[z].  The
 // queries of one launch may be positions of one prompt (one cache) or of different sessions.
 struct AttnBatch {
-    const float *kcache[PF_MAXB], *vcache[PF_MAXB];
+    const void *kcache[PF_MAXB], *vcache[PF_MAXB];
     int pos[PF_MAXB];
 };
 // a[z] through compares with constant indices: indexing the parameter by z would copy it to local memory
@@ -1668,7 +1713,8 @@ __device__ __forceinline__ int attn_lanes_per_row(int hs4) {
 }
 
 // scores for positions [t0,t1) of one head into sc[0..t1-t0); q fragments live in registers
-__device__ __forceinline__ void attn_scores(float *sc, const float *qg, const float *kbase,
+template <typename KV>
+__device__ __forceinline__ void attn_scores(float *sc, const float *qg, const KV *kbase,
                                             int kv_dim, int head_size, int t0, int t1) {
     const int hs4 = head_size >> 2;
     const int lpr = attn_lanes_per_row(hs4);
@@ -1682,10 +1728,10 @@ __device__ __forceinline__ void attn_scores(float *sc, const float *qg, const fl
         const int t = tb + rw;
         float acc = 0.0f;
         if (t < t1) {
-            const float4 *k4 = reinterpret_cast<const float4 *>(kbase + (size_t)t * kv_dim);
+            const KV *k4 = kbase + (size_t)t * kv_dim;
             for (int f = 0; f < nf; ++f) {
                 const int j = lr + f * lpr;
-                acc = dot4(__ldg(k4 + j), __ldg(q4 + j), acc);
+                acc = dot4(ldg_kv4(k4, j), __ldg(q4 + j), acc);
             }
         }
         for (int o = lpr >> 1; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
@@ -1694,7 +1740,8 @@ __device__ __forceinline__ void attn_scores(float *sc, const float *qg, const fl
 }
 
 // red[g][0..head_size) = sum over this group's rows of w[t-t0] * V[t]   (G = NT / (head_size/4))
-__device__ __forceinline__ void attn_weighted_rows(float *red, const float *w, const float *vbase,
+template <typename KV>
+__device__ __forceinline__ void attn_weighted_rows(float *red, const float *w, const KV *vbase,
                                                    int kv_dim, int head_size, int t0, int t1) {
     const int hs4 = head_size >> 2;
     const int G = NT / hs4;
@@ -1704,7 +1751,7 @@ __device__ __forceinline__ void attn_weighted_rows(float *red, const float *w, c
         float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
         for (int t = t0 + g; t < t1; t += G) {
             const float wt = w[t - t0];
-            const float4 v = __ldg(reinterpret_cast<const float4 *>(vbase + (size_t)t * kv_dim) + c);
+            const float4 v = ldg_kv4(vbase + (size_t)t * kv_dim, c);
             a.x = fmaf(v.x, wt, a.x); a.y = fmaf(v.y, wt, a.y);
             a.z = fmaf(v.z, wt, a.z); a.w = fmaf(v.w, wt, a.w);
         }
@@ -1714,6 +1761,7 @@ __device__ __forceinline__ void attn_weighted_rows(float *red, const float *w, c
 
 // The AttnBatch argument only gives it attention_flash_kernel's signature: batched launches take the
 // flash kernel (pf_prepare), so this kernel never sees one.
+template <typename KV = float>
 __global__ void __launch_bounds__(NT) attention_kernel(const AttnParams p, const AttnBatch) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     __shared__ int is_last;
@@ -1744,7 +1792,7 @@ __global__ void __launch_bounds__(NT) attention_kernel(const AttnParams p, const
     const int tid = threadIdx.x, lane = tid & 31;
     const size_t hoff = (size_t)(h / p.kv_mul) * hs;   // :369, :382
 
-    attn_scores(sc, p.q + (size_t)h * hs, p.kcache + hoff, p.kv_dim, hs, t0, t1);
+    attn_scores(sc, p.q + (size_t)h * hs, static_cast<const KV *>(p.kcache) + hoff, p.kv_dim, hs, t0, t1);
     __syncthreads();
 
     // softmax pieces (:690-705).  Every warp recomputes max and sum over the whole split from
@@ -1760,7 +1808,7 @@ __global__ void __launch_bounds__(NT) attention_kernel(const AttnParams p, const
     for (int i = lane; i < len; i += 32) l += sc[i];
     l = warp_sum(l);
 
-    attn_weighted_rows(red, sc, p.vcache + hoff, p.kv_dim, hs, t0, t1);
+    attn_weighted_rows(red, sc, static_cast<const KV *>(p.vcache) + hoff, p.kv_dim, hs, t0, t1);
     __syncthreads();
     float o = 0.0f;
     if (tid < hs) {
@@ -1842,7 +1890,7 @@ __device__ __forceinline__ void attn_warp_merge(float &m, float &l, float4 (&acc
     }
 }
 
-template <int NF>   // float4 per lane per row: head_size = 4 * NF * LPR
+template <int NF, typename KV = float>   // float4 per lane per row: head_size = 4 * NF * LPR
 __global__ void __launch_bounds__(NT) attention_flash_kernel(const AttnParams p, const AttnBatch zb) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     __shared__ int is_last;
@@ -1862,8 +1910,8 @@ __global__ void __launch_bounds__(NT) attention_flash_kernel(const AttnParams p,
     const float *qz = p.q + (size_t)z * p.q_stride;
     const size_t hoff = (size_t)(h / p.kv_mul) * hs;          // :369, :382
     const float4 *q4 = reinterpret_cast<const float4 *>(qz + (size_t)h * hs);
-    const float *kb = (p.batched ? batch_entry(zb.kcache, z) : p.kcache) + hoff;
-    const float *vb = (p.batched ? batch_entry(zb.vcache, z) : p.vcache) + hoff;
+    const KV *kb = static_cast<const KV *>(p.batched ? batch_entry(zb.kcache, z) : p.kcache) + hoff;
+    const KV *vb = static_cast<const KV *>(p.batched ? batch_entry(zb.vcache, z) : p.vcache) + hoff;
 
     // Everything whose ADDRESS does not depend on the position is requested before the position is
     // read from the control block: q, and (timeline split 0) the cache rows of this lane's first pass —
@@ -1878,16 +1926,16 @@ __global__ void __launch_bounds__(NT) attention_flash_kernel(const AttnParams p,
         acc[f] = make_float4(0.f, 0.f, 0.f, 0.f);
     }
     if (spec) {
-        const float4 *ka4 = reinterpret_cast<const float4 *>(kb + (size_t)ta0 * p.kv_dim);
-        const float4 *va4 = reinterpret_cast<const float4 *>(vb + (size_t)ta0 * p.kv_dim);
-        const float4 *kc4 = reinterpret_cast<const float4 *>(kb + (size_t)tc0 * p.kv_dim);
-        const float4 *vc4 = reinterpret_cast<const float4 *>(vb + (size_t)tc0 * p.kv_dim);
+        const KV *ka4 = kb + (size_t)ta0 * p.kv_dim;
+        const KV *va4 = vb + (size_t)ta0 * p.kv_dim;
+        const KV *kc4 = kb + (size_t)tc0 * p.kv_dim;
+        const KV *vc4 = vb + (size_t)tc0 * p.kv_dim;
 #pragma unroll
         for (int f = 0; f < NF; ++f) {
-            ka[f] = __ldcg(ka4 + lr + f * LPR);
-            vA[f] = __ldcg(va4 + lr + f * LPR);
-            kc[f] = __ldcg(kc4 + lr + f * LPR);
-            vC[f] = __ldcg(vc4 + lr + f * LPR);
+            ka[f] = ldcg_kv4(ka4, lr, f * LPR);
+            vA[f] = ldcg_kv4(va4, lr, f * LPR);
+            kc[f] = ldcg_kv4(kc4, lr, f * LPR);
+            vC[f] = ldcg_kv4(vc4, lr, f * LPR);
         }
     }
 
@@ -1938,16 +1986,16 @@ __global__ void __launch_bounds__(NT) attention_flash_kernel(const AttnParams p,
         const int ta = tbw + rw, tc = ta + NG;
         const bool va = ta < t1, vc = tc < t1;
         if (!(spec && tbw == warp * RPW)) {                   // the first pass of split 0 is already in registers
-            const float4 *ka4 = reinterpret_cast<const float4 *>(kb + (size_t)(va ? ta : t0) * p.kv_dim);
-            const float4 *va4 = reinterpret_cast<const float4 *>(vb + (size_t)(va ? ta : t0) * p.kv_dim);
-            const float4 *kc4 = reinterpret_cast<const float4 *>(kb + (size_t)(vc ? tc : t0) * p.kv_dim);
-            const float4 *vc4 = reinterpret_cast<const float4 *>(vb + (size_t)(vc ? tc : t0) * p.kv_dim);
+            const KV *ka4 = kb + (size_t)(va ? ta : t0) * p.kv_dim;
+            const KV *va4 = vb + (size_t)(va ? ta : t0) * p.kv_dim;
+            const KV *kc4 = kb + (size_t)(vc ? tc : t0) * p.kv_dim;
+            const KV *vc4 = vb + (size_t)(vc ? tc : t0) * p.kv_dim;
 #pragma unroll
             for (int f = 0; f < NF; ++f) {
-                ka[f] = __ldcg(ka4 + lr + f * LPR);
-                vA[f] = __ldcg(va4 + lr + f * LPR);
-                kc[f] = __ldcg(kc4 + lr + f * LPR);
-                vC[f] = __ldcg(vc4 + lr + f * LPR);
+                ka[f] = ldcg_kv4(ka4, lr, f * LPR);
+                vA[f] = ldcg_kv4(va4, lr, f * LPR);
+                kc[f] = ldcg_kv4(kc4, lr, f * LPR);
+                vC[f] = ldcg_kv4(vc4, lr, f * LPR);
             }
         }
         update(ka, vA, va);
@@ -2031,7 +2079,7 @@ struct AttnWoParams {
     int dim, q_dim;
 };
 
-template <int NF, typename W = float>   // float4 per lane per row: head_size = 4 * NF * LPR
+template <int NF, typename W = float, typename KV = float>   // float4 per lane per row: head_size = 4 * NF * LPR
 __global__ void __launch_bounds__(NT) attn_wo_kernel(const AttnWoParams q) {
     namespace cg = cooperative_groups;
     cg::cluster_group cluster = cg::this_cluster();
@@ -2076,7 +2124,7 @@ __global__ void __launch_bounds__(NT) attn_wo_kernel(const AttnWoParams q) {
     const int t0 = s * chunk, t1 = min(T, t0 + chunk);         // may be empty (t0 >= T)
     const size_t hoff = (size_t)(h / p.kv_mul) * hs;           // :369, :382
     const float4 *qv4 = reinterpret_cast<const float4 *>(p.q + (size_t)h * hs);
-    const float *kb = p.kcache + hoff, *vb = p.vcache + hoff;
+    const KV *kb = static_cast<const KV *>(p.kcache) + hoff, *vb = static_cast<const KV *>(p.vcache) + hoff;
     const float root_hs = sqrtf((float)hs);
 
     float4 qf[NF], acc[NF];
@@ -2110,16 +2158,16 @@ __global__ void __launch_bounds__(NT) attn_wo_kernel(const AttnWoParams q) {
         const int ta = tbw + rw, tc = ta + NG;
         const bool va = ta < t1, vc = tc < t1;
         float4 ka[NF], vA[NF], kc[NF], vC[NF];
-        const float4 *ka4 = reinterpret_cast<const float4 *>(kb + (size_t)(va ? ta : t0) * p.kv_dim);
-        const float4 *va4 = reinterpret_cast<const float4 *>(vb + (size_t)(va ? ta : t0) * p.kv_dim);
-        const float4 *kc4 = reinterpret_cast<const float4 *>(kb + (size_t)(vc ? tc : t0) * p.kv_dim);
-        const float4 *vc4 = reinterpret_cast<const float4 *>(vb + (size_t)(vc ? tc : t0) * p.kv_dim);
+        const KV *ka4 = kb + (size_t)(va ? ta : t0) * p.kv_dim;
+        const KV *va4 = vb + (size_t)(va ? ta : t0) * p.kv_dim;
+        const KV *kc4 = kb + (size_t)(vc ? tc : t0) * p.kv_dim;
+        const KV *vc4 = vb + (size_t)(vc ? tc : t0) * p.kv_dim;
 #pragma unroll
         for (int f = 0; f < NF; ++f) {
-            ka[f] = __ldcg(ka4 + lr + f * LPR);
-            vA[f] = __ldcg(va4 + lr + f * LPR);
-            kc[f] = __ldcg(kc4 + lr + f * LPR);
-            vC[f] = __ldcg(vc4 + lr + f * LPR);
+            ka[f] = ldcg_kv4(ka4, lr, f * LPR);
+            vA[f] = ldcg_kv4(va4, lr, f * LPR);
+            kc[f] = ldcg_kv4(kc4, lr, f * LPR);
+            vC[f] = ldcg_kv4(vc4, lr, f * LPR);
         }
         update(ka, vA, va);
         update(kc, vC, vc);
@@ -2524,32 +2572,36 @@ __global__ void __launch_bounds__(LOGPROB_THREADS) logprob_batch_kernel(const Lo
 
 // ---------------------------------------------------------------------------------------
 // Forking a session (l2b_fork): rows [0, n_pos) of the source's key and value caches, in every layer,
-// into up to KV_FORK_MAXD destinations of the same model.  A cache is (L, seq_len, kv_loc), so the
-// prefix of one layer of one cache is one contiguous segment of n_pos * kv_loc floats at offset
-// l * seq_len * kv_loc, the same in every session; kv_loc is a multiple of 4 (head_size is), so every
-// segment is float4-aligned.  Each source float4 is read once and stored nd times.  The fork is never
-// launched inside a step or a graph: no pdl_wait, no CTL_DONE.
+// into up to KV_FORK_MAXD destinations of the same model.  A cache is (L, seq_len, kv_loc) elements of
+// type KV, so the prefix of one layer of one cache is one contiguous segment of n_pos * kv_loc elements
+// at offset l * seq_len * kv_loc, the same in every session; kv_loc is a multiple of 4 (head_size is),
+// so every segment is a whole number of 4-element units (float4, or 8 bytes of bf16).  Each source unit
+// is read once and stored nd times.  The fork is never launched inside a step or a graph: no pdl_wait,
+// no CTL_DONE.
 // ---------------------------------------------------------------------------------------
 constexpr int KV_FORK_MAXD = 8;
+template <typename KV>
 struct KvForkParams {
-    const float *k, *v;                           // source key / value cache
-    float *dk[KV_FORK_MAXD], *dv[KV_FORK_MAXD];   // destinations [0, nd)
+    const KV *k, *v;                              // source key / value cache
+    KV *dk[KV_FORK_MAXD], *dv[KV_FORK_MAXD];      // destinations [0, nd)
     int nd;
-    long long seg;                                // floats per segment: n_pos * kv_loc
-    long long stride;                             // floats between layers: seq_len * kv_loc
+    long long seg;                                // elements per segment: n_pos * kv_loc
+    long long stride;                             // elements between layers: seq_len * kv_loc
     int L;
 };
-__global__ void __launch_bounds__(NT) kv_fork_kernel(const KvForkParams p) {
+template <typename KV>
+__global__ void __launch_bounds__(NT) kv_fork_kernel(const KvForkParams<KV> p) {
+    typedef typename std::conditional<sizeof(KV) == 2, uint2, float4>::type Unit;   // 4 elements
     const long long seg4 = p.seg >> 2;
     for (int s = blockIdx.y; s < 2 * p.L; s += gridDim.y) {   // segments 0 .. L-1: keys, L .. 2L-1: values
         const bool val = s >= p.L;
         const size_t off = (size_t)(val ? s - p.L : s) * p.stride;
-        const float4 *src = reinterpret_cast<const float4 *>((val ? p.v : p.k) + off);
+        const Unit *src = reinterpret_cast<const Unit *>((val ? p.v : p.k) + off);
         for (long long i = (long long)blockIdx.x * NT + threadIdx.x; i < seg4; i += (long long)gridDim.x * NT) {
-            const float4 x = __ldg(src + i);
+            const Unit x = __ldg(src + i);
 #pragma unroll
             for (int d = 0; d < KV_FORK_MAXD; ++d)   // constant indices: the pointers stay in parameter space
-                if (d < p.nd) reinterpret_cast<float4 *>((val ? p.dv[d] : p.dk[d]) + off)[i] = x;
+                if (d < p.nd) reinterpret_cast<Unit *>((val ? p.dv[d] : p.dk[d]) + off)[i] = x;
         }
     }
 }

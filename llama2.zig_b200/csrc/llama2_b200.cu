@@ -139,7 +139,10 @@ struct l2b_ctx {
     size_t h_call_bytes = 0;
     float *delta = nullptr;                  // L2B_TP=nccl baseline only: partial rows before the NCCL all-reduce
     float *q = nullptr, *xb = nullptr, *hb = nullptr, *logits = nullptr, *logits_loc = nullptr;
-    float *kcache = nullptr, *vcache = nullptr;     // (L, seq_len, kv_loc)
+    // KV cache, (L, seq_len, kv_loc) elements of the format `kvfmt`: 0 (fp32), L2B_KV_BF16, or
+    // L2B_KV_ROUND_BF16 (fp32 elements holding bf16-rounded values: the bf16 cache's reference)
+    int kvfmt = 0;
+    void *kcache = nullptr, *vcache = nullptr;
     float *rope_cos = nullptr, *rope_sin = nullptr; // (seq_len, head_size/2)
     float *part_o = nullptr, *part_ml = nullptr;
     unsigned int *counters = nullptr;
@@ -270,6 +273,16 @@ uint64_t fmt_ld(int fmt, uint64_t cols) {
            : fmt == L2B_WEIGHTS_Q8 ? (uint64_t)w_pitch<q8>((int)cols) : cols;
 }
 size_t w_elem(const l2b_ctx *ctx) { return fmt_elem(ctx->wfmt); }
+// ---- KV-cache format ----
+bool kv_bf16(const l2b_ctx *ctx) { return ctx->kvfmt == L2B_KV_BF16; }
+size_t kv_elem(const l2b_ctx *ctx) { return kv_bf16(ctx) ? 2 : 4; }
+// what the QKV epilogue stores: the kernels' KV type (float, bf16, kv_f32_bf16)
+enum KvStore { KS_F32, KS_BF16, KS_ROUND };
+int kv_store(const l2b_ctx *ctx) { return kv_bf16(ctx) ? KS_BF16 : ctx->kvfmt == L2B_KV_ROUND_BF16 ? KS_ROUND : KS_F32; }
+// layer `layer` of a cache (kcache or vcache) of ctx
+void *kv_layer(const l2b_ctx *ctx, void *cache, int layer) {
+    return static_cast<unsigned char *>(cache) + (size_t)layer * ctx->cfg.seq_len * ctx->kv_loc * kv_elem(ctx);   // :354
+}
 uint64_t w_ld(const l2b_ctx *ctx, uint64_t cols) { return fmt_ld(ctx->wfmt, cols); }
 // row `row` of a matrix of `cols` columns that starts at base
 const void *wrow(const l2b_ctx *ctx, const void *base, uint64_t row, uint64_t cols) {
@@ -490,25 +503,28 @@ typedef void (*gemv_fn)(const GemvParams);
 
 // Kernel instantiations by weight element type W.  EPI_XCHG (tensor parallel) has fp32 kernels only:
 // bf16 and q8 weights are single-GPU.
-template <int EPI, typename W>
+template <int EPI, typename W, typename KV = float>
 gemv_fn gemv_pick(int tpr) {
     switch (tpr) {
-    case 8: return gemv_kernel<8, EPI, W>;
-    case 16: return gemv_kernel<16, EPI, W>;
-    case 32: return gemv_kernel<32, EPI, W>;
-    case 64: return gemv_kernel<64, EPI, W>;
-    case 128: return gemv_kernel<128, EPI, W>;
-    default: return gemv_kernel<256, EPI, W>;
+    case 8: return gemv_kernel<8, EPI, W, KV>;
+    case 16: return gemv_kernel<16, EPI, W, KV>;
+    case 32: return gemv_kernel<32, EPI, W, KV>;
+    case 64: return gemv_kernel<64, EPI, W, KV>;
+    case 128: return gemv_kernel<128, EPI, W, KV>;
+    default: return gemv_kernel<256, EPI, W, KV>;
     }
 }
+// and by KV store (KvStore) for EPI_QKV, the one epilogue that writes the cache
 template <typename W>
-gemv_fn gemv_pick(int epi, int tpr) {
+gemv_fn gemv_pick(int epi, int tpr, int ks) {
     switch (epi) {
     case EPI_XCHG: return sizeof(W) == 4 ? gemv_pick<EPI_XCHG, float>(tpr) : nullptr;
     case EPI_RESID: return gemv_pick<EPI_RESID, W>(tpr);
     case EPI_STORE: return gemv_pick<EPI_STORE, W>(tpr);
     case EPI_ARGMAX: return gemv_pick<EPI_ARGMAX, W>(tpr);
-    case EPI_QKV: return gemv_pick<EPI_QKV, W>(tpr);
+    case EPI_QKV:
+        return ks == KS_BF16 ? gemv_pick<EPI_QKV, W, bf16>(tpr)
+               : ks == KS_ROUND ? gemv_pick<EPI_QKV, W, kv_f32_bf16>(tpr) : gemv_pick<EPI_QKV, W>(tpr);
     default: return gemv_pick<EPI_SILU, W>(tpr);
     }
 }
@@ -538,25 +554,29 @@ int prof_mark(l2b_ctx *ctx, const char *name, int layer, uint64_t bytes, cudaStr
 }
 
 template <typename W>
-gemv_fn gemv_tma_pick(int epi) {
+gemv_fn gemv_tma_pick(int epi, int ks) {
     switch (epi) {
     case EPI_XCHG: return sizeof(W) == 4 ? gemv_tma_kernel<EPI_XCHG, float> : nullptr;
     case EPI_RESID: return gemv_tma_kernel<EPI_RESID, W>;
     case EPI_STORE: return gemv_tma_kernel<EPI_STORE, W>;
     case EPI_ARGMAX: return gemv_tma_kernel<EPI_ARGMAX, W>;
-    case EPI_QKV: return gemv_tma_kernel<EPI_QKV, W>;
+    case EPI_QKV:
+        return ks == KS_BF16 ? gemv_tma_kernel<EPI_QKV, W, bf16>
+               : ks == KS_ROUND ? gemv_tma_kernel<EPI_QKV, W, kv_f32_bf16> : gemv_tma_kernel<EPI_QKV, W>;
     default: return gemv_tma_kernel<EPI_SILU, W>;
     }
 }
 
 template <typename W>
-gemv_fn gemv8_pick(int epi) {
+gemv_fn gemv8_pick(int epi, int ks) {
     switch (epi) {
     case EPI_XCHG: return sizeof(W) == 4 ? gemv8_kernel<EPI_XCHG, float> : nullptr;
     case EPI_RESID: return gemv8_kernel<EPI_RESID, W>;
     case EPI_STORE: return gemv8_kernel<EPI_STORE, W>;
     case EPI_ARGMAX: return gemv8_kernel<EPI_ARGMAX, W>;
-    case EPI_QKV: return gemv8_kernel<EPI_QKV, W>;
+    case EPI_QKV:
+        return ks == KS_BF16 ? gemv8_kernel<EPI_QKV, W, bf16>
+               : ks == KS_ROUND ? gemv8_kernel<EPI_QKV, W, kv_f32_bf16> : gemv8_kernel<EPI_QKV, W>;
     default: return gemv8_kernel<EPI_SILU, W>;
     }
 }
@@ -568,14 +588,15 @@ enum GemvKind { GK_LATENCY, GK_ROWS8, GK_TMA };
 // the formats an epilogue has kernels in: EPI_XCHG (tensor parallel) is fp32 only
 bool has_kernel(const l2b_ctx *ctx, int epi) { return !(ctx->wfmt != L2B_WEIGHTS_F32 && epi == EPI_XCHG); }
 
-// The one place a GEMV kernel is chosen for the context's weight format.  The shape rules that pick
-// `kind` are the same for every format (computed at 4 bytes per weight).
+// The one place a GEMV kernel is chosen for the context's weight format and KV store.  The shape rules
+// that pick `kind` are the same for every format (computed at 4 bytes per weight).
 gemv_fn pick_gemv(const l2b_ctx *ctx, GemvKind kind, int epi, int tpr) {
+    const int ks = kv_store(ctx);
     if (is_q8(ctx))
-        return kind == GK_TMA ? gemv_tma_pick<q8>(epi) : kind == GK_ROWS8 ? gemv8_pick<q8>(epi) : gemv_pick<q8>(epi, tpr);
+        return kind == GK_TMA ? gemv_tma_pick<q8>(epi, ks) : kind == GK_ROWS8 ? gemv8_pick<q8>(epi, ks) : gemv_pick<q8>(epi, tpr, ks);
     if (is_bf16(ctx))
-        return kind == GK_TMA ? gemv_tma_pick<bf16>(epi) : kind == GK_ROWS8 ? gemv8_pick<bf16>(epi) : gemv_pick<bf16>(epi, tpr);
-    return kind == GK_TMA ? gemv_tma_pick<float>(epi) : kind == GK_ROWS8 ? gemv8_pick<float>(epi) : gemv_pick<float>(epi, tpr);
+        return kind == GK_TMA ? gemv_tma_pick<bf16>(epi, ks) : kind == GK_ROWS8 ? gemv8_pick<bf16>(epi, ks) : gemv_pick<bf16>(epi, tpr, ks);
+    return kind == GK_TMA ? gemv_tma_pick<float>(epi, ks) : kind == GK_ROWS8 ? gemv8_pick<float>(epi, ks) : gemv_pick<float>(epi, tpr, ks);
 }
 
 cudaLaunchAttribute pdl_attr() {
@@ -673,53 +694,66 @@ int launch_gemv(l2b_ctx *ctx, int epi, const GemvParams &p, cudaStream_t st, con
     return L2B_OK;
 }
 
-// flash-decoding form when head_size/4 splits into 1..8 float4 per lane, else the 3-pass kernel
 typedef void (*attn_fn)(const AttnParams, const AttnBatch);
-attn_fn pick_attention(int head_size, bool flash, size_t *smem) {
+template <typename KV>
+attn_fn attention_flash_pick(int nf) {
+    switch (nf) {
+    case 1: return attention_flash_kernel<1, KV>;
+    case 2: return attention_flash_kernel<2, KV>;
+    case 3: return attention_flash_kernel<3, KV>;
+    case 4: return attention_flash_kernel<4, KV>;
+    case 5: return attention_flash_kernel<5, KV>;
+    case 6: return attention_flash_kernel<6, KV>;
+    case 8: return attention_flash_kernel<8, KV>;
+    default: return nullptr;
+    }
+}
+// the 3-pass kernel and the fork copy for cache format kvfmt
+attn_fn attention_3pass(int kvfmt) { return kvfmt == L2B_KV_BF16 ? attention_kernel<bf16> : attention_kernel<float>; }
+const void *kv_fork_pick(int kvfmt) {
+    return kvfmt == L2B_KV_BF16 ? (const void *)kv_fork_kernel<bf16> : (const void *)kv_fork_kernel<float>;
+}
+// flash-decoding form when head_size/4 splits into 1..8 float4 per lane, else the 3-pass kernel; the
+// instance for cache format kvfmt (the choice does not depend on it)
+attn_fn pick_attention(int head_size, bool flash, size_t *smem, int kvfmt = 0) {
     const int hs4 = head_size / 4;
     const int lpr = (hs4 % 8 == 0) ? 8 : (hs4 % 4 == 0) ? 4 : (hs4 % 2 == 0) ? 2 : 1;
     const int nf = hs4 / lpr;
     attn_fn f2 = nullptr;
-    if (flash) {
-        switch (nf) {
-        case 1: f2 = attention_flash_kernel<1>; break;
-        case 2: f2 = attention_flash_kernel<2>; break;
-        case 3: f2 = attention_flash_kernel<3>; break;
-        case 4: f2 = attention_flash_kernel<4>; break;
-        case 5: f2 = attention_flash_kernel<5>; break;
-        case 6: f2 = attention_flash_kernel<6>; break;
-        case 8: f2 = attention_flash_kernel<8>; break;
-        default: break;
-        }
-    }
-    if (!f2) return attention_kernel;
+    if (flash) f2 = kvfmt == L2B_KV_BF16 ? attention_flash_pick<bf16>(nf) : attention_flash_pick<float>(nf);
+    if (!f2) return attention_3pass(kvfmt);
     const int ng = NWARP * (32 / lpr);
     *smem = ((size_t)ng * head_size + 3 * (size_t)ng) * sizeof(float);
     return f2;
 }
 
 typedef void (*attn_wo_fn)(const AttnWoParams);
-template <typename W>
+template <typename W, typename KV>
 attn_wo_fn attn_wo_pick(int nf) {
     switch (nf) {
-    case 1: return attn_wo_kernel<1, W>;
-    case 2: return attn_wo_kernel<2, W>;
-    case 3: return attn_wo_kernel<3, W>;
-    case 4: return attn_wo_kernel<4, W>;
-    case 5: return attn_wo_kernel<5, W>;
-    case 6: return attn_wo_kernel<6, W>;
-    case 8: return attn_wo_kernel<8, W>;
+    case 1: return attn_wo_kernel<1, W, KV>;
+    case 2: return attn_wo_kernel<2, W, KV>;
+    case 3: return attn_wo_kernel<3, W, KV>;
+    case 4: return attn_wo_kernel<4, W, KV>;
+    case 5: return attn_wo_kernel<5, W, KV>;
+    case 6: return attn_wo_kernel<6, W, KV>;
+    case 8: return attn_wo_kernel<8, W, KV>;
     default: return nullptr;
     }
 }
-// the attention + wo kernel for head_size in weight format wfmt (whether one exists does not depend on it)
-attn_wo_fn pick_attn_wo(int head_size, size_t *smem, int wfmt = L2B_WEIGHTS_F32) {
+template <typename KV>
+attn_wo_fn attn_wo_pick(int nf, int wfmt) {
+    return wfmt == L2B_WEIGHTS_BF16 ? attn_wo_pick<bf16, KV>(nf) : wfmt == L2B_WEIGHTS_Q8 ? attn_wo_pick<q8, KV>(nf) : attn_wo_pick<float, KV>(nf);
+}
+// the attention + wo kernel for head_size in weight format wfmt and cache format kvfmt (whether one
+// exists depends on neither)
+attn_wo_fn pick_attn_wo(int head_size, size_t *smem, int wfmt = L2B_WEIGHTS_F32, int kvfmt = 0) {
     const int hs4 = head_size / 4;
     const int lpr = (hs4 % 8 == 0) ? 8 : (hs4 % 4 == 0) ? 4 : (hs4 % 2 == 0) ? 2 : 1;
     const int nf = hs4 / lpr;
     const int ng = NWARP * (32 / lpr);
     *smem = ((size_t)ng * head_size + 3 * (size_t)ng + 2 * (size_t)head_size + 4) * sizeof(float);
-    return wfmt == L2B_WEIGHTS_BF16 ? attn_wo_pick<bf16>(nf) : wfmt == L2B_WEIGHTS_Q8 ? attn_wo_pick<q8>(nf) : attn_wo_pick<float>(nf);
+    return kvfmt == L2B_KV_BF16 ? attn_wo_pick<bf16>(nf, wfmt) : attn_wo_pick<float>(nf, wfmt);
 }
 
 constexpr int kAttnClusterCtas = 8;   // CTAs per head cluster of attn_wo_kernel; 4 and 2 measured slower (DESIGN.md §4.6)
@@ -728,16 +762,15 @@ constexpr int kAttnClusterCtas = 8;   // CTAs per head cluster of attn_wo_kernel
 int launch_attn_wo(l2b_ctx *ctx, int layer, cudaStream_t st) {
     if (ctx->profiling) {
         const int hpos = ctx->n_appended > 0 ? ctx->n_appended - 1 : 0;
-        int prc = prof_mark(ctx, "attn_wo", layer, 2ull * (uint64_t)(hpos + 1) * ctx->kv_loc * 4ull + (uint64_t)ctx->dim * w_ld(ctx, ctx->q_loc) * w_elem(ctx), st);
+        int prc = prof_mark(ctx, "attn_wo", layer, 2ull * (uint64_t)(hpos + 1) * ctx->kv_loc * kv_elem(ctx) + (uint64_t)ctx->dim * w_ld(ctx, ctx->q_loc) * w_elem(ctx), st);
         if (prc) return prc;
     }
     AttnWoParams q{};
     AttnParams &a = q.a;
     a.ctl = ctx->ctl;
     a.q = ctx->q;
-    const size_t loff = (size_t)layer * ctx->cfg.seq_len * ctx->kv_loc;   // :354
-    a.kcache = ctx->kcache + loff;
-    a.vcache = ctx->vcache + loff;
+    a.kcache = kv_layer(ctx, ctx->kcache, layer);
+    a.vcache = kv_layer(ctx, ctx->vcache, layer);
     a.head_size = ctx->head_size;
     a.kv_dim = ctx->kv_loc;
     a.kv_mul = ctx->kv_mul;
@@ -747,7 +780,7 @@ int launch_attn_wo(l2b_ctx *ctx, int layer, cudaStream_t st) {
     q.dim = ctx->dim;
     q.q_dim = ctx->q_loc;
     size_t smem = 0;
-    attn_wo_fn fn = pick_attn_wo(ctx->head_size, &smem, ctx->wfmt);
+    attn_wo_fn fn = pick_attn_wo(ctx->head_size, &smem, ctx->wfmt, ctx->kvfmt);
     cudaLaunchConfig_t lc{};
     lc.gridDim = dim3(ctx->heads_loc, kAttnClusterCtas);
     lc.blockDim = dim3(NT);
@@ -773,15 +806,14 @@ int launch_attention(l2b_ctx *ctx, int layer, cudaStream_t st, const float *q, f
                      int nb = 1) {
     if (ctx->profiling) {
         const int hpos = ctx->n_appended > 0 ? ctx->n_appended - 1 : 0;
-        int prc = prof_mark(ctx, "attention", layer, 2ull * (uint64_t)(hpos + 1) * ctx->kv_loc * 4ull, st);
+        int prc = prof_mark(ctx, "attention", layer, 2ull * (uint64_t)(hpos + 1) * ctx->kv_loc * kv_elem(ctx), st);
         if (prc) return prc;
     }
     AttnParams a{};
     a.ctl = ctx->ctl;
     a.q = q;
-    const size_t loff = (size_t)layer * ctx->cfg.seq_len * ctx->kv_loc;   // :354
-    a.kcache = ctx->kcache + loff;
-    a.vcache = ctx->vcache + loff;
+    a.kcache = kv_layer(ctx, ctx->kcache, layer);
+    a.vcache = kv_layer(ctx, ctx->vcache, layer);
     a.xb = xb;
     a.part_o = part_o;
     a.part_ml = part_ml;
@@ -797,7 +829,7 @@ int launch_attention(l2b_ctx *ctx, int layer, cudaStream_t st, const float *q, f
     a.trace = zb ? nullptr : trace_slot(ctx);
     const AttnBatch none{};
     size_t smem = ctx->attn_smem;
-    attn_fn fn = pick_attention(ctx->head_size, ctx->attn_flash, &smem);
+    attn_fn fn = pick_attention(ctx->head_size, ctx->attn_flash, &smem, ctx->kvfmt);
     cudaLaunchConfig_t lc{};
     lc.gridDim = dim3(ctx->heads_loc, ctx->nsplit, nb);
     lc.blockDim = dim3(NT);
@@ -873,9 +905,8 @@ LayerGemvs layer_gemvs(const l2b_ctx *ctx, int l) {
     p.w2 = wrow(ctx, ctx->wv, (uint64_t)l * ctx->kv_loc, dim);
     p.rows0 = ctx->q_loc; p.rows1 = ctx->kv_loc; p.rows2 = ctx->kv_loc;
     p.total_rows = ctx->q_loc + 2 * ctx->kv_loc;
-    const size_t loff = (size_t)l * ctx->cfg.seq_len * ctx->kv_loc;
-    p.kcache = ctx->kcache + loff;
-    p.vcache = ctx->vcache + loff;
+    p.kcache = kv_layer(ctx, ctx->kcache, l);
+    p.vcache = kv_layer(ctx, ctx->vcache, l);
     p.rope_cos = ctx->rope_cos; p.rope_sin = ctx->rope_sin;
     p.head_size = ctx->head_size; p.kv_dim = ctx->kv_loc;
     // wo, whose result is added to the residual stream (:392-395)
@@ -1171,21 +1202,21 @@ int preload_kernels(l2b_ctx *ctx) {
         L2B_CUDA(ctx, cudaFuncGetAttributes(&fa, (const void *)pick_gemv(ctx, GK_TMA, epi, 0)));
     }
     size_t smem = 0;
-    L2B_CUDA(ctx, cudaFuncGetAttributes(&fa, (const void *)pick_attention(ctx->head_size, true, &smem)));
-    if (attn_wo_fn aw = pick_attn_wo(ctx->head_size, &smem, ctx->wfmt)) L2B_CUDA(ctx, cudaFuncGetAttributes(&fa, (const void *)aw));
-    const void *others[] = {(const void *)attention_kernel, (const void *)advance_kernel,
+    L2B_CUDA(ctx, cudaFuncGetAttributes(&fa, (const void *)pick_attention(ctx->head_size, true, &smem, ctx->kvfmt)));
+    if (attn_wo_fn aw = pick_attn_wo(ctx->head_size, &smem, ctx->wfmt, ctx->kvfmt)) L2B_CUDA(ctx, cudaFuncGetAttributes(&fa, (const void *)aw));
+    const void *others[] = {(const void *)attention_3pass(ctx->kvfmt), (const void *)advance_kernel,
                             (const void *)batch_advance_kernel, (const void *)gather_logits_kernel,
                             (const void *)resid_add_kernel, (const void *)sample_prep_kernel,
                             (const void *)sample_prep_batch_kernel, (const void *)logprob_kernel,
                             (const void *)logprob_batch_kernel, (const void *)synth_fill_kernel,
                             (const void *)synth_fill_bf16_kernel, (const void *)synth_fill_q8_kernel,
-                            (const void *)kv_fork_kernel, (const void *)verify_accept_kernel};
+                            (const void *)kv_fork_pick(ctx->kvfmt), (const void *)verify_accept_kernel};
     for (const void *f : others) L2B_CUDA(ctx, cudaFuncGetAttributes(&fa, f));
     // The kernels that run next to a TMA-ring GEMV in a decode step (the ring GEMVs, attention, the
     // token advance) all ask for the largest shared-memory carveout, so consecutive kernels never
     // need a different L1 / shared split on an SM.  (A successor was not seen to enter an SM early
     // for it, DESIGN.md §4.1; what dropping the attribute costs or gains is not measured.)
-    const void *decode[] = {(const void *)pick_attention(ctx->head_size, true, &smem), (const void *)attention_kernel,
+    const void *decode[] = {(const void *)pick_attention(ctx->head_size, true, &smem, ctx->kvfmt), (const void *)attention_3pass(ctx->kvfmt),
                             (const void *)advance_kernel};
     for (const void *f : decode)
         L2B_CUDA(ctx, cudaFuncSetAttribute(f, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
@@ -1333,8 +1364,11 @@ int create_run_state(l2b_ctx *ctx) {
     L2B_TRY(dev_alloc(ctx, &ctx->hb, (size_t)ctx->hid_loc));
     L2B_TRY(dev_alloc(ctx, &ctx->logits, V));
     if (world > 1) L2B_TRY(dev_alloc(ctx, &ctx->logits_loc, (size_t)ctx->vocab_loc));
-    L2B_TRY(dev_alloc(ctx, &ctx->kcache, L * S * ctx->kv_loc));
-    L2B_TRY(dev_alloc(ctx, &ctx->vcache, L * S * ctx->kv_loc));
+    const size_t kv_bytes = L * S * ctx->kv_loc * kv_elem(ctx);
+    unsigned char *kc = nullptr, *vc = nullptr;
+    L2B_TRY(dev_alloc(ctx, &kc, kv_bytes));
+    L2B_TRY(dev_alloc(ctx, &vc, kv_bytes));
+    ctx->kcache = kc; ctx->vcache = vc;
     L2B_TRY(dev_alloc(ctx, &ctx->ctl, (size_t)CTL_WORDS));
     L2B_TRY(dev_alloc(ctx, &ctx->amax, (size_t)1));
     L2B_TRY(dev_alloc(ctx, &ctx->gen_forced, S));
@@ -1348,8 +1382,8 @@ int create_run_state(l2b_ctx *ctx) {
     L2B_TRY(cuda_try(ctx, cudaMemsetAsync(ctx->X, 0, dim * sizeof(float), ctx->stream), "memset"));
     L2B_TRY(cuda_try(ctx, cudaMemsetAsync(ctx->amax, 0, sizeof(unsigned long long), ctx->stream), "memset"));
     L2B_TRY(cuda_try(ctx, cudaMemsetAsync(ctx->gen_forced, 0xff, S * sizeof(int), ctx->stream), "memset"));
-    L2B_TRY(cuda_try(ctx, cudaMemsetAsync(ctx->kcache, 0, L * S * ctx->kv_loc * sizeof(float), ctx->stream), "memset"));
-    L2B_TRY(cuda_try(ctx, cudaMemsetAsync(ctx->vcache, 0, L * S * ctx->kv_loc * sizeof(float), ctx->stream), "memset"));
+    L2B_TRY(cuda_try(ctx, cudaMemsetAsync(ctx->kcache, 0, kv_bytes, ctx->stream), "memset"));
+    L2B_TRY(cuda_try(ctx, cudaMemsetAsync(ctx->vcache, 0, kv_bytes, ctx->stream), "memset"));
 
     // ---- attention launch shape: enough (head, split) CTAs to cover the SMs, chunks >= min_chunk positions
     {
@@ -1370,7 +1404,7 @@ int create_run_state(l2b_ctx *ctx) {
             g_create_error = ctx->err;
             return L2B_ERR_UNSUPPORTED;
         }
-        L2B_TRY(cuda_try(ctx, cudaFuncSetAttribute(attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem), "cudaFuncSetAttribute"));
+        L2B_TRY(cuda_try(ctx, cudaFuncSetAttribute(attention_3pass(ctx->kvfmt), cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem), "cudaFuncSetAttribute"));
         L2B_TRY(dev_alloc(ctx, &ctx->part_o, (size_t)ctx->heads_loc * ns * hs));
         L2B_TRY(dev_alloc(ctx, &ctx->part_ml, (size_t)ctx->heads_loc * ns * 2));
         L2B_TRY(dev_alloc(ctx, &ctx->counters, (size_t)ctx->heads_loc));
@@ -1569,7 +1603,7 @@ void destroy_all(l2b_ctx *ctx) {
 
 int common_create(l2b_ctx **out, const l2b_config *cfg, const Source &src, uint64_t n_floats,
                   const float *rope_cos, const float *rope_sin, const l2b_shard *shard, int n_gpus,
-                  int wfmt = L2B_WEIGHTS_F32) {
+                  int wfmt = L2B_WEIGHTS_F32, int kvfmt = 0) {
     if (!out || !cfg) { g_create_error = "NULL argument"; return L2B_ERR_INVALID_ARG; }
     *out = nullptr;
     const bool in_process = n_gpus > 1;
@@ -1602,6 +1636,7 @@ int common_create(l2b_ctx **out, const l2b_config *cfg, const Source &src, uint6
         l2b_ctx *ctx = new l2b_ctx();
         ranks.push_back(ctx);
         ctx->wfmt = wfmt;
+        ctx->kvfmt = kvfmt;
         const int rank = in_process ? i : (shard ? shard->rank : 0);
         const int device = in_process ? i : device0;
         rc = create_rank(ctx, cfg, src, rope_cos, rope_sin, rank, world, device);
@@ -1638,6 +1673,7 @@ int common_create(l2b_ctx **out, const l2b_config *cfg, const Source &src, uint6
 // a context on the weights of `model` (single GPU): its own run state, caches, stream and graphs
 int create_session(l2b_ctx *ctx, const l2b_ctx *model) {
     ctx->wfmt = model->wfmt;
+    ctx->kvfmt = model->kvfmt;
     ctx->n_rounded = model->n_rounded;
     L2B_TRY(init_rank(ctx, &model->cfg, 0, 1, model->device));
     ctx->weights = model->weights;
@@ -1796,26 +1832,42 @@ int32_t l2b_create_synthetic_group(l2b_ctx **out, const l2b_config *cfg, uint64_
     return common_create(out, cfg, s, 0, nullptr, nullptr, nullptr, n_gpus);
 }
 
+// weight_format of l2b_create_format: a weight format, with L2B_KV_BF16 or L2B_KV_ROUND_BF16 or'd in.  Any
+// other value => L2B_ERR_INVALID_ARG.
+bool split_format(int32_t weight_format, int *wfmt, int *kvfmt) {
+    *kvfmt = weight_format & (L2B_KV_BF16 | L2B_KV_ROUND_BF16);
+    *wfmt = weight_format & ~(L2B_KV_BF16 | L2B_KV_ROUND_BF16);
+    if ((*wfmt != L2B_WEIGHTS_F32 && *wfmt != L2B_WEIGHTS_BF16 && *wfmt != L2B_WEIGHTS_Q8) ||
+        *kvfmt == (L2B_KV_BF16 | L2B_KV_ROUND_BF16)) {
+        g_create_error = "unknown weight format";
+        return false;
+    }
+    return true;
+}
+
 int32_t l2b_create_format(l2b_ctx **out, const l2b_config *cfg, const float *host_weights, uint64_t n_floats,
                           const float *rope_cos, const float *rope_sin, int32_t n_gpus, int32_t weight_format) {
-    if (weight_format != L2B_WEIGHTS_F32 && weight_format != L2B_WEIGHTS_BF16 && weight_format != L2B_WEIGHTS_Q8) {
-        g_create_error = "unknown weight format";
-        return L2B_ERR_INVALID_ARG;
-    }
+    int wfmt, kvfmt;
+    if (!split_format(weight_format, &wfmt, &kvfmt)) return L2B_ERR_INVALID_ARG;
     if (weight_format == L2B_WEIGHTS_F32) return l2b_create(out, cfg, host_weights, n_floats, rope_cos, rope_sin, n_gpus);
     if (!host_weights) { g_create_error = "host_weights is NULL"; return L2B_ERR_INVALID_ARG; }
-    if (n_gpus != 1) { g_create_error = "bf16 and q8 weights are single-GPU (n_gpus must be 1)"; return L2B_ERR_UNSUPPORTED; }
+    if (n_gpus != 1) { g_create_error = "bf16 and q8 weights and a bf16 KV cache are single-GPU (n_gpus must be 1)"; return L2B_ERR_UNSUPPORTED; }
     Source s; s.host = host_weights;
-    return common_create(out, cfg, s, n_floats, rope_cos, rope_sin, nullptr, 1, weight_format);
+    return common_create(out, cfg, s, n_floats, rope_cos, rope_sin, nullptr, 1, wfmt, kvfmt);
 }
 
 int32_t l2b_create_synthetic_format(l2b_ctx **out, const l2b_config *cfg, uint64_t seed, int32_t weight_format) {
-    if (weight_format != L2B_WEIGHTS_F32 && weight_format != L2B_WEIGHTS_BF16 && weight_format != L2B_WEIGHTS_Q8) {
-        g_create_error = "unknown weight format";
-        return L2B_ERR_INVALID_ARG;
-    }
+    int wfmt, kvfmt;
+    if (!split_format(weight_format, &wfmt, &kvfmt)) return L2B_ERR_INVALID_ARG;
     Source s; s.host = nullptr; s.seed = seed;
-    return common_create(out, cfg, s, 0, nullptr, nullptr, nullptr, 1, weight_format);
+    return common_create(out, cfg, s, 0, nullptr, nullptr, nullptr, 1, wfmt, kvfmt);
+}
+
+int32_t l2b_kv_info(const l2b_ctx *ctx, int32_t *kv_format, uint64_t *cache_bytes) {
+    if (!ctx) return L2B_ERR_INVALID_ARG;
+    if (kv_format) *kv_format = ctx->kvfmt;
+    if (cache_bytes) *cache_bytes = 2ull * ctx->cfg.n_layers * ctx->cfg.seq_len * ctx->kv_loc * kv_elem(ctx);
+    return L2B_OK;
 }
 
 int32_t l2b_weight_info(const l2b_ctx *ctx, int32_t *weight_format, uint64_t *n_rounded) {
@@ -1874,8 +1926,41 @@ int32_t l2b_reset(l2b_ctx *ctx) {
     return L2B_OK;
 }
 
-// Rows [0, n_pos) of src's caches into every destination: kv_fork_kernel, KV_FORK_MAXD destinations per
-// launch, on src's stream.  Everything is checked before anything launches.
+}  // extern "C" (a template below)
+
+// Rows [0, n_pos) of src's caches into every destination: kv_fork_kernel<KV>, KV_FORK_MAXD destinations per
+// launch, on src's stream.
+template <typename KV>
+int fork_launch(l2b_ctx *src, int32_t n_pos, l2b_ctx *const *dst, int32_t n_dst) {
+    const int L = src->cfg.n_layers;
+    KvForkParams<KV> p{};
+    p.k = static_cast<const KV *>(src->kcache);
+    p.v = static_cast<const KV *>(src->vcache);
+    p.seg = (long long)n_pos * src->kv_loc;
+    p.stride = (long long)src->cfg.seq_len * src->kv_loc;
+    p.L = L;
+    // One 4-element unit per thread: on llama2-7B (fp32) this grid beat one resident wave of grid-striding
+    // CTAs (8 per SM) by 5-12 % at every n_pos and destination count measured, and cudaMemcpy at one
+    // destination (DESIGN.md §4.5g).
+    const int gy = std::min(2 * L, 65535);
+    const long long chunks = ((p.seg >> 2) + NT - 1) / NT;
+    const int gx = (int)std::min(chunks, (long long)INT32_MAX);
+    for (int g = 0; g < n_dst; g += KV_FORK_MAXD) {
+        p.nd = std::min(KV_FORK_MAXD, n_dst - g);
+        for (int d = 0; d < p.nd; ++d) {
+            p.dk[d] = static_cast<KV *>(dst[g + d]->kcache);
+            p.dv[d] = static_cast<KV *>(dst[g + d]->vcache);
+        }
+        void *args[] = {&p};
+        const int rc = launch_small(src, (const void *)kv_fork_kernel<KV>, dim3(gx, gy), dim3(NT), args, src->stream, false);
+        if (rc) return rc;
+    }
+    return L2B_OK;
+}
+
+extern "C" {
+
+// Everything is checked before anything launches.
 int32_t l2b_fork(l2b_ctx *src, int32_t n_pos, l2b_ctx *const *dst, int32_t n_dst) {
     if (!src) { g_create_error = "src is NULL"; return L2B_ERR_INVALID_ARG; }
     if (!dst || n_dst < 1) return fail(src, L2B_ERR_INVALID_ARG, "dst is NULL or n_dst < 1");
@@ -1898,30 +1983,9 @@ int32_t l2b_fork(l2b_ctx *src, int32_t n_pos, l2b_ctx *const *dst, int32_t n_dst
         // below before any destination can run again.
         cudaStream_t st = src->stream;
         L2B_CUDA(src, cudaSetDevice(src->device));
-        const int L = src->cfg.n_layers;
-        KvForkParams p{};
-        p.k = src->kcache;
-        p.v = src->vcache;
-        p.seg = (long long)n_pos * src->kv_loc;
-        p.stride = (long long)src->cfg.seq_len * src->kv_loc;
-        p.L = L;
-        // One float4 per thread: on llama2-7B this grid beat one resident wave of grid-striding CTAs (8 per
-        // SM) by 5-12 % at every n_pos and destination count measured, and cudaMemcpy at one destination
-        // (DESIGN.md §4.5g).
-        const int gy = std::min(2 * L, 65535);
-        const long long chunks = ((p.seg >> 2) + NT - 1) / NT;
-        const int gx = (int)std::min(chunks, (long long)INT32_MAX);
         L2B_CUDA(src, cudaEventRecord(src->ev0, st));
-        for (int g = 0; g < n_dst; g += KV_FORK_MAXD) {
-            p.nd = std::min(KV_FORK_MAXD, n_dst - g);
-            for (int d = 0; d < p.nd; ++d) {
-                p.dk[d] = dst[g + d]->kcache;
-                p.dv[d] = dst[g + d]->vcache;
-            }
-            void *args[] = {&p};
-            const int rc = launch_small(src, (const void *)kv_fork_kernel, dim3(gx, gy), dim3(NT), args, st, false);
-            if (rc) return rc;
-        }
+        const int rc = kv_bf16(src) ? fork_launch<bf16>(src, n_pos, dst, n_dst) : fork_launch<float>(src, n_pos, dst, n_dst);
+        if (rc) return rc;
         L2B_CUDA(src, cudaEventRecord(src->ev1, st));
         L2B_CUDA(src, cudaEventSynchronize(src->ev1));
         L2B_CUDA(src, cudaEventElapsedTime(&src->last_ms, src->ev0, src->ev1));
@@ -1986,9 +2050,11 @@ int32_t l2b_forward_sample(l2b_ctx *ctx, int32_t token, int32_t pos, float tempe
 
 // ---- batched prompt prefill (prefill_gemm_kernel in l2b_device.cuh) -----------------------------
 template <int NB, typename W>
-gemv_fn pf_pick(int epi) {
+gemv_fn pf_pick(int epi, int ks) {
     switch (epi) {
-    case EPI_QKV: return prefill_gemm_kernel<EPI_QKV, NB, W>;
+    case EPI_QKV:
+        return ks == KS_BF16 ? prefill_gemm_kernel<EPI_QKV, NB, W, bf16>
+               : ks == KS_ROUND ? prefill_gemm_kernel<EPI_QKV, NB, W, kv_f32_bf16> : prefill_gemm_kernel<EPI_QKV, NB, W>;
     case EPI_SILU: return prefill_gemm_kernel<EPI_SILU, NB, W>;
     case EPI_STORE: return prefill_gemm_kernel<EPI_STORE, NB, W>;
     case EPI_ARGMAX: return prefill_gemm_kernel<EPI_ARGMAX, NB, W>;
@@ -1997,7 +2063,8 @@ gemv_fn pf_pick(int epi) {
 }
 template <int NB>
 gemv_fn pf_pick(const l2b_ctx *ctx, int epi) {
-    return is_q8(ctx) ? pf_pick<NB, q8>(epi) : is_bf16(ctx) ? pf_pick<NB, bf16>(epi) : pf_pick<NB, float>(epi);
+    const int ks = kv_store(ctx);
+    return is_q8(ctx) ? pf_pick<NB, q8>(epi, ks) : is_bf16(ctx) ? pf_pick<NB, bf16>(epi, ks) : pf_pick<NB, float>(epi, ks);
 }
 constexpr size_t kPfSmemBudget = 227 * 1024 - 8192;   // the prefill kernels keep ~6.5 KB of static shared memory
 
@@ -2016,7 +2083,7 @@ static int pf_prepare(l2b_ctx *ctx) {
     const bool shapes_ok = ctx->world == 1 && !ctx->leader && dim >= (uint64_t)ctx->big_min_n && hid >= (uint64_t)ctx->big_min_n &&
                            dim <= TMA_MAXV * TMA_PRO_THREADS * 4 && ctx->gemv8_min_bytes >= 0 &&
                            dim * dim * 4 >= (uint64_t)ctx->gemv8_min_bytes && ctx->attn_flash &&
-                           pick_attention(ctx->head_size, true, &smem) != attention_kernel &&
+                           pick_attention(ctx->head_size, true, &smem) != attention_kernel<float> &&
                            pf_ring_stages(kPfSmemBudget, PF_MAXB * dim * 4) >= 2 &&
                            pf_ring_stages(kPfSmemBudget, 2 * hid * 4) >= 2;
     if (!shapes_ok) return L2B_OK;
@@ -2076,12 +2143,11 @@ static int batched_layers(l2b_ctx *ctx, l2b_ctx *const *kv, const int *pos, int 
     cudaStream_t st = ctx->stream;
     for (int l = 0; l < ctx->cfg.n_layers; ++l) {
         LayerGemvs g = layer_gemvs(ctx, l);
-        const size_t loff = (size_t)l * ctx->cfg.seq_len * ctx->kv_loc;
         AttnBatch zb{};
         for (int b = 0; b < nb; ++b) {
             g.qkv.pos_b[b] = zb.pos[b] = pos[b];
-            g.qkv.kcache_b[b] = kv[b]->kcache + loff;
-            g.qkv.vcache_b[b] = kv[b]->vcache + loff;
+            g.qkv.kcache_b[b] = kv_layer(kv[b], kv[b]->kcache, l);
+            g.qkv.vcache_b[b] = kv_layer(kv[b], kv[b]->vcache, l);
             zb.kcache[b] = g.qkv.kcache_b[b];
             zb.vcache[b] = g.qkv.vcache_b[b];
         }
@@ -3143,7 +3209,7 @@ int32_t l2b_verify_sample_ragged(l2b_ctx *const *sessions, int32_t n, const int3
 
 int32_t l2b_read_state(l2b_ctx *ctx, int32_t which, float *dst, uint64_t n, uint64_t *n_out) {
     if (!ctx || !dst) return L2B_ERR_INVALID_ARG;
-    const float *src = nullptr;
+    const void *src = nullptr;
     uint64_t cnt = 0;
     const uint64_t L = ctx->cfg.n_layers, S = ctx->cfg.seq_len;
     switch (which) {
@@ -3158,7 +3224,18 @@ int32_t l2b_read_state(l2b_ctx *ctx, int32_t which, float *dst, uint64_t n, uint
     }
     if (n < cnt) return fail(ctx, L2B_ERR_INVALID_ARG, "dst too small");
     L2B_CUDA(ctx, cudaSetDevice(ctx->device));
-    L2B_CUDA(ctx, cudaMemcpy(dst, src, cnt * sizeof(float), cudaMemcpyDeviceToHost));
+    if ((which == 4 || which == 5) && kv_bf16(ctx)) {
+        // the bf16 cache lands in the upper half of dst and is widened in place from the front: value i is
+        // written to bytes [4i, 4i+4), below the unread values at [2 cnt + 2i, ..) for every i < cnt
+        uint16_t *h = reinterpret_cast<uint16_t *>(dst) + cnt;
+        L2B_CUDA(ctx, cudaMemcpy(h, src, cnt * 2, cudaMemcpyDeviceToHost));
+        for (uint64_t i = 0; i < cnt; ++i) {
+            const uint32_t u = (uint32_t)h[i] << 16;
+            memcpy(dst + i, &u, 4);
+        }
+    } else {
+        L2B_CUDA(ctx, cudaMemcpy(dst, src, cnt * sizeof(float), cudaMemcpyDeviceToHost));
+    }
     if (n_out) *n_out = cnt;
     return L2B_OK;
 }
@@ -3248,7 +3325,7 @@ int32_t l2b_step_bytes(const l2b_ctx *ctx, int32_t pos, uint64_t *weight_bytes, 
                               2ull * ctx->hid_loc * ld_dim + dim * ld_hid) +
                          ld_dim + (uint64_t)ctx->vocab_loc * ld_dim;
     if (weight_bytes) *weight_bytes = w_elem(ctx) * mat + 4 * (L * 2 * dim);
-    if (kv_bytes) *kv_bytes = 4ull * L * 2 * ctx->kv_loc * (uint64_t)(pos + 1);
+    if (kv_bytes) *kv_bytes = kv_elem(ctx) * L * 2 * ctx->kv_loc * (uint64_t)(pos + 1);
     return L2B_OK;
 }
 
@@ -3430,7 +3507,7 @@ int32_t l2b_op_attention_head(int32_t device, float *out, const float *q, const 
     const int G = NT / (head_size / 4);
     const size_t smem = ((size_t)G * head_size + cap) * sizeof(float);
     if (smem > (size_t)kMaxDynSmem) { g_create_error = "n_pos too large"; return L2B_ERR_UNSUPPORTED; }
-    cudaFuncSetAttribute(attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem);
+    cudaFuncSetAttribute(attention_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem);
     {
         const char *enva = getenv("L2B_ATTN");
         size_t smem2 = smem;

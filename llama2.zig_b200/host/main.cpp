@@ -32,7 +32,18 @@ static const char *usage_text =
     "     --bf16                keep the matrix weights (and the draft's) in bf16 on the GPU: half the memory and\n"
     "                           bytes per step; outputs equal an fp32 run of the bf16-rounded checkpoint (1 GPU)\n"
     "     --q8                  keep the matrix weights (and the draft's) as int8 with one scale per 64 weights: 0.53x\n"
-    "                           the bf16 bytes per step; outputs equal an fp32 run of the dequantized checkpoint (1 GPU)\n";
+    "                           the bf16 bytes per step; outputs equal an fp32 run of the dequantized checkpoint (1 GPU)\n"
+    "     --kv-bf16             keep the KV cache (and the draft's) in bf16 on the GPU: half the cache memory and\n"
+    "                           attention bytes; outputs equal an fp32-cache run that rounds each K/V value (1 GPU)\n";
+
+// -v: the KV-cache format and bytes of a context (l2b_kv_info)
+static void print_kv_info(const char *what, const l2b_ctx *ctx) {
+    int32_t fmt = 0;
+    uint64_t bytes = 0;
+    l2b_kv_info(ctx, &fmt, &bytes);
+    fprintf(stderr, "%s: %s, %llu bytes\n", what, fmt == L2B_KV_BF16 ? "bf16" : fmt == L2B_KV_ROUND_BF16 ? "fp32 (bf16-rounded)" : "fp32",
+            (unsigned long long)bytes);
+}
 
 // Generation with a draft model: the prompt positions are prefilled on target and draft, then
 // l2b_generate_speculative (-t 0) or l2h_generate_speculative_sample (-t > 0) runs the rest.  The tokens
@@ -80,7 +91,7 @@ int main(int argc, char **argv) {
     int n_gpus = 1, draft_k = 3;
     const char *draft_path = nullptr;
     bool verbose = false;
-    int32_t weight_format = L2B_WEIGHTS_F32;
+    int32_t weight_format = L2B_WEIGHTS_F32, kv_flag = 0;
     l2h_seed((uint64_t)time(nullptr));
     for (int i = 1; i < argc; ++i) {
         std::string a = argv[i];
@@ -107,6 +118,7 @@ int main(int argc, char **argv) {
         else if (a == "--draft-k") draft_k = atoi(need("draft-k"));
         else if (a == "--bf16") weight_format = L2B_WEIGHTS_BF16;
         else if (a == "--q8") weight_format = L2B_WEIGHTS_Q8;
+        else if (a == "--kv-bf16") kv_flag = L2B_KV_BF16;
         else { fprintf(stderr, "error: unknown argument '%s'\n", argv[i]); fputs(usage_text, stdout); return 0; }
     }
     if (!bin_path) { fputs(usage_text, stdout); return 0; }
@@ -120,14 +132,16 @@ int main(int argc, char **argv) {
         fprintf(stderr, "shared weights: %s\ntemperature: %g\ntop-p: %g\n\n", c.shared_weights ? "true" : "false", opt.temperature, opt.top_p);
     }
     l2b_ctx *ctx = nullptr;
-    int32_t rc = l2b_create_format(&ctx, &c, ck.data, ck.n_floats, nullptr, nullptr, n_gpus, weight_format);   // after :967
+    int32_t rc = l2b_create_format(&ctx, &c, ck.data, ck.n_floats, nullptr, nullptr, n_gpus, weight_format | kv_flag);   // after :967
     if (rc) { fprintf(stderr, "error: l2b_create: %s (%s)\n", l2b_status_string(rc), l2b_last_error(nullptr)); return 1; }
     if (verbose) {
         int32_t fmt = 0;
         uint64_t n_rounded = 0;
         l2b_weight_info(ctx, &fmt, &n_rounded);
-        fprintf(stderr, "weights: %s on the GPU, %llu matrix weights changed by rounding or quantization\n\n",
+        fprintf(stderr, "weights: %s on the GPU, %llu matrix weights changed by rounding or quantization\n",
                 fmt == L2B_WEIGHTS_BF16 ? "bf16" : fmt == L2B_WEIGHTS_Q8 ? "q8" : "fp32", (unsigned long long)n_rounded);
+        print_kv_info("kv cache", ctx);
+        fputc('\n', stderr);
     }
     l2h_free_checkpoint(&ck);   // host copy no longer needed: weights live in HBM
     l2b_ctx *draft = nullptr;
@@ -141,8 +155,9 @@ int main(int argc, char **argv) {
             return 1;
         }
         if (draft_k < 0 || draft_k > L2B_SPECULATIVE_MAX_K) { fprintf(stderr, "error: --draft-k must be in [0, %d]\n", L2B_SPECULATIVE_MAX_K); return 1; }
-        rc = l2b_create_format(&draft, &dc, dck.data, dck.n_floats, nullptr, nullptr, 1, weight_format);
+        rc = l2b_create_format(&draft, &dc, dck.data, dck.n_floats, nullptr, nullptr, 1, weight_format | kv_flag);
         if (rc) { fprintf(stderr, "error: l2b_create (draft): %s (%s)\n", l2b_status_string(rc), l2b_last_error(nullptr)); return 1; }
+        if (verbose) print_kv_info("draft kv cache", draft);
         l2h_free_checkpoint(&dck);
     }
 
