@@ -580,8 +580,48 @@ int32_t l2b_round_q8_host(float *data, uint64_t rows, uint64_t cols, uint64_t *n
 #define L2B_KV_ROUND_BF16 0x200
 /* The KV format of ctx (0: fp32, L2B_KV_BF16, L2B_KV_ROUND_BF16) and the bytes of its key and value caches
  * together: 2 * n_layers * seq_len * kv_dim * (2 for L2B_KV_BF16, else 4).  l2b_weight_info reports the
- * weight format alone.                                                                                 */
+ * weight format alone.  A paged context (below) reports the element format alone, and as cache bytes the
+ * pages it references times page_bytes: a page shared by several sessions counts in each of them
+ * (l2b_kv_pool_info gives the true total).                                                             */
 int32_t l2b_kv_info(const l2b_ctx *ctx, int32_t *kv_format, uint64_t *cache_bytes);
+
+/* ---- Paged KV layout ------------------------------------------------------------------------
+ * L2B_KV_PAGED, or'd into the weight_format of l2b_create_format / l2b_create_synthetic_format (with any
+ * weight format, and with or without L2B_KV_BF16 or L2B_KV_ROUND_BF16), keeps the caches of the model's
+ * contexts and sessions in pages of L2B_KV_PAGE_ROWS positions drawn from one pool per model.  A page
+ * holds those positions of every layer, K and V.  A session holds only the pages of the positions it has
+ * appended, and l2b_fork shares the source's full pages with its destinations instead of copying them: a
+ * destination that writes into a shared page first gets a private copy (copy-on-write).  n_gpus > 1 =>
+ * L2B_ERR_UNSUPPORTED, checked before any device is touched.  Sessions take their model's layout.
+ * Contract: a paged context returns, on every entry point, exactly what a contiguous context of the same
+ * payload, weight format and KV format returns (the outputs listed under the KV format above, and
+ * l2b_read_state of the cache rows below the appended count), after any sequence of forks, rewinds,
+ * resets and copies-on-write.  Its kernels are the contiguous kernels the same shape selects; only the
+ * row addresses differ.
+ * Changed promises of a paged context:
+ *  - Every call that appends rows first reserves the pages of every row it may write.  When the pool
+ *    limit (l2b_kv_pool_limit) or the device memory runs out, the call returns L2B_ERR_OOM and changes no
+ *    session.  After the call, every page that lies wholly at or past a session's appended count is
+ *    released, as l2b_reset releases all of them and l2b_destroy a session's.
+ *  - Rows at and past the appended count are not defined, also where a contiguous context leaves them
+ *    "untouched" or "not written": they may lie in a released page.
+ *  - l2b_read_state(4 / 5) gathers the rows into the contiguous (L, seq_len, kv_dim) fp32 layout; rows in
+ *    no page the context holds read as 0.
+ *  - l2b_fork releases each destination's pages, then shares src's full pages and copies the rows of its
+ *    last partial page (at most L2B_KV_PAGE_ROWS - 1 rows) into a fresh page per destination; when n_pos
+ *    is a multiple of L2B_KV_PAGE_ROWS nothing is copied.                                              */
+#define L2B_KV_PAGED 0x800
+#define L2B_KV_PAGE_ROWS 64
+/* The pool of ctx's model: rows per page, bytes per page (2 * n_layers * L2B_KV_PAGE_ROWS * kv_dim * the
+ * element size), pages held by some context or session, and pages allocated on the device (in use or
+ * free; free pages are kept until the model is destroyed).  Any context or session of the model; a
+ * contiguous model reports zeros.  NULL ctx or any NULL output => L2B_ERR_INVALID_ARG.                */
+int32_t l2b_kv_pool_info(const l2b_ctx *ctx, int32_t *page_rows, uint64_t *page_bytes, uint64_t *pages_in_use,
+                         uint64_t *pages_allocated);
+/* Caps the pages ctx's model may have in use (0: no cap, the default); a call that would need more returns
+ * L2B_ERR_OOM and changes no session.  A cap below the pages in use => L2B_ERR_INVALID_ARG; a contiguous
+ * model => L2B_ERR_UNSUPPORTED; NULL ctx => L2B_ERR_INVALID_ARG.                                       */
+int32_t l2b_kv_pool_limit(l2b_ctx *ctx, uint64_t max_pages);
 
 #ifdef __cplusplus
 }

@@ -139,6 +139,8 @@ def load_library():
     lib.l2b_create_synthetic_format.argtypes = [C.POINTER(vp), C.POINTER(L2BConfig), C.c_uint64, C.c_int32]
     lib.l2b_weight_info.argtypes = [vp, IP, U64P]
     lib.l2b_kv_info.argtypes = [vp, IP, U64P]
+    lib.l2b_kv_pool_info.argtypes = [vp, IP, U64P, U64P, U64P]
+    lib.l2b_kv_pool_limit.argtypes = [vp, C.c_uint64]
     lib.l2b_round_bf16_host.argtypes = [FP, C.c_uint64]
     lib.l2b_round_bf16_host.restype = None
     lib.l2b_round_q8_host.argtypes = [FP, C.c_uint64, C.c_uint64, U64P]
@@ -181,6 +183,9 @@ Q8_GROUP = 64   # L2B_Q8_GROUP
 KV_BF16 = 0x100                          # L2B_KV_BF16: or'd into the weight format of l2b_create_format
 KV_ROUND_BF16 = 0x200                    # L2B_KV_ROUND_BF16: fp32 cache of bf16-rounded values (the reference)
 KV_FORMATS = {"f32": 0, "bf16": KV_BF16, "f32-round-bf16": KV_ROUND_BF16}   # l2b_kv_info's kv_format
+KV_PAGED = 0x800                         # L2B_KV_PAGED: or'd in like the KV formats; the paged layout
+KV_PAGE_ROWS = 64                        # L2B_KV_PAGE_ROWS: positions per page
+_KV_LAYOUTS = {"contiguous": 0, "paged": KV_PAGED}
 
 
 def round_bf16_host(a):
@@ -225,21 +230,25 @@ class Transformer:
     device (l2b_create_synthetic).  weight_format="bf16" keeps the matrix weights in bf16 on the
     device, "q8" as int8 with one fp32 scale per 64 weights of a row; kv_format="bf16" keeps the KV
     cache in bf16, "f32-round-bf16" in fp32 holding bf16-rounded values, the bf16 cache's bitwise reference
-    (l2b_create_format / l2b_create_synthetic_format; single GPU, device 0).  Sessions take the model's
-    formats.
+    (l2b_create_format / l2b_create_synthetic_format; single GPU, device 0).  kv_layout="paged" keeps
+    the caches of the model's contexts and sessions in pages of KV_PAGE_ROWS positions from one pool
+    (single GPU, device 0; fork shares a prompt's pages).  Sessions take the model's formats and layout.
     """
 
     def __init__(self, ck, synthetic_seed=None, rank=0, world_size=1, device=0, comm_id=None,
-                 rope_cos=None, rope_sin=None, n_gpus=1, weight_format="f32", kv_format="f32"):
+                 rope_cos=None, rope_sin=None, n_gpus=1, weight_format="f32", kv_format="f32",
+                 kv_layout="contiguous"):
         """n_gpus > 1: ONE process drives n_gpus GPUs (l2b_create(.., n_gpus)); rank/world_size:
         one process per GPU (l2b_create_sharded)."""
         if weight_format not in _FORMATS:
             raise ValueError(f"weight_format must be one of {sorted(_FORMATS)}")
         if kv_format not in KV_FORMATS:
             raise ValueError(f"kv_format must be one of {sorted(KV_FORMATS)}")
-        fmt = _FORMATS[weight_format] | KV_FORMATS[kv_format]
+        if kv_layout not in _KV_LAYOUTS:
+            raise ValueError(f"kv_layout must be one of {sorted(_KV_LAYOUTS)}")
+        fmt = _FORMATS[weight_format] | KV_FORMATS[kv_format] | _KV_LAYOUTS[kv_layout]
         if fmt and (world_size > 1 or device != 0 or rank != 0 or n_gpus != 1):
-            raise ValueError(f"{weight_format} weights with a {kv_format} KV cache are single-GPU on device 0")
+            raise ValueError(f"{weight_format} weights with a {kv_format} {kv_layout} KV cache are single-GPU on device 0")
         self.lib = load_library()
         self.ck = ck
         self.cfg = make_config(ck)
@@ -390,6 +399,17 @@ class Transformer:
         n = C.c_uint64()
         _check(self.lib.l2b_kv_info(self.h, C.byref(fmt), C.byref(n)), self.h)
         return {v: k for k, v in KV_FORMATS.items()}[fmt.value], n.value
+
+    def kv_pool_info(self):
+        """The KV page pool of this context's model (l2b_kv_pool_info): page_rows, page_bytes,
+        pages_in_use and pages_allocated; all 0 for a contiguous model."""
+        r, b, u, a = C.c_int32(), C.c_uint64(), C.c_uint64(), C.c_uint64()
+        _check(self.lib.l2b_kv_pool_info(self.h, C.byref(r), C.byref(b), C.byref(u), C.byref(a)), self.h)
+        return {"page_rows": r.value, "page_bytes": b.value, "pages_in_use": u.value, "pages_allocated": a.value}
+
+    def kv_pool_limit(self, max_pages):
+        """Caps the pages the model may have in use (0: no cap); l2b_kv_pool_limit."""
+        _check(self.lib.l2b_kv_pool_limit(self.h, int(max_pages)), self.h)
 
     def load_stats(self):
         ms = C.c_double()

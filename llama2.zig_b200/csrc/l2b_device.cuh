@@ -273,6 +273,38 @@ __device__ __forceinline__ void kv_store2(KV *dst, float a0, float a1) {
     else
         *reinterpret_cast<float2 *>(dst) = make_float2(kv_value<KV>(a0), kv_value<KV>(a1));
 }
+// ---- paged caches (L2B_KV_PAGED).  The kernels' KV type is then kv_paged<E>, E one of the element types
+// above.  A page holds rows [jP, jP+P) of every layer, K and V: [L][K rows P | V rows P][kv_dim] elements E.
+// In place of a layer's cache base a paged kernel takes the layer's page table: entry j is the address of
+// the layer's K row jP in page j of the session, and its V row jP lies KV_PAGE_ROWS rows further on.
+// kcache and vcache both carry that table.  Entries of pages the session does not hold point at the
+// model's null page, so every row address is valid memory; rows past a stream's end are masked as before.
+constexpr int KV_PAGE_ROWS = 64;
+template <typename E> struct kv_paged {};
+template <typename KV> struct kv_traits { typedef KV elem; static constexpr bool paged = false; };
+template <typename E> struct kv_traits<kv_paged<E>> { typedef E elem; static constexpr bool paged = true; };
+template <typename KV> using kv_elem_t = typename kv_traits<KV>::elem;
+// K row t of a layer's cache c (the base, or the page table), and the V row of the same position
+template <typename KV>
+__device__ __forceinline__ kv_elem_t<KV> *kv_krow(void *c, int t, int kv_dim) {
+    if constexpr (kv_traits<KV>::paged)
+        return static_cast<kv_elem_t<KV> *const *>(c)[t / KV_PAGE_ROWS] + (size_t)(t % KV_PAGE_ROWS) * kv_dim;
+    else
+        return static_cast<kv_elem_t<KV> *>(c) + (size_t)t * kv_dim;
+}
+template <typename KV>
+__device__ __forceinline__ kv_elem_t<KV> *kv_vrow(void *c, int t, int kv_dim) {
+    if constexpr (kv_traits<KV>::paged) return kv_krow<KV>(c, t, kv_dim) + (size_t)KV_PAGE_ROWS * kv_dim;
+    else return static_cast<kv_elem_t<KV> *>(c) + (size_t)t * kv_dim;
+}
+// The attention kernels' page addresses: a split's pages [t0/P, (t1-1)/P] are staged in shared memory
+// (pg, after the kernel's own dynamic shared memory) before its row loop, so no row's address waits on a
+// global load.  A block-wide barrier follows.
+__device__ __forceinline__ void kv_stage_pages(const void *tab, int t0, int t1, const void **pg) {
+    const int j0 = t0 / KV_PAGE_ROWS, n = t1 > t0 ? (t1 - 1) / KV_PAGE_ROWS - j0 + 1 : 0;
+    for (int i = threadIdx.x; i < n; i += blockDim.x) pg[i] = static_cast<const void *const *>(tab)[j0 + i];
+    __syncthreads();
+}
 // float4 group j (ldg_kv4) or lr + k (ldcg_kv4) of a cache row, through the read-only path (ldg) or L2 only
 // (ldcg), widened exactly
 template <typename KV>
@@ -478,9 +510,16 @@ __device__ __forceinline__ void widen_emb_row(const GemvParams &p, int token, fl
 // rotated by the RoPE row (rc, rs) of position `pos`; q goes to `q`, k and v to row `pos` of the caches
 // kc / vc as KV elements.  The ring kernels' epilogue warps use it with the RoPE rows they staged in shared
 // memory.
-template <typename KV>
+template <typename KVT>
 __device__ __forceinline__ void qkv_store_pair(const GemvParams &p, float *q, void *kcv, void *vcv, int pos,
                                                const float *rc, const float *rs, int v, float a0, float a1) {
+    typedef kv_elem_t<KVT> KV;
+    if constexpr (kv_traits<KVT>::paged) {
+        // a base from which row `pos` is pos rows on, as in a contiguous cache: the contiguous
+        // instantiations keep their code unchanged
+        kcv = kv_krow<KVT>(kcv, pos, p.kv_dim) - (size_t)pos * p.kv_dim;
+        vcv = kv_vrow<KVT>(vcv, pos, p.kv_dim) - (size_t)pos * p.kv_dim;
+    }
     KV *kc = static_cast<KV *>(kcv), *vc = static_cast<KV *>(vcv);
     if (v < p.rows0 + p.rows1) {
         const bool is_q = v < p.rows0;
@@ -1713,9 +1752,11 @@ __device__ __forceinline__ int attn_lanes_per_row(int hs4) {
 }
 
 // scores for positions [t0,t1) of one head into sc[0..t1-t0); q fragments live in registers
-template <typename KV>
+// (paged KVT: the rows' pages are pg[t/P - t0/P], staged by kv_stage_pages, and kbase is unused)
+template <typename KVT, typename KV = kv_elem_t<KVT>>
 __device__ __forceinline__ void attn_scores(float *sc, const float *qg, const KV *kbase,
-                                            int kv_dim, int head_size, int t0, int t1) {
+                                            int kv_dim, int head_size, int t0, int t1,
+                                            const void *const *pg = nullptr, size_t hoff = 0) {
     const int hs4 = head_size >> 2;
     const int lpr = attn_lanes_per_row(hs4);
     const int nf = hs4 / lpr;
@@ -1728,7 +1769,11 @@ __device__ __forceinline__ void attn_scores(float *sc, const float *qg, const KV
         const int t = tb + rw;
         float acc = 0.0f;
         if (t < t1) {
-            const KV *k4 = kbase + (size_t)t * kv_dim;
+            const KV *k4;
+            if constexpr (kv_traits<KVT>::paged)
+                k4 = static_cast<const KV *>(pg[t / KV_PAGE_ROWS - t0 / KV_PAGE_ROWS]) + (size_t)(t % KV_PAGE_ROWS) * kv_dim + hoff;
+            else
+                k4 = kbase + (size_t)t * kv_dim;
             for (int f = 0; f < nf; ++f) {
                 const int j = lr + f * lpr;
                 acc = dot4(ldg_kv4(k4, j), __ldg(q4 + j), acc);
@@ -1740,9 +1785,10 @@ __device__ __forceinline__ void attn_scores(float *sc, const float *qg, const KV
 }
 
 // red[g][0..head_size) = sum over this group's rows of w[t-t0] * V[t]   (G = NT / (head_size/4))
-template <typename KV>
+template <typename KVT, typename KV = kv_elem_t<KVT>>
 __device__ __forceinline__ void attn_weighted_rows(float *red, const float *w, const KV *vbase,
-                                                   int kv_dim, int head_size, int t0, int t1) {
+                                                   int kv_dim, int head_size, int t0, int t1,
+                                                   const void *const *pg = nullptr, size_t hoff = 0) {
     const int hs4 = head_size >> 2;
     const int G = NT / hs4;
     const int tid = threadIdx.x;
@@ -1751,7 +1797,12 @@ __device__ __forceinline__ void attn_weighted_rows(float *red, const float *w, c
         float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
         for (int t = t0 + g; t < t1; t += G) {
             const float wt = w[t - t0];
-            const float4 v = ldg_kv4(vbase + (size_t)t * kv_dim, c);
+            const KV *v4;
+            if constexpr (kv_traits<KVT>::paged)
+                v4 = static_cast<const KV *>(pg[t / KV_PAGE_ROWS - t0 / KV_PAGE_ROWS]) + (size_t)(t % KV_PAGE_ROWS + KV_PAGE_ROWS) * kv_dim + hoff;
+            else
+                v4 = vbase + (size_t)t * kv_dim;
+            const float4 v = ldg_kv4(v4, c);
             a.x = fmaf(v.x, wt, a.x); a.y = fmaf(v.y, wt, a.y);
             a.z = fmaf(v.z, wt, a.z); a.w = fmaf(v.w, wt, a.w);
         }
@@ -1761,8 +1812,9 @@ __device__ __forceinline__ void attn_weighted_rows(float *red, const float *w, c
 
 // The AttnBatch argument only gives it attention_flash_kernel's signature: batched launches take the
 // flash kernel (pf_prepare), so this kernel never sees one.
-template <typename KV = float>
+template <typename KVT = float>
 __global__ void __launch_bounds__(NT) attention_kernel(const AttnParams p, const AttnBatch) {
+    typedef kv_elem_t<KVT> KV;
     extern __shared__ __align__(16) unsigned char smem_raw[];
     __shared__ int is_last;
     unsigned long long *atr = p.trace ? p.trace + ((size_t)blockIdx.y * gridDim.x) * TRACE_SLOTS : nullptr;
@@ -1792,7 +1844,10 @@ __global__ void __launch_bounds__(NT) attention_kernel(const AttnParams p, const
     const int tid = threadIdx.x, lane = tid & 31;
     const size_t hoff = (size_t)(h / p.kv_mul) * hs;   // :369, :382
 
-    attn_scores(sc, p.q + (size_t)h * hs, static_cast<const KV *>(p.kcache) + hoff, p.kv_dim, hs, t0, t1);
+    // paged: the split's page addresses after sc (chunk rounded up to an even count keeps them aligned)
+    const void **pg = reinterpret_cast<const void **>(sc + ((chunk + 1) & ~1));
+    if constexpr (kv_traits<KVT>::paged) kv_stage_pages(p.kcache, t0, t1, pg);
+    attn_scores<KVT>(sc, p.q + (size_t)h * hs, static_cast<const KV *>(p.kcache) + hoff, p.kv_dim, hs, t0, t1, pg, hoff);
     __syncthreads();
 
     // softmax pieces (:690-705).  Every warp recomputes max and sum over the whole split from
@@ -1808,7 +1863,7 @@ __global__ void __launch_bounds__(NT) attention_kernel(const AttnParams p, const
     for (int i = lane; i < len; i += 32) l += sc[i];
     l = warp_sum(l);
 
-    attn_weighted_rows(red, sc, static_cast<const KV *>(p.vcache) + hoff, p.kv_dim, hs, t0, t1);
+    attn_weighted_rows<KVT>(red, sc, static_cast<const KV *>(p.vcache) + hoff, p.kv_dim, hs, t0, t1, pg, hoff);
     __syncthreads();
     float o = 0.0f;
     if (tid < hs) {
@@ -1890,8 +1945,10 @@ __device__ __forceinline__ void attn_warp_merge(float &m, float &l, float4 (&acc
     }
 }
 
-template <int NF, typename KV = float>   // float4 per lane per row: head_size = 4 * NF * LPR
+template <int NF, typename KVT = float>   // float4 per lane per row: head_size = 4 * NF * LPR
 __global__ void __launch_bounds__(NT) attention_flash_kernel(const AttnParams p, const AttnBatch zb) {
+    typedef kv_elem_t<KVT> KV;
+    constexpr bool PG = kv_traits<KVT>::paged;
     extern __shared__ __align__(16) unsigned char smem_raw[];
     __shared__ int is_last;
     unsigned long long *atr = p.trace ? p.trace + ((size_t)blockIdx.y * gridDim.x) * TRACE_SLOTS : nullptr;
@@ -1912,6 +1969,20 @@ __global__ void __launch_bounds__(NT) attention_flash_kernel(const AttnParams p,
     const float4 *q4 = reinterpret_cast<const float4 *>(qz + (size_t)h * hs);
     const KV *kb = static_cast<const KV *>(p.batched ? batch_entry(zb.kcache, z) : p.kcache) + hoff;
     const KV *vb = static_cast<const KV *>(p.batched ? batch_entry(zb.vcache, z) : p.vcache) + hoff;
+    // paged: the page table; the rows of the first pass of split 0 come straight from it (pages 0..7,
+    // known without the position), every other row from the split's pages staged in shared memory
+    const void *const *tab = static_cast<const void *const *>(p.batched ? batch_entry(zb.kcache, z) : p.kcache);
+    const void **pg = reinterpret_cast<const void **>(smem_raw + ((size_t)NG * hs + 3 * NG) * sizeof(float));   // [pages of the split]
+    int j0 = 0;
+    // row t from page entry e (paged), or from the base
+    auto krow = [&](const void *e, int t) -> const KV * {
+        if constexpr (PG) return static_cast<const KV *>(e) + (size_t)(t % KV_PAGE_ROWS) * p.kv_dim + hoff;
+        else return kb + (size_t)t * p.kv_dim;
+    };
+    auto vrow = [&](const void *e, int t) -> const KV * {
+        if constexpr (PG) return static_cast<const KV *>(e) + (size_t)(t % KV_PAGE_ROWS + KV_PAGE_ROWS) * p.kv_dim + hoff;
+        else return vb + (size_t)t * p.kv_dim;
+    };
 
     // Everything whose ADDRESS does not depend on the position is requested before the position is
     // read from the control block: q, and (timeline split 0) the cache rows of this lane's first pass —
@@ -1926,10 +1997,11 @@ __global__ void __launch_bounds__(NT) attention_flash_kernel(const AttnParams p,
         acc[f] = make_float4(0.f, 0.f, 0.f, 0.f);
     }
     if (spec) {
-        const KV *ka4 = kb + (size_t)ta0 * p.kv_dim;
-        const KV *va4 = vb + (size_t)ta0 * p.kv_dim;
-        const KV *kc4 = kb + (size_t)tc0 * p.kv_dim;
-        const KV *vc4 = vb + (size_t)tc0 * p.kv_dim;
+        const void *ea = PG ? tab[ta0 / KV_PAGE_ROWS] : nullptr, *ec = PG ? tab[tc0 / KV_PAGE_ROWS] : nullptr;
+        const KV *ka4 = krow(ea, ta0);
+        const KV *va4 = vrow(ea, ta0);
+        const KV *kc4 = krow(ec, tc0);
+        const KV *vc4 = vrow(ec, tc0);
 #pragma unroll
         for (int f = 0; f < NF; ++f) {
             ka[f] = ldcg_kv4(ka4, lr, f * LPR);
@@ -1955,6 +2027,10 @@ __global__ void __launch_bounds__(NT) attention_flash_kernel(const AttnParams p,
     unsigned int *counters_z = p.counters + (size_t)z * gridDim.x;
     float *accp = reinterpret_cast<float *>(smem_raw);        // [NG][hs]
     float *mlp = accp + (size_t)NG * hs;                      // [NG][2]
+    if constexpr (PG) {
+        kv_stage_pages(tab, t0, t1, pg);
+        j0 = t0 / KV_PAGE_ROWS;
+    }
     const float root_hs = sqrtf((float)hs);
     float m = -INFINITY, l = 0.0f;
 
@@ -1986,10 +2062,12 @@ __global__ void __launch_bounds__(NT) attention_flash_kernel(const AttnParams p,
         const int ta = tbw + rw, tc = ta + NG;
         const bool va = ta < t1, vc = tc < t1;
         if (!(spec && tbw == warp * RPW)) {                   // the first pass of split 0 is already in registers
-            const KV *ka4 = kb + (size_t)(va ? ta : t0) * p.kv_dim;
-            const KV *va4 = vb + (size_t)(va ? ta : t0) * p.kv_dim;
-            const KV *kc4 = kb + (size_t)(vc ? tc : t0) * p.kv_dim;
-            const KV *vc4 = vb + (size_t)(vc ? tc : t0) * p.kv_dim;
+            const int sa = va ? ta : t0, sc = vc ? tc : t0;
+            const void *ea = PG ? pg[sa / KV_PAGE_ROWS - j0] : nullptr, *ec = PG ? pg[sc / KV_PAGE_ROWS - j0] : nullptr;
+            const KV *ka4 = krow(ea, sa);
+            const KV *va4 = vrow(ea, sa);
+            const KV *kc4 = krow(ec, sc);
+            const KV *vc4 = vrow(ec, sc);
 #pragma unroll
             for (int f = 0; f < NF; ++f) {
                 ka[f] = ldcg_kv4(ka4, lr, f * LPR);
@@ -2079,8 +2157,10 @@ struct AttnWoParams {
     int dim, q_dim;
 };
 
-template <int NF, typename W = float, typename KV = float>   // float4 per lane per row: head_size = 4 * NF * LPR
+template <int NF, typename W = float, typename KVT = float>   // float4 per lane per row: head_size = 4 * NF * LPR
 __global__ void __launch_bounds__(NT) attn_wo_kernel(const AttnWoParams q) {
+    typedef kv_elem_t<KVT> KV;
+    constexpr bool PG = kv_traits<KVT>::paged;
     namespace cg = cooperative_groups;
     cg::cluster_group cluster = cg::this_cluster();
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -2125,6 +2205,17 @@ __global__ void __launch_bounds__(NT) attn_wo_kernel(const AttnWoParams q) {
     const size_t hoff = (size_t)(h / p.kv_mul) * hs;           // :369, :382
     const float4 *qv4 = reinterpret_cast<const float4 *>(p.q + (size_t)h * hs);
     const KV *kb = static_cast<const KV *>(p.kcache) + hoff, *vb = static_cast<const KV *>(p.vcache) + hoff;
+    const void **pg = reinterpret_cast<const void **>(xbs + hs);   // paged: [pages of the split]
+    if constexpr (PG) kv_stage_pages(p.kcache, t0, t1, pg);
+    const int j0 = t0 / KV_PAGE_ROWS;
+    auto krow = [&](int t) -> const KV * {
+        if constexpr (PG) return static_cast<const KV *>(pg[t / KV_PAGE_ROWS - j0]) + (size_t)(t % KV_PAGE_ROWS) * p.kv_dim + hoff;
+        else return kb + (size_t)t * p.kv_dim;
+    };
+    auto vrow = [&](int t) -> const KV * {
+        if constexpr (PG) return krow(t) + (size_t)KV_PAGE_ROWS * p.kv_dim;
+        else return vb + (size_t)t * p.kv_dim;
+    };
     const float root_hs = sqrtf((float)hs);
 
     float4 qf[NF], acc[NF];
@@ -2158,10 +2249,10 @@ __global__ void __launch_bounds__(NT) attn_wo_kernel(const AttnWoParams q) {
         const int ta = tbw + rw, tc = ta + NG;
         const bool va = ta < t1, vc = tc < t1;
         float4 ka[NF], vA[NF], kc[NF], vC[NF];
-        const KV *ka4 = kb + (size_t)(va ? ta : t0) * p.kv_dim;
-        const KV *va4 = vb + (size_t)(va ? ta : t0) * p.kv_dim;
-        const KV *kc4 = kb + (size_t)(vc ? tc : t0) * p.kv_dim;
-        const KV *vc4 = vb + (size_t)(vc ? tc : t0) * p.kv_dim;
+        const KV *ka4 = krow(va ? ta : t0);
+        const KV *va4 = vrow(va ? ta : t0);
+        const KV *kc4 = krow(vc ? tc : t0);
+        const KV *vc4 = vrow(vc ? tc : t0);
 #pragma unroll
         for (int f = 0; f < NF; ++f) {
             ka[f] = ldcg_kv4(ka4, lr, f * LPR);

@@ -20,6 +20,7 @@
 #include <chrono>
 #include <set>
 #include <string>
+#include <unordered_map>
 #include <vector>
 
 #include "l2b_device.cuh"
@@ -91,9 +92,23 @@ constexpr int kCandCap = 8192;               // top-p candidates returned per st
 
 // The device weights and RoPE tables of one loaded model (one rank's shard), shared by the context that
 // loaded them and every session created on it (l2b_create_session); freed with the last of them.
+// The KV pages of a paged model (L2B_KV_PAGED): [L][K rows P | V rows P][kv_loc] elements each, P =
+// KV_PAGE_ROWS.  Released pages go to the free list, not to the device, and are not cleared: no kernel reads
+// a row past its stream's end.  The null page is what every unassigned page-table entry points at, so
+// the rows a kernel loads and then masks (split 0's first pass) are always valid memory.
+struct KvPool {
+    size_t page_bytes = 0;
+    void *null_page = nullptr;
+    std::vector<void *> all;                  // every page allocated, freed with the model
+    std::vector<void *> free_pages;
+    std::unordered_map<void *, int> refs;     // pages in use -> how many sessions hold them
+    uint64_t limit = 0;                       // l2b_kv_pool_limit (0: none)
+};
+
 struct SharedWeights {
     int refs = 1;
     std::vector<void *> owned;
+    KvPool *pool = nullptr;                   // paged models only
 };
 
 struct l2b_ctx {
@@ -143,6 +158,15 @@ struct l2b_ctx {
     // L2B_KV_ROUND_BF16 (fp32 elements holding bf16-rounded values: the bf16 cache's reference)
     int kvfmt = 0;
     void *kcache = nullptr, *vcache = nullptr;
+    // Paged layout (L2B_KV_PAGED): kcache and vcache are both the device page table kv_tab, [L][n_pages]
+    // addresses of layer l's K row jP in page j (its V rows follow P rows later); pages[j] is the page
+    // this session holds for positions [jP, jP+P), or nullptr (the table entry points at the null page).
+    // h_tab is the table's pinned host mirror; the device copy never moves, so captured graphs stay valid.
+    bool paged = false;
+    int n_pages = 0;
+    std::vector<void *> pages;
+    void **kv_tab = nullptr, **h_tab = nullptr;
+    bool tab_dirty = false;                  // h_tab has entries the device table does not
     float *rope_cos = nullptr, *rope_sin = nullptr; // (seq_len, head_size/2)
     float *part_o = nullptr, *part_ml = nullptr;
     unsigned int *counters = nullptr;
@@ -161,6 +185,7 @@ struct l2b_ctx {
     ProbIndex *h_cand = nullptr;
     // attention launch shape
     int nsplit = 1, min_chunk = 256, attn_smem = 0;   // timeline splits of >= 256 positions
+    int attn_pg_bytes = 0, attn_pg_bytes_wo = 0;      // paged: shared memory for a split's page addresses
     // streams / graphs
     cudaStream_t stream = nullptr;
     cudaGraphExec_t graphs[G_COUNT] = {};
@@ -276,11 +301,27 @@ size_t w_elem(const l2b_ctx *ctx) { return fmt_elem(ctx->wfmt); }
 // ---- KV-cache format ----
 bool kv_bf16(const l2b_ctx *ctx) { return ctx->kvfmt == L2B_KV_BF16; }
 size_t kv_elem(const l2b_ctx *ctx) { return kv_bf16(ctx) ? 2 : 4; }
-// what the QKV epilogue stores: the kernels' KV type (float, bf16, kv_f32_bf16)
-enum KvStore { KS_F32, KS_BF16, KS_ROUND };
-int kv_store(const l2b_ctx *ctx) { return kv_bf16(ctx) ? KS_BF16 : ctx->kvfmt == L2B_KV_ROUND_BF16 ? KS_ROUND : KS_F32; }
-// layer `layer` of a cache (kcache or vcache) of ctx
+// what the QKV epilogue stores: the kernels' KV type (float, bf16, kv_f32_bf16), or'd with KS_PAGED for
+// their kv_paged<> forms
+enum KvStore { KS_F32, KS_BF16, KS_ROUND, KS_PAGED = 4 };
+int kv_store(const l2b_ctx *ctx) {
+    return (kv_bf16(ctx) ? KS_BF16 : ctx->kvfmt == L2B_KV_ROUND_BF16 ? KS_ROUND : KS_F32) | (ctx->paged ? KS_PAGED : 0);
+}
+// the cache format the attention kernels are picked for: kvfmt, or'd with L2B_KV_PAGED
+int kv_kernels(const l2b_ctx *ctx) { return ctx->kvfmt | (ctx->paged ? L2B_KV_PAGED : 0); }
+template <typename T> struct type_tag { typedef T type; };
+// f(type_tag<KV>()) for the kernels' KV type of KvStore ks
+template <typename F>
+auto kv_dispatch(int ks, F f) {
+    if (ks & KS_PAGED) {
+        ks &= ~KS_PAGED;
+        return ks == KS_BF16 ? f(type_tag<kv_paged<bf16>>()) : ks == KS_ROUND ? f(type_tag<kv_paged<kv_f32_bf16>>()) : f(type_tag<kv_paged<float>>());
+    }
+    return ks == KS_BF16 ? f(type_tag<bf16>()) : ks == KS_ROUND ? f(type_tag<kv_f32_bf16>()) : f(type_tag<float>());
+}
+// layer `layer` of a cache (kcache or vcache) of ctx: its base, or (paged) its page table
 void *kv_layer(const l2b_ctx *ctx, void *cache, int layer) {
+    if (ctx->paged) return static_cast<void **>(cache) + (size_t)layer * ctx->n_pages;
     return static_cast<unsigned char *>(cache) + (size_t)layer * ctx->cfg.seq_len * ctx->kv_loc * kv_elem(ctx);   // :354
 }
 uint64_t w_ld(const l2b_ctx *ctx, uint64_t cols) { return fmt_ld(ctx->wfmt, cols); }
@@ -523,8 +564,7 @@ gemv_fn gemv_pick(int epi, int tpr, int ks) {
     case EPI_STORE: return gemv_pick<EPI_STORE, W>(tpr);
     case EPI_ARGMAX: return gemv_pick<EPI_ARGMAX, W>(tpr);
     case EPI_QKV:
-        return ks == KS_BF16 ? gemv_pick<EPI_QKV, W, bf16>(tpr)
-               : ks == KS_ROUND ? gemv_pick<EPI_QKV, W, kv_f32_bf16>(tpr) : gemv_pick<EPI_QKV, W>(tpr);
+        return kv_dispatch(ks, [tpr](auto t) { return gemv_pick<EPI_QKV, W, typename decltype(t)::type>(tpr); });
     default: return gemv_pick<EPI_SILU, W>(tpr);
     }
 }
@@ -561,8 +601,7 @@ gemv_fn gemv_tma_pick(int epi, int ks) {
     case EPI_STORE: return gemv_tma_kernel<EPI_STORE, W>;
     case EPI_ARGMAX: return gemv_tma_kernel<EPI_ARGMAX, W>;
     case EPI_QKV:
-        return ks == KS_BF16 ? gemv_tma_kernel<EPI_QKV, W, bf16>
-               : ks == KS_ROUND ? gemv_tma_kernel<EPI_QKV, W, kv_f32_bf16> : gemv_tma_kernel<EPI_QKV, W>;
+        return kv_dispatch(ks, [](auto t) { return (gemv_fn)gemv_tma_kernel<EPI_QKV, W, typename decltype(t)::type>; });
     default: return gemv_tma_kernel<EPI_SILU, W>;
     }
 }
@@ -575,8 +614,7 @@ gemv_fn gemv8_pick(int epi, int ks) {
     case EPI_STORE: return gemv8_kernel<EPI_STORE, W>;
     case EPI_ARGMAX: return gemv8_kernel<EPI_ARGMAX, W>;
     case EPI_QKV:
-        return ks == KS_BF16 ? gemv8_kernel<EPI_QKV, W, bf16>
-               : ks == KS_ROUND ? gemv8_kernel<EPI_QKV, W, kv_f32_bf16> : gemv8_kernel<EPI_QKV, W>;
+        return kv_dispatch(ks, [](auto t) { return (gemv_fn)gemv8_kernel<EPI_QKV, W, typename decltype(t)::type>; });
     default: return gemv8_kernel<EPI_SILU, W>;
     }
 }
@@ -708,8 +746,12 @@ attn_fn attention_flash_pick(int nf) {
     default: return nullptr;
     }
 }
-// the 3-pass kernel and the fork copy for cache format kvfmt
-attn_fn attention_3pass(int kvfmt) { return kvfmt == L2B_KV_BF16 ? attention_kernel<bf16> : attention_kernel<float>; }
+// the 3-pass kernel and the fork copy for cache format kvfmt (the attention kernels: or'd with L2B_KV_PAGED,
+// kv_kernels)
+attn_fn attention_3pass(int kvfmt) {
+    if (kvfmt & L2B_KV_PAGED) return (kvfmt & L2B_KV_BF16) ? attention_kernel<kv_paged<bf16>> : attention_kernel<kv_paged<float>>;
+    return kvfmt == L2B_KV_BF16 ? attention_kernel<bf16> : attention_kernel<float>;
+}
 const void *kv_fork_pick(int kvfmt) {
     return kvfmt == L2B_KV_BF16 ? (const void *)kv_fork_kernel<bf16> : (const void *)kv_fork_kernel<float>;
 }
@@ -720,7 +762,10 @@ attn_fn pick_attention(int head_size, bool flash, size_t *smem, int kvfmt = 0) {
     const int lpr = (hs4 % 8 == 0) ? 8 : (hs4 % 4 == 0) ? 4 : (hs4 % 2 == 0) ? 2 : 1;
     const int nf = hs4 / lpr;
     attn_fn f2 = nullptr;
-    if (flash) f2 = kvfmt == L2B_KV_BF16 ? attention_flash_pick<bf16>(nf) : attention_flash_pick<float>(nf);
+    if (flash && (kvfmt & L2B_KV_PAGED))
+        f2 = (kvfmt & L2B_KV_BF16) ? attention_flash_pick<kv_paged<bf16>>(nf) : attention_flash_pick<kv_paged<float>>(nf);
+    else if (flash)
+        f2 = kvfmt == L2B_KV_BF16 ? attention_flash_pick<bf16>(nf) : attention_flash_pick<float>(nf);
     if (!f2) return attention_3pass(kvfmt);
     const int ng = NWARP * (32 / lpr);
     *smem = ((size_t)ng * head_size + 3 * (size_t)ng) * sizeof(float);
@@ -753,6 +798,8 @@ attn_wo_fn pick_attn_wo(int head_size, size_t *smem, int wfmt = L2B_WEIGHTS_F32,
     const int nf = hs4 / lpr;
     const int ng = NWARP * (32 / lpr);
     *smem = ((size_t)ng * head_size + 3 * (size_t)ng + 2 * (size_t)head_size + 4) * sizeof(float);
+    if (kvfmt & L2B_KV_PAGED)
+        return (kvfmt & L2B_KV_BF16) ? attn_wo_pick<kv_paged<bf16>>(nf, wfmt) : attn_wo_pick<kv_paged<float>>(nf, wfmt);
     return kvfmt == L2B_KV_BF16 ? attn_wo_pick<bf16>(nf, wfmt) : attn_wo_pick<float>(nf, wfmt);
 }
 
@@ -780,7 +827,8 @@ int launch_attn_wo(l2b_ctx *ctx, int layer, cudaStream_t st) {
     q.dim = ctx->dim;
     q.q_dim = ctx->q_loc;
     size_t smem = 0;
-    attn_wo_fn fn = pick_attn_wo(ctx->head_size, &smem, ctx->wfmt, ctx->kvfmt);
+    attn_wo_fn fn = pick_attn_wo(ctx->head_size, &smem, ctx->wfmt, kv_kernels(ctx));
+    if (ctx->paged) smem += ctx->attn_pg_bytes_wo;
     cudaLaunchConfig_t lc{};
     lc.gridDim = dim3(ctx->heads_loc, kAttnClusterCtas);
     lc.blockDim = dim3(NT);
@@ -829,7 +877,8 @@ int launch_attention(l2b_ctx *ctx, int layer, cudaStream_t st, const float *q, f
     a.trace = zb ? nullptr : trace_slot(ctx);
     const AttnBatch none{};
     size_t smem = ctx->attn_smem;
-    attn_fn fn = pick_attention(ctx->head_size, ctx->attn_flash, &smem, ctx->kvfmt);
+    attn_fn fn = pick_attention(ctx->head_size, ctx->attn_flash, &smem, kv_kernels(ctx));
+    if (ctx->paged) smem += ctx->attn_pg_bytes;
     cudaLaunchConfig_t lc{};
     lc.gridDim = dim3(ctx->heads_loc, ctx->nsplit, nb);
     lc.blockDim = dim3(NT);
@@ -1202,9 +1251,9 @@ int preload_kernels(l2b_ctx *ctx) {
         L2B_CUDA(ctx, cudaFuncGetAttributes(&fa, (const void *)pick_gemv(ctx, GK_TMA, epi, 0)));
     }
     size_t smem = 0;
-    L2B_CUDA(ctx, cudaFuncGetAttributes(&fa, (const void *)pick_attention(ctx->head_size, true, &smem, ctx->kvfmt)));
-    if (attn_wo_fn aw = pick_attn_wo(ctx->head_size, &smem, ctx->wfmt, ctx->kvfmt)) L2B_CUDA(ctx, cudaFuncGetAttributes(&fa, (const void *)aw));
-    const void *others[] = {(const void *)attention_3pass(ctx->kvfmt), (const void *)advance_kernel,
+    L2B_CUDA(ctx, cudaFuncGetAttributes(&fa, (const void *)pick_attention(ctx->head_size, true, &smem, kv_kernels(ctx))));
+    if (attn_wo_fn aw = pick_attn_wo(ctx->head_size, &smem, ctx->wfmt, kv_kernels(ctx))) L2B_CUDA(ctx, cudaFuncGetAttributes(&fa, (const void *)aw));
+    const void *others[] = {(const void *)attention_3pass(kv_kernels(ctx)), (const void *)advance_kernel,
                             (const void *)batch_advance_kernel, (const void *)gather_logits_kernel,
                             (const void *)resid_add_kernel, (const void *)sample_prep_kernel,
                             (const void *)sample_prep_batch_kernel, (const void *)logprob_kernel,
@@ -1216,7 +1265,7 @@ int preload_kernels(l2b_ctx *ctx) {
     // token advance) all ask for the largest shared-memory carveout, so consecutive kernels never
     // need a different L1 / shared split on an SM.  (A successor was not seen to enter an SM early
     // for it, DESIGN.md §4.1; what dropping the attribute costs or gains is not measured.)
-    const void *decode[] = {(const void *)pick_attention(ctx->head_size, true, &smem, ctx->kvfmt), (const void *)attention_3pass(ctx->kvfmt),
+    const void *decode[] = {(const void *)pick_attention(ctx->head_size, true, &smem, kv_kernels(ctx)), (const void *)attention_3pass(kv_kernels(ctx)),
                             (const void *)advance_kernel};
     for (const void *f : decode)
         L2B_CUDA(ctx, cudaFuncSetAttribute(f, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
@@ -1340,6 +1389,176 @@ int create_rank(l2b_ctx *ctx, const l2b_config *cfg, const Source &src, const fl
 
 // run state, attention launch shape, pinned host buffers, tensor-parallel landing area and switches
 // of one rank whose weights are in place
+
+// ---- paged KV (L2B_KV_PAGED): the model's page pool, each session's page table, and the reservation
+// every writing call makes before it launches -----------------------------------------------------------
+size_t kv_page_bytes(const l2b_ctx *ctx) { return 2ull * ctx->cfg.n_layers * KV_PAGE_ROWS * ctx->kv_loc * kv_elem(ctx); }
+KvPool *kv_pool(const l2b_ctx *ctx) { return ctx->paged && ctx->weights ? ctx->weights->pool : nullptr; }
+
+// host table entries of page index j for every layer: `page`, or the null page when nullptr
+void kv_tab_set(l2b_ctx *ctx, int j, void *page) {
+    unsigned char *base = static_cast<unsigned char *>(page ? page : kv_pool(ctx)->null_page);
+    const size_t layer_bytes = 2ull * KV_PAGE_ROWS * ctx->kv_loc * kv_elem(ctx);
+    for (int l = 0; l < ctx->cfg.n_layers; ++l) ctx->h_tab[(size_t)l * ctx->n_pages + j] = base + (size_t)l * layer_bytes;
+    ctx->tab_dirty = true;
+}
+// The table goes up whole (n_layers * ceil(seq_len / P) addresses) and is synchronised: a batched call runs
+// on its first session's stream, and the next kernel that reads this table may be on any of them.
+int kv_tab_upload(l2b_ctx *ctx) {
+    if (!ctx->tab_dirty) return L2B_OK;
+    L2B_CUDA(ctx, cudaMemcpyAsync(ctx->kv_tab, ctx->h_tab, (size_t)ctx->cfg.n_layers * ctx->n_pages * sizeof(void *),
+                                  cudaMemcpyHostToDevice, ctx->stream));
+    L2B_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    ctx->tab_dirty = false;
+    return L2B_OK;
+}
+
+// a session's page table (every entry on the null page) and, for the model's first context, the pool
+int kv_paged_init(l2b_ctx *ctx) {
+    SharedWeights *w = ctx->weights;
+    if (!w->pool) {
+        w->pool = new KvPool();
+        w->pool->page_bytes = kv_page_bytes(ctx);
+        L2B_CUDA(ctx, cudaMalloc(&w->pool->null_page, w->pool->page_bytes));
+        L2B_CUDA(ctx, cudaMemset(w->pool->null_page, 0, w->pool->page_bytes));
+    }
+    ctx->n_pages = (ctx->cfg.seq_len + KV_PAGE_ROWS - 1) / KV_PAGE_ROWS;
+    ctx->pages.assign(ctx->n_pages, nullptr);
+    const size_t n = (size_t)ctx->cfg.n_layers * ctx->n_pages;
+    int rc = dev_alloc(ctx, &ctx->kv_tab, n);
+    if (rc) return rc;
+    L2B_CUDA(ctx, cudaHostAlloc((void **)&ctx->h_tab, n * sizeof(void *), cudaHostAllocDefault));
+    for (int j = 0; j < ctx->n_pages; ++j) kv_tab_set(ctx, j, nullptr);
+    ctx->kcache = ctx->vcache = ctx->kv_tab;
+    return kv_tab_upload(ctx);
+}
+
+int kv_page_get(l2b_ctx *ctx, KvPool *pool, void **out) {
+    if (pool->limit && pool->refs.size() >= pool->limit) return fail(ctx, L2B_ERR_OOM, "the model's KV pages are all in use (l2b_kv_pool_limit)");
+    void *pg = nullptr;
+    if (!pool->free_pages.empty()) {
+        pg = pool->free_pages.back();
+        pool->free_pages.pop_back();
+    } else {
+        if (cudaMalloc(&pg, pool->page_bytes) != cudaSuccess) { cudaGetLastError(); return fail(ctx, L2B_ERR_OOM, "cudaMalloc of a KV page failed"); }
+        pool->all.push_back(pg);
+    }
+    pool->refs[pg] = 1;
+    *out = pg;
+    return L2B_OK;
+}
+void kv_page_put(KvPool *pool, void *pg) {
+    auto it = pool->refs.find(pg);
+    if (--it->second == 0) {
+        pool->refs.erase(it);
+        pool->free_pages.push_back(pg);
+    }
+}
+// session ctx gives up page j
+void kv_drop(l2b_ctx *ctx, int j) {
+    if (!ctx->pages[j]) return;
+    kv_page_put(kv_pool(ctx), ctx->pages[j]);
+    ctx->pages[j] = nullptr;
+    kv_tab_set(ctx, j, nullptr);
+}
+// Rows [0, rows) of every layer, K and V, of page src into the nd pages dst: kv_fork_kernel with one
+// page as the "cache" (segments of rows * kv_loc elements, layers 2P rows apart), on ctx's stream.
+template <typename KV>
+int kv_page_copy(l2b_ctx *ctx, const void *src, void *const *dst, int nd, int rows) {
+    const size_t half = (size_t)KV_PAGE_ROWS * ctx->kv_loc;
+    KvForkParams<KV> p{};
+    p.k = static_cast<const KV *>(src);
+    p.v = p.k + half;
+    p.seg = (long long)rows * ctx->kv_loc;
+    p.stride = 2ll * half;
+    p.L = ctx->cfg.n_layers;
+    const int gy = std::min(2 * p.L, 65535);
+    const int gx = (int)(((p.seg >> 2) + NT - 1) / NT);
+    for (int g = 0; g < nd; g += KV_FORK_MAXD) {
+        p.nd = std::min(KV_FORK_MAXD, nd - g);
+        for (int d = 0; d < p.nd; ++d) {
+            p.dk[d] = static_cast<KV *>(dst[g + d]);
+            p.dv[d] = p.dk[d] + half;
+        }
+        void *args[] = {&p};
+        const int rc = launch_small(ctx, (const void *)kv_fork_kernel<KV>, dim3(gx, gy), dim3(NT), args, ctx->stream, false);
+        if (rc) return rc;
+    }
+    return L2B_OK;
+}
+int kv_page_copy(l2b_ctx *ctx, const void *src, void *const *dst, int nd, int rows) {
+    return kv_bf16(ctx) ? kv_page_copy<bf16>(ctx, src, dst, nd, rows) : kv_page_copy<float>(ctx, src, dst, nd, rows);
+}
+
+// rows [lo, hi) that a call may write into session s's cache (a paged session; one call lists no other)
+struct KvRange { l2b_ctx *s; int lo, hi; };
+
+// The reservation every writing entry point makes after its argument checks and before it launches: for
+// each session, the pages of its range that it does not hold are allocated, and those it shares with
+// another session (reference count above 1) are replaced by private copies (copy-on-write).  Then every
+// listed session's changed table goes up.  When a page cannot be had (the pool limit, or cudaMalloc) every
+// page this reservation took is given back and L2B_ERR_OOM returned: no session has changed.
+int kv_reserve(l2b_ctx *err_ctx, const std::vector<KvRange> &r) {
+    if (r.empty() || !r[0].s->paged) return L2B_OK;
+    L2B_CUDA(err_ctx, cudaSetDevice(r[0].s->device));
+    struct Step { l2b_ctx *s; int j; void *old; };
+    std::vector<Step> done;
+    int rc = L2B_OK;
+    for (const KvRange &x : r) {
+        KvPool *pool = kv_pool(x.s);   // a target and its draft are two models
+        const int hi = std::min(x.hi, x.s->cfg.seq_len);
+        for (int j = x.lo / KV_PAGE_ROWS; rc == L2B_OK && x.lo < hi && j <= (hi - 1) / KV_PAGE_ROWS; ++j) {
+            void *old = x.s->pages[j];
+            if (old && pool->refs[old] == 1) continue;
+            void *pg = nullptr;
+            rc = kv_page_get(err_ctx, pool, &pg);
+            if (rc) break;
+            if (old) --pool->refs[old];      // still held by another session: never 0 here
+            x.s->pages[j] = pg;
+            done.push_back(Step{x.s, j, old});
+        }
+        if (rc) break;
+    }
+    if (rc) {
+        for (size_t i = done.size(); i-- > 0;) {
+            const Step &d = done[i];
+            kv_page_put(kv_pool(d.s), d.s->pages[d.j]);
+            if (d.old) ++kv_pool(d.s)->refs[d.old];
+            d.s->pages[d.j] = d.old;
+        }
+        return rc;
+    }
+    for (const Step &d : done) {
+        if (d.old) {
+            rc = kv_page_copy(d.s, d.old, &d.s->pages[d.j], 1, KV_PAGE_ROWS);
+            if (rc) { err_ctx->err = d.s->err; return rc; }
+        }
+        kv_tab_set(d.s, d.j, d.s->pages[d.j]);
+    }
+    for (const KvRange &x : r) {
+        rc = kv_tab_upload(x.s);   // synchronises the copies above too
+        if (rc) { err_ctx->err = x.s->err; return rc; }
+    }
+    return L2B_OK;
+}
+// after a call: the pages wholly at or past the appended count go back to the pool
+void kv_release(l2b_ctx *ctx) {
+    if (!ctx->paged) return;
+    for (int j = (ctx->n_appended + KV_PAGE_ROWS - 1) / KV_PAGE_ROWS; j < ctx->n_pages; ++j) kv_drop(ctx, j);
+}
+// A writing call's pages: reserve() before the first launch; every session it listed releases its pages
+// past its appended count when the call returns, refused or not.
+struct KvCall {
+    std::vector<l2b_ctx *> s;
+    KvCall() = default;
+    KvCall(const KvCall &) = delete;
+    ~KvCall() { for (l2b_ctx *c : s) kv_release(c); }
+    int reserve(l2b_ctx *err_ctx, const std::vector<KvRange> &r) {
+        for (const KvRange &x : r) s.push_back(x.s);
+        return kv_reserve(err_ctx, r);
+    }
+};
+
 int create_run_state(l2b_ctx *ctx) {
     const l2b_config *cfg = &ctx->cfg;
     const int rank = ctx->rank, world = ctx->world;
@@ -1364,11 +1583,15 @@ int create_run_state(l2b_ctx *ctx) {
     L2B_TRY(dev_alloc(ctx, &ctx->hb, (size_t)ctx->hid_loc));
     L2B_TRY(dev_alloc(ctx, &ctx->logits, V));
     if (world > 1) L2B_TRY(dev_alloc(ctx, &ctx->logits_loc, (size_t)ctx->vocab_loc));
-    const size_t kv_bytes = L * S * ctx->kv_loc * kv_elem(ctx);
-    unsigned char *kc = nullptr, *vc = nullptr;
-    L2B_TRY(dev_alloc(ctx, &kc, kv_bytes));
-    L2B_TRY(dev_alloc(ctx, &vc, kv_bytes));
-    ctx->kcache = kc; ctx->vcache = vc;
+    const size_t kv_bytes = ctx->paged ? 0 : L * S * ctx->kv_loc * kv_elem(ctx);
+    if (ctx->paged) {
+        L2B_TRY(kv_paged_init(ctx));
+    } else {
+        unsigned char *kc = nullptr, *vc = nullptr;
+        L2B_TRY(dev_alloc(ctx, &kc, kv_bytes));
+        L2B_TRY(dev_alloc(ctx, &vc, kv_bytes));
+        ctx->kcache = kc; ctx->vcache = vc;
+    }
     L2B_TRY(dev_alloc(ctx, &ctx->ctl, (size_t)CTL_WORDS));
     L2B_TRY(dev_alloc(ctx, &ctx->amax, (size_t)1));
     L2B_TRY(dev_alloc(ctx, &ctx->gen_forced, S));
@@ -1382,8 +1605,10 @@ int create_run_state(l2b_ctx *ctx) {
     L2B_TRY(cuda_try(ctx, cudaMemsetAsync(ctx->X, 0, dim * sizeof(float), ctx->stream), "memset"));
     L2B_TRY(cuda_try(ctx, cudaMemsetAsync(ctx->amax, 0, sizeof(unsigned long long), ctx->stream), "memset"));
     L2B_TRY(cuda_try(ctx, cudaMemsetAsync(ctx->gen_forced, 0xff, S * sizeof(int), ctx->stream), "memset"));
-    L2B_TRY(cuda_try(ctx, cudaMemsetAsync(ctx->kcache, 0, kv_bytes, ctx->stream), "memset"));
-    L2B_TRY(cuda_try(ctx, cudaMemsetAsync(ctx->vcache, 0, kv_bytes, ctx->stream), "memset"));
+    if (!ctx->paged) {
+        L2B_TRY(cuda_try(ctx, cudaMemsetAsync(ctx->kcache, 0, kv_bytes, ctx->stream), "memset"));
+        L2B_TRY(cuda_try(ctx, cudaMemsetAsync(ctx->vcache, 0, kv_bytes, ctx->stream), "memset"));
+    }
 
     // ---- attention launch shape: enough (head, split) CTAs to cover the SMs, chunks >= min_chunk positions
     {
@@ -1404,7 +1629,16 @@ int create_run_state(l2b_ctx *ctx) {
             g_create_error = ctx->err;
             return L2B_ERR_UNSUPPORTED;
         }
-        L2B_TRY(cuda_try(ctx, cudaFuncSetAttribute(attention_3pass(ctx->kvfmt), cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem), "cudaFuncSetAttribute"));
+        // paged: each split's page addresses follow the kernels' shared memory (a split of `cap` rows
+        // spans at most cap / P + 2 pages; attn_wo_kernel's splits are ceil(S / 8) rows)
+        ctx->attn_pg_bytes = (int)(((size_t)cap / KV_PAGE_ROWS + 2) * sizeof(void *) + sizeof(float));
+        ctx->attn_pg_bytes_wo = (int)(((S + kAttnClusterCtas - 1) / kAttnClusterCtas / KV_PAGE_ROWS + 2) * sizeof(void *));
+        if (ctx->paged && ctx->attn_smem + ctx->attn_pg_bytes > kMaxDynSmem) {
+            ctx->err = "seq_len too large for the attention kernel's shared memory";
+            g_create_error = ctx->err;
+            return L2B_ERR_UNSUPPORTED;
+        }
+        L2B_TRY(cuda_try(ctx, cudaFuncSetAttribute(attention_3pass(kv_kernels(ctx)), cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem), "cudaFuncSetAttribute"));
         L2B_TRY(dev_alloc(ctx, &ctx->part_o, (size_t)ctx->heads_loc * ns * hs));
         L2B_TRY(dev_alloc(ctx, &ctx->part_ml, (size_t)ctx->heads_loc * ns * 2));
         L2B_TRY(dev_alloc(ctx, &ctx->counters, (size_t)ctx->heads_loc));
@@ -1573,8 +1807,16 @@ void destroy_rank(l2b_ctx *ctx) {
     if (ctx->comm && g_nccl.ok) g_nccl.CommDestroy(ctx->comm);
     for (void *p : ctx->ipc_opened) cudaIpcCloseMemHandle(p);
     for (void *p : ctx->owned) cudaFree(p);
+    if (kv_pool(ctx))
+        for (int j = 0; j < ctx->n_pages; ++j)
+            if (ctx->pages[j]) kv_page_put(kv_pool(ctx), ctx->pages[j]);
     if (ctx->weights && --ctx->weights->refs == 0) {   // the last context or session of the model
         for (void *p : ctx->weights->owned) cudaFree(p);
+        if (KvPool *pool = ctx->weights->pool) {
+            for (void *p : pool->all) cudaFree(p);
+            if (pool->null_page) cudaFree(pool->null_page);
+            delete pool;
+        }
         delete ctx->weights;
     }
     for (int i = 0; i < 2; ++i) {
@@ -1587,6 +1829,7 @@ void destroy_rank(l2b_ctx *ctx) {
     if (ctx->h_gen) cudaFreeHost(ctx->h_gen);
     if (ctx->h_cand) cudaFreeHost(ctx->h_cand);
     if (ctx->h_call) cudaFreeHost(ctx->h_call);
+    if (ctx->h_tab) cudaFreeHost(ctx->h_tab);
     if (ctx->ev0) cudaEventDestroy(ctx->ev0);
     if (ctx->ev1) cudaEventDestroy(ctx->ev1);
     if (ctx->stream) cudaStreamDestroy(ctx->stream);
@@ -1599,6 +1842,12 @@ void destroy_all(l2b_ctx *ctx) {
     // every rank must be idle before any rank's memory (a peer's landing area) goes away
     for (l2b_ctx *c : ranks) { cudaSetDevice(c->device); if (c->stream) cudaStreamSynchronize(c->stream); }
     for (size_t i = ranks.size(); i-- > 0;) destroy_rank(ranks[i]);
+}
+
+// warm_up's step at position 0 wrote through a page table that holds no page: into the null page
+int kv_null_clear(l2b_ctx *ctx) {
+    if (KvPool *pool = kv_pool(ctx)) L2B_CUDA(ctx, cudaMemset(pool->null_page, 0, pool->page_bytes));
+    return L2B_OK;
 }
 
 int common_create(l2b_ctx **out, const l2b_config *cfg, const Source &src, uint64_t n_floats,
@@ -1636,7 +1885,8 @@ int common_create(l2b_ctx **out, const l2b_config *cfg, const Source &src, uint6
         l2b_ctx *ctx = new l2b_ctx();
         ranks.push_back(ctx);
         ctx->wfmt = wfmt;
-        ctx->kvfmt = kvfmt;
+        ctx->kvfmt = kvfmt & ~L2B_KV_PAGED;
+        ctx->paged = (kvfmt & L2B_KV_PAGED) != 0;
         const int rank = in_process ? i : (shard ? shard->rank : 0);
         const int device = in_process ? i : device0;
         rc = create_rank(ctx, cfg, src, rope_cos, rope_sin, rank, world, device);
@@ -1665,6 +1915,8 @@ int common_create(l2b_ctx **out, const l2b_config *cfg, const Source &src, uint6
     }
     rc = warm_up(ranks);
     if (rc) return bail(rc);
+    rc = kv_null_clear(ranks[0]);
+    if (rc) return bail(rc);
     if (in_process) ranks[0]->members = ranks;
     *out = ranks[0];
     return L2B_OK;
@@ -1674,6 +1926,7 @@ int common_create(l2b_ctx **out, const l2b_config *cfg, const Source &src, uint6
 int create_session(l2b_ctx *ctx, const l2b_ctx *model) {
     ctx->wfmt = model->wfmt;
     ctx->kvfmt = model->kvfmt;
+    ctx->paged = model->paged;
     ctx->n_rounded = model->n_rounded;
     L2B_TRY(init_rank(ctx, &model->cfg, 0, 1, model->device));
     ctx->weights = model->weights;
@@ -1683,7 +1936,8 @@ int create_session(l2b_ctx *ctx, const l2b_ctx *model) {
     ctx->w1 = model->w1; ctx->w2 = model->w2; ctx->w3 = model->w3; ctx->wcls = model->wcls;
     ctx->rope_cos = model->rope_cos; ctx->rope_sin = model->rope_sin;
     L2B_TRY(create_run_state(ctx));
-    return warm_up(std::vector<l2b_ctx *>{ctx});
+    L2B_TRY(warm_up(std::vector<l2b_ctx *>{ctx}));
+    return kv_null_clear(ctx);
 }
 #undef L2B_TRY
 
@@ -1724,6 +1978,8 @@ int run_step(l2b_ctx *lead, int token, int pos, int which, float temperature, fl
     l2b_ctx *single[1] = {lead};
     l2b_ctx *const *ranks = lead->members.empty() ? single : lead->members.data();
     const size_t nranks = lead->members.empty() ? 1 : lead->members.size();
+    KvCall kv;
+    if (int rc = kv.reserve(lead, {{lead, pos, pos + 1}})) return rc;
     for (size_t i = 0; i < nranks; ++i) {
         l2b_ctx *ctx = ranks[i];
         if (nranks > 1 || i == 0) L2B_CUDA(lead, cudaSetDevice(ctx->device));
@@ -1835,10 +2091,10 @@ int32_t l2b_create_synthetic_group(l2b_ctx **out, const l2b_config *cfg, uint64_
 // weight_format of l2b_create_format: a weight format, with L2B_KV_BF16 or L2B_KV_ROUND_BF16 or'd in.  Any
 // other value => L2B_ERR_INVALID_ARG.
 bool split_format(int32_t weight_format, int *wfmt, int *kvfmt) {
-    *kvfmt = weight_format & (L2B_KV_BF16 | L2B_KV_ROUND_BF16);
-    *wfmt = weight_format & ~(L2B_KV_BF16 | L2B_KV_ROUND_BF16);
+    *kvfmt = weight_format & (L2B_KV_BF16 | L2B_KV_ROUND_BF16 | L2B_KV_PAGED);
+    *wfmt = weight_format & ~(L2B_KV_BF16 | L2B_KV_ROUND_BF16 | L2B_KV_PAGED);
     if ((*wfmt != L2B_WEIGHTS_F32 && *wfmt != L2B_WEIGHTS_BF16 && *wfmt != L2B_WEIGHTS_Q8) ||
-        *kvfmt == (L2B_KV_BF16 | L2B_KV_ROUND_BF16)) {
+        (*kvfmt & (L2B_KV_BF16 | L2B_KV_ROUND_BF16)) == (L2B_KV_BF16 | L2B_KV_ROUND_BF16)) {
         g_create_error = "unknown weight format";
         return false;
     }
@@ -1866,7 +2122,33 @@ int32_t l2b_create_synthetic_format(l2b_ctx **out, const l2b_config *cfg, uint64
 int32_t l2b_kv_info(const l2b_ctx *ctx, int32_t *kv_format, uint64_t *cache_bytes) {
     if (!ctx) return L2B_ERR_INVALID_ARG;
     if (kv_format) *kv_format = ctx->kvfmt;
-    if (cache_bytes) *cache_bytes = 2ull * ctx->cfg.n_layers * ctx->cfg.seq_len * ctx->kv_loc * kv_elem(ctx);
+    if (cache_bytes && ctx->paged) {
+        uint64_t held = 0;
+        for (void *pg : ctx->pages) held += pg != nullptr;
+        *cache_bytes = held * kv_page_bytes(ctx);
+    } else if (cache_bytes) {
+        *cache_bytes = 2ull * ctx->cfg.n_layers * ctx->cfg.seq_len * ctx->kv_loc * kv_elem(ctx);
+    }
+    return L2B_OK;
+}
+
+int32_t l2b_kv_pool_info(const l2b_ctx *ctx, int32_t *page_rows, uint64_t *page_bytes, uint64_t *pages_in_use,
+                         uint64_t *pages_allocated) {
+    if (!ctx || !page_rows || !page_bytes || !pages_in_use || !pages_allocated) return L2B_ERR_INVALID_ARG;
+    const KvPool *pool = kv_pool(ctx);
+    *page_rows = pool ? KV_PAGE_ROWS : 0;
+    *page_bytes = pool ? pool->page_bytes : 0;
+    *pages_in_use = pool ? pool->refs.size() : 0;
+    *pages_allocated = pool ? pool->all.size() : 0;
+    return L2B_OK;
+}
+
+int32_t l2b_kv_pool_limit(l2b_ctx *ctx, uint64_t max_pages) {
+    if (!ctx) return L2B_ERR_INVALID_ARG;
+    KvPool *pool = kv_pool(ctx);
+    if (!pool) return fail(ctx, L2B_ERR_UNSUPPORTED, "the model's KV cache is not paged");
+    if (max_pages && max_pages < pool->refs.size()) return fail(ctx, L2B_ERR_INVALID_ARG, "max_pages is below the pages in use");
+    pool->limit = max_pages;
     return L2B_OK;
 }
 
@@ -1923,6 +2205,7 @@ void l2b_destroy(l2b_ctx *ctx) { destroy_all(ctx); }
 int32_t l2b_reset(l2b_ctx *ctx) {
     if (!ctx) return L2B_ERR_INVALID_ARG;
     ctx->n_appended = 0;
+    kv_release(ctx);
     return L2B_OK;
 }
 
@@ -1958,6 +2241,52 @@ int fork_launch(l2b_ctx *src, int32_t n_pos, l2b_ctx *const *dst, int32_t n_dst)
     return L2B_OK;
 }
 
+// l2b_fork on a paged model: every destination gives up its pages, then shares src's full pages [0, n_pos/P)
+// and gets a fresh page holding a copy of the rows of src's partial last page, [n_pos/P * P, n_pos).  The
+// fresh pages are taken before any destination changes: a refused fork changes nothing.
+int fork_paged(l2b_ctx *src, int32_t n_pos, l2b_ctx *const *dst, int32_t n_dst) {
+    KvPool *pool = kv_pool(src);
+    const int full = n_pos / KV_PAGE_ROWS, tail = n_pos % KV_PAGE_ROWS;
+    L2B_CUDA(src, cudaSetDevice(src->device));
+    std::vector<void *> fresh;
+    for (int i = 0; tail && i < n_dst; ++i) {
+        void *pg = nullptr;
+        const int rc = kv_page_get(src, pool, &pg);
+        if (rc) {
+            for (void *f : fresh) kv_page_put(pool, f);
+            return rc;
+        }
+        fresh.push_back(pg);
+    }
+    for (int i = 0; i < n_dst; ++i) {
+        l2b_ctx *d = dst[i];
+        for (int j = 0; j < d->n_pages; ++j) kv_drop(d, j);
+        for (int j = 0; j < full; ++j) {
+            d->pages[j] = src->pages[j];
+            ++pool->refs[src->pages[j]];
+            kv_tab_set(d, j, d->pages[j]);
+        }
+        if (tail) {
+            d->pages[full] = fresh[i];
+            kv_tab_set(d, full, fresh[i]);
+        }
+        d->n_appended = n_pos;
+    }
+    if (tail) {
+        L2B_CUDA(src, cudaEventRecord(src->ev0, src->stream));
+        int rc = kv_page_copy(src, src->pages[full], fresh.data(), n_dst, tail);
+        if (rc) return rc;
+        L2B_CUDA(src, cudaEventRecord(src->ev1, src->stream));
+        L2B_CUDA(src, cudaEventSynchronize(src->ev1));
+        L2B_CUDA(src, cudaEventElapsedTime(&src->last_ms, src->ev0, src->ev1));
+    }
+    for (int i = 0; i < n_dst; ++i) {
+        const int rc = kv_tab_upload(dst[i]);
+        if (rc) { src->err = dst[i]->err; return rc; }
+    }
+    return L2B_OK;
+}
+
 extern "C" {
 
 // Everything is checked before anything launches.
@@ -1977,6 +2306,7 @@ int32_t l2b_fork(l2b_ctx *src, int32_t n_pos, l2b_ctx *const *dst, int32_t n_dst
     if (n_pos > src->n_appended) return fail(src, L2B_ERR_STATE, "n_pos past the positions src has appended");
     src->last_ms = 0.0f;
     src->last_launches = 0;
+    if (src->paged) return fork_paged(src, n_pos, dst, n_dst);
     if (n_pos > 0) {
         // No wait across streams: every call of this library ends in a synchronise, so neither src's
         // stream nor any destination's holds work when l2b_fork is entered, and the copy is synchronised
@@ -2053,8 +2383,7 @@ template <int NB, typename W>
 gemv_fn pf_pick(int epi, int ks) {
     switch (epi) {
     case EPI_QKV:
-        return ks == KS_BF16 ? prefill_gemm_kernel<EPI_QKV, NB, W, bf16>
-               : ks == KS_ROUND ? prefill_gemm_kernel<EPI_QKV, NB, W, kv_f32_bf16> : prefill_gemm_kernel<EPI_QKV, NB, W>;
+        return kv_dispatch(ks, [](auto t) { return (gemv_fn)prefill_gemm_kernel<EPI_QKV, NB, W, typename decltype(t)::type>; });
     case EPI_SILU: return prefill_gemm_kernel<EPI_SILU, NB, W>;
     case EPI_STORE: return prefill_gemm_kernel<EPI_STORE, NB, W>;
     case EPI_ARGMAX: return prefill_gemm_kernel<EPI_ARGMAX, NB, W>;
@@ -2378,7 +2707,12 @@ static int step_sessions(l2b_ctx *const *s, int n, const int32_t *n_tok, const i
                          StepMode mode, const float *temperature = nullptr, const float *top_p = nullptr) {
     l2b_ctx *ctx = s[0];
     const bool argmax = (mode == MODE_ARGMAX), sample = (mode == MODE_SAMPLE);
-    int rc = pf_prepare(ctx);
+    std::vector<KvRange> ranges;
+    for (int i = 0; i < n; ++i) ranges.push_back(KvRange{s[i], pos[i], pos[i] + (n_tok ? n_tok[i] : 1)});
+    KvCall kv;
+    int rc = kv.reserve(ctx, ranges);
+    if (rc) return rc;
+    rc = pf_prepare(ctx);
     if (rc) return rc;
     // the vectors: vector v runs token tokens[v]; last(v): the session it ends, or -1
     const RunVectors r = expand_runs(s, n, n_tok, pos);
@@ -2611,6 +2945,9 @@ int32_t l2b_generate_argmax(l2b_ctx *ctx, int32_t token, int32_t pos, int32_t n_
     if (rc) return rc;
     *n_done = 0;
     if (n_steps == 0) return L2B_OK;
+    KvCall kv;
+    rc = kv.reserve(ctx, {{ctx, pos, pos + n_steps}});
+    if (rc) return rc;
     int done = 0;
     rc = run_device_loop(ctx, G_ARGMAX_LOOP, token, pos, n_steps, forced, stop_on_bos, &done);
     if (rc) return rc;
@@ -2633,6 +2970,9 @@ int32_t l2b_prefill(l2b_ctx *ctx, const int32_t *tokens, int32_t n_tokens, int32
     for (int i = 0; i < n_tokens; ++i)
         if (tokens[i] < 0 || tokens[i] >= ctx->cfg.vocab_size) return fail(ctx, L2B_ERR_INVALID_ARG, "token out of range");
     const int n_silent = host_logits ? n_tokens - 1 : n_tokens;   // positions whose logits are dropped
+    KvCall kv;
+    rc = kv.reserve(ctx, {{ctx, pos0, pos0 + n_tokens}});
+    if (rc) return rc;
     rc = pf_prepare(ctx);
     if (rc) return rc;
     if (n_silent > 0 && ctx->pf_ok) {
@@ -2670,7 +3010,10 @@ int32_t l2b_score(l2b_ctx *ctx, const int32_t *tokens, int32_t n_tokens, int32_t
     ctx->last_launches = 0;
     const int n = n_tokens - 1;                               // positions scored
     if (n == 0) return L2B_OK;
-    int rc = pf_prepare(ctx);
+    KvCall kv;
+    int rc = kv.reserve(ctx, {{ctx, pos0, pos0 + n}});
+    if (rc) return rc;
+    rc = pf_prepare(ctx);
     if (rc) return rc;
     if (ctx->pf_ok) {
         rc = prefill_batched(ctx, tokens, n, pos0, true);
@@ -2894,6 +3237,11 @@ int32_t l2b_generate_argmax_batch(l2b_ctx *const *sessions, int32_t n, const int
     }
     for (int i = 0; i < n; ++i) n_done[i] = 0;
     if (n_steps == 0) return L2B_OK;
+    std::vector<KvRange> ranges;
+    for (int i = 0; i < n; ++i) ranges.push_back(KvRange{sessions[i], pos[i], pos[i] + limit[i]});
+    KvCall kv;
+    rc = kv.reserve(s0, ranges);
+    if (rc) return rc;
     rc = pf_prepare(s0);
     if (rc) return rc;
     if (s0->pf_ok) return generate_batched(sessions, n, tokens, pos, n_steps, forced, limit.data(), stop_on_bos, out_next, n_done);
@@ -2995,6 +3343,11 @@ int32_t l2b_verify_argmax_ragged(l2b_ctx *const *sessions, int32_t n, const int3
     l2b_ctx *s0 = sessions[0];
     if (!greedy || !n_accept) return fail(s0, L2B_ERR_INVALID_ARG, "greedy or n_accept is NULL");
     if (s0->world > 1) return fail(s0, L2B_ERR_UNSUPPORTED, "l2b_verify_argmax_ragged needs a single-GPU model");
+    std::vector<KvRange> ranges;
+    for (int i = 0; i < n; ++i) ranges.push_back(KvRange{sessions[i], pos0[i], pos0[i] + n_tokens[i]});
+    KvCall kv;
+    rc = kv.reserve(s0, ranges);
+    if (rc) return rc;
     rc = pf_prepare(s0);
     if (rc) return rc;
     rc = s0->pf_ok ? verify_batched(sessions, n, n_tokens, tokens, pos0, stop_on_bos, greedy, n_accept)
@@ -3027,6 +3380,13 @@ int32_t l2b_generate_speculative(l2b_ctx *target, l2b_ctx *draft, int32_t token,
     if (pos > target->n_appended || pos > draft->n_appended)
         return fail(target, L2B_ERR_STATE, "pos skips ahead of the target's or the draft's KV cache");
     if (n_steps > S - pos) n_steps = S - pos;                 // :992-993
+    // every row either model may write, up front, so a refused call changes neither; the rounds' own calls
+    // then only re-take pages they released in between
+    KvCall kv;
+    std::vector<KvRange> ranges{{target, pos, pos + n_steps}};
+    if (draft->paged) ranges.push_back(KvRange{draft, pos, pos + n_steps});
+    if (!target->paged && draft->paged) ranges.erase(ranges.begin());
+    if (int rc = kv.reserve(target, ranges)) return rc;
     float ms = 0.0f;
     int launches = 0, rounds = 0, done = 0;
     std::vector<int32_t> hist(1, token);   // hist[q - pos]: the stream's token at position q
@@ -3199,6 +3559,11 @@ int32_t l2b_verify_sample_ragged(l2b_ctx *const *sessions, int32_t n, const int3
     const int64_t cap = std::max<int64_t>((int64_t)n * (L2B_SPECULATIVE_MAX_K + 1), L2B_VERIFY_SAMPLE_STAGE_BYTES / per_pos);
     if (total > cap) return fail(s0, L2B_ERR_INVALID_ARG, "more positions than the verify staging holds (see L2B_VERIFY_SAMPLE_STAGE_BYTES)");
     if (s0->world > 1) return fail(s0, L2B_ERR_UNSUPPORTED, "l2b_verify_sample_ragged needs a single-GPU model");
+    std::vector<KvRange> ranges;
+    for (int i = 0; i < n; ++i) ranges.push_back(KvRange{sessions[i], pos0[i], pos0[i] + n_tokens[i]});
+    KvCall kv;
+    rc = kv.reserve(s0, ranges);
+    if (rc) return rc;
     rc = pf_prepare(s0);
     if (rc) return rc;
     return s0->pf_ok ? verify_sample_batched(sessions, n, n_tokens, tokens, pos0, temperature, filter_p.data(), host_probs,
@@ -3224,7 +3589,31 @@ int32_t l2b_read_state(l2b_ctx *ctx, int32_t which, float *dst, uint64_t n, uint
     }
     if (n < cnt) return fail(ctx, L2B_ERR_INVALID_ARG, "dst too small");
     L2B_CUDA(ctx, cudaSetDevice(ctx->device));
-    if ((which == 4 || which == 5) && kv_bf16(ctx)) {
+    if ((which == 4 || which == 5) && ctx->paged) {
+        // gathered page by page into the contiguous layout; rows of pages the context does not hold are 0
+        memset(dst, 0, cnt * sizeof(float));
+        const size_t el = kv_elem(ctx), P = KV_PAGE_ROWS, kvl = ctx->kv_loc;
+        std::vector<unsigned char> page(kv_page_bytes(ctx));
+        for (int j = 0; j < ctx->n_pages; ++j) {
+            if (!ctx->pages[j]) continue;
+            L2B_CUDA(ctx, cudaMemcpy(page.data(), ctx->pages[j], page.size(), cudaMemcpyDeviceToHost));
+            const uint64_t rows = std::min<uint64_t>(P, S - j * P);
+            for (uint64_t l = 0; l < L; ++l) {
+                const unsigned char *from = page.data() + ((2 * l + (which == 5)) * P) * kvl * el;
+                float *to = dst + (l * S + j * P) * kvl;
+                for (uint64_t i = 0; i < rows * kvl; ++i) {
+                    if (el == 2) {
+                        uint16_t h;
+                        memcpy(&h, from + 2 * i, 2);
+                        const uint32_t u = (uint32_t)h << 16;
+                        memcpy(to + i, &u, 4);
+                    } else {
+                        memcpy(to + i, from + 4 * i, 4);
+                    }
+                }
+            }
+        }
+    } else if ((which == 4 || which == 5) && kv_bf16(ctx)) {
         // the bf16 cache lands in the upper half of dst and is widened in place from the front: value i is
         // written to bytes [4i, 4i+4), below the unread values at [2 cnt + 2i, ..) for every i < cnt
         uint16_t *h = reinterpret_cast<uint16_t *>(dst) + cnt;
@@ -3260,6 +3649,9 @@ int32_t l2b_profile_step(l2b_ctx *ctx, int32_t token, int32_t pos, l2b_kernel_ti
     if (rc) return rc;
     if (!out || !n_out || cap <= 0) return fail(ctx, L2B_ERR_INVALID_ARG, "bad profile arguments");
     std::vector<l2b_ctx *> ranks = locals(ctx);
+    KvCall kv;
+    rc = kv.reserve(ctx, {{ctx, pos, pos + 1}});
+    if (rc) return rc;
     if (pos + 1 > ctx->n_appended) ctx->n_appended = pos + 1;   // attention bytes use this
     const int saved_appended = ctx->n_appended;
     cudaEvent_t last = nullptr;
