@@ -317,6 +317,61 @@ int32_t l2b_generate_argmax_batch(l2b_ctx *const *sessions, int32_t n, const int
                                   const int32_t *pos, int32_t n_steps, const int32_t *forced,
                                   int32_t stop_on_bos, int32_t *out_next, int32_t *n_done);
 
+/* ---- beam search ------------------------------------------------------------------------ */
+
+/* Most beams one l2b_beam_search call keeps.                                                            */
+#define L2B_BEAM_MAX 8
+
+/* Beam search of B = n_beams hypotheses from `token` at position `pos` of src's prompt, on a paged model
+ * (L2B_KV_PAGED).  Each hypothesis holds its KV rows in the pages of one of the B sessions `beams` (distinct
+ * sessions of src's model, not src; scratch during the call), and a hypothesis that continues another one
+ * takes over its parent's pages by reference instead of copying its rows.
+ * The rule.  K = 2B, T = min(n_steps, seq_len - pos).  live = [the empty hypothesis, c = 0], F = [] (finished).
+ * At step t = 0 .. T-1:
+ *   1. each live hypothesis h, in slot order, runs its last token (at t = 0: `token`) at position pos + t;
+ *   2. its candidates C_h are l2b_op_logprob_topk(logits_h, K): (lp, token) pairs, rank r_h within C_h;
+ *   3. all candidates form one pool; a candidate's score is fl(c_h + lp); the pool is ordered by score (larger
+ *      first, in argmax_key order), then by h, then by r_h;
+ *   4. the pool is walked in order, positions counted from 0: with stop_on_bos, a BOS (token 1) candidate at a
+ *      position below B goes to F, which keeps its best B, and one at position B or later is dropped; every
+ *      other candidate becomes the next live slot; the walk stops at B live;
+ *   5. with stop_on_bos, the search ends when |F| = B and the worst normalised score in F is >=
+ *      fl(c(live[0]) / (t + 1)).
+ * A hypothesis's normalised score is fl(c / len) (length penalty 1; len counts its tokens, BOS included).
+ * Hypotheses are ordered by larger normalised score, then larger c, then earlier creation (step, then
+ * position in that step's pool).  The results are the best B of F and live.  Without stop_on_bos, BOS is an
+ * ordinary token.
+ * Results, best first: result i's tokens in out_tokens[i * n_steps ..][0 .. out_len[i]) (row-major
+ * n_beams x n_steps), its cumulative natural-log probability in out_logprob[i], and its KV rows in beams[i],
+ * which has pos + out_len[i] positions appended and continues with l2b_forward(beams[i], last token,
+ * pos + out_len[i]), as after l2b_generate_argmax.  *n_run (n_run may be NULL) is the number of steps run.
+ * Contract: at every step the candidates of hypothesis [y_1 .. y_t] are l2b_op_logprob_topk of the logits
+ * l2b_forward_ragged returns for the run [token, y_1 .. y_t] at pos on an l2b_fork(src, pos, ..), bit for bit:
+ * where l2b_forward_ragged shares weight passes, the live hypotheses go 4 per pass through the same kernels
+ * (a position's arithmetic does not depend on its pass); elsewhere each runs its own single step.  So the
+ * tokens, out_len, out_logprob and the rows of beams[i] below its appended count are fixed bits, for every
+ * weight and KV format.
+ * Pages: every beam first releases its pages and shares src's [0, ceil(pos / P)); after each selection slot j
+ * takes its parent's pages; before each step a shared page the step writes into is copied first
+ * (copy-on-write, as every writing call does), so src and the siblings never change; a finished hypothesis
+ * keeps its pages until the end; at the end beams[i] take the results' pages and every other reference goes
+ * back to the pool.
+ * Refused before anything runs or changes: NULL src, beams, out_tokens, out_len or out_logprob, n_beams
+ * outside [1, L2B_BEAM_MAX] or 2 * n_beams > vocab_size, a NULL, repeated or other-model beam, src among the
+ * beams, a token out of range, pos < 0 or pos >= seq_len, n_steps < 0 => L2B_ERR_INVALID_ARG; pos past src's
+ * appended count => L2B_ERR_STATE; a contiguous model => L2B_ERR_UNSUPPORTED: reordering hypotheses there
+ * would copy O(pos) rows per beam each step (a tensor-parallel model cannot be paged, so it is refused too).
+ * n_steps == 0 runs nothing, changes nothing, and sets *n_run = 0, out_len[i] = 0 and out_logprob[i] = 0.
+ * When the pool limit (l2b_kv_pool_limit) or the device memory runs out at any step the call returns
+ * L2B_ERR_OOM: src is unchanged, every beam has 0 positions appended and no page is lost.  This is weaker
+ * than "changes no session": the beams are destinations whose streams the call replaces, as in l2b_fork.
+ * src is never changed: not its caches, its appended count or its logits.  x, xb, hb, q and logits of the
+ * beams are not defined afterwards.  Errors through l2b_last_error(src); l2b_last_timing(src) covers the
+ * whole call, host work between the steps included.  Synchronous.                                         */
+int32_t l2b_beam_search(l2b_ctx *src, int32_t token, int32_t pos, l2b_ctx *const *beams, int32_t n_beams,
+                        int32_t n_steps, int32_t stop_on_bos, int32_t *out_tokens, int32_t *out_len,
+                        float *out_logprob, int32_t *n_run);
+
 /* ---- greedy speculative decoding ------------------------------------------------------ */
 
 /* Verifies guessed ("draft") tokens of n distinct sessions in shared weight passes.  The runs are laid out
@@ -496,6 +551,13 @@ int32_t l2b_op_sample_prep(int32_t device, float *logits_inout, int32_t n, float
 /* log softmax(logits)[target] of n host logits (l2b_score's device code, see there).  NULL pointers,
  * n < 1 or a target outside [0, n) => L2B_ERR_INVALID_ARG.                                  */
 int32_t l2b_op_logprob(int32_t device, const float *logits, int32_t n, int32_t target, float *logprob);
+/* The k best log softmax(logits)[i] of n host logits, best first: out[j] = (log-probability, index), ordered
+ * by larger log-probability, then smaller index.  Each out[j].prob equals l2b_op_logprob(.., out[j].index)
+ * bit for bit.  NULL pointers, n < 1, k < 1, k > n or k > 2 * L2B_BEAM_MAX => L2B_ERR_INVALID_ARG.
+ * Here l2b_prob_index.prob holds a log-probability, not a probability.  The selection is on the
+ * log-probabilities themselves: two logits that round to one log-probability tie, and the smaller index
+ * comes first.  l2b_beam_search's candidates are this kernel's output.                                  */
+int32_t l2b_op_logprob_topk(int32_t device, const float *logits, int32_t n, int32_t k, l2b_prob_index *out);
 
 /* ---- device weight format ------------------------------------------------------------------
  * Which tensors: the token embedding, wq wk wv wo w1 w2 w3 and an unshared wcls are stored in the

@@ -33,6 +33,7 @@ from .binding import (  # noqa: F401
     KV_FORMATS,
     KV_PAGED,
     KV_PAGE_ROWS,
+    BEAM_MAX,
     QUANT_FORMATS,
     WEIGHT_FORMATS,
     vector_weighted_sum_rows,
@@ -40,6 +41,7 @@ from .binding import (  # noqa: F401
     fused_matmul,
     sample_prep,
     logprob,
+    logprob_topk,
     exported_symbols,
     forward_batch,
     forward_argmax_batch,
@@ -49,6 +51,7 @@ from .binding import (  # noqa: F401
     forward_argmax_ragged,
     forward_sample_ragged,
     fork,
+    beam_search,
     verify_argmax_ragged,
     verify_sample_ragged,
 )
@@ -56,7 +59,7 @@ from .checkpoint import Checkpoint, read_checkpoint, MODEL_SHAPES  # noqa: F401
 
 __all__ = [
     "L2BError", "L2BConfig", "L2BShard", "Transformer", "checkpoint_floats", "comm_unique_id",
-    "lib_path", "load_library", "matmul", "rmsnorm", "softmax", "synth_checkpoint_host", "round_bf16_host", "round_q8_host", "Q8_GROUP", "WEIGHT_FORMATS", "QUANT_FORMATS", "KV_BF16", "KV_ROUND_BF16", "KV_FORMATS", "KV_PAGED", "KV_PAGE_ROWS",
-    "vector_weighted_sum_rows", "attention_head", "fused_matmul", "sample_prep", "logprob", "exported_symbols", "forward_batch", "forward_argmax_batch", "forward_sample_batch", "generate_argmax_batch", "forward_ragged", "forward_argmax_ragged", "forward_sample_ragged", "fork", "verify_argmax_ragged", "verify_sample_ragged", "Checkpoint",
+    "lib_path", "load_library", "matmul", "rmsnorm", "softmax", "synth_checkpoint_host", "round_bf16_host", "round_q8_host", "Q8_GROUP", "WEIGHT_FORMATS", "QUANT_FORMATS", "KV_BF16", "KV_ROUND_BF16", "KV_FORMATS", "KV_PAGED", "KV_PAGE_ROWS", "BEAM_MAX",
+    "vector_weighted_sum_rows", "attention_head", "fused_matmul", "sample_prep", "logprob", "logprob_topk", "exported_symbols", "forward_batch", "forward_argmax_batch", "forward_sample_batch", "generate_argmax_batch", "forward_ragged", "forward_argmax_ragged", "forward_sample_ragged", "fork", "beam_search", "verify_argmax_ragged", "verify_sample_ragged", "Checkpoint",
     "read_checkpoint", "MODEL_SHAPES",
 ]

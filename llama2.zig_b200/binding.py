@@ -113,6 +113,9 @@ def load_library():
     lib.l2b_op_sample_prep.argtypes = [C.c_int32, FP, C.c_int32, C.c_float, C.c_float,
                                        C.POINTER(L2BProbIndex), C.c_int32, IP]
     lib.l2b_op_logprob.argtypes = [C.c_int32, FP, C.c_int32, C.c_int32, FP]
+    lib.l2b_op_logprob_topk.argtypes = [C.c_int32, FP, C.c_int32, C.c_int32, C.POINTER(L2BProbIndex)]
+    lib.l2b_beam_search.argtypes = [vp, C.c_int32, C.c_int32, C.POINTER(vp), C.c_int32, C.c_int32, C.c_int32,
+                                    IP, IP, FP, IP]
     lib.l2b_last_error.argtypes = [vp]
     lib.l2b_last_error.restype = C.c_char_p
     lib.l2b_status_string.argtypes = [C.c_int32]
@@ -186,6 +189,7 @@ KV_FORMATS = {"f32": 0, "bf16": KV_BF16, "f32-round-bf16": KV_ROUND_BF16}   # l2
 KV_PAGED = 0x800                         # L2B_KV_PAGED: or'd in like the KV formats; the paged layout
 KV_PAGE_ROWS = 64                        # L2B_KV_PAGE_ROWS: positions per page
 _KV_LAYOUTS = {"contiguous": 0, "paged": KV_PAGED}
+BEAM_MAX = 8                             # L2B_BEAM_MAX: most beams of one beam_search call
 
 
 def round_bf16_host(a):
@@ -653,6 +657,25 @@ def fork(src, dsts, n_pos):
     _check(load_library().l2b_fork(sh, int(n_pos), hs, n), sh)
 
 
+def beam_search(src, token, pos, beams, n_steps, stop_on_bos=True):
+    """Beam search of len(beams) hypotheses from (token, pos) on src's prompt (l2b_beam_search; a paged model).
+    Returns (tokens, logprobs, n_run), best first: tokens[i] is result i's int32 token array, logprobs[i] its
+    cumulative log-probability (float32), n_run the number of steps run.  Afterwards beams[i] holds result i's
+    KV rows with pos + len(tokens[i]) positions appended; src is not changed."""
+    n = len(beams)
+    hs = (C.c_void_p * max(n, 1))(*[b.h.value if b is not None else None for b in beams])
+    sh = src.h if src is not None else None
+    width = max(int(n_steps), 1)
+    out = np.full((max(n, 1), width), -1, dtype=np.int32)
+    lens = np.zeros(max(n, 1), dtype=np.int32)
+    lps = np.zeros(max(n, 1), dtype=np.float32)
+    ran = C.c_int32()
+    _check(load_library().l2b_beam_search(sh, int(token), int(pos), hs, n, int(n_steps), 1 if stop_on_bos else 0,
+                                          out.ctypes.data_as(IP), lens.ctypes.data_as(IP), lps.ctypes.data_as(FP),
+                                          C.byref(ran)), sh)
+    return [out[i, :lens[i]].copy() for i in range(n)], lps[:n].copy(), ran.value
+
+
 # ---- reference-named single ops on host buffers (device = cuda:0) ---------------------------
 
 def matmul(xout, x, w, device=0):
@@ -707,6 +730,16 @@ def logprob(logits, target, device=0):
     out = C.c_float()
     _check(load_library().l2b_op_logprob(device, lp_, logits.size, int(target), C.byref(out)))
     return np.float32(out.value)
+
+
+def logprob_topk(logits, k, device=0):
+    """The k best log softmax(logits)[i] on the device (l2b_op_logprob_topk: beam search's candidate kernel on
+    one row), best first, as a structured array (prob, index) like sample_prep's candidates; here `prob` is
+    the log-probability, equal to logprob(logits, index) bit for bit."""
+    logits, lp_ = _f32(logits)
+    out = (L2BProbIndex * max(int(k), 1))()
+    _check(load_library().l2b_op_logprob_topk(device, lp_, logits.size, int(k), out))
+    return np.frombuffer(out, dtype=[("prob", "<f4"), ("index", "<i4")], count=int(k)).copy()
 
 
 def rmsnorm(o, x, w, device=0):

@@ -363,6 +363,11 @@ __device__ __forceinline__ unsigned long long argmax_key(float v, int idx) {
 __device__ __forceinline__ int argmax_key_index(unsigned long long key) {
     return (int)(0xFFFFFFFFu - (unsigned int)(key & 0xFFFFFFFFull));
 }
+// the value a key was made from, bit for bit
+__device__ __forceinline__ float argmax_key_value(unsigned long long key) {
+    const uint32_t u = (uint32_t)(key >> 32);
+    return __uint_as_float((u & 0x80000000u) ? (u & 0x7FFFFFFFu) : ~u);
+}
 
 // ---------------------------------------------------------------------------------------
 // Step control block (device memory, 16 ints):
@@ -2603,9 +2608,9 @@ __global__ void __launch_bounds__(SAMP_THREADS) sample_prep_batch_kernel(const S
 // key (EPI_ARGMAX, first maximum wins), so it is exactly what l2b_forward_argmax picks.
 // ---------------------------------------------------------------------------------------
 constexpr int LOGPROB_THREADS = 1024;
-__device__ __forceinline__ float logprob_row(const float *logits, int n, int target) {
+// m = max l[i] and s = sum expf(l[i] - m) of a row in that fixed order, in every thread of the CTA
+__device__ __forceinline__ void logprob_ms(const float *logits, int n, float &m_out, float &s_out) {
     __shared__ float red[LOGPROB_THREADS / 32];
-    if (target < 0 || target >= n) return __int_as_float(0x7fffffff);
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     float m = -INFINITY;
     for (int i = tid; i < n; i += LOGPROB_THREADS) m = fmaxf(m, logits[i]);
@@ -2620,6 +2625,13 @@ __device__ __forceinline__ float logprob_row(const float *logits, int n, int tar
     if (lane == 0) red[warp] = s;
     __syncthreads();
     s = warp_sum(red[lane]);
+    m_out = m;
+    s_out = s;
+}
+__device__ __forceinline__ float logprob_row(const float *logits, int n, int target) {
+    if (target < 0 || target >= n) return __int_as_float(0x7fffffff);
+    float m, s;
+    logprob_ms(logits, n, m, s);
     return (logits[target] - m) - logf(s);
 }
 
@@ -2659,6 +2671,60 @@ __global__ void __launch_bounds__(LOGPROB_THREADS) logprob_batch_kernel(const Lo
         p.greedy[b] = argmax_key_index(p.amax[b]);
         p.amax[b] = 0ull;
     }
+}
+
+// ---------------------------------------------------------------------------------------
+// The k best log-probabilities of a row (l2b_beam_search's candidates, l2b_op_logprob_topk): m and s as
+// logprob_row forms them, then lp_i = (l_i - m) - logf(s) for every i, exactly logprob_row's value of
+// target i.  The selection is on argmax_key(lp_i, i) (larger lp first, then the smaller index), so it acts
+// on lp itself: two logits that round to one lp tie there and the smaller index wins.  Keys are unique,
+// so the TOPK_MAX largest are one set whatever order they are met in, and no atomics are involved:
+//   - each warp keeps a sorted list of the TOPK_MAX largest keys it has seen, one per lane (lane t holds
+//     the t-th), and takes 32 elements at a time; the few above the list's last key go in one by one;
+//   - the 32 warps' lists go to shared memory and warp 0 takes their 512 keys the same way.
+// Key 0 is no element's key (its low word is 0xFFFFFFFF - index, and index < n < 2^31): it stands for
+// "none yet" and for lanes past the row's end, and never enters a list.
+// ---------------------------------------------------------------------------------------
+constexpr int TOPK_MAX = 16;
+__device__ __forceinline__ void topk_warp_insert(unsigned long long &list, unsigned long long x) {
+    const int lane = threadIdx.x & 31;
+    unsigned int pend = __ballot_sync(0xffffffffu, x > __shfl_sync(0xffffffffu, list, TOPK_MAX - 1));
+    while (pend) {
+        const unsigned long long y = __shfl_sync(0xffffffffu, x, __ffs(pend) - 1);
+        pend &= pend - 1;
+        const int at = __popc(__ballot_sync(0xffffffffu, lane < TOPK_MAX && list > y));   // y's place
+        const unsigned long long prev = __shfl_up_sync(0xffffffffu, list, 1);
+        if (lane < TOPK_MAX) list = lane > at ? prev : lane == at ? y : list;   // at == TOPK_MAX: y stays out
+    }
+}
+
+// CTA b: row b of logits (stride floats apart), its k <= TOPK_MAX best to out[b * k ..], best first
+struct LogprobTopkParams {
+    const int *ctl;                 // CTL_DONE
+    const float *logits;
+    int n, stride, k;
+    ProbIndex *out;                 // [nb][k]: (log-probability, index)
+};
+__global__ void __launch_bounds__(LOGPROB_THREADS) logprob_topk_batch_kernel(const LogprobTopkParams p) {
+    __shared__ unsigned long long part[LOGPROB_THREADS / 32 * TOPK_MAX];
+    pdl_wait();
+    if (p.ctl[CTL_DONE]) return;
+    const float *row = p.logits + (size_t)blockIdx.x * p.stride;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    float m, s;
+    logprob_ms(row, p.n, m, s);
+    const float ls = logf(s);
+    unsigned long long list = 0ull;
+    for (int base = warp * 32; base < p.n; base += LOGPROB_THREADS) {   // warp-uniform: every lane shuffles
+        const int i = base + lane;
+        topk_warp_insert(list, i < p.n ? argmax_key((row[i] - m) - ls, i) : 0ull);
+    }
+    if (lane < TOPK_MAX) part[warp * TOPK_MAX + lane] = list;
+    __syncthreads();
+    if (warp != 0) return;
+    list = 0ull;
+    for (int j = 0; j < LOGPROB_THREADS / 32 * TOPK_MAX; j += 32) topk_warp_insert(list, part[j + lane]);
+    if (lane < p.k) p.out[(size_t)blockIdx.x * p.k + lane] = ProbIndex{argmax_key_value(list), argmax_key_index(list)};
 }
 
 // ---------------------------------------------------------------------------------------

@@ -1257,7 +1257,8 @@ int preload_kernels(l2b_ctx *ctx) {
                             (const void *)batch_advance_kernel, (const void *)gather_logits_kernel,
                             (const void *)resid_add_kernel, (const void *)sample_prep_kernel,
                             (const void *)sample_prep_batch_kernel, (const void *)logprob_kernel,
-                            (const void *)logprob_batch_kernel, (const void *)synth_fill_kernel,
+                            (const void *)logprob_batch_kernel, (const void *)logprob_topk_batch_kernel,
+                            (const void *)synth_fill_kernel,
                             (const void *)synth_fill_bf16_kernel, (const void *)synth_fill_q8_kernel,
                             (const void *)kv_fork_pick(ctx->kvfmt), (const void *)verify_accept_kernel};
     for (const void *f : others) L2B_CUDA(ctx, cudaFuncGetAttributes(&fa, f));
@@ -3572,6 +3573,266 @@ int32_t l2b_verify_sample_ragged(l2b_ctx *const *sessions, int32_t n, const int3
                                           cand, cand_cap, n_cand);
 }
 
+// ---- beam search (l2b_beam_search) ----------------------------------------------------------------------
+
+// logprob_topk_batch_kernel on nb rows of vocab_size logits, vocab_size apart, on ctx's stream: k best of
+// row b to out[b * k ..]
+static int launch_logprob_topk(l2b_ctx *ctx, const float *logits, int nb, int k, ProbIndex *out) {
+    LogprobTopkParams p{ctx->ctl, logits, ctx->cfg.vocab_size, ctx->cfg.vocab_size, k, out};
+    void *args[] = {&p};
+    return launch_small(ctx, (const void *)logprob_topk_batch_kernel, dim3(nb), dim3(LOGPROB_THREADS), args, ctx->stream, true);
+}
+
+// A hypothesis: its tokens after the start token, its cumulative log-probability c, when it was made (step,
+// position in that step's pool) and, once finished, its own references to its parent's pages.
+struct BeamHyp {
+    std::vector<int> toks;
+    float c = 0.0f;
+    int step = -1, at = 0, slot = -1;        // slot: the beam session a live hypothesis is in
+    std::vector<void *> pages;
+};
+static uint32_t beam_fkey(float v) {         // the order of argmax_key's high word: larger float, larger key
+    uint32_t u;
+    memcpy(&u, &v, sizeof u);
+    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+// the result order: larger normalised score fl(c / len) (length penalty 1), then larger c, then earlier
+static bool beam_better(const BeamHyp &a, const BeamHyp &b) {
+    const uint32_t na = beam_fkey(a.c / (float)a.toks.size()), nb = beam_fkey(b.c / (float)b.toks.size());
+    if (na != nb) return na > nb;
+    if (a.c != b.c) return beam_fkey(a.c) > beam_fkey(b.c);
+    return a.step != b.step ? a.step < b.step : a.at < b.at;
+}
+// new references to session s's pages [0, np)
+static std::vector<void *> beam_take(l2b_ctx *s, int np) {
+    std::vector<void *> v(s->pages.begin(), s->pages.begin() + np);
+    for (void *pg : v)
+        if (pg) ++kv_pool(s)->refs[pg];
+    return v;
+}
+static void beam_put(KvPool *pool, std::vector<void *> &v) {
+    for (void *pg : v)
+        if (pg) kv_page_put(pool, pg);
+    v.clear();
+}
+// session s gives up its pages and holds v (whose references pass to it) with n positions appended
+static void beam_assign(l2b_ctx *s, const std::vector<void *> &v, int n) {
+    for (int j = 0; j < s->n_pages; ++j) kv_drop(s, j);
+    for (size_t j = 0; j < v.size(); ++j) {
+        s->pages[j] = v[j];
+        kv_tab_set(s, (int)j, v[j]);
+    }
+    s->n_appended = n;
+}
+
+// The search of l2b_beam_search on validated arguments (n_steps > 0, a paged model).  The live hypotheses are
+// in beams[0 .. live.size()), each holding its pages; the finished ones hold theirs in fin.  Batched: the live
+// hypotheses go PF_MAXB per pass through batched_layers and batched_classifier on beams[0]'s stream and
+// buffers, and logprob_topk_batch_kernel reads pf_logits.  Otherwise each runs run_step(G_LOGITS) and the
+// kernel reads its logits.  Only live.size() * K (lp, index) pairs come back per step.
+struct BeamSearch {
+    l2b_ctx *src, *lead;
+    l2b_ctx *const *beams;
+    int B, K, pos, token;
+    bool stop;
+    std::vector<BeamHyp> live, fin;
+    int launches = 0, ran = 0;
+
+    int err_from(l2b_ctx *c, int rc) {
+        if (c != src) src->err = c->err;
+        return rc;
+    }
+    int upload_all() {
+        for (int i = 0; i < B; ++i)
+            if (int rc = kv_tab_upload(beams[i])) return err_from(beams[i], rc);
+        return L2B_OK;
+    }
+    // runs the last token of every live hypothesis at pos + t; their candidates to lead->h_cand
+    int step(int t) {
+        const int nl = (int)live.size();
+        std::vector<KvRange> r;
+        for (int j = 0; j < nl; ++j) r.push_back(KvRange{beams[j], pos + t, pos + t + 1});
+        int rc = kv_reserve(src, r);
+        if (rc) return rc;
+        std::vector<int> last(nl), at(nl, pos + t);
+        for (int j = 0; j < nl; ++j) last[j] = live[j].toks.empty() ? token : live[j].toks.back();
+        cudaStream_t st = lead->stream;
+        L2B_CUDA(src, cudaSetDevice(lead->device));
+        if (lead->pf_ok) {
+            lead->last_launches = 0;
+            L2B_CUDA(src, cudaMemcpyAsync(lead->call_ints, last.data(), nl * sizeof(int), cudaMemcpyHostToDevice, st));
+            for (int g = 0; g < nl; g += PF_MAXB) {
+                const int nb = std::min(PF_MAXB, nl - g);
+                if ((rc = batched_layers(lead, beams + g, at.data() + g, nb, lead->call_ints + g, nullptr)) ||
+                    (rc = batched_classifier(lead, nb, false)) ||
+                    (rc = launch_logprob_topk(lead, lead->pf_logits, nb, K, lead->call_cand + (size_t)g * K)))
+                    return err_from(lead, rc);
+            }
+            launches += lead->last_launches;
+        } else {
+            for (int j = 0; j < nl; ++j) {
+                if ((rc = run_step(beams[j], last[j], pos + t, G_LOGITS, 1.0f, 0.0f))) return err_from(beams[j], rc);
+                launches += beams[j]->last_launches;
+            }
+            lead->last_launches = 0;
+            for (int j = 0; j < nl; ++j)
+                if ((rc = launch_logprob_topk(lead, beams[j]->logits, 1, K, lead->call_cand + (size_t)j * K))) return err_from(lead, rc);
+            launches += lead->last_launches;
+        }
+        L2B_CUDA(src, cudaMemcpyAsync(lead->h_cand, lead->call_cand, (size_t)nl * K * sizeof(ProbIndex), cudaMemcpyDeviceToHost, st));
+        L2B_CUDA(src, cudaStreamSynchronize(st));
+        L2B_CUDA(src, cudaGetLastError());
+        for (int j = 0; j < nl; ++j) beams[j]->n_appended = pos + t + 1;
+        return L2B_OK;
+    }
+    // the selection after step t, and the page remap: slot j takes its parent's pages [0, np)
+    int select(int t) {
+        struct Cand { float score; int h, r; };
+        const int nl = (int)live.size(), np = (pos + t + 1 + KV_PAGE_ROWS - 1) / KV_PAGE_ROWS;
+        const ProbIndex *hc = lead->h_cand;
+        std::vector<Cand> cand;
+        for (int h = 0; h < nl; ++h)
+            for (int r = 0; r < K; ++r) cand.push_back(Cand{live[h].c + hc[h * K + r].prob, h, r});
+        std::sort(cand.begin(), cand.end(), [](const Cand &a, const Cand &b) {
+            const uint32_t ka = beam_fkey(a.score), kb = beam_fkey(b.score);
+            return ka != kb ? ka > kb : a.h != b.h ? a.h < b.h : a.r < b.r;
+        });
+        std::vector<BeamHyp> next;
+        std::vector<std::vector<void *>> lists;
+        for (int q = 0; q < (int)cand.size() && (int)next.size() < B; ++q) {
+            const Cand &x = cand[q];
+            BeamHyp y;
+            y.toks = live[x.h].toks;
+            y.toks.push_back(hc[x.h * K + x.r].index);
+            y.c = x.score;
+            y.step = t;
+            y.at = q;
+            if (stop && y.toks.back() == 1) {   // BOS: finished when it ranks among the first B, else dropped
+                if (q >= B) continue;
+                y.pages = beam_take(beams[x.h], np);
+                fin.push_back(std::move(y));
+                std::stable_sort(fin.begin(), fin.end(), beam_better);
+                if ((int)fin.size() > B) {
+                    beam_put(kv_pool(src), fin.back().pages);
+                    fin.pop_back();
+                }
+                continue;
+            }
+            y.slot = (int)next.size();
+            lists.push_back(beam_take(beams[x.h], np));
+            next.push_back(std::move(y));
+        }
+        for (int j = 0; j < B; ++j) beam_assign(beams[j], j < (int)lists.size() ? lists[j] : std::vector<void *>(), pos + t + 1);
+        live = std::move(next);
+        return upload_all();
+    }
+    int run(int n_steps) {
+        const int np0 = (pos + KV_PAGE_ROWS - 1) / KV_PAGE_ROWS;
+        for (int i = 0; i < B; ++i) beam_assign(beams[i], beam_take(src, np0), pos);
+        int rc = upload_all();
+        if (rc) return rc;
+        live.assign(1, BeamHyp());
+        const int T = std::min(n_steps, src->cfg.seq_len - pos);
+        for (int t = 0; t < T; ++t) {
+            if ((rc = step(t)) || (rc = select(t))) return rc;
+            ran = t + 1;
+            if (stop && (int)fin.size() == B) {
+                const BeamHyp &w = fin.back();
+                if (w.c / (float)w.toks.size() >= live[0].c / (float)(t + 1)) break;
+            }
+        }
+        return L2B_OK;
+    }
+    // beams[i] take the best B of fin and live; every other reference goes back
+    int finish(int n_steps, int32_t *out_tokens, int32_t *out_len, float *out_logprob) {
+        std::vector<BeamHyp> all = std::move(fin);
+        fin.clear();
+        for (BeamHyp &h : live) all.push_back(std::move(h));
+        std::stable_sort(all.begin(), all.end(), beam_better);
+        const int np = (pos + ran + KV_PAGE_ROWS - 1) / KV_PAGE_ROWS;
+        std::vector<std::vector<void *>> lists(B);
+        for (int i = 0; i < B; ++i) {
+            if (all[i].slot >= 0) lists[i] = beam_take(beams[all[i].slot], np);
+            else lists[i].swap(all[i].pages);
+        }
+        for (BeamHyp &h : all) beam_put(kv_pool(src), h.pages);
+        for (int i = 0; i < B; ++i) {
+            const BeamHyp &h = all[i];
+            beam_assign(beams[i], lists[i], pos + (int)h.toks.size());
+            std::copy(h.toks.begin(), h.toks.end(), out_tokens + (size_t)i * n_steps);
+            out_len[i] = (int)h.toks.size();
+            out_logprob[i] = h.c;
+        }
+        return upload_all();
+    }
+    // after a failure: every beam holds nothing and has 0 positions appended; src was never written
+    void abandon() {
+        for (int i = 0; i < B; ++i) {
+            beam_assign(beams[i], std::vector<void *>(), 0);
+            kv_tab_upload(beams[i]);
+        }
+        for (BeamHyp &h : fin) beam_put(kv_pool(src), h.pages);
+        fin.clear();
+        live.clear();
+    }
+};
+
+int32_t l2b_beam_search(l2b_ctx *src, int32_t token, int32_t pos, l2b_ctx *const *beams, int32_t n_beams,
+                        int32_t n_steps, int32_t stop_on_bos, int32_t *out_tokens, int32_t *out_len,
+                        float *out_logprob, int32_t *n_run) {
+    if (!src) { g_create_error = "src is NULL"; return L2B_ERR_INVALID_ARG; }
+    if (!beams || !out_tokens || !out_len || !out_logprob)
+        return fail(src, L2B_ERR_INVALID_ARG, "beams, out_tokens, out_len or out_logprob is NULL");
+    const int V = src->cfg.vocab_size;
+    if (n_beams < 1 || n_beams > L2B_BEAM_MAX || 2 * n_beams > V)
+        return fail(src, L2B_ERR_INVALID_ARG, "n_beams outside [1, L2B_BEAM_MAX], or 2 * n_beams > vocab_size");
+    std::set<const l2b_ctx *> seen;
+    for (int i = 0; i < n_beams; ++i) {
+        const l2b_ctx *b = beams[i];
+        if (!b) return fail(src, L2B_ERR_INVALID_ARG, "NULL beam");
+        if (b == src) return fail(src, L2B_ERR_INVALID_ARG, "src among the beams");
+        if (!seen.insert(b).second) return fail(src, L2B_ERR_INVALID_ARG, "the same beam twice");
+        if (b->weights != src->weights) return fail(src, L2B_ERR_INVALID_ARG, "a beam of another model");
+    }
+    if (token < 0 || token >= V) return fail(src, L2B_ERR_INVALID_ARG, "token out of range");
+    if (pos < 0 || pos >= src->cfg.seq_len) return fail(src, L2B_ERR_INVALID_ARG, "pos out of range");
+    if (n_steps < 0) return fail(src, L2B_ERR_INVALID_ARG, "n_steps < 0");
+    if (pos > src->n_appended) return fail(src, L2B_ERR_STATE, "pos past the positions src has appended");
+    if (!src->paged)
+        return fail(src, L2B_ERR_UNSUPPORTED,
+                    "l2b_beam_search needs a paged model (L2B_KV_PAGED): on a contiguous cache each step's reorder "
+                    "would copy O(pos) rows per beam");
+    src->last_ms = 0.0f;
+    src->last_launches = 0;
+    if (n_run) *n_run = 0;
+    if (n_steps == 0) {
+        for (int i = 0; i < n_beams; ++i) { out_len[i] = 0; out_logprob[i] = 0.0f; }
+        return L2B_OK;
+    }
+    l2b_ctx *lead = beams[0];
+    L2B_CUDA(src, cudaSetDevice(src->device));
+    int rc = pf_prepare(lead);
+    if (!rc) rc = call_buf_reserve(lead, lead->call_ints, lead->call_ints_cap, (size_t)n_beams);
+    if (!rc) rc = call_buf_reserve(lead, lead->call_cand, lead->call_cand_cap, (size_t)n_beams * 2 * n_beams);
+    if (rc) { src->err = lead->err; return rc; }
+    fill_ctl(lead, token, pos, 0, 1.0f, -1.0f);   // CTL_DONE = 0 for the batched kernels and the top-k kernel
+    L2B_CUDA(src, cudaMemcpyAsync(lead->ctl, lead->h_ctl, CTL_HOST_WORDS * sizeof(int), cudaMemcpyHostToDevice, lead->stream));
+    L2B_CUDA(src, cudaEventRecord(src->ev0, lead->stream));
+    BeamSearch bs{src, lead, beams, n_beams, 2 * n_beams, pos, token, stop_on_bos != 0};
+    rc = bs.run(n_steps);
+    if (!rc) rc = bs.finish(n_steps, out_tokens, out_len, out_logprob);
+    if (rc) {
+        bs.abandon();
+        return rc;
+    }
+    L2B_CUDA(src, cudaEventRecord(src->ev1, lead->stream));
+    L2B_CUDA(src, cudaEventSynchronize(src->ev1));
+    L2B_CUDA(src, cudaEventElapsedTime(&src->last_ms, src->ev0, src->ev1));
+    src->last_launches = bs.launches;
+    if (n_run) *n_run = bs.ran;
+    return L2B_OK;
+}
+
 int32_t l2b_read_state(l2b_ctx *ctx, int32_t which, float *dst, uint64_t n, uint64_t *n_out) {
     if (!ctx || !dst) return L2B_ERR_INVALID_ARG;
     const void *src = nullptr;
@@ -3924,6 +4185,22 @@ int32_t l2b_op_logprob(int32_t device, const float *logits, int32_t n, int32_t t
     LogprobBatchParams p{ctl, dl, n, dt, amax, dlp, dg};
     logprob_batch_kernel<<<1, LOGPROB_THREADS>>>(p);
     s.down(logprob, dlp, 1);
+    return s.rc;
+}
+
+// the k best log softmax(logits)[i] alone (logprob_topk_batch_kernel, one row): unit-test surface
+int32_t l2b_op_logprob_topk(int32_t device, const float *logits, int32_t n, int32_t k, l2b_prob_index *out) {
+    if (!logits || !out || n < 1 || k < 1 || k > n || k > 2 * L2B_BEAM_MAX) return L2B_ERR_INVALID_ARG;
+    static_assert(2 * L2B_BEAM_MAX == TOPK_MAX, "the top-k kernel keeps 2 * L2B_BEAM_MAX keys per thread");
+    static_assert(sizeof(l2b_prob_index) == sizeof(ProbIndex), "candidate layout");
+    OpScope s(device);
+    float *dl = s.up(logits, n), *dout = s.up(nullptr, (size_t)2 * k);
+    int *ctl = (int *)s.up(nullptr, CTL_WORDS);
+    if (s.rc) return s.rc;
+    cudaMemset(ctl, 0, CTL_WORDS * sizeof(int));
+    LogprobTopkParams p{ctl, dl, n, n, k, reinterpret_cast<ProbIndex *>(dout)};
+    logprob_topk_batch_kernel<<<1, LOGPROB_THREADS>>>(p);
+    s.down(reinterpret_cast<float *>(out), dout, (size_t)2 * k);
     return s.rc;
 }
 

@@ -34,7 +34,9 @@ static const char *usage_text =
     "     --q8                  keep the matrix weights (and the draft's) as int8 with one scale per 64 weights: 0.53x\n"
     "                           the bf16 bytes per step; outputs equal an fp32 run of the dequantized checkpoint (1 GPU)\n"
     "     --kv-bf16             keep the KV cache (and the draft's) in bf16 on the GPU: half the cache memory and\n"
-    "                           attention bytes; outputs equal an fp32-cache run that rounds each K/V value (1 GPU)\n";
+    "                           attention bytes; outputs equal an fp32-cache run that rounds each K/V value (1 GPU)\n"
+    "     --beam <int>          beam search with that many hypotheses (at most 8) on a paged KV cache; prints the\n"
+    "                           best one; -t and -p are ignored, -v prints every result's normalised score (1 GPU)\n";
 
 // -v: the KV-cache format and bytes of a context (l2b_kv_info)
 static void print_kv_info(const char *what, const l2b_ctx *ctx) {
@@ -84,11 +86,58 @@ static int generate_with_draft(l2b_ctx *ctx, const l2b_config &c, l2b_ctx *draft
     return L2B_OK;
 }
 
+// Beam search (--beam N): the prompt is prefilled as above, then l2b_beam_search runs N hypotheses on N
+// sessions of the paged model to the step limit, and the best one is printed.  -t and -p play no part.
+static int generate_beam(l2b_ctx *ctx, const l2b_config &c, int n_beams, const l2h_gen_options &opt,
+                         const std::vector<int32_t> &prompt, const l2h_tokenizer *tk, bool verbose) {
+    int seq_len = opt.n_steps == 0 ? c.seq_len : opt.n_steps;   // :992-993
+    seq_len = seq_len < 1 ? 1 : seq_len > c.seq_len ? c.seq_len : seq_len;
+    const int n_prompt = (int)prompt.size() < seq_len ? (int)prompt.size() : seq_len;
+    int32_t token = 1, rc = L2B_OK;                             // :988 BOS
+    if (n_prompt > 0 && n_prompt < seq_len) {
+        std::vector<int32_t> toks(1, token);
+        toks.insert(toks.end(), prompt.begin(), prompt.begin() + n_prompt - 1);
+        if ((rc = l2b_prefill(ctx, toks.data(), n_prompt, 0, nullptr))) return rc;
+    }
+    for (int i = 0; i < n_prompt; ++i) { l2h_print_token(tk, token, prompt[i]); token = prompt[i]; }
+    if (n_prompt == seq_len) return L2B_OK;
+    const int n_steps = seq_len - n_prompt;
+    std::vector<l2b_ctx *> beams;
+    for (int i = 0; i < n_beams && rc == L2B_OK; ++i) {
+        l2b_ctx *s = nullptr;
+        rc = l2b_create_session(&s, ctx);
+        if (s) beams.push_back(s);
+    }
+    std::vector<int32_t> out((size_t)n_beams * n_steps), len(n_beams);
+    std::vector<float> lp(n_beams);
+    int32_t ran = 0;
+    const auto t0 = std::chrono::steady_clock::now();
+    if (rc == L2B_OK)
+        rc = l2b_beam_search(ctx, token, n_prompt, beams.data(), n_beams, n_steps, opt.stop_on_bos, out.data(),
+                             len.data(), lp.data(), &ran);
+    const double secs = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+    for (l2b_ctx *s : beams) l2b_destroy(s);
+    if (rc) return rc;
+    for (int i = 0; i < len[0]; ++i) {
+        if (opt.stop_on_bos && out[i] == 1) break;              // :1017-1019
+        l2h_print_token(tk, token, out[i]);
+        token = out[i];
+    }
+    fflush(stdout);
+    if (verbose) {
+        fprintf(stderr, "\n\n%d steps of %d beams in %.3f s\n", ran, n_beams, secs);
+        for (int i = 0; i < n_beams; ++i)
+            fprintf(stderr, "result %d: %d tokens, log-probability %g, normalised score %g\n", i, len[i], lp[i],
+                    len[i] ? lp[i] / (float)len[i] : 0.0f);
+    }
+    return L2B_OK;
+}
+
 int main(int argc, char **argv) {
     if (argc < 2) { fputs(usage_text, stdout); return 0; }
     const char *bin_path = nullptr, *input = nullptr, *tokenizer_path = "tokenizer.bin";
     l2h_gen_options opt{1.0f, 0.9f, 0, 1, 0, 0, 0};
-    int n_gpus = 1, draft_k = 3;
+    int n_gpus = 1, draft_k = 3, n_beams = 0;
     const char *draft_path = nullptr;
     bool verbose = false;
     int32_t weight_format = L2B_WEIGHTS_F32, kv_flag = 0;
@@ -119,9 +168,14 @@ int main(int argc, char **argv) {
         else if (a == "--bf16") weight_format = L2B_WEIGHTS_BF16;
         else if (a == "--q8") weight_format = L2B_WEIGHTS_Q8;
         else if (a == "--kv-bf16") kv_flag = L2B_KV_BF16;
+        else if (a == "--beam") n_beams = atoi(need("beam"));
         else { fprintf(stderr, "error: unknown argument '%s'\n", argv[i]); fputs(usage_text, stdout); return 0; }
     }
     if (!bin_path) { fputs(usage_text, stdout); return 0; }
+    if (n_beams && (n_beams < 1 || n_beams > L2B_BEAM_MAX || n_gpus != 1 || draft_path)) {
+        fprintf(stderr, "error: --beam takes 1 to %d beams on one GPU, without --draft\n", L2B_BEAM_MAX);
+        return 1;
+    }
 
     l2h_checkpoint ck;
     if (l2h_load_checkpoint(bin_path, &ck) != L2B_OK) { fprintf(stderr, "error: cannot read checkpoint %s\n", bin_path); return 1; }
@@ -132,7 +186,8 @@ int main(int argc, char **argv) {
         fprintf(stderr, "shared weights: %s\ntemperature: %g\ntop-p: %g\n\n", c.shared_weights ? "true" : "false", opt.temperature, opt.top_p);
     }
     l2b_ctx *ctx = nullptr;
-    int32_t rc = l2b_create_format(&ctx, &c, ck.data, ck.n_floats, nullptr, nullptr, n_gpus, weight_format | kv_flag);   // after :967
+    const int32_t layout = n_beams ? L2B_KV_PAGED : 0;          // beam search needs the paged KV cache
+    int32_t rc = l2b_create_format(&ctx, &c, ck.data, ck.n_floats, nullptr, nullptr, n_gpus, weight_format | kv_flag | layout);   // after :967
     if (rc) { fprintf(stderr, "error: l2b_create: %s (%s)\n", l2b_status_string(rc), l2b_last_error(nullptr)); return 1; }
     if (verbose) {
         int32_t fmt = 0;
@@ -170,7 +225,10 @@ int main(int argc, char **argv) {
         if (n < 0) { fprintf(stderr, "error: cannot encode prompt\n"); return 1; }
         prompt.resize(n);
     }
-    if (draft) {
+    if (n_beams) {
+        rc = generate_beam(ctx, c, n_beams, opt, prompt, tk, verbose);
+        if (rc) { fprintf(stderr, "\nerror: %s (%s)\n", l2b_status_string(rc), l2b_last_error(ctx)); return 1; }
+    } else if (draft) {
         rc = generate_with_draft(ctx, c, draft, dc, draft_k, opt, prompt, tk, verbose);
         if (rc) { fprintf(stderr, "\nerror: %s (%s / %s)\n", l2b_status_string(rc), l2b_last_error(ctx), l2b_last_error(draft)); return 1; }
     } else {
