@@ -640,8 +640,9 @@ int32_t l2b_round_q8_host(float *data, uint64_t rows, uint64_t cols, uint64_t *n
  * fp32 cache's memory and bytes and the bf16 cache's accuracy.  Or'd in like L2B_KV_BF16, with the same
  * checks; both flags together => L2B_ERR_INVALID_ARG.                                                  */
 #define L2B_KV_ROUND_BF16 0x200
-/* The KV format of ctx (0: fp32, L2B_KV_BF16, L2B_KV_ROUND_BF16) and the bytes of its key and value caches
- * together: 2 * n_layers * seq_len * kv_dim * (2 for L2B_KV_BF16, else 4).  l2b_weight_info reports the
+/* The KV format of ctx (0: fp32, L2B_KV_BF16, L2B_KV_ROUND_BF16, L2B_KV_E4M3, L2B_KV_ROUND_E4M3) and the
+ * bytes of its key and value caches together: 2 * n_layers * seq_len * kv_dim * (2 for L2B_KV_BF16, 1 for
+ * L2B_KV_E4M3, else 4).  l2b_weight_info reports the
  * weight format alone.  A paged context (below) reports the element format alone, and as cache bytes the
  * pages it references times page_bytes: a page shared by several sessions counts in each of them
  * (l2b_kv_pool_info gives the true total).                                                             */
@@ -684,6 +685,38 @@ int32_t l2b_kv_pool_info(const l2b_ctx *ctx, int32_t *page_rows, uint64_t *page_
  * L2B_ERR_OOM and changes no session.  A cap below the pages in use => L2B_ERR_INVALID_ARG; a contiguous
  * model => L2B_ERR_UNSUPPORTED; NULL ctx => L2B_ERR_INVALID_ARG.                                       */
 int32_t l2b_kv_pool_limit(l2b_ctx *ctx, uint64_t max_pages);
+
+/* ---- fp8 (e4m3) KV cache ----------------------------------------------------------------------
+ * L2B_KV_E4M3, or'd into the weight_format of l2b_create_format / l2b_create_synthetic_format (with any
+ * weight format, with or without L2B_KV_PAGED), keeps the caches in OCP FP8 E4M3 ("e4m3fn": bias 7, no
+ * infinities, largest finite +-448, NaN S.1111.111): a quarter of the fp32 cache's memory and bytes, half
+ * the bf16 cache's.  Any two of L2B_KV_BF16, L2B_KV_ROUND_BF16, L2B_KV_E4M3 and L2B_KV_ROUND_E4M3 together
+ * => L2B_ERR_INVALID_ARG; n_gpus > 1 => L2B_ERR_UNSUPPORTED; both checked before any device is touched.
+ * Scales: each layer l has one fp32 scale for K, s_k[l], and one for V, s_v[l] (l2b_kv_scales; 1 by
+ * default).  An appended value v (K after RoPE, or V) with its layer's scale s is stored as the code
+ * c = e4m3(fl(v / s)): IEEE division, then the nearest e4m3 value, ties to even, subnormals rounded, the
+ * sign of zero kept, finite values past 448 and +-inf to +-448 (saturating), NaN to NaN.  Attention reads
+ * fl((float)c * s) for each element; q, scores, softmax, partials and all run state stay fp32.
+ * Contract: an e4m3-KV context returns, on every entry point, exactly what an L2B_KV_ROUND_E4M3 context of
+ * the same payload, weight format, layout and scales returns (the outputs listed under L2B_KV_BF16, and
+ * l2b_beam_search's).  Each e4m3 kernel is the fp32 kernel the same shape selects.  l2b_read_state(4 / 5)
+ * returns the caches widened with the scales (fl((float)c * s)); l2b_kv_info's cache bytes,
+ * l2b_step_bytes' kv_bytes, the attention / attn_wo bytes of l2b_profile_step and l2b_kv_pool_info's
+ * page_bytes count 1 byte per stored element.                                                         */
+#define L2B_KV_E4M3 0x1000
+/* The reference of that contract, for tests: an fp32 cache that stores fl((float)e4m3(fl(v / s)) * s) for
+ * every appended value and is read by the fp32 kernels.  Not a format to serve with.                   */
+#define L2B_KV_ROUND_E4M3 0x2000
+/* Sets the KV scales of ctx's model: scales[2l] = s_k[l], scales[2l + 1] = s_v[l], n == 2 * n_layers.  They
+ * live in the model's device memory; sessions created afterwards use them too.  Every refusal leaves the
+ * scales unchanged: NULL ctx or scales, a wrong n, or a scale that is not a finite positive normal float
+ * => L2B_ERR_INVALID_ARG; a model whose KV format is neither e4m3 flag => L2B_ERR_UNSUPPORTED; a model
+ * with a live session, or with positions appended (rows stored under the old scales would be misread),
+ * => L2B_ERR_STATE.                                                                                   */
+int32_t l2b_kv_scales(l2b_ctx *ctx, const float *scales, int32_t n);
+/* In place, the value an e4m3 cache element stands for: v -> fl((float)e4m3(fl(v / scale)) * scale), the
+ * rounding above.  NULL data does nothing.                                                             */
+void l2b_round_e4m3_host(float *data, uint64_t n, float scale);
 
 #ifdef __cplusplus
 }

@@ -27,10 +27,14 @@ from .binding import (  # noqa: F401
     synth_checkpoint_host,
     round_bf16_host,
     round_q8_host,
+    round_e4m3_host,
     Q8_GROUP,
     KV_BF16,
     KV_ROUND_BF16,
     KV_FORMATS,
+    KV_E4M3,
+    KV_ROUND_E4M3,
+    KV_E4M3_FORMATS,
     KV_PAGED,
     KV_PAGE_ROWS,
     BEAM_MAX,
@@ -59,7 +63,7 @@ from .checkpoint import Checkpoint, read_checkpoint, MODEL_SHAPES  # noqa: F401
 
 __all__ = [
     "L2BError", "L2BConfig", "L2BShard", "Transformer", "checkpoint_floats", "comm_unique_id",
-    "lib_path", "load_library", "matmul", "rmsnorm", "softmax", "synth_checkpoint_host", "round_bf16_host", "round_q8_host", "Q8_GROUP", "WEIGHT_FORMATS", "QUANT_FORMATS", "KV_BF16", "KV_ROUND_BF16", "KV_FORMATS", "KV_PAGED", "KV_PAGE_ROWS", "BEAM_MAX",
+    "lib_path", "load_library", "matmul", "rmsnorm", "softmax", "synth_checkpoint_host", "round_bf16_host", "round_q8_host", "round_e4m3_host", "Q8_GROUP", "WEIGHT_FORMATS", "QUANT_FORMATS", "KV_BF16", "KV_ROUND_BF16", "KV_FORMATS", "KV_E4M3", "KV_ROUND_E4M3", "KV_E4M3_FORMATS", "KV_PAGED", "KV_PAGE_ROWS", "BEAM_MAX",
     "vector_weighted_sum_rows", "attention_head", "fused_matmul", "sample_prep", "logprob", "logprob_topk", "exported_symbols", "forward_batch", "forward_argmax_batch", "forward_sample_batch", "generate_argmax_batch", "forward_ragged", "forward_argmax_ragged", "forward_sample_ragged", "fork", "beam_search", "verify_argmax_ragged", "verify_sample_ragged", "Checkpoint",
     "read_checkpoint", "MODEL_SHAPES",
 ]

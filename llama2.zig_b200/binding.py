@@ -147,6 +147,9 @@ def load_library():
     lib.l2b_round_bf16_host.argtypes = [FP, C.c_uint64]
     lib.l2b_round_bf16_host.restype = None
     lib.l2b_round_q8_host.argtypes = [FP, C.c_uint64, C.c_uint64, U64P]
+    lib.l2b_kv_scales.argtypes = [vp, FP, C.c_int32]
+    lib.l2b_round_e4m3_host.argtypes = [FP, C.c_uint64, C.c_float]
+    lib.l2b_round_e4m3_host.restype = None
     _lib = lib
     return lib
 
@@ -186,6 +189,10 @@ Q8_GROUP = 64   # L2B_Q8_GROUP
 KV_BF16 = 0x100                          # L2B_KV_BF16: or'd into the weight format of l2b_create_format
 KV_ROUND_BF16 = 0x200                    # L2B_KV_ROUND_BF16: fp32 cache of bf16-rounded values (the reference)
 KV_FORMATS = {"f32": 0, "bf16": KV_BF16, "f32-round-bf16": KV_ROUND_BF16}   # l2b_kv_info's kv_format
+KV_E4M3 = 0x1000                         # L2B_KV_E4M3: the fp8 (e4m3) cache, one scale per layer for K and for V
+KV_ROUND_E4M3 = 0x2000                   # L2B_KV_ROUND_E4M3: fp32 cache of e4m3-rounded values (the reference)
+KV_E4M3_FORMATS = {"e4m3": KV_E4M3, "f32-round-e4m3": KV_ROUND_E4M3}   # l2b_kv_info's kv_format, scaled
+_KV_ALL = {**KV_FORMATS, **KV_E4M3_FORMATS}
 KV_PAGED = 0x800                         # L2B_KV_PAGED: or'd in like the KV formats; the paged layout
 KV_PAGE_ROWS = 64                        # L2B_KV_PAGE_ROWS: positions per page
 _KV_LAYOUTS = {"contiguous": 0, "paged": KV_PAGED}
@@ -213,6 +220,16 @@ def round_q8_host(a):
     return n.value
 
 
+def round_e4m3_host(a, scale=1.0):
+    """In place on a C-contiguous float32 array: each value v -> fl(e4m3(fl(v / scale)) * scale), the value
+    an e4m3 cache element stands for (l2b_round_e4m3_host: nearest even, satfinite to +-448, NaN kept).
+    Returns a."""
+    if not (isinstance(a, np.ndarray) and a.dtype == np.float32 and a.flags["C_CONTIGUOUS"]):
+        raise TypeError("round_e4m3_host needs a C-contiguous float32 array")
+    load_library().l2b_round_e4m3_host(a.ctypes.data_as(FP), a.size, float(scale))
+    return a
+
+
 def synth_checkpoint_host(ck, seed):
     """Host copy of the synthetic payload l2b_create_synthetic puts on the device."""
     lib = load_library()
@@ -233,8 +250,9 @@ class Transformer:
     (l2b_create / l2b_create_sharded); with `synthetic_seed` the weights are generated on the
     device (l2b_create_synthetic).  weight_format="bf16" keeps the matrix weights in bf16 on the
     device, "q8" as int8 with one fp32 scale per 64 weights of a row; kv_format="bf16" keeps the KV
-    cache in bf16, "f32-round-bf16" in fp32 holding bf16-rounded values, the bf16 cache's bitwise reference
-    (l2b_create_format / l2b_create_synthetic_format; single GPU, device 0).  kv_layout="paged" keeps
+    cache in bf16, "f32-round-bf16" in fp32 holding bf16-rounded values, the bf16 cache's bitwise reference,
+    "e4m3" in fp8 e4m3 with one scale per layer for K and one for V (set_kv_scales), "f32-round-e4m3" its
+    fp32 reference (l2b_create_format / l2b_create_synthetic_format; single GPU, device 0).  kv_layout="paged" keeps
     the caches of the model's contexts and sessions in pages of KV_PAGE_ROWS positions from one pool
     (single GPU, device 0; fork shares a prompt's pages).  Sessions take the model's formats and layout.
     """
@@ -246,11 +264,11 @@ class Transformer:
         one process per GPU (l2b_create_sharded)."""
         if weight_format not in _FORMATS:
             raise ValueError(f"weight_format must be one of {sorted(_FORMATS)}")
-        if kv_format not in KV_FORMATS:
-            raise ValueError(f"kv_format must be one of {sorted(KV_FORMATS)}")
+        if kv_format not in _KV_ALL:
+            raise ValueError(f"kv_format must be one of {sorted(_KV_ALL)}")
         if kv_layout not in _KV_LAYOUTS:
             raise ValueError(f"kv_layout must be one of {sorted(_KV_LAYOUTS)}")
-        fmt = _FORMATS[weight_format] | KV_FORMATS[kv_format] | _KV_LAYOUTS[kv_layout]
+        fmt = _FORMATS[weight_format] | _KV_ALL[kv_format] | _KV_LAYOUTS[kv_layout]
         if fmt and (world_size > 1 or device != 0 or rank != 0 or n_gpus != 1):
             raise ValueError(f"{weight_format} weights with a {kv_format} {kv_layout} KV cache are single-GPU on device 0")
         self.lib = load_library()
@@ -397,12 +415,20 @@ class Transformer:
         return {v: k for k, v in _FORMATS.items()}[fmt.value], n.value
 
     def kv_info(self):
-        """(kv_format name, cache_bytes): the format of this context's KV cache (a KV_FORMATS key) and the
-        bytes of its key and value caches together (l2b_kv_info)."""
+        """(kv_format name, cache_bytes): the format of this context's KV cache (a KV_FORMATS or
+        KV_E4M3_FORMATS key) and the bytes of its key and value caches together (l2b_kv_info)."""
         fmt = C.c_int32()
         n = C.c_uint64()
         _check(self.lib.l2b_kv_info(self.h, C.byref(fmt), C.byref(n)), self.h)
-        return {v: k for k, v in KV_FORMATS.items()}[fmt.value], n.value
+        return {v: k for k, v in _KV_ALL.items()}[fmt.value], n.value
+
+    def set_kv_scales(self, scales):
+        """Sets the e4m3 KV scales of this model (l2b_kv_scales): scales is (n_layers, 2) floats, row l =
+        (s_k[l], s_v[l]).  Only before any session exists and any position is appended."""
+        s = np.ascontiguousarray(scales, dtype=np.float32)
+        if s.shape != (self.ck.n_layers, 2):
+            raise ValueError(f"scales must have shape ({self.ck.n_layers}, 2)")
+        _check(self.lib.l2b_kv_scales(self.h, s.ctypes.data_as(FP), s.size), self.h)
 
     def kv_pool_info(self):
         """The KV page pool of this context's model (l2b_kv_pool_info): page_rows, page_bytes,

@@ -254,24 +254,105 @@ __device__ __forceinline__ float4 widen_bf16x4(uint2 u) {
                        __uint_as_float(u.y << 16), __uint_as_float(u.y & 0xFFFF0000u));
 }
 
+// The OCP e4m3 ("e4m3fn") code of fl(v / s): nearest on the e4m3 grid, ties to even; subnormals are
+// rounded (not flushed); the sign of zero stays; finite values past 448 and +-inf become +-448 (the
+// satfinite rule of PTX cvt.rn.satfinite.e4m3x2.f32); NaN stays NaN (S.1111.111).  The one e4m3 rounding
+// of the library: the cache writers, the L2B_KV_ROUND_E4M3 reference and l2b_round_e4m3_host all use it.
+__host__ __device__ __forceinline__ uint8_t e4m3_round_bits(float v, float s) {
+#ifdef __CUDA_ARCH__
+    const uint32_t u = __float_as_uint(__fdiv_rn(v, s));
+#else
+    const float x = v / s;
+    uint32_t u;
+    memcpy(&u, &x, 4);
+#endif
+    const uint32_t sign = (u >> 24) & 0x80u, a = u & 0x7FFFFFFFu;
+    if (a > 0x7F800000u) return (uint8_t)(sign | 0x7Fu);                // NaN
+    if (a >= 0x43E00000u) return (uint8_t)(sign | 0x7Eu);               // |u| >= 448, inf included
+    if (a >= 0x3C800000u)                                               // normal: |u| >= 2^-6
+        return (uint8_t)(sign | (((a + 0x7FFFFu + ((a >> 20) & 1u)) >> 20) - 0x3C0u));
+    // subnormal: round(|u| * 2^9) to an integer 0..8 (8 is 2^-6, the smallest normal code)
+    const int e = (int)(a >> 23);
+    const uint32_t m = e ? (a & 0x7FFFFFu) | 0x800000u : a;              // |u| = m * 2^(max(e,1) - 150)
+    const int sh = 141 - (e ? e : 1);                                   // |u| * 2^9 = m / 2^sh, sh >= 21
+    if (sh >= 25) return (uint8_t)sign;                                 // below 2^-10: rounds to 0
+    uint32_t q = m >> sh;
+    const uint32_t rem = m & ((1u << sh) - 1u), half = 1u << (sh - 1);
+    q += (rem > half || (rem == half && (q & 1u))) ? 1u : 0u;
+    return (uint8_t)(sign | q);
+}
+// (float)c, exact: +-m * 2^-9 (exponent field 0) or +-(1 + m/8) * 2^(e-7), NaN for S.1111.111
+__host__ __device__ __forceinline__ float e4m3_to_float(uint8_t c) {
+    const uint32_t e = (c >> 3) & 0xFu, m = c & 7u;
+    float f;
+    if ((c & 0x7Fu) == 0x7Fu) {
+        f = NAN;
+    } else if (e) {
+        const uint32_t u = ((e + 120u) << 23) | (m << 20);
+#ifdef __CUDA_ARCH__
+        f = __uint_as_float(u);
+#else
+        memcpy(&f, &u, 4);
+#endif
+    } else {
+        f = (float)m * 0.001953125f;                                     // m * 2^-9, exact
+    }
+    return (c & 0x80u) ? -f : f;
+}
+// the value a cache element with code c stands for under scale s: fl((float)c * s)
+__host__ __device__ __forceinline__ float e4m3_widen(uint8_t c, float s) {
+#ifdef __CUDA_ARCH__
+    return __fmul_rn(e4m3_to_float(c), s);
+#else
+    return e4m3_to_float(c) * s;
+#endif
+}
+// four codes of a 32-bit word (code 0 in the low byte), widened exactly through f16 and scaled by s
+__device__ __forceinline__ float4 widen_e4m3x4(uint32_t u, float s) {
+    uint32_t lo, hi;
+    asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(lo) : "h"((unsigned short)(u & 0xFFFFu)));
+    asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(hi) : "h"((unsigned short)(u >> 16)));
+    float f0, f1, f2, f3;
+    asm("cvt.f32.f16 %0, %1;" : "=f"(f0) : "h"((unsigned short)(lo & 0xFFFFu)));
+    asm("cvt.f32.f16 %0, %1;" : "=f"(f1) : "h"((unsigned short)(lo >> 16)));
+    asm("cvt.f32.f16 %0, %1;" : "=f"(f2) : "h"((unsigned short)(hi & 0xFFFFu)));
+    asm("cvt.f32.f16 %0, %1;" : "=f"(f3) : "h"((unsigned short)(hi >> 16)));
+    return make_float4(__fmul_rn(f0, s), __fmul_rn(f1, s), __fmul_rn(f2, s), __fmul_rn(f3, s));
+}
+
 // ---- KV-cache element types.  KV is a template parameter of every kernel that writes or reads the cache:
 //   float       the fp32 cache;
 //   bf16        the bf16 cache (L2B_KV_BF16): each appended value rounded by bf16_round_bits, widened on load;
 //   kv_f32_bf16 an fp32 cache whose appended values are rounded to bf16 and stored widened (the
 //               L2B_KV_ROUND_BF16 reference).  Only the writers have it; its readers are the fp32 kernels.
+//   e4m3        the e4m3 cache (L2B_KV_E4M3): each appended value v stored as e4m3_round_bits(v, s) with its
+//               layer's scale s (s_k for K, s_v for V), read as e4m3_widen(code, s);
+//   kv_f32_e4m3 an fp32 cache holding e4m3_widen(e4m3_round_bits(v, s), s) (the L2B_KV_ROUND_E4M3
+//               reference), writers only like kv_f32_bf16.
+// The e4m3 kernels take the layer's scale pair (s_k, s_v) through GemvParams / AttnParams::kv_scale.
 struct kv_f32_bf16 { float v; };
+struct e4m3 { uint8_t c; };
+struct kv_f32_e4m3 { float v; };
 template <typename KV>
-__device__ __forceinline__ float kv_value(float x) {
-    return std::is_same<KV, float>::value ? x : __uint_as_float((uint32_t)bf16_round_bits(__float_as_uint(x)) << 16);
+constexpr bool kv_is_e4m3 = std::is_same<KV, e4m3>::value || std::is_same<KV, kv_f32_e4m3>::value;
+// the value an appended x stands for in a KV cache (s: the layer's scale, e4m3 only)
+template <typename KV>
+__device__ __forceinline__ float kv_value(float x, float s = 1.0f) {
+    if constexpr (std::is_same<KV, float>::value) return x;
+    else if constexpr (kv_is_e4m3<KV>) return e4m3_widen(e4m3_round_bits(x, s), s);
+    else return __uint_as_float((uint32_t)bf16_round_bits(__float_as_uint(x)) << 16);
 }
-// the cache pair (dst[0], dst[1]) = (a0, a1) as KV elements: one 64-bit store (fp32) or one 32-bit store (bf16)
+// the cache pair (dst[0], dst[1]) = (a0, a1) as KV elements: one 64-bit store (fp32), one 32-bit store
+// (bf16) or one 16-bit store (e4m3)
 template <typename KV>
-__device__ __forceinline__ void kv_store2(KV *dst, float a0, float a1) {
-    if constexpr (sizeof(KV) == 2)
+__device__ __forceinline__ void kv_store2(KV *dst, float a0, float a1, float s = 1.0f) {
+    if constexpr (sizeof(KV) == 1)
+        *reinterpret_cast<uint16_t *>(dst) = (uint16_t)(e4m3_round_bits(a0, s) | ((uint32_t)e4m3_round_bits(a1, s) << 8));
+    else if constexpr (sizeof(KV) == 2)
         *reinterpret_cast<uint32_t *>(dst) = (uint32_t)bf16_round_bits(__float_as_uint(a0)) |
                                              ((uint32_t)bf16_round_bits(__float_as_uint(a1)) << 16);
     else
-        *reinterpret_cast<float2 *>(dst) = make_float2(kv_value<KV>(a0), kv_value<KV>(a1));
+        *reinterpret_cast<float2 *>(dst) = make_float2(kv_value<KV>(a0, s), kv_value<KV>(a1, s));
 }
 // ---- paged caches (L2B_KV_PAGED).  The kernels' KV type is then kv_paged<E>, E one of the element types
 // above.  A page holds rows [jP, jP+P) of every layer, K and V: [L][K rows P | V rows P][kv_dim] elements E.
@@ -306,16 +387,24 @@ __device__ __forceinline__ void kv_stage_pages(const void *tab, int t0, int t1, 
     __syncthreads();
 }
 // float4 group j (ldg_kv4) or lr + k (ldcg_kv4) of a cache row, through the read-only path (ldg) or L2 only
-// (ldcg), widened exactly
+// (ldcg), widened exactly (e4m3: each element times the scale s, in fp32)
 template <typename KV>
-__device__ __forceinline__ float4 ldcg_kv4(const KV *row, int lr, int k) {
-    if constexpr (sizeof(KV) == 2) return widen_bf16x4(__ldcg(reinterpret_cast<const uint2 *>(row) + lr + k));
+__device__ __forceinline__ float4 ldcg_kv4(const KV *row, int lr, int k, float s = 1.0f) {
+    if constexpr (sizeof(KV) == 1) return widen_e4m3x4(__ldcg(reinterpret_cast<const unsigned int *>(row) + lr + k), s);
+    else if constexpr (sizeof(KV) == 2) return widen_bf16x4(__ldcg(reinterpret_cast<const uint2 *>(row) + lr + k));
     else return __ldcg(reinterpret_cast<const float4 *>(row) + lr + k);
 }
 template <typename KV>
-__device__ __forceinline__ float4 ldg_kv4(const KV *row, int j) {
-    if constexpr (sizeof(KV) == 2) return widen_bf16x4(__ldg(reinterpret_cast<const uint2 *>(row) + j));
+__device__ __forceinline__ float4 ldg_kv4(const KV *row, int j, float s = 1.0f) {
+    if constexpr (sizeof(KV) == 1) return widen_e4m3x4(__ldg(reinterpret_cast<const unsigned int *>(row) + j), s);
+    else if constexpr (sizeof(KV) == 2) return widen_bf16x4(__ldg(reinterpret_cast<const uint2 *>(row) + j));
     else return __ldg(reinterpret_cast<const float4 *>(row) + j);
+}
+// the layer's (s_k, s_v) for the e4m3 kernels; (1, 1), not read, for every other cache
+template <typename KV>
+__device__ __forceinline__ float2 kv_scales(const float *kv_scale) {
+    if constexpr (sizeof(KV) == 1) return make_float2(__ldg(kv_scale), __ldg(kv_scale + 1));
+    else return make_float2(1.0f, 1.0f);
 }
 
 // float4 column group c of a weight row of n columns in global memory (streaming, no L1 allocation;
@@ -476,6 +565,8 @@ struct GemvParams {
     // EPI_QKV of the batched kernels: vector b appends no KV row when skip_b[b] != 0 (a session that has
     // stopped in the batched generation loop), or nullptr: every vector appends
     const int *skip_b;
+    // EPI_QKV on an e4m3 cache (and its fp32 reference): the layer's (s_k, s_v) in the model's device memory
+    const float *kv_scale;
 };
 
 template <int EPI, typename W>
@@ -534,7 +625,13 @@ __device__ __forceinline__ void qkv_store_pair(const GemvParams &p, float *q, vo
         // :348-349, evaluated without FMA contraction like the reference
         const float r0 = __fsub_rn(__fmul_rn(a0, fcr), __fmul_rn(a1, fci));
         const float r1 = __fadd_rn(__fmul_rn(a0, fci), __fmul_rn(a1, fcr));
-        if (sizeof(KV) == 4 || is_q) {                   // 4-byte caches: q and k share one 64-bit store
+        if constexpr (kv_is_e4m3<KV>) {
+            if (is_q) {
+                *reinterpret_cast<float2 *>(q + i) = make_float2(r0, r1);
+            } else {
+                kv_store2(kc + (size_t)pos * p.kv_dim + i, r0, r1, __ldg(p.kv_scale));
+            }
+        } else if (sizeof(KV) == 4 || is_q) {            // 4-byte caches: q and k share one 64-bit store
             float *dst = is_q ? q + i : reinterpret_cast<float *>(kc + (size_t)pos * p.kv_dim + i);   // :355,:357
             *reinterpret_cast<float2 *>(dst) = is_q ? make_float2(r0, r1) : make_float2(kv_value<KV>(r0), kv_value<KV>(r1));
         } else {
@@ -542,7 +639,8 @@ __device__ __forceinline__ void qkv_store_pair(const GemvParams &p, float *q, vo
         }
     } else {
         const int i = v - p.rows0 - p.rows1;
-        kv_store2(vc + (size_t)pos * p.kv_dim + i, a0, a1);  // :356,:358
+        if constexpr (kv_is_e4m3<KV>) kv_store2(vc + (size_t)pos * p.kv_dim + i, a0, a1, __ldg(p.kv_scale + 1));
+        else kv_store2(vc + (size_t)pos * p.kv_dim + i, a0, a1);  // :356,:358
     }
 }
 // the decode step's form: the layer's caches of the launch
@@ -1735,6 +1833,7 @@ struct AttnParams {
     // argument.  batched == 0: one query at the control block's position on kcache / vcache.
     int batched, q_stride;
     int seq_len;           // rows of the cache (bounds the speculative first pass; 0 = no speculation)
+    const float *kv_scale; // e4m3 caches: this layer's (s_k, s_v) in the model's device memory
 };
 
 // Query z of a batched launch: position pos[z] over this layer's caches kcache[z] / vcache[z].  The
@@ -1761,7 +1860,7 @@ __device__ __forceinline__ int attn_lanes_per_row(int hs4) {
 template <typename KVT, typename KV = kv_elem_t<KVT>>
 __device__ __forceinline__ void attn_scores(float *sc, const float *qg, const KV *kbase,
                                             int kv_dim, int head_size, int t0, int t1,
-                                            const void *const *pg = nullptr, size_t hoff = 0) {
+                                            const void *const *pg = nullptr, size_t hoff = 0, float sk = 1.0f) {
     const int hs4 = head_size >> 2;
     const int lpr = attn_lanes_per_row(hs4);
     const int nf = hs4 / lpr;
@@ -1781,7 +1880,7 @@ __device__ __forceinline__ void attn_scores(float *sc, const float *qg, const KV
                 k4 = kbase + (size_t)t * kv_dim;
             for (int f = 0; f < nf; ++f) {
                 const int j = lr + f * lpr;
-                acc = dot4(ldg_kv4(k4, j), __ldg(q4 + j), acc);
+                acc = dot4(ldg_kv4(k4, j, sk), __ldg(q4 + j), acc);
             }
         }
         for (int o = lpr >> 1; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
@@ -1793,7 +1892,7 @@ __device__ __forceinline__ void attn_scores(float *sc, const float *qg, const KV
 template <typename KVT, typename KV = kv_elem_t<KVT>>
 __device__ __forceinline__ void attn_weighted_rows(float *red, const float *w, const KV *vbase,
                                                    int kv_dim, int head_size, int t0, int t1,
-                                                   const void *const *pg = nullptr, size_t hoff = 0) {
+                                                   const void *const *pg = nullptr, size_t hoff = 0, float sv = 1.0f) {
     const int hs4 = head_size >> 2;
     const int G = NT / hs4;
     const int tid = threadIdx.x;
@@ -1807,7 +1906,7 @@ __device__ __forceinline__ void attn_weighted_rows(float *red, const float *w, c
                 v4 = static_cast<const KV *>(pg[t / KV_PAGE_ROWS - t0 / KV_PAGE_ROWS]) + (size_t)(t % KV_PAGE_ROWS + KV_PAGE_ROWS) * kv_dim + hoff;
             else
                 v4 = vbase + (size_t)t * kv_dim;
-            const float4 v = ldg_kv4(v4, c);
+            const float4 v = ldg_kv4(v4, c, sv);
             a.x = fmaf(v.x, wt, a.x); a.y = fmaf(v.y, wt, a.y);
             a.z = fmaf(v.z, wt, a.z); a.w = fmaf(v.w, wt, a.w);
         }
@@ -1852,7 +1951,8 @@ __global__ void __launch_bounds__(NT) attention_kernel(const AttnParams p, const
     // paged: the split's page addresses after sc (chunk rounded up to an even count keeps them aligned)
     const void **pg = reinterpret_cast<const void **>(sc + ((chunk + 1) & ~1));
     if constexpr (kv_traits<KVT>::paged) kv_stage_pages(p.kcache, t0, t1, pg);
-    attn_scores<KVT>(sc, p.q + (size_t)h * hs, static_cast<const KV *>(p.kcache) + hoff, p.kv_dim, hs, t0, t1, pg, hoff);
+    const float2 ks = kv_scales<KV>(p.kv_scale);
+    attn_scores<KVT>(sc, p.q + (size_t)h * hs, static_cast<const KV *>(p.kcache) + hoff, p.kv_dim, hs, t0, t1, pg, hoff, ks.x);
     __syncthreads();
 
     // softmax pieces (:690-705).  Every warp recomputes max and sum over the whole split from
@@ -1868,7 +1968,7 @@ __global__ void __launch_bounds__(NT) attention_kernel(const AttnParams p, const
     for (int i = lane; i < len; i += 32) l += sc[i];
     l = warp_sum(l);
 
-    attn_weighted_rows<KVT>(red, sc, static_cast<const KV *>(p.vcache) + hoff, p.kv_dim, hs, t0, t1, pg, hoff);
+    attn_weighted_rows<KVT>(red, sc, static_cast<const KV *>(p.vcache) + hoff, p.kv_dim, hs, t0, t1, pg, hoff, ks.y);
     __syncthreads();
     float o = 0.0f;
     if (tid < hs) {
@@ -1996,6 +2096,7 @@ __global__ void __launch_bounds__(NT) attention_flash_kernel(const AttnParams p,
     float4 qf[NF], acc[NF], ka[NF], vA[NF], kc[NF], vC[NF];
     const int ta0 = warp * RPW + rw, tc0 = ta0 + NG;
     const bool spec = (s == 0) && tc0 < p.seq_len;
+    const float2 ks = kv_scales<KV>(p.kv_scale);
 #pragma unroll
     for (int f = 0; f < NF; ++f) {
         qf[f] = __ldcg(q4 + lr + f * LPR);
@@ -2009,10 +2110,10 @@ __global__ void __launch_bounds__(NT) attention_flash_kernel(const AttnParams p,
         const KV *vc4 = vrow(ec, tc0);
 #pragma unroll
         for (int f = 0; f < NF; ++f) {
-            ka[f] = ldcg_kv4(ka4, lr, f * LPR);
-            vA[f] = ldcg_kv4(va4, lr, f * LPR);
-            kc[f] = ldcg_kv4(kc4, lr, f * LPR);
-            vC[f] = ldcg_kv4(vc4, lr, f * LPR);
+            ka[f] = ldcg_kv4(ka4, lr, f * LPR, ks.x);
+            vA[f] = ldcg_kv4(va4, lr, f * LPR, ks.y);
+            kc[f] = ldcg_kv4(kc4, lr, f * LPR, ks.x);
+            vC[f] = ldcg_kv4(vc4, lr, f * LPR, ks.y);
         }
     }
 
@@ -2075,10 +2176,10 @@ __global__ void __launch_bounds__(NT) attention_flash_kernel(const AttnParams p,
             const KV *vc4 = vrow(ec, sc);
 #pragma unroll
             for (int f = 0; f < NF; ++f) {
-                ka[f] = ldcg_kv4(ka4, lr, f * LPR);
-                vA[f] = ldcg_kv4(va4, lr, f * LPR);
-                kc[f] = ldcg_kv4(kc4, lr, f * LPR);
-                vC[f] = ldcg_kv4(vc4, lr, f * LPR);
+                ka[f] = ldcg_kv4(ka4, lr, f * LPR, ks.x);
+                vA[f] = ldcg_kv4(va4, lr, f * LPR, ks.y);
+                kc[f] = ldcg_kv4(kc4, lr, f * LPR, ks.x);
+                vC[f] = ldcg_kv4(vc4, lr, f * LPR, ks.y);
             }
         }
         update(ka, vA, va);
@@ -2222,6 +2323,7 @@ __global__ void __launch_bounds__(NT) attn_wo_kernel(const AttnWoParams q) {
         else return vb + (size_t)t * p.kv_dim;
     };
     const float root_hs = sqrtf((float)hs);
+    const float2 ks = kv_scales<KV>(p.kv_scale);
 
     float4 qf[NF], acc[NF];
 #pragma unroll
@@ -2260,10 +2362,10 @@ __global__ void __launch_bounds__(NT) attn_wo_kernel(const AttnWoParams q) {
         const KV *vc4 = vrow(vc ? tc : t0);
 #pragma unroll
         for (int f = 0; f < NF; ++f) {
-            ka[f] = ldcg_kv4(ka4, lr, f * LPR);
-            vA[f] = ldcg_kv4(va4, lr, f * LPR);
-            kc[f] = ldcg_kv4(kc4, lr, f * LPR);
-            vC[f] = ldcg_kv4(vc4, lr, f * LPR);
+            ka[f] = ldcg_kv4(ka4, lr, f * LPR, ks.x);
+            vA[f] = ldcg_kv4(va4, lr, f * LPR, ks.y);
+            kc[f] = ldcg_kv4(kc4, lr, f * LPR, ks.x);
+            vC[f] = ldcg_kv4(vc4, lr, f * LPR, ks.y);
         }
         update(ka, vA, va);
         update(kc, vC, vc);
@@ -2732,7 +2834,8 @@ __global__ void __launch_bounds__(LOGPROB_THREADS) logprob_topk_batch_kernel(con
 // into up to KV_FORK_MAXD destinations of the same model.  A cache is (L, seq_len, kv_loc) elements of
 // type KV, so the prefix of one layer of one cache is one contiguous segment of n_pos * kv_loc elements
 // at offset l * seq_len * kv_loc, the same in every session; kv_loc is a multiple of 4 (head_size is),
-// so every segment is a whole number of 4-element units (float4, or 8 bytes of bf16).  Each source unit
+// so every segment is a whole number of 4-element units (float4, 8 bytes of bf16 or 4 bytes of e4m3; the
+// codes are copied raw, the scales are the model's).  Each source unit
 // is read once and stored nd times.  The fork is never launched inside a step or a graph: no pdl_wait,
 // no CTL_DONE.
 // ---------------------------------------------------------------------------------------
@@ -2748,7 +2851,8 @@ struct KvForkParams {
 };
 template <typename KV>
 __global__ void __launch_bounds__(NT) kv_fork_kernel(const KvForkParams<KV> p) {
-    typedef typename std::conditional<sizeof(KV) == 2, uint2, float4>::type Unit;   // 4 elements
+    typedef typename std::conditional<sizeof(KV) == 1, unsigned int,
+                                      typename std::conditional<sizeof(KV) == 2, uint2, float4>::type>::type Unit;   // 4 elements
     const long long seg4 = p.seg >> 2;
     for (int s = blockIdx.y; s < 2 * p.L; s += gridDim.y) {   // segments 0 .. L-1: keys, L .. 2L-1: values
         const bool val = s >= p.L;

@@ -109,6 +109,10 @@ struct SharedWeights {
     int refs = 1;
     std::vector<void *> owned;
     KvPool *pool = nullptr;                   // paged models only
+    // e4m3 KV formats only: [L][s_k, s_v] (l2b_kv_scales) on the device, read by the kernels through a
+    // pointer so captured graphs stay valid, and its host copy (l2b_read_state's widening)
+    float *kv_scale = nullptr;
+    std::vector<float> kv_scale_h;
 };
 
 struct l2b_ctx {
@@ -154,8 +158,8 @@ struct l2b_ctx {
     size_t h_call_bytes = 0;
     float *delta = nullptr;                  // L2B_TP=nccl baseline only: partial rows before the NCCL all-reduce
     float *q = nullptr, *xb = nullptr, *hb = nullptr, *logits = nullptr, *logits_loc = nullptr;
-    // KV cache, (L, seq_len, kv_loc) elements of the format `kvfmt`: 0 (fp32), L2B_KV_BF16, or
-    // L2B_KV_ROUND_BF16 (fp32 elements holding bf16-rounded values: the bf16 cache's reference)
+    // KV cache, (L, seq_len, kv_loc) elements of the format `kvfmt`: 0 (fp32), L2B_KV_BF16, L2B_KV_E4M3,
+    // or L2B_KV_ROUND_BF16 / L2B_KV_ROUND_E4M3 (fp32 elements holding rounded values: the references)
     int kvfmt = 0;
     void *kcache = nullptr, *vcache = nullptr;
     // Paged layout (L2B_KV_PAGED): kcache and vcache are both the device page table kv_tab, [L][n_pages]
@@ -300,24 +304,50 @@ uint64_t fmt_ld(int fmt, uint64_t cols) {
 size_t w_elem(const l2b_ctx *ctx) { return fmt_elem(ctx->wfmt); }
 // ---- KV-cache format ----
 bool kv_bf16(const l2b_ctx *ctx) { return ctx->kvfmt == L2B_KV_BF16; }
-size_t kv_elem(const l2b_ctx *ctx) { return kv_bf16(ctx) ? 2 : 4; }
-// what the QKV epilogue stores: the kernels' KV type (float, bf16, kv_f32_bf16), or'd with KS_PAGED for
-// their kv_paged<> forms
-enum KvStore { KS_F32, KS_BF16, KS_ROUND, KS_PAGED = 4 };
+bool kv_e4m3(const l2b_ctx *ctx) { return ctx->kvfmt == L2B_KV_E4M3; }
+// the formats whose kernels take the model's scales: the e4m3 cache and its fp32 reference
+bool kv_scaled(int kvfmt) { return kvfmt == L2B_KV_E4M3 || kvfmt == L2B_KV_ROUND_E4M3; }
+size_t kv_elem(const l2b_ctx *ctx) { return kv_bf16(ctx) ? 2 : kv_e4m3(ctx) ? 1 : 4; }
+// what the QKV epilogue stores: the kernels' KV type (float, bf16, kv_f32_bf16, e4m3, kv_f32_e4m3), or'd
+// with KS_PAGED for their kv_paged<> forms
+enum KvStore { KS_F32, KS_BF16, KS_ROUND, KS_E4M3, KS_ROUND_E4M3, KS_PAGED = 8 };
 int kv_store(const l2b_ctx *ctx) {
-    return (kv_bf16(ctx) ? KS_BF16 : ctx->kvfmt == L2B_KV_ROUND_BF16 ? KS_ROUND : KS_F32) | (ctx->paged ? KS_PAGED : 0);
+    const int ks = kv_bf16(ctx) ? KS_BF16 : ctx->kvfmt == L2B_KV_ROUND_BF16 ? KS_ROUND
+                   : kv_e4m3(ctx) ? KS_E4M3 : ctx->kvfmt == L2B_KV_ROUND_E4M3 ? KS_ROUND_E4M3 : KS_F32;
+    return ks | (ctx->paged ? KS_PAGED : 0);
 }
 // the cache format the attention kernels are picked for: kvfmt, or'd with L2B_KV_PAGED
 int kv_kernels(const l2b_ctx *ctx) { return ctx->kvfmt | (ctx->paged ? L2B_KV_PAGED : 0); }
 template <typename T> struct type_tag { typedef T type; };
+// f(type_tag<E>()) or f(type_tag<kv_paged<E>>()) for element type E
+template <typename E, typename F>
+auto kv_layout(bool paged, F f) { return paged ? f(type_tag<kv_paged<E>>()) : f(type_tag<E>()); }
 // f(type_tag<KV>()) for the kernels' KV type of KvStore ks
 template <typename F>
 auto kv_dispatch(int ks, F f) {
-    if (ks & KS_PAGED) {
-        ks &= ~KS_PAGED;
-        return ks == KS_BF16 ? f(type_tag<kv_paged<bf16>>()) : ks == KS_ROUND ? f(type_tag<kv_paged<kv_f32_bf16>>()) : f(type_tag<kv_paged<float>>());
+    const bool pg = (ks & KS_PAGED) != 0;
+    switch (ks & ~KS_PAGED) {
+    case KS_BF16: return kv_layout<bf16>(pg, f);
+    case KS_ROUND: return kv_layout<kv_f32_bf16>(pg, f);
+    case KS_E4M3: return kv_layout<e4m3>(pg, f);
+    case KS_ROUND_E4M3: return kv_layout<kv_f32_e4m3>(pg, f);
+    default: return kv_layout<float>(pg, f);
     }
-    return ks == KS_BF16 ? f(type_tag<bf16>()) : ks == KS_ROUND ? f(type_tag<kv_f32_bf16>()) : f(type_tag<float>());
+}
+// f(type_tag<KV>()) for the KV type the attention kernels read a cache of format kvfmt (kv_kernels) with:
+// the reference formats are fp32 caches and take the fp32 kernels
+template <typename F>
+auto kv_read_dispatch(int kvfmt, F f) {
+    const bool pg = (kvfmt & L2B_KV_PAGED) != 0;
+    switch (kvfmt & ~L2B_KV_PAGED) {
+    case L2B_KV_BF16: return kv_layout<bf16>(pg, f);
+    case L2B_KV_E4M3: return kv_layout<e4m3>(pg, f);
+    default: return kv_layout<float>(pg, f);
+    }
+}
+// layer l's (s_k, s_v) on the device, or nullptr for a format without scales
+const float *kv_scale_at(const l2b_ctx *ctx, int l) {
+    return ctx->weights && ctx->weights->kv_scale ? ctx->weights->kv_scale + 2 * (size_t)l : nullptr;
 }
 // layer `layer` of a cache (kcache or vcache) of ctx: its base, or (paged) its page table
 void *kv_layer(const l2b_ctx *ctx, void *cache, int layer) {
@@ -749,11 +779,11 @@ attn_fn attention_flash_pick(int nf) {
 // the 3-pass kernel and the fork copy for cache format kvfmt (the attention kernels: or'd with L2B_KV_PAGED,
 // kv_kernels)
 attn_fn attention_3pass(int kvfmt) {
-    if (kvfmt & L2B_KV_PAGED) return (kvfmt & L2B_KV_BF16) ? attention_kernel<kv_paged<bf16>> : attention_kernel<kv_paged<float>>;
-    return kvfmt == L2B_KV_BF16 ? attention_kernel<bf16> : attention_kernel<float>;
+    return kv_read_dispatch(kvfmt, [](auto t) { return (attn_fn)attention_kernel<typename decltype(t)::type>; });
 }
 const void *kv_fork_pick(int kvfmt) {
-    return kvfmt == L2B_KV_BF16 ? (const void *)kv_fork_kernel<bf16> : (const void *)kv_fork_kernel<float>;
+    return kvfmt == L2B_KV_BF16 ? (const void *)kv_fork_kernel<bf16>
+           : kvfmt == L2B_KV_E4M3 ? (const void *)kv_fork_kernel<e4m3> : (const void *)kv_fork_kernel<float>;
 }
 // flash-decoding form when head_size/4 splits into 1..8 float4 per lane, else the 3-pass kernel; the
 // instance for cache format kvfmt (the choice does not depend on it)
@@ -762,10 +792,7 @@ attn_fn pick_attention(int head_size, bool flash, size_t *smem, int kvfmt = 0) {
     const int lpr = (hs4 % 8 == 0) ? 8 : (hs4 % 4 == 0) ? 4 : (hs4 % 2 == 0) ? 2 : 1;
     const int nf = hs4 / lpr;
     attn_fn f2 = nullptr;
-    if (flash && (kvfmt & L2B_KV_PAGED))
-        f2 = (kvfmt & L2B_KV_BF16) ? attention_flash_pick<kv_paged<bf16>>(nf) : attention_flash_pick<kv_paged<float>>(nf);
-    else if (flash)
-        f2 = kvfmt == L2B_KV_BF16 ? attention_flash_pick<bf16>(nf) : attention_flash_pick<float>(nf);
+    if (flash) f2 = kv_read_dispatch(kvfmt, [nf](auto t) { return attention_flash_pick<typename decltype(t)::type>(nf); });
     if (!f2) return attention_3pass(kvfmt);
     const int ng = NWARP * (32 / lpr);
     *smem = ((size_t)ng * head_size + 3 * (size_t)ng) * sizeof(float);
@@ -798,9 +825,7 @@ attn_wo_fn pick_attn_wo(int head_size, size_t *smem, int wfmt = L2B_WEIGHTS_F32,
     const int nf = hs4 / lpr;
     const int ng = NWARP * (32 / lpr);
     *smem = ((size_t)ng * head_size + 3 * (size_t)ng + 2 * (size_t)head_size + 4) * sizeof(float);
-    if (kvfmt & L2B_KV_PAGED)
-        return (kvfmt & L2B_KV_BF16) ? attn_wo_pick<kv_paged<bf16>>(nf, wfmt) : attn_wo_pick<kv_paged<float>>(nf, wfmt);
-    return kvfmt == L2B_KV_BF16 ? attn_wo_pick<bf16>(nf, wfmt) : attn_wo_pick<float>(nf, wfmt);
+    return kv_read_dispatch(kvfmt, [nf, wfmt](auto t) { return attn_wo_pick<typename decltype(t)::type>(nf, wfmt); });
 }
 
 constexpr int kAttnClusterCtas = 8;   // CTAs per head cluster of attn_wo_kernel; 4 and 2 measured slower (DESIGN.md §4.6)
@@ -822,7 +847,8 @@ int launch_attn_wo(l2b_ctx *ctx, int layer, cudaStream_t st) {
     a.kv_dim = ctx->kv_loc;
     a.kv_mul = ctx->kv_mul;
     a.trace = nullptr;
-    q.wo = wrow(ctx, ctx->wo, (uint64_t)layer * ctx->dim, ctx->q_loc);
+    a.kv_scale = kv_scale_at(ctx, layer);
+    q.wo =wrow(ctx, ctx->wo, (uint64_t)layer * ctx->dim, ctx->q_loc);
     q.parts = ctx->attn_parts;
     q.dim = ctx->dim;
     q.q_dim = ctx->q_loc;
@@ -874,6 +900,7 @@ int launch_attention(l2b_ctx *ctx, int layer, cudaStream_t st, const float *q, f
     a.batched = zb ? 1 : 0;
     a.q_stride = q_stride;
     a.seq_len = ctx->cfg.seq_len;
+    a.kv_scale = kv_scale_at(ctx, layer);
     a.trace = zb ? nullptr : trace_slot(ctx);
     const AttnBatch none{};
     size_t smem = ctx->attn_smem;
@@ -958,6 +985,7 @@ LayerGemvs layer_gemvs(const l2b_ctx *ctx, int l) {
     p.vcache = kv_layer(ctx, ctx->vcache, l);
     p.rope_cos = ctx->rope_cos; p.rope_sin = ctx->rope_sin;
     p.head_size = ctx->head_size; p.kv_dim = ctx->kv_loc;
+    p.kv_scale = kv_scale_at(ctx, l);
     // wo, whose result is added to the residual stream (:392-395)
     g.wo.ctl = ctx->ctl;
     g.wo.n = ctx->q_loc;
@@ -1385,6 +1413,12 @@ int create_rank(l2b_ctx *ctx, const l2b_config *cfg, const Source &src, const fl
         L2B_TRY(cuda_try(ctx, cudaMemcpy(ctx->rope_cos, hc.data(), hc.size() * sizeof(float), cudaMemcpyHostToDevice), "rope upload"));
         L2B_TRY(cuda_try(ctx, cudaMemcpy(ctx->rope_sin, hsn.data(), hsn.size() * sizeof(float), cudaMemcpyHostToDevice), "rope upload"));
     }
+    if (kv_scaled(ctx->kvfmt)) {                 // the e4m3 scales, 1 until l2b_kv_scales
+        SharedWeights *w = ctx->weights;
+        w->kv_scale_h.assign(2 * L, 1.0f);
+        L2B_TRY(dev_alloc(ctx, &w->kv_scale, 2 * L, &w->owned));
+        L2B_TRY(cuda_try(ctx, cudaMemcpy(w->kv_scale, w->kv_scale_h.data(), 2 * L * sizeof(float), cudaMemcpyHostToDevice), "KV scale upload"));
+    }
     return create_run_state(ctx);
 }
 
@@ -1488,7 +1522,8 @@ int kv_page_copy(l2b_ctx *ctx, const void *src, void *const *dst, int nd, int ro
     return L2B_OK;
 }
 int kv_page_copy(l2b_ctx *ctx, const void *src, void *const *dst, int nd, int rows) {
-    return kv_bf16(ctx) ? kv_page_copy<bf16>(ctx, src, dst, nd, rows) : kv_page_copy<float>(ctx, src, dst, nd, rows);
+    return kv_bf16(ctx) ? kv_page_copy<bf16>(ctx, src, dst, nd, rows)
+           : kv_e4m3(ctx) ? kv_page_copy<e4m3>(ctx, src, dst, nd, rows) : kv_page_copy<float>(ctx, src, dst, nd, rows);
 }
 
 // rows [lo, hi) that a call may write into session s's cache (a paged session; one call lists no other)
@@ -2089,13 +2124,15 @@ int32_t l2b_create_synthetic_group(l2b_ctx **out, const l2b_config *cfg, uint64_
     return common_create(out, cfg, s, 0, nullptr, nullptr, nullptr, n_gpus);
 }
 
-// weight_format of l2b_create_format: a weight format, with L2B_KV_BF16 or L2B_KV_ROUND_BF16 or'd in.  Any
-// other value => L2B_ERR_INVALID_ARG.
+// weight_format of l2b_create_format: a weight format, with at most one of L2B_KV_BF16, L2B_KV_ROUND_BF16,
+// L2B_KV_E4M3 and L2B_KV_ROUND_E4M3 and optionally L2B_KV_PAGED or'd in.  Any other value =>
+// L2B_ERR_INVALID_ARG.
 bool split_format(int32_t weight_format, int *wfmt, int *kvfmt) {
-    *kvfmt = weight_format & (L2B_KV_BF16 | L2B_KV_ROUND_BF16 | L2B_KV_PAGED);
-    *wfmt = weight_format & ~(L2B_KV_BF16 | L2B_KV_ROUND_BF16 | L2B_KV_PAGED);
-    if ((*wfmt != L2B_WEIGHTS_F32 && *wfmt != L2B_WEIGHTS_BF16 && *wfmt != L2B_WEIGHTS_Q8) ||
-        (*kvfmt & (L2B_KV_BF16 | L2B_KV_ROUND_BF16)) == (L2B_KV_BF16 | L2B_KV_ROUND_BF16)) {
+    const int elem = L2B_KV_BF16 | L2B_KV_ROUND_BF16 | L2B_KV_E4M3 | L2B_KV_ROUND_E4M3;
+    *kvfmt = weight_format & (elem | L2B_KV_PAGED);
+    *wfmt = weight_format & ~(elem | L2B_KV_PAGED);
+    const int e = *kvfmt & elem;
+    if ((*wfmt != L2B_WEIGHTS_F32 && *wfmt != L2B_WEIGHTS_BF16 && *wfmt != L2B_WEIGHTS_Q8) || (e & (e - 1)) != 0) {
         g_create_error = "unknown weight format";
         return false;
     }
@@ -2108,7 +2145,7 @@ int32_t l2b_create_format(l2b_ctx **out, const l2b_config *cfg, const float *hos
     if (!split_format(weight_format, &wfmt, &kvfmt)) return L2B_ERR_INVALID_ARG;
     if (weight_format == L2B_WEIGHTS_F32) return l2b_create(out, cfg, host_weights, n_floats, rope_cos, rope_sin, n_gpus);
     if (!host_weights) { g_create_error = "host_weights is NULL"; return L2B_ERR_INVALID_ARG; }
-    if (n_gpus != 1) { g_create_error = "bf16 and q8 weights and a bf16 KV cache are single-GPU (n_gpus must be 1)"; return L2B_ERR_UNSUPPORTED; }
+    if (n_gpus != 1) { g_create_error = "bf16 and q8 weights and bf16, e4m3 or paged KV caches are single-GPU (n_gpus must be 1)"; return L2B_ERR_UNSUPPORTED; }
     Source s; s.host = host_weights;
     return common_create(out, cfg, s, n_floats, rope_cos, rope_sin, nullptr, 1, wfmt, kvfmt);
 }
@@ -2158,6 +2195,27 @@ int32_t l2b_weight_info(const l2b_ctx *ctx, int32_t *weight_format, uint64_t *n_
     if (weight_format) *weight_format = ctx->wfmt;
     if (n_rounded) *n_rounded = ctx->n_rounded;
     return L2B_OK;
+}
+
+int32_t l2b_kv_scales(l2b_ctx *ctx, const float *scales, int32_t n) {
+    if (!ctx) return L2B_ERR_INVALID_ARG;
+    if (!scales) return fail(ctx, L2B_ERR_INVALID_ARG, "scales is NULL");
+    if (n != 2 * ctx->cfg.n_layers) return fail(ctx, L2B_ERR_INVALID_ARG, "n must be 2 * n_layers");
+    for (int i = 0; i < n; ++i)
+        if (!std::isnormal(scales[i]) || !(scales[i] > 0.0f)) return fail(ctx, L2B_ERR_INVALID_ARG, "a KV scale is not a finite positive normal float");
+    if (!kv_scaled(ctx->kvfmt)) return fail(ctx, L2B_ERR_UNSUPPORTED, "the model's KV cache is not e4m3");
+    SharedWeights *w = ctx->weights;
+    if (w->refs > 1) return fail(ctx, L2B_ERR_STATE, "the model has a live session");
+    if (ctx->n_appended > 0) return fail(ctx, L2B_ERR_STATE, "the model has positions appended");
+    L2B_CUDA(ctx, cudaSetDevice(ctx->device));
+    L2B_CUDA(ctx, cudaMemcpy(w->kv_scale, scales, (size_t)n * sizeof(float), cudaMemcpyHostToDevice));
+    w->kv_scale_h.assign(scales, scales + n);
+    return L2B_OK;
+}
+
+void l2b_round_e4m3_host(float *data, uint64_t n, float scale) {
+    if (!data) return;
+    for (uint64_t i = 0; i < n; ++i) data[i] = e4m3_widen(e4m3_round_bits(data[i], scale), scale);
 }
 
 void l2b_round_bf16_host(float *data, uint64_t n) {
@@ -2315,7 +2373,8 @@ int32_t l2b_fork(l2b_ctx *src, int32_t n_pos, l2b_ctx *const *dst, int32_t n_dst
         cudaStream_t st = src->stream;
         L2B_CUDA(src, cudaSetDevice(src->device));
         L2B_CUDA(src, cudaEventRecord(src->ev0, st));
-        const int rc = kv_bf16(src) ? fork_launch<bf16>(src, n_pos, dst, n_dst) : fork_launch<float>(src, n_pos, dst, n_dst);
+        const int rc = kv_bf16(src) ? fork_launch<bf16>(src, n_pos, dst, n_dst)
+                       : kv_e4m3(src) ? fork_launch<e4m3>(src, n_pos, dst, n_dst) : fork_launch<float>(src, n_pos, dst, n_dst);
         if (rc) return rc;
         L2B_CUDA(src, cudaEventRecord(src->ev1, st));
         L2B_CUDA(src, cudaEventSynchronize(src->ev1));
@@ -3862,8 +3921,11 @@ int32_t l2b_read_state(l2b_ctx *ctx, int32_t which, float *dst, uint64_t n, uint
             for (uint64_t l = 0; l < L; ++l) {
                 const unsigned char *from = page.data() + ((2 * l + (which == 5)) * P) * kvl * el;
                 float *to = dst + (l * S + j * P) * kvl;
+                const float s = kv_e4m3(ctx) ? ctx->weights->kv_scale_h[2 * l + (which == 5)] : 1.0f;
                 for (uint64_t i = 0; i < rows * kvl; ++i) {
-                    if (el == 2) {
+                    if (el == 1) {
+                        to[i] = e4m3_widen(from[i], s);
+                    } else if (el == 2) {
                         uint16_t h;
                         memcpy(&h, from + 2 * i, 2);
                         const uint32_t u = (uint32_t)h << 16;
@@ -3883,6 +3945,13 @@ int32_t l2b_read_state(l2b_ctx *ctx, int32_t which, float *dst, uint64_t n, uint
             const uint32_t u = (uint32_t)h[i] << 16;
             memcpy(dst + i, &u, 4);
         }
+    } else if ((which == 4 || which == 5) && kv_e4m3(ctx)) {
+        // the codes land in the last quarter of dst and are widened from the front: value i is written to
+        // bytes [4i, 4i+4), below the unread codes at [3 cnt + i, ..) for every i < cnt
+        uint8_t *c = reinterpret_cast<uint8_t *>(dst) + 3 * cnt;
+        L2B_CUDA(ctx, cudaMemcpy(c, src, cnt, cudaMemcpyDeviceToHost));
+        const uint64_t per_layer = S * ctx->kv_loc;
+        for (uint64_t i = 0; i < cnt; ++i) dst[i] = e4m3_widen(c[i], ctx->weights->kv_scale_h[2 * (i / per_layer) + (which == 5)]);
     } else {
         L2B_CUDA(ctx, cudaMemcpy(dst, src, cnt * sizeof(float), cudaMemcpyDeviceToHost));
     }

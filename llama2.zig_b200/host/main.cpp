@@ -35,6 +35,8 @@ static const char *usage_text =
     "                           the bf16 bytes per step; outputs equal an fp32 run of the dequantized checkpoint (1 GPU)\n"
     "     --kv-bf16             keep the KV cache (and the draft's) in bf16 on the GPU: half the cache memory and\n"
     "                           attention bytes; outputs equal an fp32-cache run that rounds each K/V value (1 GPU)\n"
+    "     --kv-e4m3             keep the KV cache (and the draft's) in fp8 e4m3 with unit scales: half the bf16 cache's\n"
+    "                           memory; outputs equal an fp32-cache run that rounds each K/V value to e4m3 (1 GPU)\n"
     "     --beam <int>          beam search with that many hypotheses (at most 8) on a paged KV cache; prints the\n"
     "                           best one; -t and -p are ignored, -v prints every result's normalised score (1 GPU)\n";
 
@@ -43,7 +45,8 @@ static void print_kv_info(const char *what, const l2b_ctx *ctx) {
     int32_t fmt = 0;
     uint64_t bytes = 0;
     l2b_kv_info(ctx, &fmt, &bytes);
-    fprintf(stderr, "%s: %s, %llu bytes\n", what, fmt == L2B_KV_BF16 ? "bf16" : fmt == L2B_KV_ROUND_BF16 ? "fp32 (bf16-rounded)" : "fp32",
+    fprintf(stderr, "%s: %s, %llu bytes\n", what, fmt == L2B_KV_BF16 ? "bf16" : fmt == L2B_KV_ROUND_BF16 ? "fp32 (bf16-rounded)"
+                                    : fmt == L2B_KV_E4M3 ? "e4m3" : fmt == L2B_KV_ROUND_E4M3 ? "fp32 (e4m3-rounded)" : "fp32",
             (unsigned long long)bytes);
 }
 
@@ -168,6 +171,7 @@ int main(int argc, char **argv) {
         else if (a == "--bf16") weight_format = L2B_WEIGHTS_BF16;
         else if (a == "--q8") weight_format = L2B_WEIGHTS_Q8;
         else if (a == "--kv-bf16") kv_flag = L2B_KV_BF16;
+        else if (a == "--kv-e4m3") kv_flag = L2B_KV_E4M3;
         else if (a == "--beam") n_beams = atoi(need("beam"));
         else { fprintf(stderr, "error: unknown argument '%s'\n", argv[i]); fputs(usage_text, stdout); return 0; }
     }
