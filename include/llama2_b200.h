@@ -94,7 +94,8 @@ typedef struct l2b_ctx l2b_ctx;
  *   - a GEMV input that does not fit in shared memory: hidden_dim > 57600 on H100, or
  *     dim > 28800 where the rmsnorm gain is staged next to it;
  *   - a seq_len whose timeline split (seq_len / nsplit, at most 32 splits) no longer fits the
- *     3-pass attention kernel's 200 KB score buffer: seq_len > 1,605,632 with 8 heads or fewer.
+ *     3-pass attention kernel's 200 KB score buffer: seq_len > 1,605,632 with 8 heads or fewer;
+ *     with L2B_KV_PAGED the split's page addresses follow the buffer: seq_len > 1,556,832.
  * DESIGN.md §4.5c tabulates which kernel runs at which limit.                              */
 int32_t l2b_create(l2b_ctx **out, const l2b_config *cfg, const float *host_weights,
                    uint64_t n_floats, const float *rope_cos, const float *rope_sin,

@@ -600,6 +600,7 @@ gemv_fn gemv_pick(int epi, int tpr, int ks) {
 }
 
 constexpr int kMaxDynSmem = 200 * 1024;
+constexpr size_t kDefaultDynSmem = 48 * 1024;       // a kernel's dynamic shared memory without an opt-in
 constexpr int kMaxSmemOptin = 227 * 1024 - 2048;   // static __shared__ of the kernels stays under 2 KB
 
 int gemv_tpr(int n) {
@@ -830,6 +831,21 @@ attn_wo_fn pick_attn_wo(int head_size, size_t *smem, int wfmt = L2B_WEIGHTS_F32,
 
 constexpr int kAttnClusterCtas = 8;   // CTAs per head cluster of attn_wo_kernel; 4 and 2 measured slower (DESIGN.md §4.6)
 
+// The dynamic shared memory an attention kernel requests on ctx, page staging included: the 3-pass kernel
+// (score buffer), the flash kernel (pick_attention: the 3-pass kernel's where the head size has no flash
+// form) and attn_wo_kernel.  create_run_state checks and opts in these sizes and the launches request
+// them, so the two cannot disagree.
+enum AttnKind { ATTN_3PASS, ATTN_FLASH, ATTN_WO };
+size_t attn_request(const l2b_ctx *ctx, AttnKind k) {
+    size_t smem = ctx->attn_smem;
+    if (k == ATTN_WO) {
+        pick_attn_wo(ctx->head_size, &smem);
+        return smem + (ctx->paged ? ctx->attn_pg_bytes_wo : 0);
+    }
+    pick_attention(ctx->head_size, k == ATTN_FLASH, &smem);
+    return smem + (ctx->paged ? ctx->attn_pg_bytes : 0);
+}
+
 // attention + wo of one layer in one cluster launch (small models): partial vectors -> ctx->attn_parts
 int launch_attn_wo(l2b_ctx *ctx, int layer, cudaStream_t st) {
     if (ctx->profiling) {
@@ -852,13 +868,12 @@ int launch_attn_wo(l2b_ctx *ctx, int layer, cudaStream_t st) {
     q.parts = ctx->attn_parts;
     q.dim = ctx->dim;
     q.q_dim = ctx->q_loc;
-    size_t smem = 0;
-    attn_wo_fn fn = pick_attn_wo(ctx->head_size, &smem, ctx->wfmt, kv_kernels(ctx));
-    if (ctx->paged) smem += ctx->attn_pg_bytes_wo;
+    size_t unused = 0;
+    attn_wo_fn fn = pick_attn_wo(ctx->head_size, &unused, ctx->wfmt, kv_kernels(ctx));
     cudaLaunchConfig_t lc{};
     lc.gridDim = dim3(ctx->heads_loc, kAttnClusterCtas);
     lc.blockDim = dim3(NT);
-    lc.dynamicSmemBytes = smem;
+    lc.dynamicSmemBytes = attn_request(ctx, ATTN_WO);
     lc.stream = st;
     cudaLaunchAttribute at[2];
     at[0].id = cudaLaunchAttributeClusterDimension;
@@ -903,13 +918,12 @@ int launch_attention(l2b_ctx *ctx, int layer, cudaStream_t st, const float *q, f
     a.kv_scale = kv_scale_at(ctx, layer);
     a.trace = zb ? nullptr : trace_slot(ctx);
     const AttnBatch none{};
-    size_t smem = ctx->attn_smem;
-    attn_fn fn = pick_attention(ctx->head_size, ctx->attn_flash, &smem, kv_kernels(ctx));
-    if (ctx->paged) smem += ctx->attn_pg_bytes;
+    size_t unused = 0;
+    attn_fn fn = pick_attention(ctx->head_size, ctx->attn_flash, &unused, kv_kernels(ctx));
     cudaLaunchConfig_t lc{};
     lc.gridDim = dim3(ctx->heads_loc, ctx->nsplit, nb);
     lc.blockDim = dim3(NT);
-    lc.dynamicSmemBytes = smem;
+    lc.dynamicSmemBytes = attn_request(ctx, ctx->attn_flash ? ATTN_FLASH : ATTN_3PASS);
     lc.stream = st;
     cudaLaunchAttribute at[1] = {pdl_attr()};
     lc.attrs = at;
@@ -1660,21 +1674,27 @@ int create_run_state(l2b_ctx *ctx) {
         if (cap < ctx->min_chunk) cap = ctx->min_chunk;
         const int G = NT / (int)(hs / 4);
         ctx->attn_smem = (int)(((uint64_t)G * hs + cap) * sizeof(float));
-        if (ctx->attn_smem > kMaxDynSmem) {
-            ctx->err = "seq_len too large for the attention kernel's shared memory";
-            g_create_error = ctx->err;
-            return L2B_ERR_UNSUPPORTED;
-        }
         // paged: each split's page addresses follow the kernels' shared memory (a split of `cap` rows
         // spans at most cap / P + 2 pages; attn_wo_kernel's splits are ceil(S / 8) rows)
         ctx->attn_pg_bytes = (int)(((size_t)cap / KV_PAGE_ROWS + 2) * sizeof(void *) + sizeof(float));
         ctx->attn_pg_bytes_wo = (int)(((S + kAttnClusterCtas - 1) / kAttnClusterCtas / KV_PAGE_ROWS + 2) * sizeof(void *));
-        if (ctx->paged && ctx->attn_smem + ctx->attn_pg_bytes > kMaxDynSmem) {
+        // every attention kernel this context can launch (the 3-pass one also under L2B_ATTN=3pass) must
+        // get its request; the flash and attn_wo requests grow with seq_len only through page staging
+        const size_t req_3pass = attn_request(ctx, ATTN_3PASS), req_flash = attn_request(ctx, ATTN_FLASH);
+        const size_t req_wo = ctx->fuse_attn ? attn_request(ctx, ATTN_WO) : 0;
+        if (std::max({req_3pass, req_flash, req_wo}) > (size_t)kMaxDynSmem) {
             ctx->err = "seq_len too large for the attention kernel's shared memory";
             g_create_error = ctx->err;
             return L2B_ERR_UNSUPPORTED;
         }
         L2B_TRY(cuda_try(ctx, cudaFuncSetAttribute(attention_3pass(kv_kernels(ctx)), cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem), "cudaFuncSetAttribute"));
+        // past the 48 KiB a kernel gets without opting in (long paged contexts only); kMaxDynSmem, as for
+        // the 3-pass kernel, so another context's smaller request never lowers it
+        size_t unused = 0;
+        if (req_flash > kDefaultDynSmem)
+            L2B_TRY(cuda_try(ctx, cudaFuncSetAttribute(pick_attention((int)hs, true, &unused, kv_kernels(ctx)), cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem), "cudaFuncSetAttribute"));
+        if (req_wo > kDefaultDynSmem)
+            L2B_TRY(cuda_try(ctx, cudaFuncSetAttribute(pick_attn_wo((int)hs, &unused, ctx->wfmt, kv_kernels(ctx)), cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem), "cudaFuncSetAttribute"));
         L2B_TRY(dev_alloc(ctx, &ctx->part_o, (size_t)ctx->heads_loc * ns * hs));
         L2B_TRY(dev_alloc(ctx, &ctx->part_ml, (size_t)ctx->heads_loc * ns * 2));
         L2B_TRY(dev_alloc(ctx, &ctx->counters, (size_t)ctx->heads_loc));

@@ -12,7 +12,10 @@ rounded values widened into its fp32 cache and reads them with the fp32 kernels.
      loop), and bf16 and q8 weights on S and B: forward (logits, x, the widened caches), forward_argmax,
      forward_sample, generate_argmax, prefill, score; the batch, ragged and verify calls,
      generate_argmax_batch and fork on sessions; generate_speculative with the bf16 cache on the target or
-     on the draft (tokens, rounds and both caches); the long-context shapes L7 and L3 of test_gpu_long_context at its checked positions.
+     on the draft (tokens, rounds and both caches); the long-context shapes L7, L3 and F128 of
+     test_gpu_long_context (L7 and L3 also under L2B_FUSE=0 L2B_ATTN=3pass) on every path of its
+     check_twin: forward at the checked positions, chunked prefill, score, the batch, ragged and verify
+     calls at per-query T, forks.  The envelope shapes: test_gpu_envelope.test_envelope_kv.
   2  rounding: layer 0's K/V rows of a bf16-KV context are round_bf16_host of a plain fp32 context's layer-0
      rows, on the single step, the batched prefill, the batch and the ragged calls; every value read back
      has its low 16 bits zero.
@@ -32,6 +35,7 @@ import subprocess
 import numpy as np
 import pytest
 
+import test_gpu_long_context as LC
 from test_gpu_bf16 import _eq
 from test_gpu_bf16_shapes import STALE_PATHS
 from test_gpu_q8_shapes import filled_session
@@ -46,11 +50,11 @@ pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def kv_pair(l2b, ck, env=None, weight_format="f32"):
-    """(bf16-KV context, its fp32-KV twin) of ck under env."""
+def kv_pair(l2b, ck, env=None, weight_format="f32", seed=None):
+    """(bf16-KV context, its fp32-KV twin) of ck under env (seed: device-synthesized weights)."""
     with l2b_env(env or {}):
-        b = l2b.Transformer(ck, weight_format=weight_format, kv_format="bf16")
-        f = l2b.Transformer(ck, weight_format=weight_format, kv_format="f32-round-bf16")
+        b = l2b.Transformer(ck, seed, weight_format=weight_format, kv_format="bf16")
+        f = l2b.Transformer(ck, seed, weight_format=weight_format, kv_format="f32-round-bf16")
     return b, f
 
 
@@ -196,28 +200,15 @@ def test_speculative(l2b, name, wf):
                 _eq(db.state(s), df.state(s), f"bf16 cache on the {side}: draft {s}")
 
 
-@pytest.mark.parametrize("name", ["L7", "L3"])
-def test_twin_long_context(l2b, name):
-    """The Llama head geometry at 4096 / 8192 positions: every split-count change, the switch to long
-    chunks and the last positions (test_gpu_long_context.checked), teacher-forced and prefilled."""
-    import test_gpu_long_context as LC
+@pytest.mark.parametrize("name,env_name", LC.TWIN_PARAMS)
+def test_twin_long_context(l2b, name, env_name):
+    """The Llama head geometry at 4096 / 8192 positions on every path of test_gpu_long_context.check_twin:
+    every split-count change, the switch to long chunks and the last positions (checked), teacher-forced,
+    prefilled, scored, batched at per-query T and forked; attn_wo_kernel<4> (F128) and the 3-pass kernel."""
     ck = LC.payload(l2b, name)
-    S = ck.seq_len
-    check = LC.checked(LC.MODELS[name][0], LC.sm_count())
-    toks = teacher_tokens(S, ck.vocab_size)
-    b, f = kv_pair(l2b, ck)
+    b, f = kv_pair(l2b, ck, LC.ENVS[env_name])
     with b, f:
-        for pos, tok in enumerate(toks):
-            lb, lf = b.forward(tok, pos), f.forward(tok, pos)
-            if pos in check:
-                _eq(lb, lf, f"logits at {pos}")
-        for s in ("key_cache", "value_cache", "x"):
-            _eq(b.state(s), f.state(s), s)
-        b.reset(); f.reset()
-        tl = LC.last_short(ck.n_heads, S, LC.sm_count())
-        for a, e in zip([0, 37, tl - 1, tl + 2], [37, tl - 1, tl + 2, S]):
-            _eq(b.prefill(toks[a:e], a), f.prefill(toks[a:e], a), f"prefill {a}..{e}")
-        _eq(b.state("key_cache"), f.state("key_cache"), "prefill key cache")
+        LC.check_twin(l2b, b, f, name, env_name)
 
 
 def layer0(t, s):

@@ -13,7 +13,10 @@ least 1% of its V codes are subnormal, which the tests assert.
      and B: forward (logits, x, the widened caches), forward_argmax, forward_sample, generate_argmax, prefill,
      score; the batch, ragged and verify calls, generate_argmax_batch and fork on sessions;
      generate_speculative with the e4m3 cache on the target or on the draft; beam_search on paged models;
-     the long-context shapes L7 and L3 of test_gpu_long_context at its checked positions.
+     the long-context shapes L7, L3 and F128 of test_gpu_long_context (L7 and L3 also under L2B_FUSE=0
+     L2B_ATTN=3pass) on every path of its check_twin: forward at the checked positions, chunked prefill,
+     score, the batch, ragged and verify calls at per-query T, forks.  The envelope shapes:
+     test_gpu_envelope.test_envelope_kv.
   2  paged e4m3 against contiguous e4m3 (test_gpu_kv_paged's single-context check), and after forks,
      rewinds into shared pages (copies-on-write) and continuations.
   3  rounding: layer 0's K/V rows of an e4m3 context are round_e4m3_host of a plain fp32 context's layer-0
@@ -31,6 +34,7 @@ import subprocess
 import numpy as np
 import pytest
 
+import test_gpu_long_context as LC
 from test_gpu_bf16 import _eq
 from test_gpu_bf16_shapes import STALE_PATHS
 from test_gpu_kv_bf16 import demo_text, layer0
@@ -52,16 +56,18 @@ F = np.float32
 # ---- scales -------------------------------------------------------------------------------------------
 
 _stress = {}
+STRESS_ROWS = 258                              # stress_scales calibrates on the first min(seq_len, 258) rows
 
 
-def stress_scales(l2b, ck, wf="f32"):
+def stress_scales(l2b, ck, wf="f32", seed=None):
     """(n_layers, 2) scales from a plain fp32-KV context's caches after a prefill of the first positions:
     layer 0's s_k puts the top 3% of its |K| past 448 (saturated) and its s_v puts the bottom 3% of its
-    nonzero |V| below 2^-6 (subnormal codes); the other layers are calibrated, amax / 448."""
-    key = (id(ck), wf)
+    nonzero |V| below 2^-6 (subnormal codes); the other layers are calibrated, amax / 448.  seed: the
+    weights are device-synthesized."""
+    key = (id(ck), wf, seed)
     if key not in _stress or _stress[key][0] is not ck:
-        n = min(ck.seq_len, 258)
-        with l2b.Transformer(ck, weight_format=wf) as f:
+        n = min(ck.seq_len, STRESS_ROWS)
+        with l2b.Transformer(ck, seed, weight_format=wf) as f:
             f.prefill(teacher_tokens(n, ck.vocab_size), want_logits=False)
             K = np.abs(rows(f, "key_cache", n, ck))
             V = np.abs(rows(f, "value_cache", n, ck))
@@ -75,15 +81,16 @@ def stress_scales(l2b, ck, wf="f32"):
     return _stress[key][1]
 
 
-def scales_for(l2b, ck, which, wf="f32"):
-    return np.ones((ck.n_layers, 2), F) if which == "unit" else stress_scales(l2b, ck, wf)
+def scales_for(l2b, ck, which, wf="f32", seed=None):
+    return np.ones((ck.n_layers, 2), F) if which == "unit" else stress_scales(l2b, ck, wf, seed)
 
 
-def kv_pair(l2b, ck, scales, env=None, weight_format="f32", kv_layout="contiguous"):
-    """(e4m3-KV context, its fp32-KV twin) of ck under env, both with `scales`."""
+def kv_pair(l2b, ck, scales, env=None, weight_format="f32", kv_layout="contiguous", seed=None):
+    """(e4m3-KV context, its fp32-KV twin) of ck under env, both with `scales` (seed: device-synthesized
+    weights)."""
     with l2b_env(env or {}):
-        b = l2b.Transformer(ck, weight_format=weight_format, kv_format="e4m3", kv_layout=kv_layout)
-        f = l2b.Transformer(ck, weight_format=weight_format, kv_format="f32-round-e4m3", kv_layout=kv_layout)
+        b = l2b.Transformer(ck, seed, weight_format=weight_format, kv_format="e4m3", kv_layout=kv_layout)
+        f = l2b.Transformer(ck, seed, weight_format=weight_format, kv_format="f32-round-e4m3", kv_layout=kv_layout)
     b.set_kv_scales(scales)
     f.set_kv_scales(scales)
     return b, f
@@ -282,28 +289,15 @@ def test_beam_search(l2b, name, sc):
 
 
 @pytest.mark.parametrize("sc", SCALES)
-@pytest.mark.parametrize("name", ["L7", "L3"])
-def test_twin_long_context(l2b, name, sc):
-    """The Llama head geometry at 4096 / 8192 positions: every split-count change, the switch to long
-    chunks and the last positions (test_gpu_long_context.checked), teacher-forced and prefilled."""
-    import test_gpu_long_context as LC
+@pytest.mark.parametrize("name,env_name", LC.TWIN_PARAMS)
+def test_twin_long_context(l2b, name, env_name, sc):
+    """The Llama head geometry at 4096 / 8192 positions on every path of test_gpu_long_context.check_twin:
+    every split-count change, the switch to long chunks and the last positions (checked), teacher-forced,
+    prefilled, scored, batched at per-query T and forked; attn_wo_kernel<4> (F128) and the 3-pass kernel."""
     ck = LC.payload(l2b, name)
-    S = ck.seq_len
-    check = LC.checked(LC.MODELS[name][0], LC.sm_count())
-    toks = teacher_tokens(S, ck.vocab_size)
-    b, f = kv_pair(l2b, ck, scales_for(l2b, ck, sc))
+    b, f = kv_pair(l2b, ck, scales_for(l2b, ck, sc), LC.ENVS[env_name])
     with b, f:
-        for pos, tok in enumerate(toks):
-            lb, lf = b.forward(tok, pos), f.forward(tok, pos)
-            if pos in check:
-                _eq(lb, lf, f"logits at {pos}")
-        for s in ("key_cache", "value_cache", "x"):
-            _eq(b.state(s), f.state(s), s)
-        b.reset(); f.reset()
-        tl = LC.last_short(ck.n_heads, S, LC.sm_count())
-        for a, e in zip([0, 37, tl - 1, tl + 2], [37, tl - 1, tl + 2, S]):
-            _eq(b.prefill(toks[a:e], a), f.prefill(toks[a:e], a), f"prefill {a}..{e}")
-        _eq(b.state("key_cache"), f.state("key_cache"), "prefill key cache")
+        LC.check_twin(l2b, b, f, name, env_name)
 
 
 # ---- 2: paged against contiguous ----------------------------------------------------------------------

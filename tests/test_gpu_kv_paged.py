@@ -24,10 +24,18 @@ compared below that count.
      no page.
   9  slow, llama2-7B: best-of-8 from a 1984-token prompt at seq_len 2048 in bf16 KV: tokens equal the
      contiguous twin's and the pool holds 47 pages.
+ 10  long context: L7, L3 and F128 of test_gpu_long_context (default; L2B_FUSE=0 L2B_ATTN=3pass on L7 and
+     L3) in f32, bf16 and e4m3 (stress scales) KV, through test_gpu_long_context.check_twin: forward at
+     the checked positions, the prefill chunks around last_short, score, forward_batch / forward_ragged /
+     verify_argmax_ragged at per-query T, forks at 3, 299, last_short and 4000 rows.  Flash splits of up to
+     911 rows over 16 staged pages, attn_wo_kernel's 8 cluster splits of 512 rows, the 3-pass kernel's
+     456 / 911-row score buffers.  The envelope shapes and the paged seq_len limits are in
+     test_gpu_envelope.
 """
 import numpy as np
 import pytest
 
+import test_gpu_long_context as LC
 from test_gpu_bf16 import _eq
 from test_gpu_transformer import teacher_tokens
 from test_gpu_variants import CASES, MODELS, l2b_env, payload
@@ -37,11 +45,11 @@ pytestmark = pytest.mark.gpu
 P = 64
 
 
-def twin(l2b, ck, env=None, weight_format="f32", kv_format="f32"):
-    """(paged context, its contiguous twin) of ck under env."""
+def twin(l2b, ck, env=None, weight_format="f32", kv_format="f32", seed=None):
+    """(paged context, its contiguous twin) of ck under env (seed: device-synthesized weights)."""
     with l2b_env(env or {}):
-        a = l2b.Transformer(ck, weight_format=weight_format, kv_format=kv_format, kv_layout="paged")
-        b = l2b.Transformer(ck, weight_format=weight_format, kv_format=kv_format)
+        a = l2b.Transformer(ck, seed, weight_format=weight_format, kv_format=kv_format, kv_layout="paged")
+        b = l2b.Transformer(ck, seed, weight_format=weight_format, kv_format=kv_format)
     return a, b
 
 
@@ -507,6 +515,22 @@ def test_accounting(l2b):
             s.close()
             a.reset()
             assert a.kv_pool_info()["pages_in_use"] == 0
+
+
+@pytest.mark.parametrize("kv", ["f32", "bf16", "e4m3"])
+@pytest.mark.parametrize("name,env_name", LC.TWIN_PARAMS)
+def test_twin_long_context(l2b, name, env_name, kv):
+    """The Llama head geometry at 4096 / 8192 positions (test_gpu_long_context.check_twin): splits of up to
+    911 rows staged over 16 pages, attn_wo_kernel's 8 cluster splits of 512 rows, the 3-pass kernel's
+    456 / 911-row score buffers.  e4m3 runs with stress scales."""
+    ck = LC.payload(l2b, name)
+    a, b = twin(l2b, ck, LC.ENVS[env_name], kv_format=kv)
+    with a, b:
+        if kv == "e4m3":
+            from test_gpu_kv_e4m3 import stress_scales
+            for t in (a, b):
+                t.set_kv_scales(stress_scales(l2b, ck))
+        LC.check_twin(l2b, a, b, name, env_name)
 
 
 @pytest.mark.slow

@@ -44,6 +44,9 @@ Ledger: geometry / split regime / path / kernel -> test id (test_long_context[..
   attn_wo_kernel<4>, 8 cluster splits                                            [F128-*-default]
   64 heads, 5 splits of 820 rows, gemv8_kernel                                   [L70-*-default] (slow)
 
+  KV caches (paged; bf16, e4m3 and their paged forms), bit for bit against their twins: check_twin, run
+  by test_gpu_kv_paged, test_gpu_kv_bf16 and test_gpu_kv_e4m3 on L7, L3 and F128 (TWIN_PARAMS)
+
 Bounds.  e(r) = max|r - ref64| / max|ref64| (log-probabilities: scaled by the position's max|logit|).
 Every result is within REL_TOL = 1e-4, and within K[family, kernel class] * e_att.  The strict oracle
 would take an hour per model at these sizes on a CPU host, so the yardstick is a float32 restatement
@@ -266,6 +269,81 @@ def bound(path, case, kclass, e_dev, e_att):
     assert e_dev <= REL_TOL, (path, e_dev)
     k = K[FAMILY[path], kclass]
     assert e_dev <= k * max(e_att, ATT_FLOOR), (path, e_dev, e_att, k)
+
+
+# (model, environment) of the KV-cache twins (test_gpu_kv_paged, test_gpu_kv_bf16, test_gpu_kv_e4m3); the
+# default environment's id is the model's name alone
+TWIN_PARAMS = [pytest.param(m, e, id=m if e == "default" else f"{m}-{e}")
+               for m in ("L7", "L3", "F128") for e in (("default", "3pass") if m != "F128" else ("default",))]
+
+
+def check_twin(l2b, a, b, name, env_name):
+    """a == b bit for bit, two contexts of model `name` created under ENVS[env_name] whose KV caches differ
+    only in a way their contract says does not show (a paged context and its contiguous twin; a bf16 or
+    e4m3 cache and the fp32 cache of its rounded values), on test_long_context's paths: teacher-forced
+    forward at the checked positions, the caches below the appended count, the chunked prefill across
+    last_short, score, forward_batch / forward_ragged / verify_argmax_ragged at per-query T, and forks at
+    page-unaligned positions, the last one followed by decode steps."""
+    from test_gpu_bf16 import _eq
+    from test_gpu_kv_paged import same_rows
+    sms = sm_count()
+    ck = a.ck
+    S = ck.seq_len
+    check = checked(MODELS[name][0], sms)
+    tl = last_short(ck.n_heads, S, sms)
+    toks = teacher_tokens(S, ck.vocab_size)
+    for pos, tok in enumerate(toks):
+        la, lb = a.forward(tok, pos), b.forward(tok, pos)
+        if pos in check:
+            _eq(la, lb, f"logits at {pos}")
+    same_rows(a, b, S, "forward")
+    _eq(a.state("x"), b.state("x"), "x")
+    for x in (a, b):
+        x.reset()
+    for lo, hi in zip([0, 37, tl - 1, tl + 2], [37, tl - 1, tl + 2, S]):
+        _eq(a.prefill(toks[lo:hi], lo), b.prefill(toks[lo:hi], lo), f"prefill {lo}..{hi}")
+    same_rows(a, b, S, "prefill")
+    for x in (a, b):
+        x.reset()
+    for x, y, what in zip(a.score(toks), b.score(toks), ("log-probs", "greedy")):
+        _eq(x, y, f"score {what}")                      # a and b now hold S - 1 positions
+
+    with l2b_env(ENVS[env_name]):
+        sa, sb = [a.session() for _ in range(3)], [b.session() for _ in range(3)]
+    try:
+        ta, tb = [a] + sa, [b] + sb
+        ps = [S - 1, 3, 299, tl]                       # the sessions take 3, 299 and tl rows by fork
+        for t in (ta, tb):
+            for s, q in zip(t[1:], ps[1:]):
+                l2b.fork(t[0], [s], q)
+        _eq(l2b.forward_batch(ta, [toks[q] for q in ps], ps),
+            l2b.forward_batch(tb, [toks[q] for q in ps], ps), "forward_batch")
+        for x, y, q in zip(ta, tb, ps):
+            same_rows(x, y, q + 1, "forward_batch")
+        # session 1's prompt crosses tl / tl + 1 in chunks while the context decodes its last 3 positions
+        cuts = [0, 37, tl - 1, tl + 1]
+        for i in range(3):
+            runs, pos = [toks[cuts[i]:cuts[i + 1]], [toks[S - 3 + i]]], [cuts[i], S - 3 + i]
+            _eq(l2b.forward_ragged([ta[1], a], runs, pos), l2b.forward_ragged([tb[1], b], runs, pos),
+                f"forward_ragged {i}")
+        same_rows(ta[1], tb[1], tl + 1, "forward_ragged")
+        same_rows(a, b, S, "forward_ragged")
+        runs, pos = [toks[S - 4:S], toks[tl:tl + 1]], [S - 4, tl]
+        va = l2b.verify_argmax_ragged([a, ta[3]], runs, pos)
+        vb = l2b.verify_argmax_ragged([b, tb[3]], runs, pos)
+        _eq(va[1], vb[1], "n_accept")
+        for x, y in zip(va[0], vb[0]):
+            _eq(x, y, "verify greedy")
+        n_fork = 4000                                  # 62.5 pages of 64 rows
+        for t in (ta, tb):
+            l2b.fork(t[0], t[1:3], n_fork)
+        for s, u in zip(ta[1:3], tb[1:3]):
+            same_rows(s, u, n_fork, "fork")
+            for q in range(n_fork, n_fork + 4):
+                _eq(s.forward(toks[q], q), u.forward(toks[q], q), f"after the fork at {q}")
+    finally:
+        for s in sa + sb:
+            s.close()
 
 
 def test_split_rows_regimes():
