@@ -292,59 +292,79 @@ int dev_alloc(l2b_ctx *ctx, T **p, size_t count, std::vector<void *> *owner = nu
     return L2B_OK;
 }
 
-// ---- device weight format ----
-bool is_bf16(const l2b_ctx *ctx) { return ctx->wfmt == L2B_WEIGHTS_BF16; }
-bool is_q8(const l2b_ctx *ctx) { return ctx->wfmt == L2B_WEIGHTS_Q8; }
-// bytes of a stored element and elements from one row to the next, of a matrix in format fmt
-size_t fmt_elem(int fmt) { return fmt == L2B_WEIGHTS_BF16 ? 2 : fmt == L2B_WEIGHTS_Q8 ? 1 : 4; }
-uint64_t fmt_ld(int fmt, uint64_t cols) {
-    return fmt == L2B_WEIGHTS_BF16 ? (uint64_t)w_pitch<bf16>((int)cols)
-           : fmt == L2B_WEIGHTS_Q8 ? (uint64_t)w_pitch<q8>((int)cols) : cols;
-}
-size_t w_elem(const l2b_ctx *ctx) { return fmt_elem(ctx->wfmt); }
-// ---- KV-cache format ----
-bool kv_bf16(const l2b_ctx *ctx) { return ctx->kvfmt == L2B_KV_BF16; }
-bool kv_e4m3(const l2b_ctx *ctx) { return ctx->kvfmt == L2B_KV_E4M3; }
-// the formats whose kernels take the model's scales: the e4m3 cache and its fp32 reference
-bool kv_scaled(int kvfmt) { return kvfmt == L2B_KV_E4M3 || kvfmt == L2B_KV_ROUND_E4M3; }
-size_t kv_elem(const l2b_ctx *ctx) { return kv_bf16(ctx) ? 2 : kv_e4m3(ctx) ? 1 : 4; }
-// what the QKV epilogue stores: the kernels' KV type (float, bf16, kv_f32_bf16, e4m3, kv_f32_e4m3), or'd
-// with KS_PAGED for their kv_paged<> forms
-enum KvStore { KS_F32, KS_BF16, KS_ROUND, KS_E4M3, KS_ROUND_E4M3, KS_PAGED = 8 };
-int kv_store(const l2b_ctx *ctx) {
-    const int ks = kv_bf16(ctx) ? KS_BF16 : ctx->kvfmt == L2B_KV_ROUND_BF16 ? KS_ROUND
-                   : kv_e4m3(ctx) ? KS_E4M3 : ctx->kvfmt == L2B_KV_ROUND_E4M3 ? KS_ROUND_E4M3 : KS_F32;
-    return ks | (ctx->paged ? KS_PAGED : 0);
-}
-// the cache format the attention kernels are picked for: kvfmt, or'd with L2B_KV_PAGED
-int kv_kernels(const l2b_ctx *ctx) { return ctx->kvfmt | (ctx->paged ? L2B_KV_PAGED : 0); }
+// ---- formats: the one place a weight or KV format value becomes the C++ type the kernels are templated on.
+// Each visitor calls f(type_tag<T>()) and has a case for every format; split_format admits no other value,
+// so anything else is a defect here and aborts.
 template <typename T> struct type_tag { typedef T type; };
+
+// ---- device weight format: the weight element W (float, bf16 or q8)
+template <typename F>
+auto with_w(int wfmt, F f) {
+    switch (wfmt) {
+    case L2B_WEIGHTS_F32: return f(type_tag<float>());
+    case L2B_WEIGHTS_BF16: return f(type_tag<bf16>());
+    case L2B_WEIGHTS_Q8: return f(type_tag<q8>());
+    }
+    abort();
+}
+// bytes of a stored element and elements from one row to the next, of a matrix in the context's format
+size_t w_elem(const l2b_ctx *ctx) { return with_w(ctx->wfmt, [](auto w) { return sizeof(typename decltype(w)::type); }); }
+uint64_t w_ld(const l2b_ctx *ctx, uint64_t cols) {
+    return with_w(ctx->wfmt, [cols](auto w) { return (uint64_t)w_pitch<typename decltype(w)::type>((int)cols); });
+}
+
+// ---- KV-cache format (kvfmt, with the layout flag `paged` apart)
+// the element E a cache stores: the round-trip references are fp32 caches
+template <typename F>
+auto with_kv_elem(int kvfmt, F f) {
+    switch (kvfmt) {
+    case 0:                                       // fp32
+    case L2B_KV_ROUND_BF16:
+    case L2B_KV_ROUND_E4M3: return f(type_tag<float>());
+    case L2B_KV_BF16: return f(type_tag<bf16>());
+    case L2B_KV_E4M3: return f(type_tag<e4m3>());
+    }
+    abort();
+}
 // f(type_tag<E>()) or f(type_tag<kv_paged<E>>()) for element type E
 template <typename E, typename F>
 auto kv_layout(bool paged, F f) { return paged ? f(type_tag<kv_paged<E>>()) : f(type_tag<E>()); }
-// f(type_tag<KV>()) for the kernels' KV type of KvStore ks
+// the KV type the QKV epilogue writes the context's cache with: float, bf16, kv_f32_bf16, e4m3 or kv_f32_e4m3,
+// in its kv_paged<> form on a paged cache
 template <typename F>
-auto kv_dispatch(int ks, F f) {
-    const bool pg = (ks & KS_PAGED) != 0;
-    switch (ks & ~KS_PAGED) {
-    case KS_BF16: return kv_layout<bf16>(pg, f);
-    case KS_ROUND: return kv_layout<kv_f32_bf16>(pg, f);
-    case KS_E4M3: return kv_layout<e4m3>(pg, f);
-    case KS_ROUND_E4M3: return kv_layout<kv_f32_e4m3>(pg, f);
-    default: return kv_layout<float>(pg, f);
+auto with_kv_store(const l2b_ctx *ctx, F f) {
+    switch (ctx->kvfmt) {
+    case 0: return kv_layout<float>(ctx->paged, f);
+    case L2B_KV_BF16: return kv_layout<bf16>(ctx->paged, f);
+    case L2B_KV_ROUND_BF16: return kv_layout<kv_f32_bf16>(ctx->paged, f);
+    case L2B_KV_E4M3: return kv_layout<e4m3>(ctx->paged, f);
+    case L2B_KV_ROUND_E4M3: return kv_layout<kv_f32_e4m3>(ctx->paged, f);
+    }
+    abort();
+}
+// the KV type the attention kernels read the context's cache with: its element, kv_paged<> on a paged cache
+template <typename F>
+auto with_kv_read(const l2b_ctx *ctx, F f) {
+    return with_kv_elem(ctx->kvfmt, [ctx, &f](auto e) { return kv_layout<typename decltype(e)::type>(ctx->paged, f); });
+}
+size_t kv_elem(const l2b_ctx *ctx) { return with_kv_elem(ctx->kvfmt, [](auto e) { return sizeof(typename decltype(e)::type); }); }
+// n stored elements at `from` widened on the host to the fp32 values they stand for (e4m3: under the layer's
+// scale s).  Front to back, each element read before its value is written, so `to` may overlap `from` where
+// value i ends at or below element i + 1 (the in-place widening of l2b_read_state).
+void kv_widen(type_tag<float>, const unsigned char *from, float *to, uint64_t n, float) { memmove(to, from, n * 4); }
+void kv_widen(type_tag<bf16>, const unsigned char *from, float *to, uint64_t n, float) {
+    for (uint64_t i = 0; i < n; ++i) {
+        uint16_t h;
+        memcpy(&h, from + 2 * i, 2);
+        const uint32_t u = (uint32_t)h << 16;
+        memcpy(to + i, &u, 4);
     }
 }
-// f(type_tag<KV>()) for the KV type the attention kernels read a cache of format kvfmt (kv_kernels) with:
-// the reference formats are fp32 caches and take the fp32 kernels
-template <typename F>
-auto kv_read_dispatch(int kvfmt, F f) {
-    const bool pg = (kvfmt & L2B_KV_PAGED) != 0;
-    switch (kvfmt & ~L2B_KV_PAGED) {
-    case L2B_KV_BF16: return kv_layout<bf16>(pg, f);
-    case L2B_KV_E4M3: return kv_layout<e4m3>(pg, f);
-    default: return kv_layout<float>(pg, f);
-    }
+void kv_widen(type_tag<e4m3>, const unsigned char *from, float *to, uint64_t n, float s) {
+    for (uint64_t i = 0; i < n; ++i) to[i] = e4m3_widen(from[i], s);
 }
+// the formats whose kernels take the model's scales: the e4m3 cache and its fp32 reference
+bool kv_scaled(int kvfmt) { return kvfmt == L2B_KV_E4M3 || kvfmt == L2B_KV_ROUND_E4M3; }
 // layer l's (s_k, s_v) on the device, or nullptr for a format without scales
 const float *kv_scale_at(const l2b_ctx *ctx, int l) {
     return ctx->weights && ctx->weights->kv_scale ? ctx->weights->kv_scale + 2 * (size_t)l : nullptr;
@@ -354,7 +374,6 @@ void *kv_layer(const l2b_ctx *ctx, void *cache, int layer) {
     if (ctx->paged) return static_cast<void **>(cache) + (size_t)layer * ctx->n_pages;
     return static_cast<unsigned char *>(cache) + (size_t)layer * ctx->cfg.seq_len * ctx->kv_loc * kv_elem(ctx);   // :354
 }
-uint64_t w_ld(const l2b_ctx *ctx, uint64_t cols) { return fmt_ld(ctx->wfmt, cols); }
 // row `row` of a matrix of `cols` columns that starts at base
 const void *wrow(const l2b_ctx *ctx, const void *base, uint64_t row, uint64_t cols) {
     return static_cast<const unsigned char *>(base) + row * w_ld(ctx, cols) * w_elem(ctx);
@@ -434,7 +453,22 @@ int64_t quantize_q8_row(const float *w, uint64_t cols, unsigned char *rec) {
     return changed;
 }
 
-int upload(l2b_ctx *ctx, void *dst, const float *src, uint64_t rows, uint64_t cols, uint64_t src_pitch, int fmt) {
+// Rounds one row of cols fp32 weights to bf16 (bf16_round_bits) into d, zero-padded to ld elements; returns
+// how many weights the rounding changed.
+int64_t round_bf16_row(const float *w, uint64_t cols, uint64_t ld, uint16_t *d) {
+    int64_t changed = 0;
+    for (uint64_t c = 0; c < cols; ++c) {
+        uint32_t u;
+        memcpy(&u, w + c, 4);
+        d[c] = bf16_round_bits(u);
+        changed += ((uint32_t)d[c] << 16) != u;
+    }
+    for (uint64_t c = cols; c < ld; ++c) d[c] = 0;
+    return changed;
+}
+
+template <typename W>
+int upload(l2b_ctx *ctx, void *dst, const float *src, uint64_t rows, uint64_t cols, uint64_t src_pitch) {
     if (!ctx->stage[0]) {
         size_t want = 32ull << 20;
         const char *env = getenv("L2B_STAGE_MB");
@@ -445,13 +479,12 @@ int upload(l2b_ctx *ctx, void *dst, const float *src, uint64_t rows, uint64_t co
             L2B_CUDA(ctx, cudaEventCreateWithFlags(&ctx->stage_ev[i], cudaEventDisableTiming));
         }
     }
-    // bf16: each row is rounded (bf16_round_bits) and padded with zeros to w_ld elements while it is
-    // packed into the stage, so the DMA moves dense bf16 rows.  q8: each row is quantized into its row
-    // record (quantize_q8_row).
-    const bool bf16w = fmt == L2B_WEIGHTS_BF16, q8w = fmt == L2B_WEIGHTS_Q8;
-    const uint64_t ld = fmt_ld(fmt, cols);
-    const uint64_t row_bytes = ld * fmt_elem(fmt);
-    const bool dense = (src_pitch == cols) && fmt == L2B_WEIGHTS_F32;
+    // Each row is packed into the stage in its stored form, so the DMA moves dense rows: bf16 rows are
+    // rounded and padded with zeros to w_pitch elements (round_bf16_row), q8 rows quantized into their row
+    // records (quantize_q8_row).
+    const uint64_t ld = (uint64_t)w_pitch<W>((int)cols);
+    const uint64_t row_bytes = ld * sizeof(W);
+    const bool dense = (src_pitch == cols) && std::is_same<W, float>::value;
     const uint64_t total = rows * row_bytes;
     uint64_t done = 0;                       // bytes of the dense destination already issued
     while (done < total) {
@@ -459,45 +492,29 @@ int upload(l2b_ctx *ctx, void *dst, const float *src, uint64_t rows, uint64_t co
         ctx->stage_next ^= 1;
         L2B_CUDA(ctx, cudaEventSynchronize(ctx->stage_ev[b]));   // previous DMA out of this buffer finished
         uint64_t chunk = total - done < ctx->stage_bytes ? total - done : ctx->stage_bytes;
-        if (bf16w) {
+        if (dense) {
+            memcpy(ctx->stage[b], reinterpret_cast<const unsigned char *>(src) + done, chunk);
+        } else {
+            // whole rows only (a chunk never splits a row of a sharded window)
             const uint64_t r = chunk / row_bytes;
             if (r == 0) return fail(ctx, L2B_ERR_UNSUPPORTED, "row larger than the upload staging buffer");
             chunk = r * row_bytes;
             const uint64_t row0 = done / row_bytes;
-            uint16_t *o = reinterpret_cast<uint16_t *>(ctx->stage[b]);
-            uint64_t changed = 0;
             for (uint64_t i = 0; i < r; ++i) {
                 const float *s = src + (row0 + i) * src_pitch;
-                uint16_t *d = o + i * ld;
-                for (uint64_t c = 0; c < cols; ++c) {
-                    uint32_t u;
-                    memcpy(&u, s + c, 4);
-                    d[c] = bf16_round_bits(u);
-                    changed += ((uint32_t)d[c] << 16) != u;
+                unsigned char *d = ctx->stage[b] + i * row_bytes;
+                int64_t changed = 0;
+                if constexpr (std::is_same<W, q8>::value) {
+                    changed = quantize_q8_row(s, cols, d);
+                    if (changed < 0) return fail(ctx, L2B_ERR_INVALID_ARG, "non-finite matrix weight in a q8 payload");
+                } else if constexpr (std::is_same<W, bf16>::value) {
+                    changed = round_bf16_row(s, cols, ld, reinterpret_cast<uint16_t *>(d));
+                } else {
+                    static_assert(std::is_same<W, float>::value, "a weight element type");
+                    memcpy(d, s, row_bytes);
                 }
-                for (uint64_t c = cols; c < ld; ++c) d[c] = 0;
-            }
-            ctx->n_rounded += changed;
-        } else if (q8w) {
-            const uint64_t r = chunk / row_bytes;
-            if (r == 0) return fail(ctx, L2B_ERR_UNSUPPORTED, "row larger than the upload staging buffer");
-            chunk = r * row_bytes;
-            const uint64_t row0 = done / row_bytes;
-            for (uint64_t i = 0; i < r; ++i) {
-                const int64_t changed = quantize_q8_row(src + (row0 + i) * src_pitch, cols, ctx->stage[b] + i * row_bytes);
-                if (changed < 0) return fail(ctx, L2B_ERR_INVALID_ARG, "non-finite matrix weight in a q8 payload");
                 ctx->n_rounded += (uint64_t)changed;
             }
-        } else if (!dense) {
-            // whole rows only (a chunk never splits a row of a sharded window)
-            uint64_t r = chunk / row_bytes;
-            if (r == 0) return fail(ctx, L2B_ERR_UNSUPPORTED, "row larger than the upload staging buffer");
-            chunk = r * row_bytes;
-            const uint64_t row0 = done / row_bytes;
-            for (uint64_t i = 0; i < r; ++i)
-                memcpy(ctx->stage[b] + i * row_bytes, src + (row0 + i) * src_pitch, row_bytes);
-        } else {
-            memcpy(ctx->stage[b], reinterpret_cast<const unsigned char *>(src) + done, chunk);
         }
         L2B_CUDA(ctx, cudaMemcpyAsync(reinterpret_cast<unsigned char *>(dst) + done, ctx->stage[b], chunk,
                                       cudaMemcpyHostToDevice, ctx->stream));
@@ -508,18 +525,18 @@ int upload(l2b_ctx *ctx, void *dst, const float *src, uint64_t rows, uint64_t co
     return L2B_OK;
 }
 
-// matrix: a weight matrix, stored in the context's format (wfmt); otherwise fp32 (RMSNorm gains).
-// A bf16 or q8 matrix is only ever whole (single GPU).
+// A tensor stored as elements W.  A bf16 or q8 matrix is only ever whole (single GPU).
+template <typename W>
 int materialize(l2b_ctx *ctx, void **dptr, const Source &src, uint64_t payload_off, int tensor_id,
-                uint64_t L, uint64_t rows, uint64_t cols, ShardMode mode, Dist dist, bool matrix) {
+                uint64_t L, uint64_t rows, uint64_t cols, ShardMode mode, Dist dist) {
     const uint64_t g = ctx->world, r = ctx->rank;
     const uint64_t rows_loc = (mode == SH_ROWS) ? rows / g : rows;
     const uint64_t cols_loc = (mode == SH_COLS) ? cols / g : cols;
     const uint64_t row0 = (mode == SH_ROWS) ? r * rows_loc : 0;
     const uint64_t col0 = (mode == SH_COLS) ? r * cols_loc : 0;
-    const int fmt = matrix ? ctx->wfmt : L2B_WEIGHTS_F32;
-    const uint64_t ld = fmt_ld(fmt, cols_loc);
-    const size_t esize = fmt_elem(fmt);
+    const uint64_t ld = (uint64_t)w_pitch<W>((int)cols_loc);
+    const size_t esize = sizeof(W);
+    constexpr bool f32 = std::is_same<W, float>::value;
     unsigned char *base = nullptr;
     int rc = dev_alloc(ctx, &base, L * rows_loc * ld * esize, &ctx->weights->owned);
     if (rc) return rc;
@@ -528,13 +545,20 @@ int materialize(l2b_ctx *ctx, void **dptr, const Source &src, uint64_t payload_o
     const bool whole = (rows_loc == rows && cols_loc == cols);
     const uint64_t nl = whole ? 1 : L;            // one shot when nothing is cut
     const uint64_t rr = whole ? L * rows : rows_loc;
-    if (fmt != L2B_WEIGHTS_F32 && !src.host)     // the row padding; the upload writes its own zeros
+    if (!f32 && !src.host) {
+        // the row padding (the upload writes its own zeros), and the device count of weights the synthesis
+        // rounds, read back when the weights are in place
         L2B_CUDA(ctx, cudaMemsetAsync(base, 0, L * rows_loc * ld * esize, ctx->stream));
+        if (!ctx->d_rounded) {
+            if ((rc = dev_alloc(ctx, &ctx->d_rounded, 1))) return rc;
+            L2B_CUDA(ctx, cudaMemsetAsync(ctx->d_rounded, 0, sizeof(unsigned long long), ctx->stream));
+        }
+    }
     for (uint64_t l = 0; l < nl; ++l) {
         void *dst = base + l * rows_loc * ld * esize;
         const uint64_t first = l * rows * cols + row0 * cols + col0;
         if (src.host) {
-            rc = upload(ctx, dst, src.host + payload_off + first, rr, cols_loc, cols, fmt);
+            rc = upload<W>(ctx, dst, src.host + payload_off + first, rr, cols_loc, cols);
             if (rc) return rc;
         } else {
             const uint64_t total = rr * cols_loc;
@@ -542,24 +566,32 @@ int materialize(l2b_ctx *ctx, void **dptr, const Source &src, uint64_t payload_o
                                    ? (total + 255) / 256
                                    : (uint64_t)(ctx->num_sms * 16));
             if (blocks < 1) blocks = 1;
-            if (fmt == L2B_WEIGHTS_Q8) {
+            if constexpr (std::is_same<W, q8>::value) {
                 const uint64_t groups = rr * (uint64_t)q8_groups((int)cols_loc);   // one thread per group
                 const int gblocks = (int)std::min<uint64_t>((groups + 255) / 256, (uint64_t)ctx->num_sms * 16);
                 synth_fill_q8_kernel<<<gblocks < 1 ? 1 : gblocks, 256, 0, ctx->stream>>>(
                     static_cast<unsigned char *>(dst), rr, cols_loc, first, cols, tensor_seed, dist.mean,
                     dist.sigma * kSynthInvStd, dist.lo, dist.hi, ctx->d_rounded);
-            } else if (fmt == L2B_WEIGHTS_BF16)
+            } else if constexpr (std::is_same<W, bf16>::value) {
                 synth_fill_bf16_kernel<<<blocks, 256, 0, ctx->stream>>>(
                     static_cast<uint16_t *>(dst), rr, cols_loc, first, cols, tensor_seed, dist.mean,
                     dist.sigma * kSynthInvStd, dist.lo, dist.hi, ctx->d_rounded);
-            else
+            } else {
+                static_assert(f32, "a weight element type");
                 synth_fill_kernel<<<blocks, 256, 0, ctx->stream>>>(static_cast<float *>(dst), rr, cols_loc, first, cols,
                                                                    tensor_seed, dist.mean, dist.sigma * kSynthInvStd,
                                                                    dist.lo, dist.hi);
+            }
             L2B_CUDA(ctx, cudaGetLastError());
         }
     }
     return L2B_OK;
+}
+// matrix: a weight matrix, stored in the context's format (wfmt); otherwise fp32 (RMSNorm gains)
+int materialize(l2b_ctx *ctx, void **dptr, const Source &src, uint64_t payload_off, int tensor_id,
+                uint64_t L, uint64_t rows, uint64_t cols, ShardMode mode, Dist dist, bool matrix) {
+    auto as = [&](auto w) { return materialize<typename decltype(w)::type>(ctx, dptr, src, payload_off, tensor_id, L, rows, cols, mode, dist); };
+    return matrix ? with_w(ctx->wfmt, as) : as(type_tag<float>());
 }
 int materialize(l2b_ctx *ctx, float **dptr, const Source &src, uint64_t payload_off, int tensor_id,
                 uint64_t L, uint64_t rows, uint64_t cols, ShardMode mode, Dist dist) {
@@ -572,9 +604,28 @@ int materialize(l2b_ctx *ctx, float **dptr, const Source &src, uint64_t payload_
 // ---- GEMV launch ---------------------------------------------------------------------------
 typedef void (*gemv_fn)(const GemvParams);
 
-// Kernel instantiations by weight element type W.  EPI_XCHG (tensor parallel) has fp32 kernels only:
-// bf16 and q8 weights are single-GPU.
-template <int EPI, typename W, typename KV = float>
+// The kernel of epilogue epi in one GEMV family for weights W: fam(std::integral_constant<int, EPI>(),
+// type_tag<KV>()) names the family's instance.  KV is the context's store type for EPI_QKV, the one epilogue
+// that writes the cache, and float otherwise.  EPI_XCHG (tensor parallel) has kernels only for fp32 weights
+// (bf16 and q8 weights are single-GPU) and only in the families that declare it (XCHG); nullptr where there
+// is no kernel.
+template <typename W, bool XCHG, typename F>
+gemv_fn pick_epi(const l2b_ctx *ctx, int epi, F fam) {
+    auto f32 = type_tag<float>();
+    switch (epi) {
+    case EPI_STORE: return fam(std::integral_constant<int, EPI_STORE>(), f32);
+    case EPI_ARGMAX: return fam(std::integral_constant<int, EPI_ARGMAX>(), f32);
+    case EPI_QKV: return with_kv_store(ctx, [&fam](auto kv) { return fam(std::integral_constant<int, EPI_QKV>(), kv); });
+    case EPI_SILU: return fam(std::integral_constant<int, EPI_SILU>(), f32);
+    case EPI_XCHG:
+        if constexpr (XCHG && std::is_same<W, float>::value) return fam(std::integral_constant<int, EPI_XCHG>(), f32);
+        return nullptr;
+    case EPI_RESID: return fam(std::integral_constant<int, EPI_RESID>(), f32);
+    }
+    return nullptr;
+}
+// the latency kernel's instance for tpr threads per row pair
+template <int EPI, typename W, typename KV>
 gemv_fn gemv_pick(int tpr) {
     switch (tpr) {
     case 8: return gemv_kernel<8, EPI, W, KV>;
@@ -582,21 +633,9 @@ gemv_fn gemv_pick(int tpr) {
     case 32: return gemv_kernel<32, EPI, W, KV>;
     case 64: return gemv_kernel<64, EPI, W, KV>;
     case 128: return gemv_kernel<128, EPI, W, KV>;
-    default: return gemv_kernel<256, EPI, W, KV>;
+    case 256: return gemv_kernel<256, EPI, W, KV>;
     }
-}
-// and by KV store (KvStore) for EPI_QKV, the one epilogue that writes the cache
-template <typename W>
-gemv_fn gemv_pick(int epi, int tpr, int ks) {
-    switch (epi) {
-    case EPI_XCHG: return sizeof(W) == 4 ? gemv_pick<EPI_XCHG, float>(tpr) : nullptr;
-    case EPI_RESID: return gemv_pick<EPI_RESID, W>(tpr);
-    case EPI_STORE: return gemv_pick<EPI_STORE, W>(tpr);
-    case EPI_ARGMAX: return gemv_pick<EPI_ARGMAX, W>(tpr);
-    case EPI_QKV:
-        return kv_dispatch(ks, [tpr](auto t) { return gemv_pick<EPI_QKV, W, typename decltype(t)::type>(tpr); });
-    default: return gemv_pick<EPI_SILU, W>(tpr);
-    }
+    return nullptr;
 }
 
 constexpr int kMaxDynSmem = 200 * 1024;
@@ -624,48 +663,26 @@ int prof_mark(l2b_ctx *ctx, const char *name, int layer, uint64_t bytes, cudaStr
     return L2B_OK;
 }
 
-template <typename W>
-gemv_fn gemv_tma_pick(int epi, int ks) {
-    switch (epi) {
-    case EPI_XCHG: return sizeof(W) == 4 ? gemv_tma_kernel<EPI_XCHG, float> : nullptr;
-    case EPI_RESID: return gemv_tma_kernel<EPI_RESID, W>;
-    case EPI_STORE: return gemv_tma_kernel<EPI_STORE, W>;
-    case EPI_ARGMAX: return gemv_tma_kernel<EPI_ARGMAX, W>;
-    case EPI_QKV:
-        return kv_dispatch(ks, [](auto t) { return (gemv_fn)gemv_tma_kernel<EPI_QKV, W, typename decltype(t)::type>; });
-    default: return gemv_tma_kernel<EPI_SILU, W>;
-    }
-}
-
-template <typename W>
-gemv_fn gemv8_pick(int epi, int ks) {
-    switch (epi) {
-    case EPI_XCHG: return sizeof(W) == 4 ? gemv8_kernel<EPI_XCHG, float> : nullptr;
-    case EPI_RESID: return gemv8_kernel<EPI_RESID, W>;
-    case EPI_STORE: return gemv8_kernel<EPI_STORE, W>;
-    case EPI_ARGMAX: return gemv8_kernel<EPI_ARGMAX, W>;
-    case EPI_QKV:
-        return kv_dispatch(ks, [](auto t) { return (gemv_fn)gemv8_kernel<EPI_QKV, W, typename decltype(t)::type>; });
-    default: return gemv8_kernel<EPI_SILU, W>;
-    }
-}
-
 // GEMV kernel families: the latency kernel (gemv_kernel, tpr threads per row pair), the register-fed
 // 8-row kernel and the TMA ring
 enum GemvKind { GK_LATENCY, GK_ROWS8, GK_TMA };
 
-// the formats an epilogue has kernels in: EPI_XCHG (tensor parallel) is fp32 only
-bool has_kernel(const l2b_ctx *ctx, int epi) { return !(ctx->wfmt != L2B_WEIGHTS_F32 && epi == EPI_XCHG); }
-
-// The one place a GEMV kernel is chosen for the context's weight format and KV store.  The shape rules
-// that pick `kind` are the same for every format (computed at 4 bytes per weight).
+// The one place a GEMV kernel is chosen for the context's weight format and KV store; nullptr where the
+// format has none.  The shape rules that pick `kind` are the same for every format (computed at 4 bytes
+// per weight).
 gemv_fn pick_gemv(const l2b_ctx *ctx, GemvKind kind, int epi, int tpr) {
-    const int ks = kv_store(ctx);
-    if (is_q8(ctx))
-        return kind == GK_TMA ? gemv_tma_pick<q8>(epi, ks) : kind == GK_ROWS8 ? gemv8_pick<q8>(epi, ks) : gemv_pick<q8>(epi, tpr, ks);
-    if (is_bf16(ctx))
-        return kind == GK_TMA ? gemv_tma_pick<bf16>(epi, ks) : kind == GK_ROWS8 ? gemv8_pick<bf16>(epi, ks) : gemv_pick<bf16>(epi, tpr, ks);
-    return kind == GK_TMA ? gemv_tma_pick<float>(epi, ks) : kind == GK_ROWS8 ? gemv8_pick<float>(epi, ks) : gemv_pick<float>(epi, tpr, ks);
+    return with_w(ctx->wfmt, [&](auto w) -> gemv_fn {
+        using W = typename decltype(w)::type;
+        switch (kind) {
+        case GK_LATENCY:
+            return pick_epi<W, true>(ctx, epi, [tpr](auto e, auto kv) { return gemv_pick<decltype(e)::value, W, typename decltype(kv)::type>(tpr); });
+        case GK_ROWS8:
+            return pick_epi<W, true>(ctx, epi, [](auto e, auto kv) { return (gemv_fn)gemv8_kernel<decltype(e)::value, W, typename decltype(kv)::type>; });
+        case GK_TMA:
+            return pick_epi<W, true>(ctx, epi, [](auto e, auto kv) { return (gemv_fn)gemv_tma_kernel<decltype(e)::value, W, typename decltype(kv)::type>; });
+        }
+        return nullptr;
+    });
 }
 
 cudaLaunchAttribute pdl_attr() {
@@ -700,7 +717,7 @@ int launch_gemv(l2b_ctx *ctx, int epi, const GemvParams &p, cudaStream_t st, con
     }
     const size_t xbytes = (size_t)p.n * 4 * (1 + (p.gamma ? 1 : 0) + (p.parts ? 1 : 0));
     const size_t xonly = (size_t)p.n * 4;
-    const size_t slot_bytes = is_q8(ctx) ? (size_t)DecodeRing<q8>::SLOT_BYTES : (size_t)DecodeRing<float>::SLOT_BYTES;   // = DecodeRing<bf16>'s
+    const size_t slot_bytes = with_w(ctx->wfmt, [](auto w) { return (size_t)DecodeRing<typename decltype(w)::type>::SLOT_BYTES; });
     // Decision from the shape.  Bandwidth-bound shapes take the TMA-ring kernel, latency-bound ones
     // the fine-grained kernel.  The ring kernel stages only x in shared memory; the rest of the
     // opt-in limit is its ring of 16 KB slots (13 next to a 16 KB x; DESIGN.md §4.1).
@@ -723,8 +740,8 @@ int launch_gemv(l2b_ctx *ctx, int epi, const GemvParams &p, cudaStream_t st, con
     if (smem > (size_t)kMaxSmemOptin) return fail(ctx, L2B_ERR_UNSUPPORTED, "activation vector too large for shared memory");
     if (tma && nstage < 2) return fail(ctx, L2B_ERR_UNSUPPORTED, "TMA ring of fewer than 2 stages");
     const int tpr = gemv_tpr(p.n);
-    if (!has_kernel(ctx, epi)) return fail(ctx, L2B_ERR_UNSUPPORTED, "no kernel for this epilogue in the context's weight format");
     gemv_fn fn = pick_gemv(ctx, tma ? GK_TMA : big ? GK_ROWS8 : GK_LATENCY, epi, tpr);
+    if (!fn) return fail(ctx, L2B_ERR_UNSUPPORTED, "no kernel for this epilogue in the context's weight format");
     if (!ctx->attr_done.count((const void *)fn)) {
         L2B_CUDA(ctx, cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmemOptin));
         ctx->attr_done.insert((const void *)fn);
@@ -764,69 +781,61 @@ int launch_gemv(l2b_ctx *ctx, int epi, const GemvParams &p, cudaStream_t st, con
 }
 
 typedef void (*attn_fn)(const AttnParams, const AttnBatch);
-template <typename KV>
-attn_fn attention_flash_pick(int nf) {
-    switch (nf) {
-    case 1: return attention_flash_kernel<1, KV>;
-    case 2: return attention_flash_kernel<2, KV>;
-    case 3: return attention_flash_kernel<3, KV>;
-    case 4: return attention_flash_kernel<4, KV>;
-    case 5: return attention_flash_kernel<5, KV>;
-    case 6: return attention_flash_kernel<6, KV>;
-    case 8: return attention_flash_kernel<8, KV>;
-    default: return nullptr;
-    }
-}
-// the 3-pass kernel and the fork copy for cache format kvfmt (the attention kernels: or'd with L2B_KV_PAGED,
-// kv_kernels)
-attn_fn attention_3pass(int kvfmt) {
-    return kv_read_dispatch(kvfmt, [](auto t) { return (attn_fn)attention_kernel<typename decltype(t)::type>; });
-}
-const void *kv_fork_pick(int kvfmt) {
-    return kvfmt == L2B_KV_BF16 ? (const void *)kv_fork_kernel<bf16>
-           : kvfmt == L2B_KV_E4M3 ? (const void *)kv_fork_kernel<e4m3> : (const void *)kv_fork_kernel<float>;
-}
-// flash-decoding form when head_size/4 splits into 1..8 float4 per lane, else the 3-pass kernel; the
-// instance for cache format kvfmt (the choice does not depend on it)
-attn_fn pick_attention(int head_size, bool flash, size_t *smem, int kvfmt = 0) {
+typedef void (*attn_wo_fn)(const AttnWoParams);
+
+// The flash-decoding shape of head_size: lpr lanes share a row, each holding nf float4; a CTA covers ng rows.
+// The flash kernel's dynamic shared memory follows from it, and attn_wo_kernel's adds the CTA's
+// unnormalised output with its M and L, and the merged head output (page staging apart: attn_request).
+struct AttnShape { int nf; size_t flash_smem, wo_smem; };
+AttnShape attn_shape(int head_size) {
     const int hs4 = head_size / 4;
     const int lpr = (hs4 % 8 == 0) ? 8 : (hs4 % 4 == 0) ? 4 : (hs4 % 2 == 0) ? 2 : 1;
-    const int nf = hs4 / lpr;
-    attn_fn f2 = nullptr;
-    if (flash) f2 = kv_read_dispatch(kvfmt, [nf](auto t) { return attention_flash_pick<typename decltype(t)::type>(nf); });
-    if (!f2) return attention_3pass(kvfmt);
-    const int ng = NWARP * (32 / lpr);
-    *smem = ((size_t)ng * head_size + 3 * (size_t)ng) * sizeof(float);
-    return f2;
+    const size_t ng = NWARP * (32 / lpr);
+    const size_t flash = (ng * head_size + 3 * ng) * sizeof(float);
+    return {hs4 / lpr, flash, flash + (2 * (size_t)head_size + 4) * sizeof(float)};
+}
+// f(std::integral_constant<int, NF>()) for the flash kernels' nf in {1..6, 8}; nullptr for any other nf
+template <typename Fn, typename F>
+Fn with_nf(int nf, F f) {
+    switch (nf) {
+    case 1: return f(std::integral_constant<int, 1>());
+    case 2: return f(std::integral_constant<int, 2>());
+    case 3: return f(std::integral_constant<int, 3>());
+    case 4: return f(std::integral_constant<int, 4>());
+    case 5: return f(std::integral_constant<int, 5>());
+    case 6: return f(std::integral_constant<int, 6>());
+    case 8: return f(std::integral_constant<int, 8>());
+    }
+    return nullptr;
 }
 
-typedef void (*attn_wo_fn)(const AttnWoParams);
-template <typename W, typename KV>
-attn_wo_fn attn_wo_pick(int nf) {
-    switch (nf) {
-    case 1: return attn_wo_kernel<1, W, KV>;
-    case 2: return attn_wo_kernel<2, W, KV>;
-    case 3: return attn_wo_kernel<3, W, KV>;
-    case 4: return attn_wo_kernel<4, W, KV>;
-    case 5: return attn_wo_kernel<5, W, KV>;
-    case 6: return attn_wo_kernel<6, W, KV>;
-    case 8: return attn_wo_kernel<8, W, KV>;
-    default: return nullptr;
-    }
+// flash-decoding form for KV when head_size has one (*smem: its request), else the 3-pass kernel
+template <typename KV = float>
+attn_fn pick_attention(int head_size, bool flash, size_t *smem) {
+    const AttnShape sh = attn_shape(head_size);
+    attn_fn f = nullptr;
+    if (flash) f = with_nf<attn_fn>(sh.nf, [](auto nf) { return attention_flash_kernel<decltype(nf)::value, KV>; });
+    if (!f) return attention_kernel<KV>;
+    *smem = sh.flash_smem;
+    return f;
 }
-template <typename KV>
-attn_wo_fn attn_wo_pick(int nf, int wfmt) {
-    return wfmt == L2B_WEIGHTS_BF16 ? attn_wo_pick<bf16, KV>(nf) : wfmt == L2B_WEIGHTS_Q8 ? attn_wo_pick<q8, KV>(nf) : attn_wo_pick<float, KV>(nf);
+// the instance for the context's cache (which kernel it is does not depend on the cache)
+attn_fn pick_attention(const l2b_ctx *ctx, bool flash) {
+    size_t unused = 0;
+    return with_kv_read(ctx, [&](auto kv) { return pick_attention<typename decltype(kv)::type>(ctx->head_size, flash, &unused); });
 }
-// the attention + wo kernel for head_size in weight format wfmt and cache format kvfmt (whether one
-// exists depends on neither)
-attn_wo_fn pick_attn_wo(int head_size, size_t *smem, int wfmt = L2B_WEIGHTS_F32, int kvfmt = 0) {
-    const int hs4 = head_size / 4;
-    const int lpr = (hs4 % 8 == 0) ? 8 : (hs4 % 4 == 0) ? 4 : (hs4 % 2 == 0) ? 2 : 1;
-    const int nf = hs4 / lpr;
-    const int ng = NWARP * (32 / lpr);
-    *smem = ((size_t)ng * head_size + 3 * (size_t)ng + 2 * (size_t)head_size + 4) * sizeof(float);
-    return kv_read_dispatch(kvfmt, [nf, wfmt](auto t) { return attn_wo_pick<typename decltype(t)::type>(nf, wfmt); });
+
+// the attention + wo kernel for head_size, weights W and cache type KV; nullptr where head_size has no
+// flash form
+template <typename W = float, typename KV = float>
+attn_wo_fn pick_attn_wo(int head_size) {
+    return with_nf<attn_wo_fn>(attn_shape(head_size).nf, [](auto nf) { return attn_wo_kernel<decltype(nf)::value, W, KV>; });
+}
+// the instance for the context's weights and cache (whether one exists depends on neither)
+attn_wo_fn pick_attn_wo(const l2b_ctx *ctx) {
+    return with_w(ctx->wfmt, [ctx](auto w) {
+        return with_kv_read(ctx, [ctx](auto kv) { return pick_attn_wo<typename decltype(w)::type, typename decltype(kv)::type>(ctx->head_size); });
+    });
 }
 
 constexpr int kAttnClusterCtas = 8;   // CTAs per head cluster of attn_wo_kernel; 4 and 2 measured slower (DESIGN.md §4.6)
@@ -837,11 +846,8 @@ constexpr int kAttnClusterCtas = 8;   // CTAs per head cluster of attn_wo_kernel
 // them, so the two cannot disagree.
 enum AttnKind { ATTN_3PASS, ATTN_FLASH, ATTN_WO };
 size_t attn_request(const l2b_ctx *ctx, AttnKind k) {
+    if (k == ATTN_WO) return attn_shape(ctx->head_size).wo_smem + (ctx->paged ? ctx->attn_pg_bytes_wo : 0);
     size_t smem = ctx->attn_smem;
-    if (k == ATTN_WO) {
-        pick_attn_wo(ctx->head_size, &smem);
-        return smem + (ctx->paged ? ctx->attn_pg_bytes_wo : 0);
-    }
     pick_attention(ctx->head_size, k == ATTN_FLASH, &smem);
     return smem + (ctx->paged ? ctx->attn_pg_bytes : 0);
 }
@@ -868,8 +874,7 @@ int launch_attn_wo(l2b_ctx *ctx, int layer, cudaStream_t st) {
     q.parts = ctx->attn_parts;
     q.dim = ctx->dim;
     q.q_dim = ctx->q_loc;
-    size_t unused = 0;
-    attn_wo_fn fn = pick_attn_wo(ctx->head_size, &unused, ctx->wfmt, kv_kernels(ctx));
+    attn_wo_fn fn = pick_attn_wo(ctx);
     cudaLaunchConfig_t lc{};
     lc.gridDim = dim3(ctx->heads_loc, kAttnClusterCtas);
     lc.blockDim = dim3(NT);
@@ -918,8 +923,7 @@ int launch_attention(l2b_ctx *ctx, int layer, cudaStream_t st, const float *q, f
     a.kv_scale = kv_scale_at(ctx, layer);
     a.trace = zb ? nullptr : trace_slot(ctx);
     const AttnBatch none{};
-    size_t unused = 0;
-    attn_fn fn = pick_attention(ctx->head_size, ctx->attn_flash, &unused, kv_kernels(ctx));
+    attn_fn fn = pick_attention(ctx, ctx->attn_flash);
     cudaLaunchConfig_t lc{};
     lc.gridDim = dim3(ctx->heads_loc, ctx->nsplit, nb);
     lc.blockDim = dim3(NT);
@@ -1287,35 +1291,34 @@ int preload_kernels(l2b_ctx *ctx) {
     cudaFuncAttributes fa;
     const int tprs[] = {8, 16, 32, 64, 128, 256};
     for (int epi = 0; epi < EPI_COUNT; ++epi) {
-        if (!has_kernel(ctx, epi)) continue;
+        if (!pick_gemv(ctx, GK_TMA, epi, 0)) continue;   // EPI_XCHG: no kernel in a bf16 or q8 family
         for (int tpr : tprs) L2B_CUDA(ctx, cudaFuncGetAttributes(&fa, (const void *)pick_gemv(ctx, GK_LATENCY, epi, tpr)));
         L2B_CUDA(ctx, cudaFuncGetAttributes(&fa, (const void *)pick_gemv(ctx, GK_ROWS8, epi, 0)));
         L2B_CUDA(ctx, cudaFuncGetAttributes(&fa, (const void *)pick_gemv(ctx, GK_TMA, epi, 0)));
     }
-    size_t smem = 0;
-    L2B_CUDA(ctx, cudaFuncGetAttributes(&fa, (const void *)pick_attention(ctx->head_size, true, &smem, kv_kernels(ctx))));
-    if (attn_wo_fn aw = pick_attn_wo(ctx->head_size, &smem, ctx->wfmt, kv_kernels(ctx))) L2B_CUDA(ctx, cudaFuncGetAttributes(&fa, (const void *)aw));
-    const void *others[] = {(const void *)attention_3pass(kv_kernels(ctx)), (const void *)advance_kernel,
+    L2B_CUDA(ctx, cudaFuncGetAttributes(&fa, (const void *)pick_attention(ctx, true)));
+    if (attn_wo_fn aw = pick_attn_wo(ctx)) L2B_CUDA(ctx, cudaFuncGetAttributes(&fa, (const void *)aw));
+    const void *fork = with_kv_elem(ctx->kvfmt, [](auto e) { return (const void *)kv_fork_kernel<typename decltype(e)::type>; });
+    const void *others[] = {(const void *)pick_attention(ctx, false), (const void *)advance_kernel,
                             (const void *)batch_advance_kernel, (const void *)gather_logits_kernel,
                             (const void *)resid_add_kernel, (const void *)sample_prep_kernel,
                             (const void *)sample_prep_batch_kernel, (const void *)logprob_kernel,
                             (const void *)logprob_batch_kernel, (const void *)logprob_topk_batch_kernel,
                             (const void *)synth_fill_kernel,
                             (const void *)synth_fill_bf16_kernel, (const void *)synth_fill_q8_kernel,
-                            (const void *)kv_fork_pick(ctx->kvfmt), (const void *)verify_accept_kernel};
+                            fork, (const void *)verify_accept_kernel};
     for (const void *f : others) L2B_CUDA(ctx, cudaFuncGetAttributes(&fa, f));
     // The kernels that run next to a TMA-ring GEMV in a decode step (the ring GEMVs, attention, the
     // token advance) all ask for the largest shared-memory carveout, so consecutive kernels never
     // need a different L1 / shared split on an SM.  (A successor was not seen to enter an SM early
     // for it, DESIGN.md §4.1; what dropping the attribute costs or gains is not measured.)
-    const void *decode[] = {(const void *)pick_attention(ctx->head_size, true, &smem, kv_kernels(ctx)), (const void *)attention_3pass(kv_kernels(ctx)),
+    const void *decode[] = {(const void *)pick_attention(ctx, true), (const void *)pick_attention(ctx, false),
                             (const void *)advance_kernel};
     for (const void *f : decode)
         L2B_CUDA(ctx, cudaFuncSetAttribute(f, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
     for (int epi = 0; epi < EPI_COUNT; ++epi)
-        if (has_kernel(ctx, epi))
-            L2B_CUDA(ctx, cudaFuncSetAttribute((const void *)pick_gemv(ctx, GK_TMA, epi, 0),
-                                               cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+        if (gemv_fn f = pick_gemv(ctx, GK_TMA, epi, 0))
+            L2B_CUDA(ctx, cudaFuncSetAttribute((const void *)f, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
     return L2B_OK;
 }
 
@@ -1373,10 +1376,6 @@ int create_rank(l2b_ctx *ctx, const l2b_config *cfg, const Source &src, const fl
     const uint64_t o_wcls = off;
 
     const auto t_load0 = std::chrono::steady_clock::now();
-    if (ctx->wfmt != L2B_WEIGHTS_F32 && !src.host) {
-        L2B_TRY(dev_alloc(ctx, &ctx->d_rounded, 1));
-        L2B_TRY(cuda_try(ctx, cudaMemsetAsync(ctx->d_rounded, 0, sizeof(unsigned long long), ctx->stream), "memset"));
-    }
     L2B_TRY(materialize(ctx, &ctx->emb, src, o_emb, 1, 1, V, dim, SH_NONE, {0.0, 0.04, -BIG, BIG}, true));
     L2B_TRY(materialize(ctx, &ctx->rms_att, src, o_ratt, 2, 1, L, dim, SH_NONE, {1.35, 0.35, 0.25f, 2.4f}));
     L2B_TRY(materialize(ctx, &ctx->wq, src, o_wq, 3, L, dim, dim, SH_ROWS, {0.0, 0.04 * sd, -BIG, BIG}, true));
@@ -1510,34 +1509,44 @@ void kv_drop(l2b_ctx *ctx, int j) {
     ctx->pages[j] = nullptr;
     kv_tab_set(ctx, j, nullptr);
 }
-// Rows [0, rows) of every layer, K and V, of page src into the nd pages dst: kv_fork_kernel with one
-// page as the "cache" (segments of rows * kv_loc elements, layers 2P rows apart), on ctx's stream.
-template <typename KV>
-int kv_page_copy(l2b_ctx *ctx, const void *src, void *const *dst, int nd, int rows) {
-    const size_t half = (size_t)KV_PAGE_ROWS * ctx->kv_loc;
-    KvForkParams<KV> p{};
-    p.k = static_cast<const KV *>(src);
-    p.v = p.k + half;
-    p.seg = (long long)rows * ctx->kv_loc;
-    p.stride = 2ll * half;
-    p.L = ctx->cfg.n_layers;
-    const int gy = std::min(2 * p.L, 65535);
-    const int gx = (int)(((p.seg >> 2) + NT - 1) / NT);
-    for (int g = 0; g < nd; g += KV_FORK_MAXD) {
-        p.nd = std::min(KV_FORK_MAXD, nd - g);
-        for (int d = 0; d < p.nd; ++d) {
-            p.dk[d] = static_cast<KV *>(dst[g + d]);
-            p.dv[d] = p.dk[d] + half;
+// kv_fork_kernel on ctx's stream: in every layer l, the segments of seg elements at k + l * stride and
+// v + l * stride into the same offsets from every destination pair dst[d] = (K base, V base), KV_FORK_MAXD
+// destinations per launch.  One 4-element unit per thread: on llama2-7B (fp32) this grid beat one resident
+// wave of grid-striding CTAs (8 per SM) by 5-12 % at every n_pos and destination count measured, and
+// cudaMemcpy at one destination (DESIGN.md §4.5g).
+int kv_fork_launch(l2b_ctx *ctx, const void *k, const void *v, long long seg, long long stride,
+                   const std::vector<std::pair<void *, void *>> &dst) {
+    return with_kv_elem(ctx->kvfmt, [&](auto e) -> int {
+        using E = typename decltype(e)::type;
+        KvForkParams<E> p{};
+        p.k = static_cast<const E *>(k);
+        p.v = static_cast<const E *>(v);
+        p.seg = seg;
+        p.stride = stride;
+        p.L = ctx->cfg.n_layers;
+        const int gy = std::min(2 * p.L, 65535);
+        const int gx = (int)std::min(((seg >> 2) + NT - 1) / NT, (long long)INT32_MAX);
+        for (size_t g = 0; g < dst.size(); g += KV_FORK_MAXD) {
+            p.nd = (int)std::min(dst.size() - g, (size_t)KV_FORK_MAXD);
+            for (int d = 0; d < p.nd; ++d) {
+                p.dk[d] = static_cast<E *>(dst[g + d].first);
+                p.dv[d] = static_cast<E *>(dst[g + d].second);
+            }
+            void *args[] = {&p};
+            const int rc = launch_small(ctx, (const void *)kv_fork_kernel<E>, dim3(gx, gy), dim3(NT), args, ctx->stream, false);
+            if (rc) return rc;
         }
-        void *args[] = {&p};
-        const int rc = launch_small(ctx, (const void *)kv_fork_kernel<KV>, dim3(gx, gy), dim3(NT), args, ctx->stream, false);
-        if (rc) return rc;
-    }
-    return L2B_OK;
+        return L2B_OK;
+    });
 }
+// Rows [0, rows) of every layer, K and V, of page src into the nd pages dst: one page as the "cache" (layers
+// 2P rows apart, V rows P rows after K rows).
 int kv_page_copy(l2b_ctx *ctx, const void *src, void *const *dst, int nd, int rows) {
-    return kv_bf16(ctx) ? kv_page_copy<bf16>(ctx, src, dst, nd, rows)
-           : kv_e4m3(ctx) ? kv_page_copy<e4m3>(ctx, src, dst, nd, rows) : kv_page_copy<float>(ctx, src, dst, nd, rows);
+    const long long half = (long long)KV_PAGE_ROWS * ctx->kv_loc;   // elements
+    const size_t half_bytes = (size_t)half * kv_elem(ctx);
+    std::vector<std::pair<void *, void *>> d;
+    for (int i = 0; i < nd; ++i) d.emplace_back(dst[i], static_cast<unsigned char *>(dst[i]) + half_bytes);
+    return kv_fork_launch(ctx, src, static_cast<const unsigned char *>(src) + half_bytes, (long long)rows * ctx->kv_loc, 2 * half, d);
 }
 
 // rows [lo, hi) that a call may write into session s's cache (a paged session; one call lists no other)
@@ -1623,8 +1632,7 @@ int create_run_state(l2b_ctx *ctx) {
         // results/h100_policy_ab.txt)
         const char *ef = getenv("L2B_FUSE");
         const int want = ef ? atoi(ef) : (dim <= 512 ? 1 : 0);
-        size_t smem_aw = 0;
-        ctx->fuse_attn = (want & 1) && world == 1 && dim < 1024 && pick_attn_wo((int)hs, &smem_aw) != nullptr;
+        ctx->fuse_attn = (want & 1) && world == 1 && dim < 1024 && pick_attn_wo((int)hs) != nullptr;
         if (ctx->fuse_attn) L2B_TRY(dev_alloc(ctx, &ctx->attn_parts, (size_t)cfg->n_heads * dim));
     }
     L2B_TRY(dev_alloc(ctx, &ctx->delta, dim));
@@ -1687,14 +1695,13 @@ int create_run_state(l2b_ctx *ctx) {
             g_create_error = ctx->err;
             return L2B_ERR_UNSUPPORTED;
         }
-        L2B_TRY(cuda_try(ctx, cudaFuncSetAttribute(attention_3pass(kv_kernels(ctx)), cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem), "cudaFuncSetAttribute"));
+        L2B_TRY(cuda_try(ctx, cudaFuncSetAttribute(pick_attention(ctx, false), cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem), "cudaFuncSetAttribute"));
         // past the 48 KiB a kernel gets without opting in (long paged contexts only); kMaxDynSmem, as for
         // the 3-pass kernel, so another context's smaller request never lowers it
-        size_t unused = 0;
         if (req_flash > kDefaultDynSmem)
-            L2B_TRY(cuda_try(ctx, cudaFuncSetAttribute(pick_attention((int)hs, true, &unused, kv_kernels(ctx)), cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem), "cudaFuncSetAttribute"));
+            L2B_TRY(cuda_try(ctx, cudaFuncSetAttribute(pick_attention(ctx, true), cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem), "cudaFuncSetAttribute"));
         if (req_wo > kDefaultDynSmem)
-            L2B_TRY(cuda_try(ctx, cudaFuncSetAttribute(pick_attn_wo((int)hs, &unused, ctx->wfmt, kv_kernels(ctx)), cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem), "cudaFuncSetAttribute"));
+            L2B_TRY(cuda_try(ctx, cudaFuncSetAttribute(pick_attn_wo(ctx), cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem), "cudaFuncSetAttribute"));
         L2B_TRY(dev_alloc(ctx, &ctx->part_o, (size_t)ctx->heads_loc * ns * hs));
         L2B_TRY(dev_alloc(ctx, &ctx->part_ml, (size_t)ctx->heads_loc * ns * 2));
         L2B_TRY(dev_alloc(ctx, &ctx->counters, (size_t)ctx->heads_loc));
@@ -1908,7 +1915,7 @@ int kv_null_clear(l2b_ctx *ctx) {
 
 int common_create(l2b_ctx **out, const l2b_config *cfg, const Source &src, uint64_t n_floats,
                   const float *rope_cos, const float *rope_sin, const l2b_shard *shard, int n_gpus,
-                  int wfmt = L2B_WEIGHTS_F32, int kvfmt = 0) {
+                  int wfmt = L2B_WEIGHTS_F32, int kvfmt = 0, bool paged = false) {
     if (!out || !cfg) { g_create_error = "NULL argument"; return L2B_ERR_INVALID_ARG; }
     *out = nullptr;
     const bool in_process = n_gpus > 1;
@@ -1941,8 +1948,8 @@ int common_create(l2b_ctx **out, const l2b_config *cfg, const Source &src, uint6
         l2b_ctx *ctx = new l2b_ctx();
         ranks.push_back(ctx);
         ctx->wfmt = wfmt;
-        ctx->kvfmt = kvfmt & ~L2B_KV_PAGED;
-        ctx->paged = (kvfmt & L2B_KV_PAGED) != 0;
+        ctx->kvfmt = kvfmt;
+        ctx->paged = paged;
         const int rank = in_process ? i : (shard ? shard->rank : 0);
         const int device = in_process ? i : device0;
         rc = create_rank(ctx, cfg, src, rope_cos, rope_sin, rank, world, device);
@@ -2145,14 +2152,14 @@ int32_t l2b_create_synthetic_group(l2b_ctx **out, const l2b_config *cfg, uint64_
 }
 
 // weight_format of l2b_create_format: a weight format, with at most one of L2B_KV_BF16, L2B_KV_ROUND_BF16,
-// L2B_KV_E4M3 and L2B_KV_ROUND_E4M3 and optionally L2B_KV_PAGED or'd in.  Any other value =>
-// L2B_ERR_INVALID_ARG.
-bool split_format(int32_t weight_format, int *wfmt, int *kvfmt) {
+// L2B_KV_E4M3 and L2B_KV_ROUND_E4M3 and optionally L2B_KV_PAGED or'd in; split into the weight format, the
+// KV element format and the layout.  Any other value => L2B_ERR_INVALID_ARG.
+bool split_format(int32_t weight_format, int *wfmt, int *kvfmt, bool *paged) {
     const int elem = L2B_KV_BF16 | L2B_KV_ROUND_BF16 | L2B_KV_E4M3 | L2B_KV_ROUND_E4M3;
-    *kvfmt = weight_format & (elem | L2B_KV_PAGED);
+    *kvfmt = weight_format & elem;
+    *paged = (weight_format & L2B_KV_PAGED) != 0;
     *wfmt = weight_format & ~(elem | L2B_KV_PAGED);
-    const int e = *kvfmt & elem;
-    if ((*wfmt != L2B_WEIGHTS_F32 && *wfmt != L2B_WEIGHTS_BF16 && *wfmt != L2B_WEIGHTS_Q8) || (e & (e - 1)) != 0) {
+    if ((*wfmt != L2B_WEIGHTS_F32 && *wfmt != L2B_WEIGHTS_BF16 && *wfmt != L2B_WEIGHTS_Q8) || (*kvfmt & (*kvfmt - 1)) != 0) {
         g_create_error = "unknown weight format";
         return false;
     }
@@ -2162,19 +2169,21 @@ bool split_format(int32_t weight_format, int *wfmt, int *kvfmt) {
 int32_t l2b_create_format(l2b_ctx **out, const l2b_config *cfg, const float *host_weights, uint64_t n_floats,
                           const float *rope_cos, const float *rope_sin, int32_t n_gpus, int32_t weight_format) {
     int wfmt, kvfmt;
-    if (!split_format(weight_format, &wfmt, &kvfmt)) return L2B_ERR_INVALID_ARG;
+    bool paged;
+    if (!split_format(weight_format, &wfmt, &kvfmt, &paged)) return L2B_ERR_INVALID_ARG;
     if (weight_format == L2B_WEIGHTS_F32) return l2b_create(out, cfg, host_weights, n_floats, rope_cos, rope_sin, n_gpus);
     if (!host_weights) { g_create_error = "host_weights is NULL"; return L2B_ERR_INVALID_ARG; }
     if (n_gpus != 1) { g_create_error = "bf16 and q8 weights and bf16, e4m3 or paged KV caches are single-GPU (n_gpus must be 1)"; return L2B_ERR_UNSUPPORTED; }
     Source s; s.host = host_weights;
-    return common_create(out, cfg, s, n_floats, rope_cos, rope_sin, nullptr, 1, wfmt, kvfmt);
+    return common_create(out, cfg, s, n_floats, rope_cos, rope_sin, nullptr, 1, wfmt, kvfmt, paged);
 }
 
 int32_t l2b_create_synthetic_format(l2b_ctx **out, const l2b_config *cfg, uint64_t seed, int32_t weight_format) {
     int wfmt, kvfmt;
-    if (!split_format(weight_format, &wfmt, &kvfmt)) return L2B_ERR_INVALID_ARG;
+    bool paged;
+    if (!split_format(weight_format, &wfmt, &kvfmt, &paged)) return L2B_ERR_INVALID_ARG;
     Source s; s.host = nullptr; s.seed = seed;
-    return common_create(out, cfg, s, 0, nullptr, nullptr, nullptr, 1, wfmt, kvfmt);
+    return common_create(out, cfg, s, 0, nullptr, nullptr, nullptr, 1, wfmt, kvfmt, paged);
 }
 
 int32_t l2b_kv_info(const l2b_ctx *ctx, int32_t *kv_format, uint64_t *cache_bytes) {
@@ -2288,37 +2297,7 @@ int32_t l2b_reset(l2b_ctx *ctx) {
     return L2B_OK;
 }
 
-}  // extern "C" (a template below)
-
-// Rows [0, n_pos) of src's caches into every destination: kv_fork_kernel<KV>, KV_FORK_MAXD destinations per
-// launch, on src's stream.
-template <typename KV>
-int fork_launch(l2b_ctx *src, int32_t n_pos, l2b_ctx *const *dst, int32_t n_dst) {
-    const int L = src->cfg.n_layers;
-    KvForkParams<KV> p{};
-    p.k = static_cast<const KV *>(src->kcache);
-    p.v = static_cast<const KV *>(src->vcache);
-    p.seg = (long long)n_pos * src->kv_loc;
-    p.stride = (long long)src->cfg.seq_len * src->kv_loc;
-    p.L = L;
-    // One 4-element unit per thread: on llama2-7B (fp32) this grid beat one resident wave of grid-striding
-    // CTAs (8 per SM) by 5-12 % at every n_pos and destination count measured, and cudaMemcpy at one
-    // destination (DESIGN.md §4.5g).
-    const int gy = std::min(2 * L, 65535);
-    const long long chunks = ((p.seg >> 2) + NT - 1) / NT;
-    const int gx = (int)std::min(chunks, (long long)INT32_MAX);
-    for (int g = 0; g < n_dst; g += KV_FORK_MAXD) {
-        p.nd = std::min(KV_FORK_MAXD, n_dst - g);
-        for (int d = 0; d < p.nd; ++d) {
-            p.dk[d] = static_cast<KV *>(dst[g + d]->kcache);
-            p.dv[d] = static_cast<KV *>(dst[g + d]->vcache);
-        }
-        void *args[] = {&p};
-        const int rc = launch_small(src, (const void *)kv_fork_kernel<KV>, dim3(gx, gy), dim3(NT), args, src->stream, false);
-        if (rc) return rc;
-    }
-    return L2B_OK;
-}
+}  // extern "C" (a helper below)
 
 // l2b_fork on a paged model: every destination gives up its pages, then shares src's full pages [0, n_pos/P)
 // and gets a fresh page holding a copy of the rows of src's partial last page, [n_pos/P * P, n_pos).  The
@@ -2393,8 +2372,10 @@ int32_t l2b_fork(l2b_ctx *src, int32_t n_pos, l2b_ctx *const *dst, int32_t n_dst
         cudaStream_t st = src->stream;
         L2B_CUDA(src, cudaSetDevice(src->device));
         L2B_CUDA(src, cudaEventRecord(src->ev0, st));
-        const int rc = kv_bf16(src) ? fork_launch<bf16>(src, n_pos, dst, n_dst)
-                       : kv_e4m3(src) ? fork_launch<e4m3>(src, n_pos, dst, n_dst) : fork_launch<float>(src, n_pos, dst, n_dst);
+        std::vector<std::pair<void *, void *>> d;
+        for (int i = 0; i < n_dst; ++i) d.emplace_back(dst[i]->kcache, dst[i]->vcache);
+        const int rc = kv_fork_launch(src, src->kcache, src->vcache, (long long)n_pos * src->kv_loc,
+                                      (long long)src->cfg.seq_len * src->kv_loc, d);
         if (rc) return rc;
         L2B_CUDA(src, cudaEventRecord(src->ev1, st));
         L2B_CUDA(src, cudaEventSynchronize(src->ev1));
@@ -2459,21 +2440,13 @@ int32_t l2b_forward_sample(l2b_ctx *ctx, int32_t token, int32_t pos, float tempe
 }  // extern "C" (templates below)
 
 // ---- batched prompt prefill (prefill_gemm_kernel in l2b_device.cuh) -----------------------------
-template <int NB, typename W>
-gemv_fn pf_pick(int epi, int ks) {
-    switch (epi) {
-    case EPI_QKV:
-        return kv_dispatch(ks, [](auto t) { return (gemv_fn)prefill_gemm_kernel<EPI_QKV, NB, W, typename decltype(t)::type>; });
-    case EPI_SILU: return prefill_gemm_kernel<EPI_SILU, NB, W>;
-    case EPI_STORE: return prefill_gemm_kernel<EPI_STORE, NB, W>;
-    case EPI_ARGMAX: return prefill_gemm_kernel<EPI_ARGMAX, NB, W>;
-    default: return prefill_gemm_kernel<EPI_RESID, NB, W>;
-    }
-}
+// the batched-prefill kernel of NB vectors for the context's formats (no EPI_XCHG: single GPU only)
 template <int NB>
 gemv_fn pf_pick(const l2b_ctx *ctx, int epi) {
-    const int ks = kv_store(ctx);
-    return is_q8(ctx) ? pf_pick<NB, q8>(epi, ks) : is_bf16(ctx) ? pf_pick<NB, bf16>(epi, ks) : pf_pick<NB, float>(epi, ks);
+    return with_w(ctx->wfmt, [&](auto w) {
+        using W = typename decltype(w)::type;
+        return pick_epi<W, false>(ctx, epi, [](auto e, auto kv) { return (gemv_fn)prefill_gemm_kernel<decltype(e)::value, NB, W, typename decltype(kv)::type>; });
+    });
 }
 constexpr size_t kPfSmemBudget = 227 * 1024 - 8192;   // the prefill kernels keep ~6.5 KB of static shared memory
 
@@ -2521,7 +2494,7 @@ static int pf_launch(l2b_ctx *ctx, int epi, GemvParams p, cudaStream_t st) {
     const size_t xbytes = (size_t)NB * p.n * 4;
     const int nstage = pf_ring_stages(kPfSmemBudget, xbytes);
     // the same ring bytes in the format's stages: 32 KB fp32, 16 KB bf16, 17 KB q8
-    p.nstage = is_q8(ctx) ? pf_stages<q8>(nstage) : is_bf16(ctx) ? pf_stages<bf16>(nstage) : nstage;
+    p.nstage = with_w(ctx->wfmt, [nstage](auto w) { return pf_stages<typename decltype(w)::type>(nstage); });
     int grid = ctx->num_sms;
     const int npairs = (p.total_rows + 1) / 2;
     if (grid > npairs) grid = npairs;
@@ -2536,7 +2509,9 @@ static int pf_launch(l2b_ctx *ctx, int epi, GemvParams p, cudaStream_t st) {
     cudaLaunchAttribute at[1] = {pdl_attr()};
     lc.attrs = at;
     lc.numAttrs = ctx->use_pdl ? 1 : 0;
-    L2B_CUDA(ctx, cudaLaunchKernelEx(&lc, pf_pick<NB>(ctx, epi), p));
+    const gemv_fn fn = pf_pick<NB>(ctx, epi);
+    if (!fn) return fail(ctx, L2B_ERR_UNSUPPORTED, "batched prefill: no kernel for this epilogue");
+    L2B_CUDA(ctx, cudaLaunchKernelEx(&lc, fn, p));
     ++ctx->last_launches;
     return L2B_OK;
 }
@@ -3929,54 +3904,38 @@ int32_t l2b_read_state(l2b_ctx *ctx, int32_t which, float *dst, uint64_t n, uint
     }
     if (n < cnt) return fail(ctx, L2B_ERR_INVALID_ARG, "dst too small");
     L2B_CUDA(ctx, cudaSetDevice(ctx->device));
-    if ((which == 4 || which == 5) && ctx->paged) {
-        // gathered page by page into the contiguous layout; rows of pages the context does not hold are 0
-        memset(dst, 0, cnt * sizeof(float));
-        const size_t el = kv_elem(ctx), P = KV_PAGE_ROWS, kvl = ctx->kv_loc;
-        std::vector<unsigned char> page(kv_page_bytes(ctx));
-        for (int j = 0; j < ctx->n_pages; ++j) {
-            if (!ctx->pages[j]) continue;
-            L2B_CUDA(ctx, cudaMemcpy(page.data(), ctx->pages[j], page.size(), cudaMemcpyDeviceToHost));
-            const uint64_t rows = std::min<uint64_t>(P, S - j * P);
-            for (uint64_t l = 0; l < L; ++l) {
-                const unsigned char *from = page.data() + ((2 * l + (which == 5)) * P) * kvl * el;
-                float *to = dst + (l * S + j * P) * kvl;
-                const float s = kv_e4m3(ctx) ? ctx->weights->kv_scale_h[2 * l + (which == 5)] : 1.0f;
-                for (uint64_t i = 0; i < rows * kvl; ++i) {
-                    if (el == 1) {
-                        to[i] = e4m3_widen(from[i], s);
-                    } else if (el == 2) {
-                        uint16_t h;
-                        memcpy(&h, from + 2 * i, 2);
-                        const uint32_t u = (uint32_t)h << 16;
-                        memcpy(to + i, &u, 4);
-                    } else {
-                        memcpy(to + i, from + 4 * i, 4);
-                    }
-                }
-            }
-        }
-    } else if ((which == 4 || which == 5) && kv_bf16(ctx)) {
-        // the bf16 cache lands in the upper half of dst and is widened in place from the front: value i is
-        // written to bytes [4i, 4i+4), below the unread values at [2 cnt + 2i, ..) for every i < cnt
-        uint16_t *h = reinterpret_cast<uint16_t *>(dst) + cnt;
-        L2B_CUDA(ctx, cudaMemcpy(h, src, cnt * 2, cudaMemcpyDeviceToHost));
-        for (uint64_t i = 0; i < cnt; ++i) {
-            const uint32_t u = (uint32_t)h[i] << 16;
-            memcpy(dst + i, &u, 4);
-        }
-    } else if ((which == 4 || which == 5) && kv_e4m3(ctx)) {
-        // the codes land in the last quarter of dst and are widened from the front: value i is written to
-        // bytes [4i, 4i+4), below the unread codes at [3 cnt + i, ..) for every i < cnt
-        uint8_t *c = reinterpret_cast<uint8_t *>(dst) + 3 * cnt;
-        L2B_CUDA(ctx, cudaMemcpy(c, src, cnt, cudaMemcpyDeviceToHost));
-        const uint64_t per_layer = S * ctx->kv_loc;
-        for (uint64_t i = 0; i < cnt; ++i) dst[i] = e4m3_widen(c[i], ctx->weights->kv_scale_h[2 * (i / per_layer) + (which == 5)]);
-    } else {
+    if (which != 4 && which != 5) {
         L2B_CUDA(ctx, cudaMemcpy(dst, src, cnt * sizeof(float), cudaMemcpyDeviceToHost));
+        if (n_out) *n_out = cnt;
+        return L2B_OK;
     }
-    if (n_out) *n_out = cnt;
-    return L2B_OK;
+    // The cache widened to fp32 layer by layer, each e4m3 layer with its own scale.  A paged cache is gathered
+    // page by page into the contiguous layout, and rows of pages the context does not hold are 0.  A contiguous
+    // cache of el-byte elements lands in the last el/4 of dst and is widened in place from the front: value i
+    // is written to bytes [4i, 4i+4), below the unread elements at [cnt (4 - el) + el (i+1), ..).
+    const int v = which == 5;
+    const uint64_t kvl = ctx->kv_loc, P = KV_PAGE_ROWS;
+    return with_kv_elem(ctx->kvfmt, [&](auto e) -> int32_t {
+        const size_t el = sizeof(typename decltype(e)::type);
+        auto widen = [&](const unsigned char *from, uint64_t l, uint64_t row0, uint64_t rows) {
+            kv_widen(e, from, dst + (l * S + row0) * kvl, rows * kvl, kv_scaled(ctx->kvfmt) ? ctx->weights->kv_scale_h[2 * l + v] : 1.0f);
+        };
+        if (ctx->paged) {
+            memset(dst, 0, cnt * sizeof(float));
+            std::vector<unsigned char> page(kv_page_bytes(ctx));
+            for (int j = 0; j < ctx->n_pages; ++j) {
+                if (!ctx->pages[j]) continue;
+                L2B_CUDA(ctx, cudaMemcpy(page.data(), ctx->pages[j], page.size(), cudaMemcpyDeviceToHost));
+                for (uint64_t l = 0; l < L; ++l) widen(page.data() + (2 * l + v) * P * kvl * el, l, j * P, std::min<uint64_t>(P, S - j * P));
+            }
+        } else {
+            unsigned char *h = reinterpret_cast<unsigned char *>(dst) + cnt * (4 - el);
+            L2B_CUDA(ctx, cudaMemcpy(h, src, cnt * el, cudaMemcpyDeviceToHost));
+            for (uint64_t l = 0; l < L; ++l) widen(h + l * S * kvl * el, l, 0, S);
+        }
+        if (n_out) *n_out = cnt;
+        return L2B_OK;
+    });
 }
 
 int32_t l2b_last_timing(const l2b_ctx *ctx, float *device_ms, int32_t *kernel_launches) {
